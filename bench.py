@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the READ per-frame render hot path on B200 (driver contract: one JSON line on stdout).
+"""Benchmark of the READ per-frame render hot path on H100 (one JSON line on stdout).
 
-    python bench.py --gpus 1 --steps K --warmup W [--config c1|c2|c3]   # our arm
+    python bench.py --gpus 1 --steps K --warmup W [--config c1|c2|c3] [--dump-outputs DIR]   # our arm
     python bench.py --impl reference --gpus 1 ...                       # the reference's CPU path (oracle port) on host cores
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
@@ -15,10 +15,14 @@ views, ONE NCCL reduce-scatter(min) of the packed level-0 z-buffers so that rank
 
 Output keys (DESIGN.md "Measurement"): value = frames/s with all inputs resident in HBM; e2e = frames/s through the public plugin
 call (FrameRenderer.infer: host matrix inverse, H2D of the camera, D2H of the displayable frame, stream sync) - the headline;
-roofline = the dominant kernel family (tcgen05 3x3 gated convs, tensor bound) measured live with CUDA events against the BURST
+roofline = the dominant kernel family (wgmma 3x3 gated convs, tensor bound) measured live with CUDA events against the dense
 bf16 peak (launches timed in sequence, CUDA events between them); roofline_raster = rasterizer + gather against HBM bandwidth; parity = the timed frame
 checked against the oracle (index maps bit-exact, RGB within the stated tolerance); cpu_baseline = the oracle port on the host
-cores (one full frame); reference_gpu = the reference's own GPU path (its pcpr kernel + torch/cuDNN fp32 net) on this box.
+cores (one full frame); reference_gpu = the reference's own GPU path (its pcpr kernel + torch/cuDNN fp32 net) on this machine.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (the RGB frame [1, 3, H, W], float32) as
+DIR/frame.npy; scene, descriptors, weights and cameras are seeded, so two builds run with the same arguments can be compared
+output for output.
 """
 import argparse
 import json
@@ -51,26 +55,14 @@ def metric_name(cfg):
     return f"frames/sec @{w}x{hn}, {n // 1_000_000}M pts" if n >= 1_000_000 else f"frames/sec @{w}x{hn}, {n // 1000}k pts"
 
 
-def measured_traffic():
-    """DRAM bytes per launch from the committed ncu captures (profiles/r02_traffic.json, else r01); None if absent."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        try:
-            d = json.load(open(p))
-            d["_src"] = "profiles/" + name
-            return d
-        except Exception:
-            continue
-    return None
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "MEASURED_PEAKS.json"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 - a ceiling, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -203,7 +195,7 @@ def base_config(cfg):
 
 def run_reference_arm(args):
     """The reference's own CPU implementation of the path (oracle port: the reference's GPU rasterizer has no CPU build and its
-    Python modules cannot travel to the GPU box) on this box's host cores, full frames, same workload / config keys as our arm.
+    Python modules are not part of this repository) on this box's host cores, full frames, same workload / config keys as our arm.
     --steps / --warmup are honoured up to a wall-clock budget (a C3 frame costs ~20 s of CPU time); the line says what ran."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -247,7 +239,7 @@ def run_reference_arm(args):
 
 # ---------------------------------------------------------------------------------------------- reference GPU path
 def reference_gpu_block(cfg, xyz_np, tex_cn, sd, dev, frames=3):
-    """What a READ user has on this box today (SURVEY §8d "kernel to beat"): the UNMODIFIED reference rasterizer (oracle/_ref,
+    """What a READ user has on this machine today (SURVEY §8d "kernel to beat"): the UNMODIFIED reference rasterizer (oracle/_ref,
     compiled from its own sources) called like src/READ/gl/myrender.py:32-40 - CPU tensors in, one pcpr.forward per level, CPU
     tensors out - followed by the reference's torch modules on the GPU in fp32 (oracle/unet_ref.py restates them op for op:
     index_select gather + cuDNN convs), with cuDNN's TF32 default and with TF32 off."""
@@ -256,7 +248,7 @@ def reference_gpu_block(cfg, xyz_np, tex_cn, sd, dev, frames=3):
     from read_b200 import synth
     pcpr = build_ref.load()
     if pcpr is None:
-        return {"unavailable": "oracle/_ref/pcpr*.so not built (needs /root/reference at build time)"}
+        return {"unavailable": "oracle/_ref/pcpr*.so not built (needs a checkout of the reference at build time, oracle/build_ref.py)"}
     _, W, H, _, _, _ = CONFIGS[cfg]
     pts = torch.from_numpy(xyz_np)
     sd_d = {k: v.to(dev) for k, v in sd.items()}
@@ -390,8 +382,10 @@ def run_ours(args):
             ms = float(t.item())
         return ms
 
+    last_out = [None]
+
     def resident_step(s):
-        step(mats_dev[s], mats_dev[s + 1] if s + 1 < total else None)
+        last_out[0] = step(mats_dev[s], mats_dev[s + 1] if s + 1 < total else None)
 
     if world == 1:
         def e2e_step(s):
@@ -441,7 +435,7 @@ def run_ours(args):
     torch.cuda.synchronize()
     launches_per_step = (2 + eng.n_launches()) if world == 1 else (4 + eng.n_launches())
     if args.profile_timed_region:
-        # ncu --profile-from-start off: the capture holds exactly the launches of the timed steps (the launch list under profiles/);
+        # ncu --profile-from-start off: the capture holds exactly the launches of the timed steps;
         # numbers printed by such a run are not bench values, so nothing else is measured
         torch.cuda.synchronize()
         torch.cuda.cudart().cudaProfilerStart()
@@ -455,6 +449,9 @@ def run_ours(args):
     join_side = (lambda: torch.cuda.current_stream().wait_stream(sfs.side)) if world > 1 else None   # K rasters inside K timed steps
     ms_res = timed(resident_step, args.steps, args.warmup, finish=join_side)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "frame.npy"), last_out[0].float().cpu().numpy())
     if world == 1:
         pyr.clear()
     for s in range(min(3, args.warmup)):
@@ -553,22 +550,19 @@ def run_ours(args):
     # feature write (8 * s).  The packed z is counted ONCE.
     rg_bytes = 12 * count + P * (8 + 32 + 8 * feat_bytes)
     hbm = pk["hbm_gbs"]
-    tens_peak = pk["bf16_tflops"]            # the conservative denominator: the burst peak, although the layers are timed in sequence
+    tens_peak = pk["bf16_tflops"]
     roof_tc = None
-    traf = measured_traffic()
     if tc_ms > 0:
         ach = tc_flops / (tc_ms * 1e-3) / 1e12
-        kern = {"C32": "gated_conv_tc_kernel (one CTA, resident weights)", "C64": "gated_conv_tc2_kernel (CTA pair, resident weights)",
-                "C128": "gated_conv_tc2s_kernel (CTA pair, streamed weights)", "C256": "gated_conv_tc2s_kernel (CTA pair, streamed weights)"}
-        roof_tc = {"kernel": "tcgen05 implicit-GEMM gated conv, 3x3 stride-1 instances (gated_conv_tc_kernel / gated_conv_tc2_kernel / "
-                             f"gated_conv_tc2s_kernel) = {100.0 * tc_flops / max(eng.flops, 1):.1f}% of the net's conv FLOPs", "bound": "tensor",
+        kern = {"C32": "gated_conv_tc_kernel (resident weights)", "C64": "gated_conv_tc_kernel (resident weights)",
+                "C128": "gated_conv_tc_kernel (streamed weights)", "C256": "gated_conv_tc_kernel (streamed weights)"}
+        roof_tc = {"kernel": "wgmma implicit-GEMM gated conv, 3x3 stride-1 instances (gated_conv_tc_kernel) = "
+                             f"{100.0 * tc_flops / max(eng.flops, 1):.1f}% of the net's conv FLOPs", "bound": "tensor",
                    "by_class": {k_: {"layers": v_[0], "us_per_layer": 1e3 * v_[1] / v_[0], "tflops": v_[2] / (v_[1] * 1e-3) / 1e12,
                                      "frac": v_[2] / (v_[1] * 1e-3) / 1e12 / tens_peak, "kernel": kern[k_]} for k_, v_ in tc_classes.items()},
                    "achieved": ach, "peak": tens_peak, "unit": "TFLOP/s", "frac": ach / tens_peak,
-                   "peak_src": pk["src"] + " bf16_tflops (burst figure; launches timed in sequence inside the eager replay of the net)",
+                   "peak_src": pk["src"] + " bf16_tflops (launches timed in sequence inside the eager replay of the net)",
                    "frac_of_sustained": ach / pk["bf16_tflops_sustained"], "sustained_peak": pk["bf16_tflops_sustained"],
-                   "traffic": (traf or {}).get("gated_conv_tc_kernel_avg_bytes_per_launch"),
-                   "traffic_src": (traf or {}).get("_src"),
                    "ms_per_frame": tc_ms,
                    "whole_net_tflops_in_graph": eng.flops / (ms_res / args.steps * 1e-3) / 1e12,
                    "layers": sum(1 for l_ in eng.layers if l_.impl == L.CONV_TCGEN05 and l_.k == 3 and l_.stride == 1)}
@@ -576,8 +570,6 @@ def run_ours(args):
     roof_raster = {"kernel": "raster_stream_kernel + pyramid_resolve_gather_kernel",
                    "bound": "hbm",
                    "achieved": ach_r, "peak": hbm, "unit": "GB/s", "frac": ach_r / hbm, "peak_src": pk["src"],
-                   "traffic": ((traf.get("raster_stream_kernel_bytes_per_launch", traf.get("raster_sorted_kernel_bytes_per_launch", 0))
-                                + traf.get("pyramid_resolve_gather_bytes_per_launch", 0)) if traf else None),
                    "algorithmic_bytes": rg_bytes, "ms_per_frame": rg_ms,
                    "note": "algorithmic bytes = 12 B per point + 56 B per pyramid pixel (SURVEY 8d, bf16 features); the sorted store holds 16 B per point (xyz + original id)",
                    "project_ms": project_ms, "resolve_gather_ms": resolve_ms}
@@ -718,10 +710,10 @@ def run_ours(args):
             "roofline": roof_tc if roof_tc else roof_raster,
             "roofline_raster": roof_raster,
             "breakdown_ms_per_frame": {"raster_project": project_ms, "pyramid_resolve_gather": resolve_ms, "raster_total": rg_ms,
-                                       "conv_tcgen05_tma_3x3": tc_ms, "conv_tcgen05_tma_other": tco_ms,
-                                       "conv_tcgen05_tma_other_tflops": (tco_flops / (tco_ms * 1e-3) / 1e12 if tco_ms > 0 else None),
-                                       "conv_tcgen05_gather": tcg_ms,
-                                       "conv_tcgen05_gather_tflops": tcg_ach, "conv_generic": gen_ms, "upsample_kernels": aux_ms,
+                                       "conv_wgmma_tma_3x3": tc_ms, "conv_wgmma_tma_other": tco_ms,
+                                       "conv_wgmma_tma_other_tflops": (tco_flops / (tco_ms * 1e-3) / 1e12 if tco_ms > 0 else None),
+                                       "conv_wgmma_gather": tcg_ms,
+                                       "conv_wgmma_gather_tflops": tcg_ach, "conv_generic": gen_ms, "upsample_kernels": aux_ms,
                                        "conv_generic_tflops": gen_ach, "net_flops": eng.flops,
                                        "note": "eager launches timed in sequence with CUDA events between them (PDL off); the frame replays them as one CUDA graph with PDL"},
             "parity": parity,
@@ -916,11 +908,15 @@ def main():
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-reference-gpu", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's output frame as DIR/frame.npy (float32)")
     ap.add_argument("--profile-timed-region", action="store_true",
                     help="cudaProfilerStart/Stop around the timed steps and exit (for ncu --profile-from-start off)")
     ap.add_argument("--layer-times", default=None, help="write per-layer CUDA-event timings (JSON) to this path")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
+    if args.dump_outputs and (args.impl != "ours" or args.config == "c5"):
+        ap.error("--dump-outputs applies to the frame configs (c1 / c2 / c3) of our arm")
     if args.config == "c5":
         if args.impl == "reference":
             print(json.dumps({"impl": "reference", "unavailable": "config c5 (training) has no CPU arm: the reference's training step needs its CUDA rasterizer"}))

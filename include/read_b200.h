@@ -1,5 +1,5 @@
 /*
- * read_b200 — C ABI of the B200-native READ render hot path.
+ * read_b200 — C ABI of the H100-native (sm_90a) READ render hot path.
  *
  * Plain C: pointers, sizes, ints.  No torch / C++ types cross this boundary.
  * All data pointers are CALLER-OWNED DEVICE memory unless a parameter is named
@@ -37,23 +37,16 @@ enum {
 
 int read_version(void);
 const char *read_last_error(void);
-/* Tuning options.  Results are bit-identical for every accepted setting (one exception: "tc_pair_wide" selects a kernel whose K order
- * differs - within one bf16 ulp per layer output); unknown names and out-of-range values are rejected.
+/* Tuning options.  Results are bit-identical for every accepted setting; unknown names and out-of-range values are rejected.
  *   rasterizer: "raster_pipelined" (1), "raster_bulk_tma" (1), "raster_mode" (0..3, default 2), "raster_occupancy" (0 = auto), "raster_stream" (1),
  *               "raster_dedup" (0), "raster_run" (0 = auto), "raster_nbr_filter" (0), "raster_stages" (2; 3 = deeper point ring),
  *               "raster_carveout" (45: preferred shared-memory carveout in percent for the streaming kernel, -1 = driver default)
- *   convs:      read when a plan is created: "tc_mt" (supertile width 1 (default) / 2 / 4, 0 = auto-widen), "tc_merge_done" (1),
- *               "tc_commit_late" (0), "tc_bpair" (0), "tc_probe" (0), "tc_pair" (1: CTA-pair cta_group::2 kernel for the Cin 64 layers and
- *               the Cin 32 layers without a residual, 2: every eligible layer, 0: off), "tc_pair_wide" (1: streamed-weight CTA-pair kernel for
- *               the Cin, Cout = 128 / 256 layers), "tc_wide_ntile" (256; 128 = narrower units for Cout 256, measured slower),
- *               "tc_tma_store" (1: epilogue items staged in shared memory and written by TMA stores; also read at launch by the pair kernel);
- *               read at launch: "tc_role_rot" (1), "tc_pdl" (1: programmatic dependent launch between consecutive conv kernels)
+ *   convs:      read at launch: "tc_pdl" (1: programmatic dependent launch between consecutive conv kernels)
  *   The Python host applies READ_B200_OPTIONS="name=value,..." from the environment when it loads the library.
  * The options are process-wide tuning state (plain ints): set them before creating plans / launching, not concurrently with
- * launches from other threads.  Diagnostic knobs that skip work and therefore corrupt the output ("tc_debug", "tcg_debug",
- * raster_mode 4 / 5) exist only in builds compiled with -DREAD_DIAG and are absent from the shipped library. */
+ * launches from other threads.  Diagnostic knobs that skip work and therefore corrupt the output (raster_mode 4 / 5) exist only in builds compiled with -DREAD_DIAG and are absent from the shipped library. */
 int read_set_option(const char *name, int value);
-/* 1 if the current device is sm_100 (B200); the library refuses to launch elsewhere. */
+/* 1 if the current device is sm_90 (H100); the library refuses to launch elsewhere. */
 int read_device_ok(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -185,7 +178,7 @@ typedef struct read_conv_desc {
     int32_t k, stride, pad;
     int32_t elu;                    /* 1: A = ELU(alpha=1); 0: identity */
     const float *w_generic;         /* packed f32 [k*k*Cin][Npad] (read_pack_weights_generic) or NULL */
-    const void *w_tc;               /* packed bf16 for the tcgen05 kernel (read_pack_weights_tc) or NULL */
+    const void *w_tc;               /* packed bf16 for the wgmma kernels (read_pack_weights_tc) or NULL */
     const float *bias_f, *bias_m;   /* [Cout] */
     const float *bn_scale, *bn_shift; /* [Cout] folded eval-mode BatchNorm */
     const void *residual;           /* optional [B,Hout,Wout,Cout] added after BN (ResBlock / FAM skip) */
@@ -198,7 +191,7 @@ typedef struct read_conv_desc {
      * accumulators BEFORE bias / activation.  A 1x1 conv commutes with nearest upsampling, so
      *   conv1x1(cat[a, up2(b)]) == conv1x1_a(a) + up2(conv1x1_b(b)):
      * the coarse sources of the AFF heads (unet.py:79-89,252-254) are convolved at their own resolution into RAW tensors
-     * and enter here, instead of being gathered 4..64 times each at the fine resolution.  tcgen05 TMA kernel only. */
+     * and enter here, instead of being gathered 4..64 times each at the fine resolution.  TMA-fed wgmma kernel only. */
     const void *addin;
     int32_t addin_H, addin_W;
 } read_conv_desc;
@@ -220,10 +213,10 @@ int read_pack_weights_tc_strided(const float *wf, const float *wm, int Cout, int
 int read_pack_weights_tc_for(const read_conv_desc *d, const float *wf, const float *wm, void *out_bf16, void *stream);
 int read_pack_weights_tc(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16,
                          void *stream);
-/* 1 if the tcgen05 TMA kernel supports this layer (stride-1 k x k / stride-2 3x3, 4x4 single source; 1x1 virtual concat of
+/* 1 if the TMA-fed wgmma kernel supports this layer (stride-1 k x k / stride-2 3x3, 4x4 single source; 1x1 virtual concat of
  * identity / nearest-down sources), else 0. */
 int read_conv_tc_supported(const read_conv_desc *d);
-/* Same for the tcgen05 kernel with a gathered A operand (any stride / concat / resampling, bf16 activations);
+/* Same for the wgmma kernel with a gathered A operand (any stride / concat / resampling, bf16 activations);
  * it has its own weight packing. */
 int read_conv_tcg_supported(const read_conv_desc *d);
 int64_t read_tcg_weight_elems(int Cout, int Cin, int k);

@@ -1,9 +1,9 @@
 """ORACLE — test infrastructure only.
 
-Compile the UNMODIFIED reference extension (MyRender/CloudProjection/{pcpr_cuda.cpp,point_render.cu}) from where
-it lies under /root/reference into oracle/_ref/pcpr*.so with a direct nvcc/g++ recipe (not the reference's
-setup.py).  Only possible in the build container; the built .so travels to the GPU box with the snapshot, where
-tests/test_gpu_reference_kernel.py uses it as "the kernel to beat" and checks ref_depth >= oracle_depth.
+Compile the UNMODIFIED reference extension (MyRender/CloudProjection/{pcpr_cuda.cpp,point_render.cu}) from a checkout of
+the reference (READ_REFERENCE_ROOT, default /root/reference) into oracle/_ref/pcpr*.so with a direct nvcc/g++ recipe (not
+the reference's setup.py).  tests/golden/make_ref_pcpr_golden.py runs it on a GPU and stores its outputs, which
+tests/test_gpu_reference_kernel.py compares against.
 No reference SOURCE is copied into this repository.
 """
 import os
@@ -12,7 +12,8 @@ import sysconfig
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT_DIR = os.path.join(HERE, "_ref")
-SRC = "/root/reference/MyRender/CloudProjection"
+REFERENCE_ROOT = os.environ.get("READ_REFERENCE_ROOT", "/root/reference")
+SRC = os.path.join(REFERENCE_ROOT, "MyRender", "CloudProjection")
 
 
 def so_path():
@@ -36,7 +37,7 @@ def build(force=False):
     o1, o2 = os.path.join(OUT_DIR, "pcpr_cuda.o"), os.path.join(OUT_DIR, "point_render.o")
     subprocess.check_call(["g++", "-O2", "-fPIC", "-std=c++17", "-w"] + defs + inc + ["-c", os.path.join(SRC, "pcpr_cuda.cpp"), "-o", o1])
     subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-O2", "-std=c++17", "-w", "-Xcompiler", "-fPIC",
-                           "-gencode", "arch=compute_100,code=sm_100"] + defs + inc +
+                           "-gencode", "arch=compute_90,code=sm_90"] + defs + inc +
                           ["-c", os.path.join(SRC, "point_render.cu"), "-o", o2])
     libdir = os.path.join(os.path.dirname(torch.__file__), "lib")
     subprocess.check_call(["g++", "-shared", o1, o2, "-o", out, "-L" + libdir, "-L/usr/local/cuda/lib64",

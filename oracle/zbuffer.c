@@ -20,9 +20,9 @@
  *
  * Parity status: the reference ships no golden vectors for this path
  * (SURVEY.md §4) — "parity unpinned" by reference tests; this restatement is
- * pinned by hand-derived known-answer tests (tests/test_oracle_kat.py) and, on
- * the GPU box, against the reference extension built from source
- * (oracle/_ref/pcpr*.so) on collision-free scenes.
+ * pinned by hand-derived known-answer tests (tests/test_oracle_kat.py) and
+ * against the recorded outputs of the reference extension built from source
+ * (tests/golden/ref_pcpr_*.npz) on collision-free scenes.
  *
  * Documented deviations from a literal execution of the racy reference kernel:
  *   - NaN clip coordinates (w == 0 and numerator 0) are culled; the reference

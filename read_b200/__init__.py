@@ -1,4 +1,4 @@
-"""read_b200 — B200-native (sm_100a) implementation of READ's per-frame render hot path.
+"""read_b200 — H100-native (sm_90a) implementation of READ's per-frame render hot path.
 
     points -> packed z-buffer pyramid -> descriptor feature pyramid -> gated-conv refinement net -> RGB
 

@@ -1,13 +1,13 @@
 """ctypes binding of the C-ABI library (include/read_b200.h).
 
-The product path fails LOUDLY when the CUDA library is missing or the device is not a B200:
+The product path fails LOUDLY when the CUDA library is missing or the device is not an H100 (sm_90):
 there is no CPU or eager-PyTorch fallback anywhere in this package.
 """
 import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# READ_B200_LIB: timing-experiment scripts point this at the -DREAD_DIAG build (python -m read_b200.build --diag)
+# READ_B200_LIB: load another build of the library (e.g. the -DREAD_DIAG build: python -m read_b200.build --diag)
 LIB_PATH = os.environ.get("READ_B200_LIB") or os.path.join(_HERE, "libread_b200.so")
 
 c_int, c_i64, c_u32 = ctypes.c_int, ctypes.c_int64, ctypes.c_uint32
@@ -21,7 +21,7 @@ TEXACT = {"none": 0, "sigmoid": 1, "tanh": 2}
 ACT_F32, ACT_BF16 = 0, 1
 SRC_IDENTITY, SRC_NEAREST_DOWN, SRC_NEAREST_UP, SRC_BILINEAR_UP4 = 0, 1, 2, 3
 OUT_NHWC, OUT_NCHW_F32, OUT_RAW_NHWC = 0, 1, 2
-CONV_AUTO, CONV_GENERIC, CONV_TCGEN05, CONV_TCGEN05_GATHER = 0, 1, 2, 3
+CONV_AUTO, CONV_GENERIC, CONV_TCGEN05, CONV_TCGEN05_GATHER = 0, 1, 2, 3   # names kept from the ABI; 2 / 3 are the wgmma kernels
 
 
 class ReadSrc(ctypes.Structure):
@@ -148,16 +148,16 @@ _device_checked = set()
 
 
 def require_device(device_index=None):
-    """Raise unless torch sees a CUDA device of compute capability 10.x (B200)."""
+    """Raise unless torch sees a CUDA device of compute capability 9.0 (H100): the kernels are built for sm_90a only."""
     import torch
     if not torch.cuda.is_available():
         raise RuntimeError("read_b200: no CUDA device; this package has no CPU fallback")
     idx = torch.cuda.current_device() if device_index is None else device_index
     if idx in _device_checked:
         return
-    major, _ = torch.cuda.get_device_capability(idx)
-    if major != 10:
-        raise RuntimeError(f"read_b200: kernels are built for sm_100a only, device {idx} is sm_{major}x")
+    major, minor = torch.cuda.get_device_capability(idx)
+    if (major, minor) != (9, 0):
+        raise RuntimeError(f"read_b200: kernels are built for sm_90a only, device {idx} is sm_{major}{minor}")
     _device_checked.add(idx)
 
 

@@ -1,8 +1,8 @@
-"""Build the C-ABI CUDA library in-tree with nvcc for sm_100a (no JIT, no torch build system).
+"""Build the C-ABI CUDA library in-tree with nvcc for sm_90a (no JIT, no torch build system).
 
     python -m read_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the object files are build products (git-ignored).
 """
 import glob
 import os
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libread_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -61,7 +61,7 @@ def _build(LIB, objdir, extra, verbose):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed building libread_b200.so")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -83,7 +83,7 @@ static int validate_conv(const read_conv_desc &d)
     RB_CHECK_ARG(d.addin == nullptr || (d.addin_H == (d.Hout + 1) / 2 && d.addin_W == (d.Wout + 1) / 2),
                  "conv: addin must be [B, ceil(Hout/2), ceil(Wout/2), 2*Cout]");
     RB_CHECK_ARG((d.out_mode != READ_OUT_RAW_NHWC && d.addin == nullptr) || d.impl == READ_CONV_TCGEN05,
-                 "conv: RAW output / addin are served by the tcgen05 TMA kernel only");
+                 "conv: RAW output / addin are served by the TMA tensor-core kernel only");
     RB_CHECK_ARG((d.out2 == nullptr) == (d.out2_mul == nullptr), "conv: out2 and out2_mul come together");
     RB_CHECK_ARG(d.out2 == nullptr || d.out_mode == READ_OUT_NHWC, "conv: out2 needs NHWC output");
     return READ_OK;
@@ -97,10 +97,11 @@ int64_t read_launch_count(void) { return g_launches.load(); }
 
 int read_device_ok(void)
 {
-    int dev = 0, major = 0;
+    int dev = 0, major = 0, minor = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return 0;
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-    return major == 10 ? 1 : 0;
+    if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+    return (major == 9 && minor == 0) ? 1 : 0;
 }
 
 int read_conv_tc_supported(const read_conv_desc *d)
@@ -131,11 +132,11 @@ int read_conv_plan_create(const read_conv_desc *d, read_conv_plan **out)
     int impl = d->impl;
     RB_CHECK_ARG(impl != READ_CONV_AUTO, "conv plan: choose impl explicitly (the weight packing differs per kernel)");
     if (impl == READ_CONV_TCGEN05) {
-        RB_CHECK_ARG(d->w_tc != nullptr, "conv plan: tcgen05 requested without packed bf16 weights");
-        if (!tc_supported(*d)) { set_error("conv plan: layer shape not supported by the tcgen05 TMA kernel"); return READ_ERR_UNSUPPORTED; }
+        RB_CHECK_ARG(d->w_tc != nullptr, "conv plan: tensor-core kernel requested without packed bf16 weights");
+        if (!tc_supported(*d)) { set_error("conv plan: layer shape not supported by the TMA tensor-core kernel"); return READ_ERR_UNSUPPORTED; }
     } else if (impl == READ_CONV_TCGEN05_GATHER) {
-        RB_CHECK_ARG(d->w_tc != nullptr, "conv plan: tcgen05 requested without packed bf16 weights");
-        if (!tcg_supported(*d)) { set_error("conv plan: layer not supported by the tcgen05 gather kernel"); return READ_ERR_UNSUPPORTED; }
+        RB_CHECK_ARG(d->w_tc != nullptr, "conv plan: tensor-core kernel requested without packed bf16 weights");
+        if (!tcg_supported(*d)) { set_error("conv plan: layer not supported by the gather tensor-core kernel"); return READ_ERR_UNSUPPORTED; }
     } else {
         RB_CHECK_ARG(impl == READ_CONV_GENERIC, "conv plan: unknown impl %d", impl);
         RB_CHECK_ARG(d->w_generic != nullptr, "conv plan: generic kernel needs w_generic");

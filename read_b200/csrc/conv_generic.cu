@@ -1,4 +1,4 @@
-// Generic fused gated convolution on CUDA cores (fp32 accumulate) for sm_100a.
+// Generic fused gated convolution on CUDA cores (fp32 accumulate) for sm_90a.
 //
 // Covers EVERY BasicConv shape of the refinement net (READ/models/unet.py:22-53): k in {1,3,4},
 // stride in {1,2}, any channel count that is a multiple of 8, with the surrounding graph ops fused
@@ -10,7 +10,7 @@
 //   * bias, ELU / identity, sigmoid gate, eval-mode BatchNorm affine (unet.py:44-51)
 //   * residual add (ResBlock unet.py:20, FAM unet.py:116)
 // This is the shape-complete kernel and the fp32 "parity mode" of the net; the dominant 3x3 layers run on
-// the tcgen05 kernel in conv_tc.cu when activations are bf16.
+// the wgmma kernel in conv_tc.cu when activations are bf16.
 #include "common.cuh"
 #include "conv_common.cuh"
 
@@ -283,8 +283,8 @@ __global__ void nhwc_to_nchw_kernel(const TI *__restrict__ in, int B, int C, int
 // One thread per LOW-resolution pixel and 8 channels: the 4x4 output block of a source pixel (X, Y) depends on
 // the 3x3 neighbourhood only, with constant weights (output column 4X + j samples X - 0.375 + j / 4: {3/8 L + 5/8 C,
 // 1/8 L + 7/8 C, 7/8 C + 1/8 R, 5/8 C + 3/8 R}; borders clamp L / R onto C exactly as torch's max(src, 0) / min(i0 + 1, n - 1)).
-// 9 loads, vertical then horizontal lerp in registers, 16 stores: ~35 instructions per output vector instead of ~250 (the
-// round-1 per-output kernel spent its time in three 64-bit divisions per 16 bytes written: 1.5 TB/s).
+// 9 loads, vertical then horizontal lerp in registers, 16 stores: ~35 instructions per output vector instead of ~250 (a
+// per-output kernel spends its time in three 64-bit divisions per 16 bytes written).
 template <typename T>
 __global__ void __launch_bounds__(128) upsample_bilinear4_block_kernel(const T *__restrict__ in, int B, int h, int w, int C, T *__restrict__ out)
 {

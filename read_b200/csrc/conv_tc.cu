@@ -1,33 +1,30 @@
-// Gated convolution as an implicit GEMM on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a.
+// Gated convolution as an implicit GEMM on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 // One kernel computes  y = BN( A(conv_f(x)+b_f) * sigmoid(conv_m(x)+b_m) ) [+ residual]  (BasicConv,
-// READ/models/unet.py:22-53) for stride-1 k x k convolutions over NHWC bf16 activations:
+// READ/models/unet.py:22-53) for stride-1 k x k and stride-2 3x3 / 4x4 convolutions over NHWC bf16 activations:
 //
 //   GEMM view   D[M = 128 output pixels (16 rows x 8 cols of one image), N = f|m channels] +=
 //               A[M, K = one filter tap x CIN_BLK input channels] * B[N, K]
-//   A operand   ONE TMA 4-D tile load {c, x, y, b} per tile and K chunk: the (16+k-1)-row x (8+k-1)-column halo tile.
-//               Every filter tap (ky, kx) reads it through a UMMA descriptor whose start address is advanced by
-//               (ky * halo_w + kx) pixel rows and whose 8-row-group stride (SBO) is halo_w pixel rows: tcgen05.mma
-//               addresses the rows of a swizzled K-major operand linearly (start + (r/8)*SBO + (r%8)*row_bytes) and
-//               applies the swizzle XOR on ABSOLUTE shared-memory address bits, exactly like the TMA unit that wrote
-//               the tile (scripts/experiments/umma_rowshift.cu, verified on B200 for 64B / 128B swizzle, every start
-//               row and group stride tried).  An M tile is therefore 8 pixels wide x 16 rows: its 8-row groups are
-//               8 consecutive pixels of one halo row.  The input is fetched from L2 ONCE per tile (x1.41 halo) instead
-//               of once per filter column (x3.75).  Pixels outside the image are ZERO-FILLED by the TMA unit == the
-//               conv's zero padding (unet.py:29,36).  Rows are CIN_BLK bf16 (64 or 128 bytes) with the matching
-//               64B/128B swizzle: the canonical K-major UMMA layout, no im2col is ever materialised.
-//   B operand   packed weights [tap][kchunk][n][CIN_BLK] bf16, conv_f and conv_m side by side in N so ONE
-//               accumulator tile holds both gates of the same output channels.  When the whole layer fits
-//               (<= 144 KB: the C=32 and C=64 layers) the weights are loaded ONCE per CTA and stay resident in
-//               shared memory; otherwise they stream through their own mbarrier ring.
-//   D           fp32 in TMEM, double buffered (2 x up to 256 columns): the epilogue of tile i overlaps the
-//               MMAs of tile i+1.
-//   epilogue    tcgen05.ld -> bias, ELU, sigmoid gate, BN affine, residual add, bf16 pack -> global
+//   A operand   ONE TMA 4-D tile load {c, x, y, b} per tile and K chunk: the (16+k-1)-row x (8+k-1)-column halo tile, rows of
+//               CIN_BLK bf16 with the matching 32/64/128-byte swizzle.  Every filter tap (ky, kx) reads its 128 pixel rows out of
+//               that tile with ldmatrix (pixel (py + ky, px + kx) of the halo) into wgmma's register A operand, so the input is
+//               fetched once per tile (x1.41 halo) and no im2col is ever materialised.  Pixels outside the image are ZERO-FILLED by
+//               the TMA unit == the conv's zero padding (unet.py:29,36).
+//   B operand   packed weights [tap][kchunk][n][CIN_BLK] bf16, conv_f and conv_m side by side in N so ONE accumulator tile
+//               holds both gates of the same output channels; read by wgmma through K-major shared-memory descriptors.
+//               When the whole layer fits (<= 144 KB: the C=32 and C=64 layers) the weights are loaded ONCE per CTA and stay
+//               resident in shared memory; otherwise they stream through their own mbarrier ring.
+//   D           fp32 in registers: two consumer warpgroups, each owning 64 pixels (8 rows) of the tile.
+//   epilogue    bias, ELU, sigmoid gate, BN affine, residual add, bf16 pack -> global, straight from the accumulators
 //               (optionally a second output y*z for the following FAM, unet.py:115).
 //
-// Warp roles (384 or 640 threads, 1 CTA/SM, persistent over tiles): warp0 = TMA producer, warps 1 and 3 = MMA issuers
-// (alternate tiles), warp2 = TMEM allocator, warps 4.. = epilogue (TMEM lane quadrant = warp%4).  The issuing roles
-// keep their ring indices/phases incrementally: no integer division on the per-k-step path.
+// Warp roles (288 threads, persistent over tiles): warps 0..7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA
+// producer, which runs ahead through the A (and streamed B) rings while the consumers compute.  Layers with N <= 64 whose
+// weights and four A stages fit half the shared-memory budget run two CTAs per SM: one CTA's epilogue overlaps the other's MMAs.
+//
+// Stride 2 (3x3 / 4x4, pad 1): input column 2x + kx - 1 is an EVEN column for kx odd and an ODD one for kx even, so a stage
+// holds four phase tiles E/O x E/O, each loaded by one TMA with traversal stride 2 in x and y (tile[j][i] = in(sx + 2i, sy + 2j),
+// sx = 2*X0 for E, 2*X0 - 1 for O); tap (ky, kx) reads phase tile ((ky+1)&1, (kx+1)&1) at pixel offset (ky>>1, kx>>1).
 #include "common.cuh"
 #include "conv_common.cuh"
 #include "ptx.cuh"
@@ -37,41 +34,22 @@
 
 namespace rb {
 
-// Diagnostic knobs (skip MMAs / loads / epilogue work: WRONG output, timing experiments only) exist only in -DREAD_DIAG builds;
-// the shipped library compiles them out (scripts/tc_debug_times.py builds its own copy).
-#ifdef READ_DIAG
-#define TC_DBG(a_, bit_) (((a_).debug & (bit_)) != 0)
-// per-role timeline of CTA 0: trace[role * 2048 + 1 + i] = (code << 56) | clock64, trace[role * 2048] = count
-#define TC_TRACE(role_, code_)                                                                                          \
-    do {                                                                                                                \
-        if (a.trace != nullptr && blockIdx.x == 0 && lane == 0 && trc_n < 2046u) {                                      \
-            a.trace[(role_) * 2048 + 1 + trc_n] = ((unsigned long long)(code_) << 56) | ((unsigned long long)clock64() & 0x00FFFFFFFFFFFFFFull); \
-            a.trace[(role_) * 2048] = ++trc_n;                                                                          \
-        }                                                                                                               \
-    } while (0)
-#else
-#define TC_DBG(a_, bit_) false
-#define TC_TRACE(role_, code_) do { } while (0)
-#endif
-
-constexpr int TC_TW = 8, TC_TH = 16;          // 128-pixel M tile: 16 rows of 8 pixels (one 8-row UMMA group per image row)
-constexpr int TC_MAX_STAGES = 16;           // ring depth bounds the bytes in flight per SM (latency-bound small-C layers)
-constexpr uint32_t TC_SMEM_BUDGET = 218 * 1024;
+constexpr int TC_TW = 8, TC_TH = 16;          // 128-pixel M tile: 16 rows of 8 pixels
+constexpr int TC_THREADS = 288;               // two consumer warpgroups + one producer warp
+constexpr int TC_PRODUCER_WARP = 8;
+constexpr int TC_MAX_STAGES = 16;
+constexpr uint32_t TC_SMEM_BUDGET = 200 * 1024;
+constexpr uint32_t TC_SMEM_BUDGET_SMALL_N = 100 * 1024;   // N <= 64: two CTAs per SM
+__host__ __device__ constexpr int tc_ctas_per_sm(int n_tile) { return n_tile <= 64 ? 2 : 1; }
 constexpr uint32_t TC_RESIDENT_MAX = 144 * 1024;
-constexpr int TC_TMEM_COLS = 512;
 // barrier slots (uint64 each)
-constexpr int TC_MAX_ACC = 8;               // TMEM accumulator ring: 512 columns / n_tile, at most 8
-constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_TFULL = 64, BAR_TEMPTY = 72,
-              BAR_BRES = 80, BAR_TMEMPTR = 82, BAR_RFULL = 84, BAR_PARAMS = 132;
-// lean epilogue output staging (see the item loop): 16 warps x TC_NBUF buffers of one item (32 pixels x 16 channels bf16 = 1 KB)
-constexpr int TC_STAGE_BYTES = 1024, TC_NBUF = 3;
-constexpr uint32_t TC_STAGING_BYTES = 16u * TC_NBUF * TC_STAGE_BYTES;
+constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_BRES = 64, BAR_PARAMS = 66;
+constexpr uint32_t TC_CONSUMER_WARPS = 8;
 
 // activation tensor maps: one per source of a virtual concat (1x1 convs: torch.cat along channels, unet.py:88,105,263;
 // a nearest-DOWN resampled source is a traversal-stride load of the full-resolution tensor)
 struct TcMaps {
     CUtensorMap a[READ_MAX_SRC];
-    CUtensorMap o, r;        // lean epilogue items of the NHWC output (TMA store) / the residual tensor (TMA load), when args.tma_out
 };
 
 struct TcArgs {
@@ -88,110 +66,36 @@ struct TcArgs {
     int n_src;                             // sources of the virtual concat (> 1 only for 1x1 convs)
     int src_kc_end[READ_MAX_SRC];          // K chunks [src_kc_end[s-1], src_kc_end[s]) come from source s
     int src_shift[READ_MAX_SRC];           // log2 of the source's nearest-down factor (coordinate multiplier)
-    float inv_tx, inv_ty;                  // 1/tiles_x, 1/tiles_y for the division-free tile decode
-    int nacc;                              // accumulator ring depth (each n_tile TMEM columns wide)
-    int dual;                              // two MMA issuer warps, each with its own half of the A ring (resident weights only)
-    int debug;                             // diagnostic knobs (read_set_option "tc_debug"): 1 = lean epilogue only hand-shakes,
-                                           // 2 = issuers skip the MMAs, 4 = producer skips the A loads, 8 = lean epilogue
-                                           // computes but does not touch global memory, 16 = single MMA issuer
-    uint32_t a_bytes, b_bytes, b_region_off;   // halo tile bytes, one weight tile bytes, byte offset of the B region
-    int elu;
+    uint32_t a_bytes, b_bytes, b_region_off;   // halo stage bytes, one weight tile bytes, byte offset of the B region
+    int pdl;                               // launched with programmatic stream serialization (griddepcontrol in the kernel)
+    int ctas_per_sm;                       // 2: the layer fits half the shared-memory budget and its kernel instance two CTAs' registers
+    int rev_total;                         // 0, or the number of work units: unit t is mapped to rev_total - 1 - t (read_conv_plan_set_tile_order)
     const float *bias_f, *bias_m, *scale, *shift;
-    const __nv_bfloat16 *residual;
-    __nv_bfloat16 *out;
-    float *out_nchw;                      // final layer only
-    __nv_bfloat16 *out2;
-    const __nv_bfloat16 *out2_mul;
-    const __nv_bfloat16 *addin;           // RAW [B, addin_H, addin_W, n_tile] added (nearest x2) to the accumulators, or null
-    int addin_H, addin_W;
-    int raw;                              // RAW output: store the accumulators themselves, [.., n_tile] channels
-    int mt;                               // M tiles per SUPERTILE (1, 2 or 4 horizontally adjacent 8x16-pixel tiles share ONE halo load,
-                                          // one ring stage and one set of hand-shakes; each keeps its own TMEM accumulator slot)
-    int mt_log2, nacc_log2;
-    int stiles_x;                         // supertiles per image row: ceil(tiles_x / mt)
-    float inv_stx;
-    int role_rot;                         // 1: the single-issuer roles (TMA producers, MMA issuers) run in the HIGHEST warp ids
-    int pdl;                              // launched with programmatic stream serialization (griddepcontrol in the kernel)
-    int commit_late;                      // supertiles: commit the M tiles' tfull barriers together at the end of the supertile
-    int merge_done;                       // resident weights, kchunks == 1, mt == 1: ONE "tile done" commit per tile - the producers wait
-                                          // on the accumulator's tfull barrier (A stage j of issuer me <-> accumulator slot 2j + me)
-    int bpair;                            // streamed weights: one tcgen05.commit per PAIR of B stages
-    int rev_total;                        // 0, or the number of work units: unit t is mapped to rev_total - 1 - t (read_conv_plan_set_tile_order)
-    int tma_out;                          // lean epilogue: items are staged in shared memory and written by TMA stores (plan: fits, no out2)
-    uint32_t stage_bytes;                 // TC_STAGING_BYTES when the plan reserved the staging buffers (between the B region and the barriers)
-    int probe;                            // issuers try_wait the NEXT tile's barriers before issuing the current tile's MMAs
-    unsigned long long *trace;            // READ_DIAG builds: per-role timeline buffer (see TC_TRACE), else null
+    EpiArgs epi;
 };
 
-// tile index -> (n tile, tile x, tile y, image) without integer division: fdiv_small, conv_common.cuh
 struct TileCoord {
     int nt, tx, ty, b;
 };
-// t indexes the CTA's work units: (supertile, n tile).  A supertile is a.mt horizontally adjacent M tiles.
-__device__ __forceinline__ TileCoord decode_tile(long long t, const TcArgs &a)
+__device__ __forceinline__ TileCoord decode_tile(int t, const TcArgs &a)
 {
+    if (a.rev_total) t = a.rev_total - 1 - t;
     TileCoord c;
-    if (a.rev_total) t = (long long)a.rev_total - 1 - t;
-    int mt = (int)t;
-    c.nt = 0;
-    if (a.n_tiles == 2) { c.nt = mt & 1; mt >>= 1; }
-    else if (a.n_tiles > 2) { c.nt = (int)(t % a.n_tiles); mt = (int)(t / a.n_tiles); }
-    // mt indexes SUPERTILES; tx is the x index of the supertile's first M tile
-    const int q = fdiv_small(mt, a.inv_stx);
-    c.tx = (mt - q * a.stiles_x) * a.mt;
-    c.b = fdiv_small(q, a.inv_ty);
-    c.ty = q - c.b * a.tiles_y;
+    c.nt = t % a.n_tiles;
+    int m = t / a.n_tiles;
+    c.tx = m % a.tiles_x;
+    m /= a.tiles_x;
+    c.ty = m % a.tiles_y;
+    c.b = m / a.tiles_y;
     return c;
-}
-// same for layers with a single n tile (work unit == supertile)
-__device__ __forceinline__ TileCoord decode_supertile(int s, const TcArgs &a)
-{
-    TileCoord c;
-    c.nt = 0;
-    if (a.rev_total) s = a.rev_total - 1 - s;
-    const int q = fdiv_small(s, a.inv_stx);
-    c.tx = (s - q * a.stiles_x) * a.mt;
-    c.b = fdiv_small(q, a.inv_ty);
-    c.ty = q - c.b * a.tiles_y;
-    return c;
-}
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b)
-{
-    __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&v);
-}
-// one F2FP per pair: lo -> bits [0,16) (lower address), hi -> bits [16,32)
-__device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi)
-{
-    uint32_t d;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
-}
-__device__ __forceinline__ float2 unpack_bf16x2(uint32_t u)
-{
-    return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 *>(&u));
 }
 
 // ------------------------------------------------------------------ the kernel
-// KS = filter size (1 or 3), KKN = UMMA K-steps per tap chunk (cin_blk / 16), RES = weights resident in smem.
-// Compile-time so the single-thread MMA issue loop is straight-line code: round-1 profiling showed that thread, not
-// the tensor pipe, bounded every layer (85 scalar instructions per filter tap with runtime loop bounds).
-// NTHR = 384: 8 epilogue warps, 16-column chunks, software-pipelined (wide layers, Cout >= 128).
-// NTHR = 640: 16 epilogue warps, 8-column chunks (Cout <= 64): those layers have so little MMA work per tile (576 / 2304
-//             tensor cycles) that the epilogue's instruction stream bounds them; twice the warps halve each warp's
-//             share and give the schedulers 4 warps per SMSP to hide the MUFU / TMEM / global-load latencies.
-// A ring stage = one halo tile (all k x k taps of one K chunk): one wait, one expect_tx, one TMA load and one
-//       tcgen05.commit per tile and K chunk (round-1 knob experiments: with ALL work disabled the C=32 kernel still took
-//       1600 cycles per tile in the serial wait / expect_tx / TMA / commit chains of per-filter-column stages).
-// STR = conv stride.  STR == 2 (3x3 / 4x4, pad 1): input column 2x + kx - 1 is an EVEN column for kx odd and an ODD one for kx
-//       even, so a stage holds four phase tiles E/O x E/O, each loaded by one TMA with traversal stride 2 in x and y
-//       (tile[j][i] = in(sx + 2i, sy + 2j), sx = 2*X0 for E, 2*X0 - 1 for O); tap (ky, kx) reads phase tile
-//       ((ky+1)&1, (kx+1)&1) at pixel offset (ky>>1, kx>>1) through the same row-linear descriptors.
-template <int KS, int KKN, bool RES, int NTHR, int EPI, int STR>
-__global__ void __launch_bounds__(NTHR, 1)
-gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB,
-                     const __grid_constant__ TcArgs a)
+// KS = filter size, STR = stride, KKN = 16-element K steps per K chunk (cin_blk / 16), N = n_tile (wgmma N).  Filter size and
+// stride are compile-time so that the tap loop unrolls into constant shared-memory offsets.
+template <int KS, int STR, int KKN, int N>
+__global__ void __launch_bounds__(TC_THREADS, tc_ctas_per_sm(N))
+gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
 {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (s_u32(smem_raw) + 1023u) & ~1023u;
@@ -199,657 +103,157 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
 
     constexpr int ntaps = KS * KS;
     const uint32_t b_region = smem_base + a.b_region_off;
-    const uint32_t b_region_bytes = RES ? (uint32_t)(ntaps * a.kchunks) * a.b_bytes : (uint32_t)a.b_stages * a.b_bytes;
-    const uint32_t stage_region = smem_base + a.b_region_off + b_region_bytes;            // 1 KB aligned (b_bytes is a multiple of 1 KB)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.b_region_off + b_region_bytes + a.stage_bytes);
+    const uint32_t b_region_bytes = a.b_resident ? (uint32_t)(ntaps * a.kchunks) * a.b_bytes : (uint32_t)a.b_stages * a.b_bytes;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.b_region_off + b_region_bytes);
     const uint32_t bar0 = s_u32(bars);
     const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY;
-    const uint32_t bfull0 = bar0 + 8 * BAR_BFULL, bempty0 = bar0 + 8 * BAR_BEMPTY;
-    const uint32_t tfull0 = bar0 + 8 * BAR_TFULL, tempty0 = bar0 + 8 * BAR_TEMPTY, bres = bar0 + 8 * BAR_BRES;
-    uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(bars + BAR_TMEMPTR);
-    float *s_par = reinterpret_cast<float *>(bars + BAR_PARAMS);   // 4 x Cout floats
+    const uint32_t bfull0 = bar0 + 8 * BAR_BFULL, bempty0 = bar0 + 8 * BAR_BEMPTY, bres = bar0 + 8 * BAR_BRES;
+    float4 *s_par = reinterpret_cast<float4 *>(bars + BAR_PARAMS);
 
-    // Role warp index.  The SM's warp arbiter prefers the highest warp id among eligible warps (B300_MICROARCH.md "Multi-warp
-    // arbiter"): with role_rot the four single-issuer warps (TMA producers, MMA issuers) are the LAST four warps of the CTA so the
-    // epilogue's instruction stream cannot starve the ~10 scalar instructions behind every tcgen05.mma.  The epilogue keeps
-    // TMEM lane quadrant = hardware warp id % 4 because the rotation is a multiple of 4.
     const int lane = threadIdx.x & 31;
-    const int warp = a.role_rot ? (int)(((threadIdx.x >> 5) + 4u) % (NTHR / 32)) : (int)(threadIdx.x >> 5);
+    const int warp = threadIdx.x >> 5;
     if (a.pdl) pdl_launch_dependents();
-#ifdef READ_DIAG
-    unsigned trc_n = 0;
-#endif
-
-    for (int i = threadIdx.x; i < a.cout_pad; i += NTHR) {
-        // one float4 per channel: {bias_f, bias_m, bn_scale, bn_shift} -> a single LDS.128 in the epilogue
-        // (the lean path stores them pre-folded for gate_folded: {bias_f, bias_m / 2, bn_scale / 2, bn_shift})
-        const float hs = NTHR == 640 ? 0.5f : 1.f;
-        reinterpret_cast<float4 *>(s_par)[i] = i < a.Cout ? make_float4(a.bias_f[i], hs * a.bias_m[i], hs * a.scale[i], a.shift[i])
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (warp == 0 && lane == 0) {
+    for (int i = threadIdx.x; i < a.cout_pad; i += TC_THREADS)
+        s_par[i] = i < a.Cout ? make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
         for (int i = 0; i < a.n_src; ++i) tma_prefetch_desc(&tm.a[i]);
         tma_prefetch_desc(&tmB);
-        if (a.tma_out) {
-            tma_prefetch_desc(&tm.o);
-            if (a.residual != nullptr) tma_prefetch_desc(&tm.r);
-        }
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < TC_MAX_STAGES; ++s) {
             mbar_init(afull0 + 8 * s, 1);
-            mbar_init(aempty0 + 8 * s, 1);
+            mbar_init(aempty0 + 8 * s, TC_CONSUMER_WARPS);
             mbar_init(bfull0 + 8 * s, 1);
-            mbar_init(bempty0 + 8 * s, 1);
-        }
-        for (int i = 0; i < TC_MAX_ACC; ++i) {
-            mbar_init(tfull0 + 8 * i, 1);
-            mbar_init(tempty0 + 8 * i, NTHR == 640 ? (a.raw ? 16u : (uint32_t)(a.n_tile >> 3)) : ((a.n_tile >> 1) == 8 ? 4u : (NTHR - 128) / 32));   // arrivals per tile: lean = 4 quadrants x nch16 warps, else every epilogue warp
+            mbar_init(bempty0 + 8 * s, TC_CONSUMER_WARPS);
         }
         mbar_init(bres, 1);
-        if (NTHR == 640)
-            for (int i = 0; i < 16 * TC_NBUF; ++i) mbar_init(bar0 + 8 * (BAR_RFULL + i), 1);
         mbar_fence_init();
     }
-    if (warp == 2) tmem_alloc(s_u32(tmem_ptr_smem), TC_TMEM_COLS);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
-    const int m_tiles = a.stiles_x * a.tiles_y * a.B;             // supertiles
-    const long long total_tiles = (long long)m_tiles * a.n_tiles;  // work units of the persistent loops below
+    const int total_tiles = a.tiles_x * a.tiles_y * a.B * a.n_tiles;   // < 2^31 (checked by the host)
     const int n_total = a.n_tile * a.n_tiles;
 
-    if (warp == 0 || (warp == 2 && a.dual)) {
-        // ===================== TMA producer(s) (whole warp loops, one elected lane issues) =====================
-        // With dual issuers there are two producers as well: warp 0 feeds ring 0 (even tiles), warp 2 ring 1 (odd tiles).
-        const uint32_t pme = (warp == 2) ? 1u : 0u;
-        if (RES && pme == 0u && elect_one()) {
-            const int nb = KS * KS * a.kchunks;
+    if (warp == TC_PRODUCER_WARP) {
+        // ===================== TMA producer (whole warp loops, one elected lane issues) =====================
+        if (a.b_resident && elect_one()) {
+            const int nb = ntaps * a.kchunks;
             mbar_arrive_expect_tx(bres, (uint32_t)nb * a.b_bytes);
             for (int i = 0; i < nb; ++i) tma_load_2d(&tmB, bres, b_region + (uint32_t)i * a.b_bytes, 0, i * n_total);
         }
         __syncwarp();
         if (a.pdl) pdl_wait();        // activations come from the previous kernel; the (static) weights above do not
-        // A ring(s): one ring, or (dual issuers) two half rings used by alternate tiles - each ring is then a plain
-        // single-producer / single-consumer queue, so mbarrier phase parity can never alias
-        const uint32_t ring_n = a.dual ? (uint32_t)a.a_stages / 2u : (uint32_t)a.a_stages;
-        const uint32_t ring_base = a.dual ? pme * ring_n : 0u;
-        uint32_t as = 0, aph = 0;
-        uint32_t bs = 0, bph = 0, tile_it = 0;
-        uint32_t b_addr = b_region;
-        const int row_step = KS * a.kchunks * n_total;                 // +1 filter row in the packed weights
-        const long long pf_dist = (a.dual ? 4 : 2) * (long long)gridDim.x;   // this producer's tile after next
-        for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tile_it) {
-            if (a.dual && (tile_it & 1u) != pme) continue;             // the other producer's tile
+        uint32_t as = 0, aph = 0, bs = 0, bph = 0;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const TileCoord tc_ = decode_tile(t, a);
-            const int nt = tc_.nt, tx = tc_.tx, ty = tc_.ty, b = tc_.b;
-            const int x0 = tx * TC_TW - a.pad, y0 = ty * TC_TH - a.pad;
-            // warm L2 with the halo tile this producer will need two of its tiles from now (DRAM latency is what bounds
-            // the small-C layers: the ring can only keep a_stages * a_bytes in flight per SM)
-            const long long tp = t + pf_dist;
-            if (STR == 1 && a.n_src == 1 && tp < total_tiles && elect_one()) {
-                const TileCoord pc = decode_tile(tp, a);
-                for (int kc = 0; kc < a.kchunks; ++kc)
-                    tma_prefetch_4d(&tm.a[0], kc * a.cin_blk, pc.tx * TC_TW - a.pad, pc.ty * TC_TH - a.pad, pc.b);
-            }
-            __syncwarp();
+            const int x0 = tc_.tx * TC_TW - a.pad, y0 = tc_.ty * TC_TH - a.pad;
             for (int kc = 0; kc < a.kchunks; ++kc) {
-                const uint32_t slot = ring_base + as;
-                // merged mode: the stage is free when the tile that used it is complete = its accumulator's tfull barrier
-                mbar_wait(a.merge_done ? tfull0 + 8 * (a.dual ? 2u * as + pme : as) : aempty0 + 8 * slot, aph ^ 1u);
-                TC_TRACE(pme, 1);
+                mbar_wait(aempty0 + 8 * as, aph ^ 1u);
                 if (elect_one()) {
-                    if (TC_DBG(a, 4)) {
-                        mbar_arrive(afull0 + 8 * slot);
+                    const uint32_t full = afull0 + 8 * as, dst = smem_base + as * a.a_bytes;
+                    if (STR == 1) {
+                        mbar_arrive_expect_tx(full, a.a_tx_bytes);
+                        // virtual concat (1x1, pad 0): chunk kc belongs to source si; a down-sampled source is read with
+                        // traversal stride 2^shift from coordinate (x0, y0) << shift
+                        int si = 0, kc0 = 0;
+                        for (int q = 0; q < READ_MAX_SRC - 1; ++q)
+                            if (q + 1 < a.n_src && kc >= a.src_kc_end[q]) { si = q + 1; kc0 = a.src_kc_end[q]; }
+                        const int sh = a.src_shift[si];
+                        tma_load_4d(&tm.a[si], full, dst, (kc - kc0) * a.cin_blk, x0 << sh, y0 << sh, tc_.b);
                     } else {
-                        if (STR == 1) {
-                            mbar_arrive_expect_tx(afull0 + 8 * slot, a.a_tx_bytes);
-                            if (a.n_src == 1) {
-                                tma_load_4d(&tm.a[0], afull0 + 8 * slot, smem_base + slot * a.a_bytes, kc * a.cin_blk, x0, y0, b);
-                            } else {
-                                // virtual concat (1x1, pad 0): chunk kc belongs to source si; a down-sampled source is read
-                                // with traversal stride 2^shift from coordinate (x0, y0) << shift
-                                int si = 0, kc0 = 0;
-                                for (int q = 0; q < READ_MAX_SRC - 1; ++q)
-                                    if (q + 1 < a.n_src && kc >= a.src_kc_end[q]) { si = q + 1; kc0 = a.src_kc_end[q]; }
-                                const int sh = a.src_shift[si];
-                                tma_load_4d(&tm.a[si], afull0 + 8 * slot, smem_base + slot * a.a_bytes, (kc - kc0) * a.cin_blk,
-                                            x0 << sh, y0 << sh, b);
-                            }
-                        } else {
-                            mbar_arrive_expect_tx(afull0 + 8 * slot, 4u * a.a_tx_bytes);
-                            const int ex = 2 * tx * TC_TW, ey = 2 * ty * TC_TH;        // even-phase origin in the input
+                        mbar_arrive_expect_tx(full, 4u * a.a_tx_bytes);
+                        const int ex = 2 * tc_.tx * TC_TW, ey = 2 * tc_.ty * TC_TH;        // even-phase origin in the input
 #pragma unroll
-                            for (int ph4 = 0; ph4 < 4; ++ph4)
-                                tma_load_4d(&tm.a[0], afull0 + 8 * slot, smem_base + slot * a.a_bytes + (uint32_t)ph4 * a.tile_bytes,
-                                            kc * a.cin_blk, ex - (ph4 & 1), ey - (ph4 >> 1), b);
-                        }
+                        for (int ph4 = 0; ph4 < 4; ++ph4)
+                            tma_load_4d(&tm.a[0], full, dst + (uint32_t)ph4 * a.tile_bytes, kc * a.cin_blk, ex - (ph4 & 1), ey - (ph4 >> 1), tc_.b);
                     }
                 }
                 __syncwarp();
-                TC_TRACE(pme, 2);
-                if (++as == ring_n) { as = 0; aph ^= 1u; }
-                if (!RES) {
-#pragma unroll
-                    for (int kx = 0; kx < KS; ++kx) {
-                        int row = (kx * a.kchunks + kc) * n_total + nt * a.n_tile;       // tap = ky*KS + kx
-#pragma unroll
-                        for (int ky = 0; ky < KS; ++ky, row += row_step) {
-                            mbar_wait(bempty0 + 8 * (a.bpair ? (bs | 1u) : bs), bph ^ 1u);   // pair mode: the pair's (odd) barrier
-                            if (elect_one()) {
-                                mbar_arrive_expect_tx(bfull0 + 8 * bs, a.b_bytes);
-                                tma_load_2d(&tmB, bfull0 + 8 * bs, b_addr, 0, row);
-                            }
-                            __syncwarp();
-                            b_addr += a.b_bytes;
-                            if (++bs == (uint32_t)a.b_stages) { bs = 0; bph ^= 1u; b_addr = b_region; }
+                if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
+                if (!a.b_resident) {
+                    for (int tap = 0; tap < ntaps; ++tap) {
+                        mbar_wait(bempty0 + 8 * bs, bph ^ 1u);
+                        if (elect_one()) {
+                            mbar_arrive_expect_tx(bfull0 + 8 * bs, a.b_bytes);
+                            tma_load_2d(&tmB, bfull0 + 8 * bs, b_region + bs * a.b_bytes, 0, (tap * a.kchunks + kc) * n_total + tc_.nt * a.n_tile);
                         }
+                        __syncwarp();
+                        if (++bs == (uint32_t)a.b_stages) { bs = 0; bph ^= 1u; }
                     }
                 }
             }
         }
-    } else if (warp == 1 || warp == 3) {
-        // ===================== MMA issuers (whole warp loops, one elected lane issues) =====================
-        // TWO issuer warps take alternate tiles (accumulator 0 / 1): every tcgen05.mma costs its issuing thread ~10 scalar
-        // instructions (~100+ cycles for a lone warp) - more than the 8..64 tensor cycles of the small-N layers' MMAs - so
-        // two independent instruction streams into the tensor pipe nearly double its occupancy.  A/B ring stages are
-        // produced in tile order; each issuer consumes its own tiles' stages and skips over the other issuer's.
-        const uint32_t me = (warp == 3) ? 1u : 0u;
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(a.n_tile >> 3) << 17) | ((128u >> 4) << 24);
-        constexpr uint32_t row_bytes = KKN * 16u * 2u;                 // cin_blk bf16
-        constexpr uint32_t layout_type = (KKN == 4) ? 2u : (KKN == 2 ? 4u : 6u);   // SWIZZLE_128B : SWIZZLE_64B : SWIZZLE_32B
-        // SBO = stride between consecutive 8-row groups = one halo row (halo_w pixels)
-        const uint32_t desc_hi = (uint32_t)(make_kmajor_desc(0, (uint32_t)a.halo_w * row_bytes, layout_type) >> 32);
-        const uint32_t desc_hi_b = (uint32_t)(make_kmajor_desc(0, 8u * row_bytes, layout_type) >> 32);   // weights: dense rows
-        constexpr uint32_t lo_lbo = 1u << 16;                          // LBO field (ignored for swizzled K-major), kept = 1
-        constexpr uint32_t px16 = row_bytes >> 4;                       // one pixel row, in 16-byte units
-        const uint32_t ky_step = (uint32_t)a.halo_w * px16;            // one halo row of pixels
-        const uint32_t a16 = a.a_bytes >> 4, b16 = a.b_bytes >> 4, tile16 = a.tile_bytes >> 4;
-        // tap (ky, kx) -> 16-byte offset of its A rows inside the stage
-        auto tap_off = [&](int ky, int kx) -> uint32_t {
-            if (STR == 1) return (uint32_t)ky * ky_step + (uint32_t)kx * px16;
-            return (uint32_t)((((ky + 1) & 1) << 1) | ((kx + 1) & 1)) * tile16 + (uint32_t)(ky >> 1) * ky_step + (uint32_t)(kx >> 1) * px16;
-        };
-        const uint32_t st16 = a16;                                     // one ring stage, in 16-byte units
-        const uint32_t a_lo0 = ((smem_base & 0x3FFFFu) >> 4) | lo_lbo, b_lo0 = ((b_region & 0x3FFFFu) >> 4) | lo_lbo;
-        const uint32_t tap16 = (uint32_t)a.kchunks * b16;              // resident weights: +1 tap
-        if (RES) mbar_wait(bres, 0);
-        uint32_t as = 0, aph = 0, bs = 0, bph = 0, tile_it = 0;
-        uint32_t a_lo = a_lo0, b_lo = b_lo0;
-        const uint32_t ring_n = a.dual ? (uint32_t)a.a_stages / 2u : (uint32_t)a.a_stages;
-        const uint32_t ring_lo0 = a_lo0 + (a.dual ? me * ring_n * st16 : 0u);
-        const uint32_t ring_bar = a.dual ? me * ring_n : 0u;
-        a_lo = ring_lo0;
-        // The accumulators form a ring of a.nacc TMEM slots (tile i -> slot i % nacc): round-1 knob experiments showed the
-        // hand-shake chain issuer -> tcgen05.commit -> epilogue -> tempty -> issuer costs ~1600 cycles per tile even with
-        // all work disabled, so with one slot per issuer every small-tile layer ran at the chain's latency.
-        uint32_t acc_c = 0, acc_p = 0;
-        const uint32_t MT = (uint32_t)a.mt;
-        const bool probe = RES && a.probe != 0;       // host: resident weights, one K chunk, plain tiles
-        bool ready_t = false, ready_a = false;
-        const uint32_t mt16 = (uint32_t)TC_TW * px16;                 // +1 M tile inside the supertile's halo, 16-byte units
-        for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tile_it) {
-            // a supertile owns MT consecutive accumulator slots (nacc % MT == 0: it never straddles the ring's wrap)
-            const uint32_t acc = acc_c, acc_ph = acc_p;
-            acc_c += MT;
-            if (acc_c >= (uint32_t)a.nacc) { acc_c = 0; acc_p ^= 1u; }
-            if (a.dual ? ((tile_it & 1u) != me) : (me != 0u)) continue;   // not this issuer's supertile
-            if (!(probe && ready_t))
-                for (uint32_t mi = 0; mi < MT; ++mi) mbar_wait(tempty0 + 8 * (acc + mi), acc_ph ^ 1u);
-            TC_TRACE(2 + me, 3);
-            tcgen05_fence_after();
-            const uint32_t d_tmem0 = tmem_base + acc * (uint32_t)a.n_tile;
-            uint32_t bkc = b_lo0;                                      // resident weights: chunk kc of tap 0
-            for (int kc = 0; kc < a.kchunks; ++kc, bkc += b16) {
-                if (!(probe && ready_a)) mbar_wait(afull0 + 8 * (ring_bar + as), aph);
-                if (probe) {
-                    // look at the NEXT own tile's barriers now: their ~90-cycle try_wait latency overlaps the MMAs still queued in the
-                    // tensor pipe instead of sitting between this tile's last MMA and the next tile's first
-                    uint32_t an = acc + (a.dual ? 2u : 1u), apn = acc_ph;
-                    if (an >= (uint32_t)a.nacc) { an -= (uint32_t)a.nacc; apn ^= 1u; }
-                    uint32_t sn = as + 1u, spn = aph;
-                    if (sn == ring_n) { sn = 0; spn ^= 1u; }
-                    ready_t = __all_sync(0xFFFFFFFFu, mbar_try_wait(tempty0 + 8 * an, apn ^ 1u));
-                    ready_a = __all_sync(0xFFFFFFFFu, mbar_try_wait(afull0 + 8 * (ring_bar + sn), spn));
-                }
-                TC_TRACE(2 + me, 4);
-                tcgen05_fence_after();
-                const bool last_kc = kc == a.kchunks - 1;
-                if (RES) {
-                    // resident weights: nothing to wait for between taps - ONE elected block issues the whole stage
-                    // (MT * k*k*KKN MMAs + the commits) instead of an elect / syncwarp pair per tap
-                    if (elect_one()) {
-                        for (uint32_t mi = 0; mi < MT; ++mi) {
-                            const uint32_t d_tmem = d_tmem0 + mi * (uint32_t)a.n_tile;
-                            const uint32_t a_mt = a_lo + mi * mt16;
-#pragma unroll
-                            for (int kx = 0; kx < KS; ++kx) {
-#pragma unroll
-                                for (int ky = 0; ky < KS; ++ky) {
-                                    const uint32_t bl = bkc + (uint32_t)(ky * KS + kx) * tap16;
-                                    const uint32_t al = a_mt + tap_off(ky, kx);
-#pragma unroll
-                                    for (int kk = 0; kk < KKN; ++kk) {
-                                        if (TC_DBG(a, 2)) continue;
-                                        const uint32_t accum = (kx | ky | kk) != 0 ? 1u : (kc != 0 ? 1u : 0u);
-                                        umma_bf16_lohi2(d_tmem, al + 2u * kk, desc_hi, bl + 2u * kk, desc_hi_b, idesc, accum);
-                                    }
-                                }
-                            }
-                            if (last_kc && !a.commit_late) umma_commit(tfull0 + 8 * (acc + mi));    // this M tile's accumulator is complete
-                        }
-                        if (last_kc && a.commit_late)
-                            for (uint32_t mi = 0; mi < MT; ++mi) umma_commit(tfull0 + 8 * (acc + mi));
-                        if (!a.merge_done) umma_commit(aempty0 + 8 * (ring_bar + as));
-                    }
-                    __syncwarp();
-                } else {
-#pragma unroll
-                    for (int kx = 0; kx < KS; ++kx) {
-#pragma unroll
-                        for (int ky = 0; ky < KS; ++ky) {
-                            mbar_wait(bfull0 + 8 * bs, bph);
-                            tcgen05_fence_after();
-                            if (elect_one()) {
-                                for (uint32_t mi = 0; mi < MT; ++mi) {
-                                    const uint32_t al = a_lo + mi * mt16 + tap_off(ky, kx);
-                                    const uint32_t d_tmem = d_tmem0 + mi * (uint32_t)a.n_tile;
-#pragma unroll
-                                    for (int kk = 0; kk < KKN; ++kk) {
-                                        if (TC_DBG(a, 2)) continue;
-                                        // +16 bf16 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
-                                        const uint32_t accum = (kx | ky | kk) != 0 ? 1u : (kc != 0 ? 1u : 0u);
-                                        umma_bf16_lohi2(d_tmem, al + 2u * kk, desc_hi, b_lo + 2u * kk, desc_hi_b, idesc, accum);
-                                    }
-                                }
-                                if (!a.bpair || (bs & 1u)) umma_commit(bempty0 + 8 * bs);
-                            }
-                            __syncwarp();
-                            b_lo += b16;
-                            if (++bs == (uint32_t)a.b_stages) { bs = 0; bph ^= 1u; b_lo = b_lo0; }
-                        }
-                    }
-                    if (elect_one()) {
-                        umma_commit(aempty0 + 8 * (ring_bar + as));
-                        if (last_kc)
-                            for (uint32_t mi = 0; mi < MT; ++mi) umma_commit(tfull0 + 8 * (acc + mi));
-                    }
-                    __syncwarp();
-                }
-                TC_TRACE(2 + me, 5);
-                a_lo += st16;
-                if (++as == ring_n) { as = 0; aph ^= 1u; a_lo = ring_lo0; }
-            }
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue (8 warps: 2 per TMEM lane quadrant, interleaved over 16-column chunks) =====
-        // Software pipelined: the TMEM load of chunk c+1 and the residual/FAM-multiplier loads of chunk c+1 are in
-        // flight while chunk c is computed; the first chunk's global loads are issued BEFORE waiting for the MMAs.
-        const int q = warp & 3;
-        const int sub = (warp - 4) >> 2;          // 0 or 1: which chunks of the tile this warp owns
-        const int r = q * 32 + lane;              // accumulator row == pixel within the tile
-        const int py = r / TC_TW, px = r % TC_TW;
-        const int half = a.n_tile >> 1;
-        const int nchunks = half >> 4;
-        const float4 *par4 = reinterpret_cast<const float4 *>(s_par);
-        unsigned tile_seq = 0;                      // this CTA's tile counter (final layer: tiles alternate between the quadrant's two warps)
-        uint32_t acc_c = 0, acc_p = 0;
-        if (a.pdl) pdl_wait();        // residual / add-in / FAM-multiplier tensors come from earlier kernels
-        if (NTHR == 640 && (EPI != 0 || !a.raw)) {
-            // ---------------- lean 16-warp item loop (Cout 16 / 32 / 64, one n tile) ----------------
-            // Work item = (TMEM lane quadrant q, 16-column chunk) of one M tile: 4 * nch16 items per tile.  Warp -> (q, chunk)
-            // is FIXED; with nch16 = 1 / 2 / 4 chunks per tile a warp serves every 4th / 2nd / every M tile of the CTA's
-            // sequence.  A lane owns 32 contiguous output bytes of its pixel (full sectors for the residual read and the store).
-            // Round-2 role timelines (profiles/r02_role_timelines.md) showed the epilogue - not the tensor pipe - bounding the
-            // C=32 / C=64 layers, and the epilogue itself issue-bound: ~560 warp instructions per item of which only 180 were
-            // the 16 outputs' math; the rest was the per-tile header (tile decode, 64-bit offsets, ring bookkeeping) executed
-            // by EVERY warp for EVERY tile, including the tiles it skips.  This loop visits only the warp's own items and
-            // derives tile / accumulator slot / phase from the item index with shifts.
-            // EPI fixes the layer kind at compile time (1: ELU, no residual - ResBlock main.0; 2: no activation + residual -
-            // ResBlock main.1; 0: runtime flags).
-            const bool elu = EPI == 1 ? true : (EPI == 2 ? false : a.elu != 0);
-            const bool has_res = EPI == 2 ? true : (EPI == 1 ? false : a.residual != nullptr);
-            const bool has_out2 = EPI != 0 ? false : a.out2 != nullptr;
-            const int nch16 = half >> 4;                       // 1, 2 or 4 (host: lean only for Cout 16 / 32 / 64)
-            const int lg = nch16 >> 1;                         // log2(nch16)
-            const int chunk = sub & (nch16 - 1);
-            const uint32_t item_step = 4u >> lg;               // M tiles between two items of this warp
-            const uint32_t n_units = (uint32_t)((total_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);   // this CTA's supertiles
-            const uint32_t n_mtiles = n_units << a.mt_log2;
-            // accumulator slot / phase of item `it`: it % nacc, (it / nacc) & 1 - kept incrementally (nacc need not be a power of two)
-            uint32_t acc = ((uint32_t)sub >> lg) % (uint32_t)a.nacc, acc_ph = (((uint32_t)sub >> lg) / (uint32_t)a.nacc) & 1u;
-            // Output path (a.tma_out).  Timing experiments (scripts/ab_pair_dbg.py, profiles/r02_conv_experiments.md): a lane's two
-            // 16-byte stores at a Cout * 2 byte lane stride cost 32 LSU wavefronts per instruction and bounded the epilogue (C=32:
-            // 89 -> 65 us with the stores switched off).  The item (32 pixels x 16 channels = 1 KB) is staged in a per-warp buffer
-            // (conflict-free under the 32-byte TMA swizzle) and written by ONE TMA store; a residual tile is TMA-loaded into the same
-            // buffer one item ahead and updated in place.  No cross-warp synchronisation: each warp's lane 0 owns its bulk groups.
-            // Ragged edges are clipped by the TMA unit.
-            const bool tma_out = a.tma_out != 0;
-            const uint32_t sbuf0 = stage_region + (uint32_t)(warp - 4) * (TC_NBUF * TC_STAGE_BYTES);
-            const uint32_t rfull0 = bar0 + 8 * (BAR_RFULL + (warp - 4) * TC_NBUF);
-            const uint32_t lane_off = (uint32_t)lane * 32u, sw = (((uint32_t)lane >> 2) & 1u) * 16u;     // SWIZZLE_32B: bit 4 ^= bit 7
-            uint32_t kb = 0, kph = 0;
-            if (tma_out && has_res && lane == 0 && ((uint32_t)sub >> lg) < n_mtiles) {
-                const uint32_t it0 = (uint32_t)sub >> lg;
-                const TileCoord t0 = decode_supertile((int)(blockIdx.x + (it0 >> a.mt_log2) * gridDim.x), a);
-                mbar_arrive_expect_tx(rfull0, TC_STAGE_BYTES);
-                tma_load_4d(&tm.r, rfull0, sbuf0, chunk * 16, (t0.tx + (int)(it0 & (uint32_t)(a.mt - 1))) * TC_TW, t0.ty * TC_TH + q * 4, t0.b);
-            }
-            for (uint32_t it = (uint32_t)sub >> lg; it < n_mtiles; it += item_step) {
-                const uint32_t su = it >> a.mt_log2, mi = it & (uint32_t)(a.mt - 1);
-                const TileCoord tc_ = decode_supertile((int)(blockIdx.x + su * gridDim.x), a);
-                const int b = tc_.b;
-                const int x = (tc_.tx + (int)mi) * TC_TW + px, y = tc_.ty * TC_TH + py;
-                const bool inside = (x < a.W) && (y < a.H);
-                const uint32_t trow = tmem_base + acc * (uint32_t)a.n_tile + ((uint32_t)(q * 32) << 16);
-                const int co = chunk * 16;                                              // lean layers have ONE n tile
-                const int o = ((b * a.H + y) * a.W + x) * a.Cout + co;                  // < 2^31 (checked by the host)
-                uint4 rs0 = make_uint4(0, 0, 0, 0), rs1 = rs0, ml0 = rs0, ml1 = rs0;
-                uint4 af0 = rs0, af1 = rs0, am0 = rs0, am1 = rs0;            // add-in: f and m columns of this item
-                const bool has_addin = EPI == 0 && a.addin != nullptr;
-                if (has_addin && inside) {
-                    const __nv_bfloat16 *ap = a.addin + ((b * a.addin_H + (y >> 1)) * a.addin_W + (x >> 1)) * a.n_tile + chunk * 16;
-                    af0 = __ldg(reinterpret_cast<const uint4 *>(ap));
-                    af1 = __ldg(reinterpret_cast<const uint4 *>(ap) + 1);
-                    am0 = __ldg(reinterpret_cast<const uint4 *>(ap + half));
-                    am1 = __ldg(reinterpret_cast<const uint4 *>(ap + half) + 1);
-                }
-                const uint32_t kn = kb + 1 == TC_NBUF ? 0u : kb + 1;
-                if (tma_out) {
-                    if (lane == 0) {
-                        bulk_wait_group_read<1>();      // only the previous item's store may still be reading: buffers kb and kn are free
-                        const uint32_t itn = it + item_step;
-                        if (has_res && itn < n_mtiles) {
-                            const TileCoord tn = decode_supertile((int)(blockIdx.x + (itn >> a.mt_log2) * gridDim.x), a);
-                            mbar_arrive_expect_tx(rfull0 + 8 * kn, TC_STAGE_BYTES);
-                            tma_load_4d(&tm.r, rfull0 + 8 * kn, sbuf0 + kn * TC_STAGE_BYTES, co,
-                                        (tn.tx + (int)(itn & (uint32_t)(a.mt - 1))) * TC_TW, tn.ty * TC_TH + q * 4, tn.b);
-                        }
-                    }
-                } else if (inside) {
-                    if (has_res) {
-                        rs0 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o));
-                        rs1 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o) + 1);
-                    }
-                    if (has_out2) {
-                        ml0 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o));
-                        ml1 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o) + 1);
-                    }
-                }
-                TC_TRACE(warp, 9);
-                mbar_wait(tfull0 + 8 * acc, acc_ph);
-                TC_TRACE(warp, 6);
-                tcgen05_fence_after();
-                uint32_t f16[16], m16[16];
-                tmem_ld16(trow + (uint32_t)(chunk * 16), f16);
-                tmem_ld16(trow + (uint32_t)(half + chunk * 16), m16);
-                tmem_ld_wait();
-                TC_TRACE(warp, 7);
-                // the accumulator is in registers: hand the TMEM slot back before the math
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                if (has_addin) {        // pre-activation terms computed at the coarser resolution (nearest x2)
-                    const uint32_t fa[8] = {af0.x, af0.y, af0.z, af0.w, af1.x, af1.y, af1.z, af1.w};
-                    const uint32_t ma[8] = {am0.x, am0.y, am0.z, am0.w, am1.x, am1.y, am1.z, am1.w};
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        f16[2 * j] = __float_as_uint(__uint_as_float(f16[2 * j]) + __uint_as_float(fa[j] << 16));
-                        f16[2 * j + 1] = __float_as_uint(__uint_as_float(f16[2 * j + 1]) + __uint_as_float(fa[j] & 0xFFFF0000u));
-                        m16[2 * j] = __float_as_uint(__uint_as_float(m16[2 * j]) + __uint_as_float(ma[j] << 16));
-                        m16[2 * j + 1] = __float_as_uint(__uint_as_float(m16[2 * j + 1]) + __uint_as_float(ma[j] & 0xFFFF0000u));
-                    }
-                }
-                float yv[16];
-                if (elu) {              // warp-uniform: the no-activation layers skip the ex2 path entirely
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) yv[j] = gate_folded<true>(__uint_as_float(f16[j]), __uint_as_float(m16[j]), par4[co + j]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) yv[j] = gate_folded<false>(__uint_as_float(f16[j]), __uint_as_float(m16[j]), par4[co + j]);
-                }
-                if (tma_out) {
-                    const uint32_t sb = sbuf0 + kb * TC_STAGE_BYTES + lane_off;
-                    if (has_res) {
-                        mbar_wait(rfull0 + 8 * kb, kph);
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rs0.x), "=r"(rs0.y), "=r"(rs0.z), "=r"(rs0.w) : "r"(sb + sw));
-                        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(rs1.x), "=r"(rs1.y), "=r"(rs1.z), "=r"(rs1.w) : "r"(sb + (sw ^ 16u)));
-                        const uint32_t rr[8] = {rs0.x, rs0.y, rs0.z, rs0.w, rs1.x, rs1.y, rs1.z, rs1.w};
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            yv[2 * j] += __uint_as_float(rr[j] << 16);
-                            yv[2 * j + 1] += __uint_as_float(rr[j] & 0xFFFF0000u);
-                        }
-                    }
-                    uint32_t pk[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) pk[j] = cvt_bf16x2(yv[2 * j], yv[2 * j + 1]);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sb + sw), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sb + (sw ^ 16u)), "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7]) : "memory");
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (!TC_DBG(a, 8)) tma_store_4d(&tm.o, sbuf0 + kb * TC_STAGE_BYTES, co, (tc_.tx + (int)mi) * TC_TW, tc_.ty * TC_TH + q * 4, b);
-                        bulk_commit_group();
-                    }
-                    kb = kn;
-                    if (kb == 0) kph ^= 1u;
-                } else if (inside) {
-                    if (has_res) {
-                        const uint32_t rr[8] = {rs0.x, rs0.y, rs0.z, rs0.w, rs1.x, rs1.y, rs1.z, rs1.w};
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            yv[2 * j] += __uint_as_float(rr[j] << 16);
-                            yv[2 * j + 1] += __uint_as_float(rr[j] & 0xFFFF0000u);
-                        }
-                    }
-                    uint32_t pk[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) pk[j] = cvt_bf16x2(yv[2 * j], yv[2 * j + 1]);
-                    uint4 *op = reinterpret_cast<uint4 *>(a.out + o);
-                    op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                    op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                    if (has_out2) {
-                        const uint32_t mm[8] = {ml0.x, ml0.y, ml0.z, ml0.w, ml1.x, ml1.y, ml1.z, ml1.w};
-                        uint32_t p2[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float2 ys = unpack_bf16x2(pk[j]);   // the stored (rounded) activation
-                            const float2 mv = unpack_bf16x2(mm[j]);
-                            p2[j] = cvt_bf16x2(ys.x * mv.x, ys.y * mv.y);
-                        }
-                        uint4 *o2 = reinterpret_cast<uint4 *>(a.out2 + o);
-                        o2[0] = make_uint4(p2[0], p2[1], p2[2], p2[3]);
-                        o2[1] = make_uint4(p2[4], p2[5], p2[6], p2[7]);
-                    }
-                }
-                TC_TRACE(warp, 8);
-                acc += item_step;
-                while (acc >= (uint32_t)a.nacc) { acc -= (uint32_t)a.nacc; acc_ph ^= 1u; }
-            }
-            if (tma_out && lane == 0) bulk_wait_group<0>();      // staging buffers read and stores performed before the CTA retires
-        } else
-        for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x)
-        for (int mi = 0; mi < a.mt; ++mi) {                           // the M tiles of the supertile, one accumulator slot each
-            const TileCoord tc_ = decode_tile(t, a);
-            const int nt = tc_.nt, tx = tc_.tx + mi, ty = tc_.ty, b = tc_.b;
-            const int x = tx * TC_TW + px, y = ty * TC_TH + py;
-            const bool inside = (x < a.W) && (y < a.H);
-            const long long pixo = (((long long)b * a.H + y) * a.W + x) * a.Cout + nt * half;
-            const uint32_t acc = acc_c, acc_ph = acc_p;
-            if (++acc_c == (uint32_t)a.nacc) { acc_c = 0; acc_p ^= 1u; }
-            const uint32_t trow = tmem_base + acc * (uint32_t)a.n_tile + ((uint32_t)(q * 32) << 16);
-
-            if (half == 8) {
-                // final layer (unet.py:285: BasicConv(32 -> 3), Cout padded to 8): one 8-column chunk, NCHW fp32 output.
-                // The two warps of a TMEM lane quadrant take ALTERNATE tiles (tempty counts 4 arrivals): a warp's wait / load / store
-                // chain is ~1400 cycles per tile and nothing else bounds this layer, so two chains in flight halve the tile period.
-                const bool mine = ((unsigned)tile_seq++ & 1u) == (unsigned)sub;
-                if (!mine) continue;
-                mbar_wait(tfull0 + 8 * acc, acc_ph);
-                tcgen05_fence_after();
-                {
-                    uint32_t f8[8], m8[8];
-                    tmem_ld8(trow, f8);
-                    tmem_ld8(trow + 8u, m8);
-                    tmem_ld_wait();
-                    if (inside) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            if (j < a.Cout) {
-                                const float4 pp = par4[j];
-                                a.out_nchw[(((long long)b * a.Cout + j) * a.H + y) * a.W + x] =
-                                    gated_epilogue_fast(__uint_as_float(f8[j]) + pp.x, __uint_as_float(m8[j]) + pp.y, a.elu, pp.z, pp.w);
-                            }
-                        }
-                    }
-                }
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                continue;
-            }
-            if (NTHR == 640) {
-                // lean 16-warp path.  Work item = (TMEM lane quadrant q, 16-column chunk): 4 * nch16 items per tile, dealt
-                // to the 16 warps as warp -> (q, chunk k % nch16) of every G-th tile, G = 4 / nch16 (Cout 32: each warp
-                // serves alternate tiles; Cout 64: every tile).  A lane then owns 32 contiguous output bytes of its
-                // pixel: full 32-byte sectors for the residual read and the store (8-column items touched half sectors
-                // from two different warps at different times) and half as many per-tile hand-shakes per output.
-                // EPI fixes the layer kind at compile time (1: ELU, no residual - ResBlock main.0; 2: no activation +
-                // residual - ResBlock main.1; 0: runtime flags).
-                if (EPI == 0 && a.raw) {
-                    // RAW output (one term of a 1x1 conv over a multi-resolution concat): every warp, every tile; 16-column
-                    // chunks sub, sub + 4, .. of the accumulator; optional add-in of the next-coarser RAW tensor
-                    const int opix = ((b * a.H + y) * a.W + x) * a.n_tile;
-                    const int apix = ((b * a.addin_H + (y >> 1)) * a.addin_W + (x >> 1)) * a.n_tile;
-                    mbar_wait(tfull0 + 8 * acc, acc_ph);
-                    tcgen05_fence_after();
-                    for (int c = sub; c < (a.n_tile >> 4); c += 4) {
-                        uint32_t v[16];
-                        tmem_ld16(trow + (uint32_t)(c * 16), v);
-                        uint4 a0 = make_uint4(0, 0, 0, 0), a1 = a0;
-                        if (a.addin != nullptr && inside) {
-                            a0 = __ldg(reinterpret_cast<const uint4 *>(a.addin + apix + c * 16));
-                            a1 = __ldg(reinterpret_cast<const uint4 *>(a.addin + apix + c * 16) + 1);
-                        }
-                        tmem_ld_wait();
-                        if (inside) {
-                            const uint32_t aa[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                            uint32_t pk[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j)
-                                pk[j] = cvt_bf16x2(__uint_as_float(v[2 * j]) + __uint_as_float(aa[j] << 16),
-                                                   __uint_as_float(v[2 * j + 1]) + __uint_as_float(aa[j] & 0xFFFF0000u));
-                            uint4 *op = reinterpret_cast<uint4 *>(a.out + opix + c * 16);
-                            op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                            op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                        }
-                    }
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                    continue;
-                }
-                // (the gated lean items are served by the item loop above; only RAW terms reach this point)
-                continue;
-            }
-            // two statically named register buffers (A/B): runtime-indexed arrays would be demoted to local memory
-            uint4 resA[2], resB[2], mulA[2], mulB[2];
-            uint32_t rfA[16], rmA[16], rfB[16], rmB[16];
-            auto prefetch = [&](int c, uint4 (&res)[2], uint4 (&mul)[2]) {
-                if (inside && c < nchunks) {
-                    const long long o = pixo + c * 16;
-                    if (a.residual) {
-                        res[0] = __ldg(reinterpret_cast<const uint4 *>(a.residual + o));
-                        res[1] = __ldg(reinterpret_cast<const uint4 *>(a.residual + o) + 1);
-                    }
-                    if (a.out2) {
-                        mul[0] = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o));
-                        mul[1] = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o) + 1);
-                    }
-                }
-            };
-            // computes chunk c from (rf, rm, res, mul) while the loads of chunk c+2 go into (rfn, rmn, resn, muln)
-            auto stage = [&](int c, uint32_t (&rf)[16], uint32_t (&rm)[16], uint4 (&res)[2], uint4 (&mul)[2],
-                             uint32_t (&rfn)[16], uint32_t (&rmn)[16], uint4 (&resn)[2], uint4 (&muln)[2]) {
-                tmem_ld_wait();
-                const int cn = c + 2;
-                if (cn < nchunks) {
-                    tmem_ld16(trow + (uint32_t)(cn * 16), rfn);
-                    tmem_ld16(trow + (uint32_t)(half + cn * 16), rmn);
-                }
-                prefetch(cn, resn, muln);
-                const int co = nt * half + c * 16;
-                float yv[16];
-                if (a.elu) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float4 pp = par4[co + j];
-                        yv[j] = gate_fast<true>(__uint_as_float(rf[j]) + pp.x, __uint_as_float(rm[j]) + pp.y, pp.z, pp.w);
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float4 pp = par4[co + j];
-                        yv[j] = gate_fast<false>(__uint_as_float(rf[j]) + pp.x, __uint_as_float(rm[j]) + pp.y, pp.z, pp.w);
-                    }
-                }
-                if (inside) {
-                    const long long o = pixo + c * 16;
-                    if (a.residual) {
-                        const uint32_t rr[8] = {res[0].x, res[0].y, res[0].z, res[0].w, res[1].x, res[1].y, res[1].z, res[1].w};
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float2 f = unpack_bf16x2(rr[j]);
-                            yv[2 * j] += f.x;
-                            yv[2 * j + 1] += f.y;
-                        }
-                    }
-                    uint32_t pk[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) pk[j] = pack_bf16x2(yv[2 * j], yv[2 * j + 1]);
-                    uint4 *op = reinterpret_cast<uint4 *>(a.out + o);
-                    op[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                    op[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                    if (a.out2) {
-                        const uint32_t mm[8] = {mul[0].x, mul[0].y, mul[0].z, mul[0].w, mul[1].x, mul[1].y, mul[1].z, mul[1].w};
-                        uint32_t p2[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float2 ys = unpack_bf16x2(pk[j]);   // the stored (rounded) activation
-                            const float2 mv = unpack_bf16x2(mm[j]);
-                            p2[j] = pack_bf16x2(ys.x * mv.x, ys.y * mv.y);
-                        }
-                        uint4 *o2 = reinterpret_cast<uint4 *>(a.out2 + o);
-                        o2[0] = make_uint4(p2[0], p2[1], p2[2], p2[3]);
-                        o2[1] = make_uint4(p2[4], p2[5], p2[6], p2[7]);
-                    }
-                }
-            };
-            prefetch(sub, resA, mulA);
-            mbar_wait(tfull0 + 8 * acc, acc_ph);
-            tcgen05_fence_after();
-            if (sub < nchunks) {
-                tmem_ld16(trow + (uint32_t)(sub * 16), rfA);
-                tmem_ld16(trow + (uint32_t)(half + sub * 16), rmA);
-            }
-            for (int c = sub; c < nchunks; c += 4) {
-                stage(c, rfA, rmA, resA, mulA, rfB, rmB, resB, mulB);
-                if (c + 2 < nchunks) stage(c + 2, rfB, rmB, resB, mulB, rfA, rmA, resA, mulA);
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-        }
+        return;
     }
 
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, TC_TMEM_COLS);
+    // ===================== consumers: two warpgroups, 64 pixels (8 tile rows) each =====================
+    const int wg = warp >> 2, wiw = warp & 3;
+    constexpr uint32_t row_bytes = KKN * 32u;                  // cin_blk bf16
+    // this lane's ldmatrix row (pixel of the tile) and 8-element half of the K step
+    constexpr int HALO_W = STR == 1 ? TC_TW + KS - 1 : TC_TW + 1;     // halo tile width in pixels (== a.halo_w)
+    const int lr = 64 * wg + 16 * wiw + (lane & 7) + 8 * ((lane >> 3) & 1);
+    const uint32_t a_base = (uint32_t)((lr >> 3) * HALO_W + (lr & 7)) * row_bytes;   // tap (0, 0) of this lane's pixel
+    const uint32_t khalf = (uint32_t)(lane >> 4) * 16u;
+    if (a.pdl) pdl_wait();        // residual / add-in / FAM-multiplier tensors come from earlier kernels
+    if (a.b_resident) mbar_wait(bres, 0);
+    uint32_t as = 0, aph = 0, bs = 0, bph = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const TileCoord tc_ = decode_tile(t, a);
+        float acc[N / 2];
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+        for (int kc = 0; kc < a.kchunks; ++kc) {
+            mbar_wait(afull0 + 8 * as, aph);
+            const uint32_t stage = smem_base + as * a.a_bytes;
+            // A fragments of tap t+1 are loaded while the MMAs of tap t run: two register buffers, the tap loop fully unrolled
+            uint32_t fr[2][KKN][4];
+            auto load_a = [&](int tap, uint32_t (&f)[KKN][4]) {
+                const int ky = tap / KS, kx = tap % KS;
+                const uint32_t off = STR == 1
+                    ? a_base + (uint32_t)(ky * HALO_W + kx) * row_bytes
+                    : a_base + (uint32_t)((((ky + 1) & 1) << 1) | ((kx + 1) & 1)) * a.tile_bytes + (uint32_t)((ky >> 1) * HALO_W + (kx >> 1)) * row_bytes;
+#pragma unroll
+                for (int kk = 0; kk < KKN; ++kk) ldmatrix_x4(stage + swz(off + 32u * kk + khalf, row_bytes), f[kk]);
+            };
+            uint32_t prev_bs = 0;
+            load_a(0, fr[0]);
+#pragma unroll
+            for (int tap = 0; tap < ntaps; ++tap) {
+                uint32_t b_addr;
+                if (a.b_resident) {
+                    b_addr = b_region + (uint32_t)(tap * a.kchunks + kc) * a.b_bytes;
+                } else {
+                    mbar_wait(bfull0 + 8 * bs, bph);
+                    b_addr = b_region + bs * a.b_bytes;
+                }
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < KKN; ++kk) Wgmma<N>::mma(acc, fr[tap & 1][kk], wgmma_desc(b_addr + 32u * kk, row_bytes), 1u);
+                wgmma_commit();
+                wgmma_wait<1>();          // tap t-1 retired: its A buffer and (streamed) B stage are free
+                if (!a.b_resident) {
+                    if (tap > 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(bempty0 + 8 * prev_bs);
+                    }
+                    prev_bs = bs;
+                    if (++bs == (uint32_t)a.b_stages) { bs = 0; bph ^= 1u; }
+                }
+                if (tap + 1 < ntaps) load_a(tap + 1, fr[(tap + 1) & 1]);
+            }
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            __syncwarp();
+            if (lane == 0) {
+                if (!a.b_resident) mbar_arrive(bempty0 + 8 * prev_bs);
+                mbar_arrive(aempty0 + 8 * as);
+            }
+            if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
+        }
+        EpiArgs e = a.epi;
+        e.par = s_par;
+        const int x0 = tc_.tx * TC_TW + (lane >> 2), y0 = tc_.ty * TC_TH + 8 * wg + 2 * wiw;
+        const int xs[2] = {x0, x0}, ys[2] = {y0, y0 + 1};
+        const bool in[2] = {x0 < a.W && y0 < a.H, x0 < a.W && y0 + 1 < a.H};
+        epilogue_tile<N>(acc, lane, tc_.b, ys, xs, in, tc_.nt, e);
     }
 }
 
@@ -884,14 +288,6 @@ __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__rest
 struct TcGeom {
     int cin_blk, kchunks, n_tile, n_tiles, cout_pad;
 };
-// Issue-side tuning, read at plan creation (read_set_option).  Measured ABAB on the C3 layers (profiles/r02_conv_experiments.md):
-//   tc_merge_done 1: ONE tcgen05.commit per tile for resident-weight, single-K-chunk layers (C=32: 87 -> 79 us, 97 -> 87 us)
-//   tc_commit_late / tc_bpair: fewer commits for supertiles / streamed weights - no gain, off
-int g_tc_commit_late = 0, g_tc_merge_done = 1, g_tc_bpair = 0, g_tc_probe = 0;
-extern int g_tc_tma_store;   // conv_tc2.cu
-int g_tc_pair_wide = 1;   // ... and its streamed-weight variant for the Cin, Cout = 128 / 256 layers ("tc_pair_wide")
-int g_tc_pair = 1;        // CTA-pair (cta_group::2) kernel, conv_tc2.cu (read_set_option "tc_pair"): 0 = off, 1 = Cin 64 layers and Cin 32 layers without a residual (measured ABAB: 81 -> 73 us; with a residual the pair is 2 us slower), 2 = every eligible layer
-int g_tc_mt = 1;          // supertile width (read_set_option "tc_mt"): 1 = plain 8x16 tiles (default: measured fastest), 0 = auto-widen, 2 / 4 = force where legal
 // K-chunk granularity of a layer: the widest block (64 or 32 channels) that divides EVERY source of a virtual concat
 static int desc_chan_gran(const read_conv_desc &d)
 {
@@ -916,7 +312,7 @@ static bool tc_geom(int Cin, int Cout, int stride, TcGeom *g, int chan_gran = 64
     if (Cout <= 8) cout_pad = 8;                 // final layer: N = 16 (f|m of 8 padded channels)
     else if (Cout % 16 != 0) return false;
     const int n_total = 2 * cout_pad;
-    const int n_tile = n_total <= 256 ? n_total : 256;
+    const int n_tile = n_total <= 128 ? n_total : 128;   // accumulators in registers: 64 fp32 per thread
     if (n_total % n_tile != 0) return false;
     if (cout_pad > 8 && (n_tile / 2) % 16 != 0) return false;
     if (cin_blk == 16 && (n_total / n_tile != 1 || cout_pad <= 8 || !(cout_pad == 16 || cout_pad == 32 || cout_pad == 64))) return false;
@@ -997,7 +393,6 @@ struct TcPlan {
     CUtensorMap tmB;
     TcArgs args;
     size_t smem_bytes;
-    Tc2Plan *pair;           // CTA-pair variant (conv_tc2.cu) when the layer qualifies and "tc_pair" is on
     int reverse;
 };
 
@@ -1005,55 +400,26 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
 {
     TcGeom g;
     if (!tc_supported(d) || !tc_geom(d.Cin, d.Cout, d.stride, &g, desc_chan_gran(d))) {
-        set_error("tcgen05 conv: unsupported layer");
+        set_error("wgmma conv: unsupported layer");
         return READ_ERR_UNSUPPORTED;
     }
     PFN_encodeTiled enc = get_encode_tiled();
     if (!enc) {
-        set_error("tcgen05 conv: cuTensorMapEncodeTiled not available from the driver");
+        set_error("wgmma conv: cuTensorMapEncodeTiled not available from the driver");
         return READ_ERR_CUDA;
     }
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.w_tc) & 127) == 0, "tcgen05 conv: packed weights must be 128B aligned");
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "tcgen05 conv: output must be 16B aligned");
-    RB_CHECK_ARG(d.residual == nullptr || (reinterpret_cast<uintptr_t>(d.residual) & 15) == 0, "tcgen05 conv: residual must be 16B aligned");
-    RB_CHECK_ARG(d.addin == nullptr || (reinterpret_cast<uintptr_t>(d.addin) & 15) == 0, "tcgen05 conv: addin must be 16B aligned");
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.w_tc) & 127) == 0, "wgmma conv: packed weights must be 128B aligned");
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "wgmma conv: output must be 16B aligned");
+    RB_CHECK_ARG(d.residual == nullptr || (reinterpret_cast<uintptr_t>(d.residual) & 15) == 0, "wgmma conv: residual must be 16B aligned");
+    RB_CHECK_ARG(d.addin == nullptr || (reinterpret_cast<uintptr_t>(d.addin) & 15) == 0, "wgmma conv: addin must be 16B aligned");
+    const long long tiles = (long long)((d.Wout + TC_TW - 1) / TC_TW) * ((d.Hout + TC_TH - 1) / TC_TH) * d.B * g.n_tiles;
+    RB_CHECK_ARG(tiles < (1ll << 31), "wgmma conv: too many tiles");
     TcPlan *p = new (std::nothrow) TcPlan{};
-    RB_CHECK_ARG(p != nullptr, "tcgen05 conv: out of host memory");
-    // measured ABAB at C3 (profiles/r02_conv_experiments.md): the pair kernel takes the C=64 layers from 73 to 56-68 us, but the C=32
-    // layers (HBM-bound at 3-4.5 TB/s, they live on bytes in flight, not on tensor cycles) from 86 to 97 us -> pairs for Cin 64 only
-    if (g_tc_pair && tc2_supported(d) && d.out_mode == READ_OUT_NHWC && (d.Cin == 64 || (d.Cin == 32 && d.residual == nullptr) || (d.Cin > 64 && g_tc_pair_wide) || g_tc_pair >= 2)) {
-        const int rc2 = tc2_plan_create(d, &p->pair);
-        if (rc2 != READ_OK) { delete p; return rc2; }
-    }
+    RB_CHECK_ARG(p != nullptr, "wgmma conv: out of host memory");
 
     const bool s2 = d.stride == 2;
     const int halo_rows = s2 ? TC_TH + 1 : TC_TH + d.k - 1;
-    const int tiles_x0 = (d.Wout + TC_TW - 1) / TC_TW;
-    const int nacc0 = TC_TMEM_COLS / g.n_tile > TC_MAX_ACC ? TC_MAX_ACC : TC_TMEM_COLS / g.n_tile;
-    // Supertile width (M tiles sharing one halo load / ring stage / hand-shake set).  Round-1 knob experiments: with ALL work
-    // disabled the C=32 kernel still spent 850 cycles per 128-pixel tile in the producer -> issuer -> epilogue hand-shake chains,
-    // half of the layer's time; a supertile amortises them over mt tiles and shrinks the halo overhead (x1.41 -> x1.20 for mt 4).
-    // Constraints: two supertiles of accumulators fit TMEM (mt * n_tile <= 256), nacc % mt == 0, resident weights keep >= 4
-    // stages (two per issuer), streamed weights keep 3; images narrower than a few supertiles stay at mt 1.
-    int mt = 1;
-    if (!s2 && g.n_tiles == 1) {
-        const uint32_t total_b0 = (uint32_t)(d.k * d.k * g.kchunks) * (uint32_t)g.n_tile * g.cin_blk * 2u;
-        const uint32_t ab1 = (((uint32_t)halo_rows * (uint32_t)(TC_TW + d.k - 1) * g.cin_blk * 2u) + 1023u) & ~1023u;
-        const bool res1 = total_b0 <= TC_RESIDENT_MAX && TC_SMEM_BUDGET - total_b0 >= 2 * ab1;   // resident weights at mt 1
-        for (int cand = 4; cand >= 2; cand >>= 1) {
-            if (g_tc_mt > 0 && cand != g_tc_mt) continue;
-            if (cand * g.n_tile > 256 || nacc0 % cand != 0) continue;
-            if (g_tc_mt <= 0 && tiles_x0 < 4 * cand) continue;
-            const uint32_t ab = (((uint32_t)halo_rows * (uint32_t)(TC_TW * cand + d.k - 1) * g.cin_blk * 2u) + 1023u) & ~1023u;
-            // never trade resident weights for a wider supertile (the C=64 layers: 144 KB of weights leave room for mt 1 only)
-            if (res1 ? ((TC_SMEM_BUDGET - total_b0) / ab < (uint32_t)(4 * g.kchunks))
-                     : (3 * ab + 4u * (uint32_t)g.n_tile * g.cin_blk * 2u > TC_SMEM_BUDGET)) continue;
-            mt = cand;
-            break;
-        }
-        if (g_tc_mt == 1) mt = 1;
-    }
-    const int halo_w = s2 ? TC_TW + 1 : TC_TW * mt + d.k - 1;
+    const int halo_w = s2 ? TC_TW + 1 : TC_TW + d.k - 1;
     const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
                                   : (g.cin_blk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
     for (int si = 0; si < d.n_src; ++si) {   // activations: dims {C, W, H, B}; box = one halo tile (all filter taps)
@@ -1069,7 +435,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
                          estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
-            set_error("tcgen05 conv: cuTensorMapEncodeTiled(activations, source %d) failed with %d", si, (int)r);
+            set_error("wgmma conv: cuTensorMapEncodeTiled(activations, source %d) failed with %d", si, (int)r);
             delete p;
             return READ_ERR_CUDA;
         }
@@ -1085,7 +451,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
-            set_error("tcgen05 conv: cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
+            set_error("wgmma conv: cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
             delete p;
             return READ_ERR_CUDA;
         }
@@ -1096,10 +462,6 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     a.cin_blk = g.cin_blk; a.kchunks = g.kchunks; a.n_tile = g.n_tile; a.n_tiles = g.n_tiles;
     a.tiles_x = (d.Wout + TC_TW - 1) / TC_TW;
     a.tiles_y = (d.Hout + TC_TH - 1) / TC_TH;
-    a.mt = mt;
-    a.mt_log2 = mt == 4 ? 2 : (mt == 2 ? 1 : 0);
-    a.stiles_x = (a.tiles_x + mt - 1) / mt;
-    a.inv_stx = 1.0f / (float)a.stiles_x;
     a.halo_w = halo_w;
     a.stride = d.stride;
     a.n_src = d.n_src;
@@ -1111,6 +473,8 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
                 kc += d.src[si].C / g.cin_blk;
                 if (d.n_src > 1 && d.src[si].mode == READ_SRC_NEAREST_DOWN)
                     while ((1 << sh) < d.src[si].factor) ++sh;
+            } else {
+                kc = 1 << 30;
             }
             a.src_kc_end[si] = kc;
             a.src_shift[si] = sh;
@@ -1121,33 +485,11 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
-    a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && TC_SMEM_BUDGET - total_b >= 2 * a.a_bytes) ? 1 : 0;
-    // Lean-epilogue layers (Cout 16 / 32 / 64, NHWC bf16 output, no second output) stage their output items for TMA stores when
-    // reserving the staging buffers does not cost them ring depth that matters (>= 6 stages or as many as without).
-    uint32_t budget = TC_SMEM_BUDGET;
-    a.tma_out = 0;
-    a.stage_bytes = 0;
-    {
-        const int half_n = g.n_tile >> 1;
-        const bool lean = (half_n == 16 || half_n == 32 || half_n == 64) && g.n_tiles == 1 && d.Cout == g.cout_pad &&
-                          (long long)d.B * d.Hout * d.Wout * d.Cout < (1ll << 31);
-        if (g_tc_tma_store && lean && d.out_mode == READ_OUT_NHWC && d.out2 == nullptr && budget > TC_STAGING_BYTES) {
-            const uint32_t small = budget - TC_STAGING_BYTES;
-            bool ok;
-            if (a.b_resident) {
-                const uint32_t full_st = (budget - total_b) / a.a_bytes, st = small > total_b ? (small - total_b) / a.a_bytes : 0;
-                ok = st >= 2 && (st >= 6 || st >= full_st || st >= (uint32_t)TC_MAX_STAGES);
-            } else {
-                const uint32_t full_st = (budget - 3 * a.a_bytes) / a.b_bytes, st = small > 3 * a.a_bytes ? (small - 3 * a.a_bytes) / a.b_bytes : 0;
-                ok = st >= 2 && (st >= 6 || st >= full_st || st >= (uint32_t)TC_MAX_STAGES);
-            }
-            if (ok) {
-                a.tma_out = 1;
-                a.stage_bytes = TC_STAGING_BYTES;
-                budget = small;
-            }
-        }
-    }
+    // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights + >= 4 A stages in half the budget
+    a.ctas_per_sm = (tc_ctas_per_sm(g.n_tile) > 1 && g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX &&
+                     total_b + 4 * a.a_bytes <= TC_SMEM_BUDGET_SMALL_N) ? 2 : 1;
+    const uint32_t budget = a.ctas_per_sm > 1 ? TC_SMEM_BUDGET_SMALL_N : TC_SMEM_BUDGET;
+    a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && total_b + 2 * a.a_bytes <= budget) ? 1 : 0;
     uint32_t b_region_bytes;
     if (a.b_resident) {
         int st = (int)((budget - total_b) / a.a_bytes);
@@ -1157,7 +499,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     } else {
         a.a_stages = 3;
         if (3 * a.a_bytes + 2 * a.b_bytes > budget) {
-            set_error("tcgen05 conv: layer does not fit shared memory (A stage %u B, B tile %u B)", a.a_bytes, a.b_bytes);
+            set_error("wgmma conv: layer does not fit shared memory (A stage %u B, B tile %u B)", a.a_bytes, a.b_bytes);
             delete p;
             return READ_ERR_UNSUPPORTED;
         }
@@ -1165,80 +507,63 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         a.b_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
     }
-    if (a.tma_out) {   // epilogue items: 16 channels x 8 x 4 pixels of the NHWC output (store) / residual (load), 32-byte swizzle
-        cuuint64_t dims[4] = {(cuuint64_t)d.Cout, (cuuint64_t)d.Wout, (cuuint64_t)d.Hout, (cuuint64_t)d.B};
-        cuuint64_t strides[3] = {(cuuint64_t)d.Cout * 2, (cuuint64_t)d.Wout * d.Cout * 2, (cuuint64_t)d.Hout * d.Wout * d.Cout * 2};
-        cuuint32_t box[4] = {16, (cuuint32_t)TC_TW, 4, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&p->tmA.o, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r == CUDA_SUCCESS)
-            r = enc(&p->tmA.r, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, d.residual ? const_cast<void *>(d.residual) : d.out, dims, strides, box,
-                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) {
-            set_error("tcgen05 conv: cuTensorMapEncodeTiled(output items) failed with %d", (int)r);
-            delete p;
-            return READ_ERR_CUDA;
-        }
-    }
-    a.inv_tx = 1.0f / (float)a.tiles_x;
-    a.inv_ty = 1.0f / (float)a.tiles_y;
-    a.nacc = TC_TMEM_COLS / g.n_tile > TC_MAX_ACC ? TC_MAX_ACC : TC_TMEM_COLS / g.n_tile;
-    a.nacc_log2 = 0;
-    while ((1 << a.nacc_log2) < a.nacc) ++a.nacc_log2;     // n_tile is 16 * 2^k here: nacc is 2, 4 or 8
-    a.dual = (a.b_resident && a.a_stages >= 4 * g.kchunks) ? 1 : 0;      // >= 2 tiles of A per issuer
-    if (a.dual) a.a_stages &= ~1;            // two equal half rings
-    a.commit_late = g_tc_commit_late ? 1 : 0;
-    a.merge_done = 0;
-    if (g_tc_merge_done && a.b_resident && g.kchunks == 1 && mt == 1 && a.a_stages >= 2) {
-        // A ring depth == accumulator ring depth: stage <-> slot is one-to-one.  The shallower ring wins (C=64: 144 KB of
-        // resident weights leave 3 A stages, so 3 of the 4 accumulator slots are used); two issuers need an even split.
-        a.merge_done = 1;
-        const int depth = a.a_stages < a.nacc ? a.a_stages : a.nacc;
-        a.dual = depth >= 4 ? 1 : 0;
-        a.a_stages = a.nacc = a.dual ? (depth & ~1) : depth;
-    }
-    a.probe = (g_tc_probe && a.b_resident && g.kchunks == 1 && mt == 1) ? 1 : 0;
-    a.bpair = 0;
-    if (g_tc_bpair && !a.b_resident && a.b_stages >= 4) {
-        a.bpair = 1;
-        a.b_stages &= ~1;
-        b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
-    }
     a.b_region_off = (uint32_t)a.a_stages * a.a_bytes;
-    a.elu = d.elu;
     a.bias_f = d.bias_f; a.bias_m = d.bias_m; a.scale = d.bn_scale; a.shift = d.bn_shift;
-    a.residual = static_cast<const __nv_bfloat16 *>(d.residual);
-    a.out = static_cast<__nv_bfloat16 *>(d.out);
-    a.out_nchw = static_cast<float *>(d.out);
-    a.out2 = static_cast<__nv_bfloat16 *>(d.out2);
-    a.out2_mul = static_cast<const __nv_bfloat16 *>(d.out2_mul);
-    a.addin = static_cast<const __nv_bfloat16 *>(d.addin);
-    a.addin_H = d.addin_H; a.addin_W = d.addin_W;
-    a.raw = d.out_mode == READ_OUT_RAW_NHWC ? 1 : 0;
-    p->smem_bytes = 1024 + (size_t)a.b_region_off + b_region_bytes + a.stage_bytes + 8 * BAR_PARAMS + 16 * (size_t)g.cout_pad + 64;
+    EpiArgs &e = a.epi;
+    e.H = d.Hout; e.W = d.Wout; e.Cout = d.Cout;
+    e.elu = d.elu;
+    e.raw = d.out_mode == READ_OUT_RAW_NHWC ? 1 : 0;
+    e.nchw = d.out_mode == READ_OUT_NCHW_F32 ? 1 : 0;
+    e.par = nullptr;
+    e.residual = static_cast<const __nv_bfloat16 *>(d.residual);
+    e.out2_mul = static_cast<const __nv_bfloat16 *>(d.out2_mul);
+    e.addin = static_cast<const __nv_bfloat16 *>(d.addin);
+    e.out = d.out;
+    e.out2 = static_cast<__nv_bfloat16 *>(d.out2);
+    e.addin_H = d.addin_H; e.addin_W = d.addin_W;
+    p->smem_bytes = 1024 + (size_t)a.b_region_off + b_region_bytes + 8 * BAR_PARAMS + 16 * (size_t)g.cout_pad + 64;
     *out = p;
     return READ_OK;
 }
 
-int g_tc_debug = 0;
-unsigned long long *g_tc_trace = nullptr;    // READ_DIAG builds only (read_set_trace_buffer)
-int g_tc_role_rot = 1;    // single-issuer roles in the highest warp ids (read_set_option "tc_role_rot")
 int g_tc_pdl = 1;         // programmatic dependent launch between consecutive conv kernels (read_set_option "tc_pdl")
+
+template <int KS, int STR, int KKN, int N>
+static int launch_tc(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_kernel<KS, STR, KKN, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
+    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_kernel<KS, STR, KKN, N>, p->tmA, p->tmB, a));
+    return READ_OK;
+}
+
+template <int KS, int STR>
+static int launch_tc_kn(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    const int kkn = a.cin_blk / 16;
+#define RB_TC_N(KKN_)                                                                       \
+    switch (a.n_tile) {                                                                     \
+    case 16: return launch_tc<KS, STR, KKN_, 16>(p, a, lcfg);                               \
+    case 32: return launch_tc<KS, STR, KKN_, 32>(p, a, lcfg);                               \
+    case 64: return launch_tc<KS, STR, KKN_, 64>(p, a, lcfg);                               \
+    case 128: return launch_tc<KS, STR, KKN_, 128>(p, a, lcfg);                             \
+    default: break;                                                                         \
+    }
+    if (kkn == 1) { RB_TC_N(1) }
+    else if (kkn == 2) { RB_TC_N(2) }
+    else if (kkn == 4) { RB_TC_N(4) }
+#undef RB_TC_N
+    set_error("wgmma conv: no kernel instance for cin_blk=%d n_tile=%d", a.cin_blk, a.n_tile);
+    return READ_ERR_UNSUPPORTED;
+}
 
 int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
 {
-    if (p->pair != nullptr) return tc2_plan_launch(p->pair, st, max_ctas);
     TcArgs a = p->args;
-    a.debug = g_tc_debug;
-    a.role_rot = g_tc_role_rot ? 1 : 0;
     a.pdl = g_tc_pdl ? 1 : 0;
-    a.trace = g_tc_trace;
-    const long long total_tiles = (long long)a.stiles_x * a.tiles_y * a.B * a.n_tiles;
+    const long long total_tiles = (long long)a.tiles_x * a.tiles_y * a.B * a.n_tiles;
     if (total_tiles == 0) return READ_OK;
     a.rev_total = p->reverse ? (int)total_tiles : 0;
-    long long grid = num_sms();
+    long long grid = (long long)num_sms() * a.ctas_per_sm;
     if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
     if (grid > total_tiles) grid = total_tiles;
     // cudaLaunchKernelEx with programmatic stream serialization: the kernel may be scheduled while its predecessor in the
@@ -1248,80 +573,28 @@ int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
     lattr[0].val.programmaticStreamSerializationAllowed = 1;
     cudaLaunchConfig_t lcfg{};
     lcfg.gridDim = dim3((unsigned)grid);
+    lcfg.blockDim = dim3(TC_THREADS);
     lcfg.dynamicSmemBytes = p->smem_bytes;
     lcfg.stream = st;
     lcfg.attrs = lattr;
     lcfg.numAttrs = a.pdl ? 1 : 0;
-#define RB_TC_LAUNCH_I(KS_, KKN_, RES_, NT_, EPI_, STR_)                                                               \
-    do {                                                                                                                \
-        RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_kernel<KS_, KKN_, RES_, NT_, EPI_, STR_>,                            \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));                 \
-        lcfg.blockDim = dim3(NT_);                                                                                      \
-        RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_kernel<KS_, KKN_, RES_, NT_, EPI_, STR_>, p->tmA, p->tmB, a));  \
-    } while (0)
-#define RB_TC_LAUNCH(KS_, KKN_, RES_, STR_)                                                                             \
-    do {                                                                                                                \
-        if (lean) RB_TC_LAUNCH_I(KS_, KKN_, RES_, 640, 0, STR_);                                                        \
-        else RB_TC_LAUNCH_I(KS_, KKN_, RES_, 384, 0, STR_);                                                             \
-    } while (0)
-#define RB_TC_LAUNCH_K(KS_, STR_)                                                                                       \
-    do {                                                                                                                \
-        if (kkn == 4 && a.b_resident) RB_TC_LAUNCH(KS_, 4, true, STR_);                                                 \
-        else if (kkn == 4) RB_TC_LAUNCH(KS_, 4, false, STR_);                                                           \
-        else if (a.b_resident) RB_TC_LAUNCH(KS_, 2, true, STR_);                                                        \
-        else RB_TC_LAUNCH(KS_, 2, false, STR_);                                                                         \
-    } while (0)
-    // lean 16-warp epilogue: Cout 16 / 32 / 64 and 32-bit output offsets
-    const int half_n = a.n_tile >> 1;
-    const bool lean = (half_n == 16 || half_n == 32 || half_n == 64) && a.Cout == a.cout_pad &&
-                      (long long)a.B * a.H * a.W * a.Cout < (1ll << 31);
-    const int kkn = a.cin_blk / 16;
-    // the two ResBlock layer kinds of the C=32 / C=64 stages get compile-time epilogues
-    const int epi = (lean && a.stride == 1 && a.ksize == 3 && a.b_resident && !a.out2)
-                        ? ((a.elu && !a.residual) ? 1 : ((!a.elu && a.residual) ? 2 : 0)) : 0;
-    if (kkn != 1 && kkn != 2 && kkn != 4) {
-        set_error("tcgen05 conv: no kernel instance for cin_blk=%d", a.cin_blk);
-        return READ_ERR_UNSUPPORTED;
-    }
-    if (kkn == 1) {        // 8- / 16-channel inputs: resident weights, lean epilogue (tc_geom admits nothing else)
-        if (!(lean && a.b_resident && a.stride == 1)) {
-            set_error("tcgen05 conv: 16-channel K steps need resident weights and Cout 16 / 32 / 64");
-            return READ_ERR_UNSUPPORTED;
-        }
-        if (a.ksize == 3) { if (epi == 1) RB_TC_LAUNCH_I(3, 1, true, 640, 1, 1); else RB_TC_LAUNCH_I(3, 1, true, 640, 0, 1); }
-        else RB_TC_LAUNCH_I(1, 1, true, 640, 0, 1);
-    }
-    else if (epi == 1 && kkn == 2) RB_TC_LAUNCH_I(3, 2, true, 640, 1, 1);
-    else if (epi == 2 && kkn == 2) RB_TC_LAUNCH_I(3, 2, true, 640, 2, 1);
-    else if (epi == 1 && kkn == 4) RB_TC_LAUNCH_I(3, 4, true, 640, 1, 1);
-    else if (epi == 2 && kkn == 4) RB_TC_LAUNCH_I(3, 4, true, 640, 2, 1);
-    else if (a.stride == 1 && a.ksize == 3) RB_TC_LAUNCH_K(3, 1);
-    else if (a.stride == 1 && a.ksize == 1) RB_TC_LAUNCH_K(1, 1);
-    else if (a.stride == 2 && a.ksize == 3 && kkn == 2) { if (a.b_resident) RB_TC_LAUNCH(3, 2, true, 2); else RB_TC_LAUNCH(3, 2, false, 2); }
-    else if (a.stride == 2 && a.ksize == 4 && kkn == 2) { if (a.b_resident) RB_TC_LAUNCH(4, 2, true, 2); else RB_TC_LAUNCH(4, 2, false, 2); }
+    int rc;
+    if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
+    else if (a.stride == 1 && a.ksize == 3) rc = launch_tc_kn<3, 1>(p, a, lcfg);
+    else if (a.stride == 2 && a.ksize == 3) rc = launch_tc_kn<3, 2>(p, a, lcfg);
+    else if (a.stride == 2 && a.ksize == 4) rc = launch_tc_kn<4, 2>(p, a, lcfg);
     else {
-        set_error("tcgen05 conv: no kernel instance for k=%d stride=%d", a.ksize, a.stride);
+        set_error("wgmma conv: no kernel instance for k=%d stride=%d", a.ksize, a.stride);
         return READ_ERR_UNSUPPORTED;
     }
-#undef RB_TC_LAUNCH_K
-#undef RB_TC_LAUNCH_I
-#undef RB_TC_LAUNCH
+    if (rc != READ_OK) return rc;
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
 
-void tc2_plan_set_reverse(Tc2Plan *p, int reverse);
-void tc_plan_set_reverse(TcPlan *p, int reverse)
-{
-    p->reverse = reverse ? 1 : 0;
-    if (p->pair) tc2_plan_set_reverse(p->pair, reverse);
-}
+void tc_plan_set_reverse(TcPlan *p, int reverse) { p->reverse = reverse ? 1 : 0; }
 
-void tc_plan_destroy(TcPlan *p)
-{
-    if (p && p->pair) tc2_plan_destroy(p->pair);
-    delete p;
-}
+void tc_plan_destroy(TcPlan *p) { delete p; }
 
 }  // namespace rb
 
@@ -1331,10 +604,6 @@ static int pack_tc_impl(const float *wf, const float *wm, int Cout, int Cin, int
                         void *stream);
 
 extern "C" {
-
-#ifdef READ_DIAG
-void read_set_trace_buffer(void *buf) { g_tc_trace = static_cast<unsigned long long *>(buf); }
-#endif
 
 int64_t read_tc_weight_elems(int Cout, int Cin, int k)
 {

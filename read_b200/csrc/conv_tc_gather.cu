@@ -1,22 +1,20 @@
-// General gated convolution on the tcgen05 tensor cores: implicit GEMM whose A operand is GATHERED by four
-// producer warps (cp.async 16-byte chunks, zero-fill for padding) directly into the 128B-swizzled K-major
-// layout the UMMA descriptor expects.  Covers every BasicConv shape of READ/models/unet.py that the pure-TMA kernel
-// (conv_tc.cu) cannot express as shifted tile loads:
-//   * stride-2 3x3 and 4x4 convolutions (feat_extract[1,2,6], [3,4,7])
+// General gated convolution on the Hopper tensor cores (wgmma): implicit GEMM whose A operand is GATHERED by four
+// producer warps (cp.async 16-byte chunks, zero-fill for padding) into 128B-swizzled rows of shared memory.  Covers every
+// BasicConv shape of READ/models/unet.py that the TMA kernel (conv_tc.cu) cannot express as shifted tile loads:
+//   * stride-2 3x3 and 4x4 convolutions with channel counts the TMA kernel does not take (feat_extract[1,2,6], [3,4,7])
 //   * virtual concat of up to 4 sources (SCM / AFF / decoder merges: unet.py:88,105,263,271,279)
 //   * nearest up/down resampling of a source (F.interpolate, unet.py:239-250) and bilinear x4 (nn.Upsample, :200)
 //   * channel counts that are only multiples of 8 (8->32 first conv, 32->3 last conv, SCM 16/56/120/248)
 //   * NCHW fp32 output for the final layer
 //
 // GEMM view: M = 128 output pixels (8 rows x 16 cols), K = (tap, cin) flattened in 8-channel chunks and padded to
-// 64-element blocks, N = conv_f | conv_m channels (<= 256 per tile).  Weights arrive by TMA; accumulators live in
-// TMEM (double buffered); the epilogue is the same fused bias/ELU/sigmoid/BN/residual tail as conv_tc.cu.
+// 64-element blocks, N = conv_f | conv_m channels (<= 128 per tile).  Weights arrive by TMA and are read by wgmma through
+// shared-memory descriptors; the A rows are read with ldmatrix into wgmma's register operand; accumulators live in the
+// registers of two consumer warpgroups (64 pixels each), whose epilogue is the fused bias/ELU/sigmoid/BN/residual tail of
+// conv_common.cuh.
 //
-// Warp roles (832 threads, 1 CTA/SM, persistent): warp0 = weight TMA + TMEM alloc, warp1 = MMA issuer,
-// warps2-9 = A gather producers, one warp per ring stage (lane -> fixed 16-byte K chunk, 4 tile columns x 8 rows),
-// warps10-25 = epilogue (TMEM lane quadrant = warp%4, four warps per quadrant interleaved over 8-column chunks).
-// Stride is a template parameter, row validity replaces clamps, source offsets are 32-bit, the tile decode is
-// division-free, accumulators form a TMEM ring.
+// Warp roles (384 threads, 1 CTA/SM, persistent): warps 0-3 = producers, one warp per ring stage: lane 0 loads the stage's
+// weights by TMA and every lane gathers a fixed 16-byte K chunk of 4 tile columns x 8 rows of A; warps 4-11 = consumers.
 #include "common.cuh"
 #include "conv_common.cuh"
 #include "ptx.cuh"
@@ -26,20 +24,11 @@
 
 namespace rb {
 
-#ifdef READ_DIAG
-#define TCG_DBG(a_, bit_) (((a_).debug & (bit_)) != 0)
-#else
-#define TCG_DBG(a_, bit_) false
-#endif
-
-constexpr int G_THREADS = 832;
-constexpr int G_EPI_WARP0 = 10;              // warps 10..25
-constexpr int G_EPI_WARPS = 16;
+constexpr int G_THREADS = 384;
+constexpr int G_CONS_WARP0 = 4;              // warps 0..3 produce, warps 4..11 are two consumer warpgroups
 constexpr int G_TW = 16, G_TH = 8;
-constexpr int G_MAX_STAGES = 8;
+constexpr int G_MAX_STAGES = 4;              // one gather warp per ring stage
 constexpr uint32_t G_SMEM_BUDGET = 200 * 1024;
-constexpr int G_TMEM_COLS = 512;
-constexpr int G_MAX_ACC = 8;
 constexpr int G_KBLK = 64;                     // elements per K block (128-byte rows, SWIZZLE_128B)
 
 struct GSrc {
@@ -69,18 +58,10 @@ struct GArgs {
     int tiles_x, tiles_y;
     float inv_tx, inv_ty, inv_nt;   // reciprocals for the division-free tile decode
     int stages;
-    int nacc;                  // TMEM accumulator ring depth (each n_tile columns wide)
     int pdl;                   // launched with programmatic stream serialization
-    int lean16;                // epilogue work items = (quadrant, 16-column chunk) dealt over tiles (NHWC, Cout 16 / 32 / 64)
-    int debug;                 // diagnostic knobs ("tcg_debug"): 1 = epilogue only hand-shakes, 2 = no MMAs, 4 = no gather copies
     uint32_t a_bytes, b_bytes;
-    int elu;
     const float *bias_f, *bias_m, *scale, *shift;
-    const __nv_bfloat16 *residual;
-    void *out;
-    int out_mode;
-    __nv_bfloat16 *out2;
-    const __nv_bfloat16 *out2_mul;
+    EpiArgs epi;
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32_t src_bytes)
@@ -92,19 +73,11 @@ __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar)
 {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t g_pack2(float a, float b)
 {
     __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t *>(&v);
-}
-// one F2FP per pair: lo -> bits [0,16) (lower address)
-__device__ __forceinline__ uint32_t g_cvt2(float lo, float hi)
-{
-    uint32_t d;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
-    return d;
 }
 __device__ __forceinline__ float2 g_unpack2(uint32_t u) { return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162 *>(&u)); }
 
@@ -143,7 +116,7 @@ __device__ __noinline__ void gather_bilinear_row(const SrcS &sv, const __nv_bflo
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(o.x), "r"(o.y), "r"(o.z), "r"(o.w) : "memory");
 }
 
-template <int STRIDE>
+template <int STRIDE, int N>
 __global__ void __launch_bounds__(G_THREADS, 1)
 gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ GArgs a)
 {
@@ -156,10 +129,7 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + ring_bytes);
     const uint32_t full0 = s_u32(bars);
     const uint32_t empty0 = full0 + 8 * G_MAX_STAGES;
-    const uint32_t tfull0 = empty0 + 8 * G_MAX_STAGES;
-    const uint32_t tempty0 = tfull0 + 8 * G_MAX_ACC;
-    uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(bars + 2 * G_MAX_STAGES + 2 * G_MAX_ACC);
-    float4 *s_par4 = reinterpret_cast<float4 *>(bars + 2 * G_MAX_STAGES + 2 * G_MAX_ACC + 2);   // Cout_pad x {bias_f, bias_m, scale, shift}
+    float4 *s_par4 = reinterpret_cast<float4 *>(bars + 2 * G_MAX_STAGES);   // Cout_pad x {bias_f, bias_m, scale, shift}
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int CP = a.Cout_pad;
@@ -195,25 +165,16 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
         s_tab[i] = e;
     }
     for (int i = threadIdx.x; i < CP; i += G_THREADS)
-        s_par4[i] = i < a.Cout ? make_float4(a.bias_f[i], 0.5f * a.bias_m[i], 0.5f * a.scale[i], a.shift[i])   // gate_folded
-                               : make_float4(0.f, 0.f, 0.f, 0.f);
-    if (warp == 1 && lane == 0) {
+        s_par4[i] = i < a.Cout ? make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < a.stages; ++s) {
-            mbar_init(full0 + 8 * s, 32 + 1);   // the 32 lanes of the stage's gather warp + the weight-TMA thread
-            mbar_init(empty0 + 8 * s, 1);
-        }
-        for (int i = 0; i < G_MAX_ACC; ++i) {
-            mbar_init(tfull0 + 8 * i, 1);
-            mbar_init(tempty0 + 8 * i, a.lean16 ? (uint32_t)(a.n_tile >> 3) : (uint32_t)G_EPI_WARPS);   // arrivals per tile
+            mbar_init(full0 + 8 * s, 32 + 1);   // the 32 lanes of the stage's gather warp + its lane 0's weight TMA
+            mbar_init(empty0 + 8 * s, 8);       // the 8 consumer warps
         }
         mbar_fence_init();
     }
-    if (warp == 0) tmem_alloc(s_u32(tmem_ptr_smem), G_TMEM_COLS);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     // everything above touched only static data (weights' descriptors, folded constants): with programmatic dependent launch
     // it overlapped the previous kernel's tail; activations / residuals below need that kernel to have completed
     if (a.pdl) pdl_wait();
@@ -222,73 +183,14 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
     const long long total_tiles = (long long)m_tiles * a.n_tiles;
     const int n_total = a.n_tile * a.n_tiles;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            // ===================== weight TMA producer =====================
-            uint32_t s = 0, ph = 0;
-            for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                const int nt = (int)t - fdiv_small((int)t, a.inv_nt) * a.n_tiles;
-                int row = nt * a.n_tile;
-                for (int kb = 0; kb < a.kblocks; ++kb, row += n_total) {
-                    mbar_wait(empty0 + 8 * s, ph ^ 1u);
-                    const uint32_t fb = full0 + 8 * s;
-                    mbar_arrive_expect_tx(fb, a.b_bytes);
-                    tma_load_2d(&tmB, fb, smem_base + s * stage_bytes + a.a_bytes, 0, row);
-                    if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===================== MMA issuer =====================
-            // (Two issuers on alternate tiles were tried and dropped: both would walk the SAME stage ring, and an issuer
-            // skipping the other's stages can get more than one mbarrier phase ahead of a slot - the parity wait then
-            // aliases.  conv_tc.cu can do it because each of its issuers owns a half ring.)
-            // The ~90-cycle latency of try_wait is taken off the per-stage chain by probing the NEXT stage's barrier
-            // before the current stage's MMAs are issued.
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(a.n_tile >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t desc_hi = (uint32_t)(make_kmajor_desc(0, 1024u, 2u) >> 32);
-            const uint32_t st16 = stage_bytes >> 4, ab16 = a.a_bytes >> 4;
-            const uint32_t lo0 = ((smem_base & 0x3FFFFu) >> 4) | (1u << 16);
-            uint32_t s = 0, ph = 0, lo = lo0;
-            uint32_t acc = 0, acc_ph = 0;              // accumulator ring (see conv_tc.cu): tile i -> slot i % nacc
-            bool ready = false;                        // the current stage's full barrier was already seen complete
-            for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                mbar_wait(tempty0 + 8 * acc, acc_ph ^ 1u);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * (uint32_t)a.n_tile;
-                for (int kb = 0; kb < a.kblocks; ++kb) {
-                    if (!ready) mbar_wait(full0 + 8 * s, ph);
-                    uint32_t sn = s + 1, phn = ph;
-                    if (sn == (uint32_t)a.stages) { sn = 0; phn ^= 1u; }
-                    ready = mbar_try_wait(full0 + 8 * sn, phn);      // probe (the ring is continuous across tiles)
-                    fence_proxy_async();          // gathered A rows were written through the generic proxy
-                    tcgen05_fence_after();
-#pragma unroll
-                    for (int kk = 0; kk < G_KBLK / 16; ++kk) {
-                        if (TCG_DBG(a, 2)) continue;
-                        umma_bf16_lohi(d_tmem, lo + 2u * kk, lo + ab16 + 2u * kk, desc_hi, idesc,
-                                       kk != 0 ? 1u : (kb != 0 ? 1u : 0u));
-                    }
-                    umma_commit(empty0 + 8 * s);
-                    lo += st16;
-                    s = sn; ph = phn;
-                    if (s == 0) lo = lo0;
-                }
-                umma_commit(tfull0 + 8 * acc);
-                if (++acc == (uint32_t)a.nacc) { acc = 0; acc_ph ^= 1u; }
-            }
-        }
-    } else if (warp < G_EPI_WARP0) {
-        // ===================== A gather producers: 8 warps, ONE WARP PER RING STAGE =====================
-        // Warp w owns ring slot w (stages <= 8 warps; a slot must have ONE producer that sees every one of its phases, or
-        // the parity wait on its empty barrier could alias two phases) and fills it on its own: lane -> (16-byte K chunk j = lane & 7, tile
-        // column px = 4*g + (lane >> 3), g = 0..3), 8 tile rows each, 32 copies per lane and stage.  Round-1 knob
-        // experiments: with 256 threads per stage the 256 serialised mbarrier arrivals alone cost ~380 cycles per
-        // stage (3x the stage's MMA time) and every warp paid the wait / decode / table latencies of every stage; here
-        // a stage costs 32 arrivals and its per-stage set-up is paid once per lane, while 8 stages are gathered
-        // concurrently by the 8 warps.
-        const uint32_t w = (uint32_t)(warp - 2);
+    if (warp < G_CONS_WARP0) {
+        // ===================== producers: 4 warps, ONE WARP PER RING STAGE =====================
+        // Warp w owns ring slot w (a slot must have ONE producer that sees every one of its phases, or the parity wait on its
+        // empty barrier could alias two phases) and fills it on its own: lane 0 starts the TMA of the stage's weight block,
+        // then lane -> (16-byte K chunk j = lane & 7, tile column px = 4*g + (lane >> 3), g = 0..3), 8 tile rows each, 32
+        // copies per lane and stage.  The stages are gathered concurrently by the 4 warps.
+        const uint32_t w = (uint32_t)warp;
+        if (w >= (uint32_t)a.stages) return;
         const uint32_t my_empty = empty0 + 8 * w;
         const int j = lane & 7;
         const int pq = lane >> 3;
@@ -296,6 +198,7 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
         const int4 *tab = s_tab + j;
         for (long long tl = blockIdx.x; tl < total_tiles; tl += gridDim.x) {
             const int mt = fdiv_small((int)tl, a.inv_nt);
+            const int nt = (int)tl - mt * a.n_tiles;
             const int q_ = fdiv_small(mt, a.inv_tx);
             const int tx = mt - q_ * a.tiles_x;
             const int b = fdiv_small(q_, a.inv_ty);
@@ -307,69 +210,67 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
                 if (s == w) {
                     mbar_wait(my_empty, ph ^ 1u);
                     const uint32_t dst0 = smem_base + s * stage_bytes;
-                    if (TCG_DBG(a, 4)) {
-                        mbar_arrive(full0 + 8 * s);
-                    } else {
-                        const int4 e = tab[kb * 8];
-                        const SrcS &sv = s_src[e.x < 0 ? 0 : e.x];
-                        const __nv_bfloat16 *sbase = sv.ptr + (long long)b * sv.plane;
-                        const int iy0 = iyb + e.y;
-                        if (!sv.bil) {
-                            const int shl = sv.shl, shr = sv.shr, rs = sv.rs, C = sv.C;
-                            // per-row source offsets (elements), -1 = row outside the image / the output
-                            int roff[G_TH];
+                    if (lane == 0) {
+                        mbar_arrive_expect_tx(full0 + 8 * s, a.b_bytes);
+                        tma_load_2d(&tmB, full0 + 8 * s, dst0 + a.a_bytes, 0, nt * a.n_tile + kb * n_total);
+                    }
+                    const int4 e = tab[kb * 8];
+                    const SrcS &sv = s_src[e.x < 0 ? 0 : e.x];
+                    const __nv_bfloat16 *sbase = sv.ptr + (long long)b * sv.plane;
+                    const int iy0 = iyb + e.y;
+                    if (!sv.bil) {
+                        const int shl = sv.shl, shr = sv.shr, rs = sv.rs, C = sv.C;
+                        // per-row source offsets (elements), -1 = row outside the image / the output
+                        int roff[G_TH];
+#pragma unroll
+                        for (int i = 0; i < G_TH; ++i) {
+                            const int iy = iy0 + i * STRIDE;
+                            const bool rv = (e.x >= 0) && (i < rows_ok) && ((unsigned)iy < (unsigned)a.Hin);
+                            roff[i] = rv ? ((iy << shl) >> shr) * rs + e.w : -1;
+                        }
+#pragma unroll
+                        for (int g = 0; g < 4; ++g) {
+                            const int px = g * 4 + pq;
+                            const int ox = tx * G_TW + px;
+                            const int ix = ox * STRIDE - a.pad + e.z;
+                            const bool xv = (ox < a.Wout) && ((unsigned)ix < (unsigned)a.Win);
+                            const int xoff = ((ix << shl) >> shr) * C;
+                            const uint32_t dcol = dst0 + (uint32_t)px * 128u + (uint32_t)((j ^ (px & 7)) << 4);
 #pragma unroll
                             for (int i = 0; i < G_TH; ++i) {
-                                const int iy = iy0 + i * STRIDE;
-                                const bool rv = (e.x >= 0) && (i < rows_ok) && ((unsigned)iy < (unsigned)a.Hin);
-                                roff[i] = rv ? ((iy << shl) >> shr) * rs + e.w : -1;
+                                const bool valid = xv && roff[i] >= 0;
+                                cp_async16(dcol + (uint32_t)i * 2048u, sbase + (valid ? roff[i] + xoff : 0), valid ? 16u : 0u);
                             }
-#pragma unroll
-                            for (int g = 0; g < 4; ++g) {
-                                const int px = g * 4 + pq;
-                                const int ox = tx * G_TW + px;
-                                const int ix = ox * STRIDE - a.pad + e.z;
-                                const bool xv = (ox < a.Wout) && ((unsigned)ix < (unsigned)a.Win);
-                                const int xoff = ((ix << shl) >> shr) * C;
-                                const uint32_t dcol = dst0 + (uint32_t)px * 128u + (uint32_t)((j ^ (px & 7)) << 4);
-#pragma unroll
-                                for (int i = 0; i < G_TH; ++i) {
-                                    const bool valid = xv && roff[i] >= 0;
-                                    cp_async16(dcol + (uint32_t)i * 2048u, sbase + (valid ? roff[i] + xoff : 0), valid ? 16u : 0u);
-                                }
-                            }
-                            // asynchronous arrival: the barrier counts this lane in when its copies above have landed (no
-                            // wait, no writer-side proxy fence: the MMA thread fences once per stage after its wait)
-                            cp_async_arrive_noinc(full0 + 8 * s);
-                        } else {
-                            for (int g = 0; g < 4; ++g) {
-                                const int px = g * 4 + pq;
-                                const int ox = tx * G_TW + px;
-                                const int ix = ox * STRIDE - a.pad + e.z;
-                                const bool xv = (e.x >= 0) && (ox < a.Wout) && ((unsigned)ix < (unsigned)a.Win);
-                                const uint32_t dcol = dst0 + (uint32_t)px * 128u + (uint32_t)((j ^ (px & 7)) << 4);
-                                for (int i = 0; i < G_TH; ++i) {
-                                    const int iy = iy0 + i * STRIDE;
-                                    const bool valid = xv && (i < rows_ok) && (iy >= 0) && (iy < a.Hin);
-                                    gather_bilinear_row(sv, sbase + e.w, ix, iy, valid, dcol + (uint32_t)i * 2048u);
-                                }
-                            }
-                            fence_proxy_async();          // plain st.shared data: writer-side fence + ordinary arrive
-                            mbar_arrive(full0 + 8 * s);
                         }
+                        // asynchronous arrival: the barrier counts this lane in when its copies above have landed
+                        cp_async_arrive_noinc(full0 + 8 * s);
+                    } else {
+                        for (int g = 0; g < 4; ++g) {
+                            const int px = g * 4 + pq;
+                            const int ox = tx * G_TW + px;
+                            const int ix = ox * STRIDE - a.pad + e.z;
+                            const bool xv = (e.x >= 0) && (ox < a.Wout) && ((unsigned)ix < (unsigned)a.Win);
+                            const uint32_t dcol = dst0 + (uint32_t)px * 128u + (uint32_t)((j ^ (px & 7)) << 4);
+                            for (int i = 0; i < G_TH; ++i) {
+                                const int iy = iy0 + i * STRIDE;
+                                const bool valid = xv && (i < rows_ok) && (iy >= 0) && (iy < a.Hin);
+                                gather_bilinear_row(sv, sbase + e.w, ix, iy, valid, dcol + (uint32_t)i * 2048u);
+                            }
+                        }
+                        mbar_arrive(full0 + 8 * s);
                     }
                 }
                 if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
             }
         }
-    } else if (warp < G_EPI_WARP0 + G_EPI_WARPS) {
-        // ===================== epilogue (warps 10-25) =====================
-        const int q = warp & 3;                       // TMEM lane quadrant this warp may read
-        const int sub = (warp - G_EPI_WARP0) >> 2;    // 0..3: 8-column chunks sub, sub + 4, ...
-        const int r = q * 32 + lane;
-        const int py = r / G_TW, pxl = r % G_TW;
-        const int half = a.n_tile >> 1;
-        uint32_t acc_c = 0, acc_p = 0, lean_it = 0;
+    } else {
+        // ===================== consumers: two warpgroups, 64 pixels (4 tile rows) each =====================
+        const int wg = (warp - G_CONS_WARP0) >> 2, wiw = warp & 3;
+        const uint32_t lrow = (uint32_t)(64 * wg + 16 * wiw + (lane & 7) + 8 * ((lane >> 3) & 1));   // this lane's ldmatrix row
+        const uint32_t khalf = (uint32_t)(lane >> 4) * 16u;
+        uint32_t s = 0, ph = 0;
+        EpiArgs e = a.epi;
+        e.par = s_par4;
         for (long long t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const int mt = fdiv_small((int)t, a.inv_nt);
             const int nt = (int)t - mt * a.n_tiles;
@@ -377,171 +278,31 @@ gated_conv_tc_gather_kernel(const __grid_constant__ CUtensorMap tmB, const __gri
             const int tx = mt - q_ * a.tiles_x;
             const int b = fdiv_small(q_, a.inv_ty);
             const int ty = q_ - b * a.tiles_y;
-            const int x = tx * G_TW + pxl, y = ty * G_TH + py;
-            const bool inside = (x < a.Wout) && (y < a.Hout);
-            const int pix = (b * a.Hout + y) * a.Wout + x;                  // output elements < 2^31 (checked by the host)
-            const uint32_t acc = acc_c, acc_ph = acc_p;
-            if (++acc_c == (uint32_t)a.nacc) { acc_c = 0; acc_p ^= 1u; }
-            const bool nhwc = a.out_mode != READ_OUT_NCHW_F32;
-            const bool has_res = a.residual != nullptr, has_out2 = a.out2 != nullptr;
-            if (a.lean16) {
-                // (quadrant, 16-column chunk) items, 4 * nch16 per tile, dealt warp -> chunk (sub % nch16) of every G-th
-                // tile (G = 4 / nch16): a lane owns 32 contiguous output bytes (full sectors), see conv_tc.cu
-                const int nch16 = half >> 4;
-                const int chunk = sub & (nch16 - 1);
-                if (((lean_it++) & (uint32_t)((4 >> (nch16 >> 1)) - 1)) != (uint32_t)(sub >> (nch16 >> 1))) continue;
-                const int co = chunk * 16;
-                const int o = pix * a.Cout + co;
-                uint4 rs0 = make_uint4(0, 0, 0, 0), rs1 = rs0, ml0 = rs0, ml1 = rs0;
-                if (inside) {
-                    if (has_res) {
-                        rs0 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o));
-                        rs1 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o) + 1);
-                    }
-                    if (has_out2) {
-                        ml0 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o));
-                        ml1 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o) + 1);
-                    }
-                }
-                mbar_wait(tfull0 + 8 * acc, acc_ph);
-                tcgen05_fence_after();
-                const uint32_t trow = tmem_base + acc * (uint32_t)a.n_tile + ((uint32_t)(q * 32) << 16);
-                if (TCG_DBG(a, 1)) {
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                    continue;
-                }
-                // two 8-column halves in sequence (register budget: 72 per thread at 832 threads)
+            float acc[N / 2];
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    uint32_t f8[8], m8[8];
-                    tmem_ld8(trow + (uint32_t)(co + 8 * hh), f8);
-                    tmem_ld8(trow + (uint32_t)(half + co + 8 * hh), m8);
-                    tmem_ld_wait();
-                    if (hh == 1) {                    // accumulator fully read: hand the TMEM slot back before the math
-                        tcgen05_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                    }
-                    float yv[8];
-                    if (a.elu) {
+            for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+            for (int kb = 0; kb < a.kblocks; ++kb) {
+                mbar_wait(full0 + 8 * s, ph);
+                const uint32_t stage = smem_base + s * stage_bytes;
+                uint32_t fr[G_KBLK / 16][4];
 #pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) yv[jj] = gate_folded<true>(__uint_as_float(f8[jj]), __uint_as_float(m8[jj]), s_par4[co + 8 * hh + jj]);
-                    } else {
+                for (int kk = 0; kk < G_KBLK / 16; ++kk) ldmatrix_x4(stage + swz(lrow * 128u + 32u * kk + khalf, 128u), fr[kk]);
+                wgmma_fence();
+                wgmma_fence_acc(acc);
 #pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) yv[jj] = gate_folded<false>(__uint_as_float(f8[jj]), __uint_as_float(m8[jj]), s_par4[co + 8 * hh + jj]);
-                    }
-                    if (inside) {
-                        const uint4 rs = hh ? rs1 : rs0, ml = hh ? ml1 : ml0;
-                        if (has_res) {
-                            const uint32_t rr[4] = {rs.x, rs.y, rs.z, rs.w};
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                yv[2 * jj] += __uint_as_float(rr[jj] << 16);
-                                yv[2 * jj + 1] += __uint_as_float(rr[jj] & 0xFFFF0000u);
-                            }
-                        }
-                        uint32_t pk[4];
-#pragma unroll
-                        for (int jj = 0; jj < 4; ++jj) pk[jj] = g_cvt2(yv[2 * jj], yv[2 * jj + 1]);
-                        reinterpret_cast<uint4 *>(static_cast<__nv_bfloat16 *>(a.out) + o)[hh] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                        if (has_out2) {
-                            const uint32_t mm[4] = {ml.x, ml.y, ml.z, ml.w};
-                            uint32_t p2[4];
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                const float2 ys = g_unpack2(pk[jj]);
-                                const float2 mv = g_unpack2(mm[jj]);
-                                p2[jj] = g_cvt2(ys.x * mv.x, ys.y * mv.y);
-                            }
-                            reinterpret_cast<uint4 *>(a.out2 + o)[hh] = make_uint4(p2[0], p2[1], p2[2], p2[3]);
-                        }
-                    }
-                }
-                continue;
-            }
-            const int c_first = sub * 8;
-            // first chunk's residual / FAM multiplier: issued before the wait for the MMAs
-            uint4 r0 = make_uint4(0, 0, 0, 0), m0 = make_uint4(0, 0, 0, 0);
-            if (inside && nhwc && c_first < half && nt * half + c_first < a.Cout) {
-                const int o = pix * a.Cout + nt * half + c_first;
-                if (has_res) r0 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o));
-                if (has_out2) m0 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o));
-            }
-            mbar_wait(tfull0 + 8 * acc, acc_ph);
-            tcgen05_fence_after();
-            if (TCG_DBG(a, 1)) {
-                tcgen05_fence_before();
+                for (int kk = 0; kk < G_KBLK / 16; ++kk) Wgmma<N>::mma(acc, fr[kk], wgmma_desc(stage + a.a_bytes + 32u * kk, 128u), 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_acc(acc);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-                continue;
+                if (lane == 0) mbar_arrive(empty0 + 8 * s);
+                if (++s == (uint32_t)a.stages) { s = 0; ph ^= 1u; }
             }
-            const uint32_t trow = tmem_base + acc * (uint32_t)a.n_tile + ((uint32_t)(q * 32) << 16);
-            for (int c0 = c_first; c0 < half; c0 += 8 * (G_EPI_WARPS / 4)) {
-                const int co = nt * half + c0;
-                if (co >= a.Cout) break;             // padded channels (warp-uniform)
-                uint32_t rf[8], rm[8];
-                tmem_ld8(trow + (uint32_t)c0, rf);
-                tmem_ld8(trow + (uint32_t)(half + c0), rm);
-                const int o = pix * a.Cout + co;
-                if (c0 != c_first && inside && nhwc) {
-                    if (has_res) r0 = __ldg(reinterpret_cast<const uint4 *>(a.residual + o));
-                    if (has_out2) m0 = __ldg(reinterpret_cast<const uint4 *>(a.out2_mul + o));
-                }
-                tmem_ld_wait();
-                float yv[8];
-                if (a.elu) {
-#pragma unroll
-                    for (int jj = 0; jj < 8; ++jj) yv[jj] = gate_folded<true>(__uint_as_float(rf[jj]), __uint_as_float(rm[jj]), s_par4[co + jj]);
-                } else {
-#pragma unroll
-                    for (int jj = 0; jj < 8; ++jj) yv[jj] = gate_folded<false>(__uint_as_float(rf[jj]), __uint_as_float(rm[jj]), s_par4[co + jj]);
-                }
-                if (inside) {
-                    if (!nhwc) {
-                        float *op = static_cast<float *>(a.out);
-#pragma unroll
-                        for (int jj = 0; jj < 8; ++jj)
-                            if (co + jj < a.Cout) op[(((long long)b * a.Cout + co + jj) * a.Hout + y) * a.Wout + x] = yv[jj];
-                    } else {
-                        if (has_res) {
-                            const uint32_t rr[4] = {r0.x, r0.y, r0.z, r0.w};
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                yv[2 * jj] += __uint_as_float(rr[jj] << 16);
-                                yv[2 * jj + 1] += __uint_as_float(rr[jj] & 0xFFFF0000u);
-                            }
-                        }
-                        uint32_t pk[4];
-#pragma unroll
-                        for (int jj = 0; jj < 4; ++jj) pk[jj] = g_cvt2(yv[2 * jj], yv[2 * jj + 1]);
-                        *reinterpret_cast<uint4 *>(static_cast<__nv_bfloat16 *>(a.out) + o) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                        if (has_out2) {
-                            const uint32_t mm[4] = {m0.x, m0.y, m0.z, m0.w};
-                            uint32_t p2[4];
-#pragma unroll
-                            for (int jj = 0; jj < 4; ++jj) {
-                                const float2 ys = g_unpack2(pk[jj]);
-                                const float2 mv = g_unpack2(mm[jj]);
-                                p2[jj] = g_cvt2(ys.x * mv.x, ys.y * mv.y);
-                            }
-                            *reinterpret_cast<uint4 *>(a.out2 + o) = make_uint4(p2[0], p2[1], p2[2], p2[3]);
-                        }
-                    }
-                }
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
+            const int y0 = ty * G_TH + 4 * wg + wiw, x0 = tx * G_TW + (lane >> 2);
+            const int xs[2] = {x0, x0 + 8}, ys[2] = {y0, y0};
+            const bool in[2] = {x0 < a.Wout && y0 < a.Hout, x0 + 8 < a.Wout && y0 < a.Hout};
+            epilogue_tile<N>(acc, lane, b, ys, xs, in, nt, e);
         }
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, G_TMEM_COLS);
     }
 }
 
@@ -583,16 +344,16 @@ static bool g_geom(int Cin, int Cout, int k, GGeom *g)
 {
     if (Cin % 8 != 0 || Cout < 1) return false;
     int cp, n_tile, n_tiles;
-    if (Cout <= 128) {
+    if (Cout <= 64) {
         cp = ((Cout + 7) / 8) * 8;
         n_tile = 2 * cp;
         n_tiles = 1;
-    } else {
-        cp = ((Cout + 127) / 128) * 128;
-        n_tile = 256;
-        n_tiles = cp / 128;
+    } else {                                   // accumulators in registers: at most 128 columns (64 fp32 per thread)
+        cp = ((Cout + 63) / 64) * 64;
+        n_tile = 128;
+        n_tiles = cp / 64;
     }
-    if (n_tile % 16 != 0 || n_tile > 256) return false;
+    if (n_tile % 16 != 0 || n_tile > 128) return false;
     if (g) *g = GGeom{cp, n_tile, n_tiles, (k * k * Cin + G_KBLK - 1) / G_KBLK};
     return true;
 }
@@ -626,18 +387,18 @@ int tcg_plan_create(const read_conv_desc &d, TcgPlan **out)
 {
     GGeom g;
     if (!tcg_supported(d) || !g_geom(d.Cin, d.Cout, d.k, &g)) {
-        set_error("tcgen05 gather conv: unsupported layer");
+        set_error("wgmma gather conv: unsupported layer");
         return READ_ERR_UNSUPPORTED;
     }
     PFN_encodeTiled enc = get_encode_tiled();
     if (!enc) {
-        set_error("tcgen05 gather conv: cuTensorMapEncodeTiled not available from the driver");
+        set_error("wgmma gather conv: cuTensorMapEncodeTiled not available from the driver");
         return READ_ERR_CUDA;
     }
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.w_tc) & 127) == 0, "tcgen05 gather conv: packed weights must be 128B aligned");
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "tcgen05 gather conv: output must be 16B aligned");
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.w_tc) & 127) == 0, "wgmma gather conv: packed weights must be 128B aligned");
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "wgmma gather conv: output must be 16B aligned");
     TcgPlan *p = new (std::nothrow) TcgPlan{};
-    RB_CHECK_ARG(p != nullptr, "tcgen05 gather conv: out of host memory");
+    RB_CHECK_ARG(p != nullptr, "wgmma gather conv: out of host memory");
     {
         const cuuint64_t rows = (cuuint64_t)g.kblocks * g.n_tile * g.n_tiles;
         cuuint64_t dims[2] = {(cuuint64_t)G_KBLK, rows};
@@ -648,7 +409,7 @@ int tcg_plan_create(const read_conv_desc &d, TcgPlan **out)
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
-            set_error("tcgen05 gather conv: cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
+            set_error("wgmma gather conv: cuTensorMapEncodeTiled(weights) failed with %d", (int)r);
             delete p;
             return READ_ERR_CUDA;
         }
@@ -674,17 +435,13 @@ int tcg_plan_create(const read_conv_desc &d, TcgPlan **out)
     a.inv_tx = 1.0f / (float)a.tiles_x;
     a.inv_ty = 1.0f / (float)a.tiles_y;
     a.inv_nt = 1.0f / (float)a.n_tiles;
-    a.nacc = G_TMEM_COLS / g.n_tile > G_MAX_ACC ? G_MAX_ACC : G_TMEM_COLS / g.n_tile;
     if ((long long)d.B * d.Hout * d.Wout * d.Cout >= (1ll << 31)) {
-        set_error("tcgen05 gather conv: output too large for 32-bit offsets");
+        set_error("wgmma gather conv: output too large for 32-bit offsets");
         delete p;
         return READ_ERR_UNSUPPORTED;
     }
-    a.debug = 0;
-    a.lean16 = (d.out_mode == READ_OUT_NHWC && g.n_tiles == 1 && g.cout_pad == d.Cout &&
-                (d.Cout == 16 || d.Cout == 32 || d.Cout == 64)) ? 1 : 0;
     if ((long long)a.tiles_x * a.tiles_y * d.B * a.n_tiles >= (1ll << 22)) {
-        set_error("tcgen05 gather conv: too many tiles for the division-free decode");
+        set_error("wgmma gather conv: too many tiles for the division-free decode");
         delete p;
         return READ_ERR_UNSUPPORTED;
     }
@@ -694,28 +451,57 @@ int tcg_plan_create(const read_conv_desc &d, TcgPlan **out)
     if (stages > G_MAX_STAGES) stages = G_MAX_STAGES;
     a.stages = stages;
     if (stages < 3 || (d.stride != 1 && d.stride != 2)) {
-        set_error("tcgen05 gather conv: unsupported geometry (stages %d, stride %d)", stages, d.stride);
+        set_error("wgmma gather conv: unsupported geometry (stages %d, stride %d)", stages, d.stride);
         delete p;
         return READ_ERR_UNSUPPORTED;
     }
-    a.elu = d.elu;
     a.bias_f = d.bias_f; a.bias_m = d.bias_m; a.scale = d.bn_scale; a.shift = d.bn_shift;
-    a.residual = static_cast<const __nv_bfloat16 *>(d.residual);
-    a.out = d.out; a.out_mode = d.out_mode;
-    a.out2 = static_cast<__nv_bfloat16 *>(d.out2);
-    a.out2_mul = static_cast<const __nv_bfloat16 *>(d.out2_mul);
-    p->smem_bytes = 1024 + (size_t)stages * (a.a_bytes + a.b_bytes) + 8 * (2 * G_MAX_STAGES + 2 * G_MAX_ACC + 2) + 16 * (size_t)g.cout_pad + 16 * (size_t)g.kblocks * 8 + sizeof(SrcS) * READ_MAX_SRC + 64;
+    EpiArgs &e = a.epi;
+    e.H = d.Hout; e.W = d.Wout; e.Cout = d.Cout;
+    e.elu = d.elu;
+    e.raw = 0;
+    e.nchw = d.out_mode == READ_OUT_NCHW_F32 ? 1 : 0;
+    e.par = nullptr;
+    e.residual = static_cast<const __nv_bfloat16 *>(d.residual);
+    e.out2_mul = static_cast<const __nv_bfloat16 *>(d.out2_mul);
+    e.addin = nullptr;
+    e.out = d.out;
+    e.out2 = static_cast<__nv_bfloat16 *>(d.out2);
+    e.addin_H = e.addin_W = 0;
+    p->smem_bytes = 1024 + (size_t)stages * (a.a_bytes + a.b_bytes) + 8 * (2 * G_MAX_STAGES) + 16 * (size_t)g.cout_pad + 16 * (size_t)g.kblocks * 8 + sizeof(SrcS) * READ_MAX_SRC + 64;
     *out = p;
     return READ_OK;
 }
 
-int g_tcg_debug = 0;
 extern int g_tc_pdl;
+
+template <int STRIDE, int N>
+static int launch_tcg(const TcgPlan *p, const GArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_gather_kernel<STRIDE, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
+    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_gather_kernel<STRIDE, N>, p->tmB, a));
+    return READ_OK;
+}
+
+template <int STRIDE>
+static int launch_tcg_n(const TcgPlan *p, const GArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    switch (a.n_tile) {
+    case 16: return launch_tcg<STRIDE, 16>(p, a, lcfg);
+    case 32: return launch_tcg<STRIDE, 32>(p, a, lcfg);
+    case 48: return launch_tcg<STRIDE, 48>(p, a, lcfg);
+    case 64: return launch_tcg<STRIDE, 64>(p, a, lcfg);
+    case 80: return launch_tcg<STRIDE, 80>(p, a, lcfg);
+    case 96: return launch_tcg<STRIDE, 96>(p, a, lcfg);
+    case 112: return launch_tcg<STRIDE, 112>(p, a, lcfg);
+    case 128: return launch_tcg<STRIDE, 128>(p, a, lcfg);
+    default: set_error("wgmma gather conv: no kernel instance for n_tile=%d", a.n_tile); return READ_ERR_UNSUPPORTED;
+    }
+}
 
 int tcg_plan_launch(const TcgPlan *p, cudaStream_t st, int max_ctas)
 {
     GArgs a = p->args;
-    a.debug = g_tcg_debug;
     const long long total_tiles = (long long)a.tiles_x * a.tiles_y * a.B * a.n_tiles;
     if (total_tiles == 0) return READ_OK;
     long long grid = num_sms();
@@ -732,13 +518,8 @@ int tcg_plan_launch(const TcgPlan *p, cudaStream_t st, int max_ctas)
     lcfg.stream = st;
     lcfg.attrs = lattr;
     lcfg.numAttrs = a.pdl ? 1 : 0;
-    if (a.stride == 1) {
-        RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_gather_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
-        RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_gather_kernel<1>, p->tmB, a));
-    } else {
-        RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_gather_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
-        RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_gather_kernel<2>, p->tmB, a));
-    }
+    const int rc = a.stride == 1 ? launch_tcg_n<1>(p, a, lcfg) : launch_tcg_n<2>(p, a, lcfg);
+    if (rc != READ_OK) return rc;
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

@@ -1,4 +1,4 @@
-// Descriptor gather / scatter-add for sm_100a.
+// Descriptor gather / scatter-add for sm_90a.
 // Replaces PointTexture.forward and its autograd backward (READ/models/texture.py:42-70):
 //   feat[b,c,y,x] = texture_[0,c,(int64)idx[b,0,y,x]]      (empty pixel carries idx 0 -> point 0)
 // Descriptors are read from a point-major [N,D] shadow so a pixel touches one 32-byte sector.
@@ -146,8 +146,8 @@ template <> __device__ __forceinline__ void write_desc8<float>(float *out, long 
     o[1] = d[1];
 }
 
-int g_gather_variant = 3;     // read_set_option("gather_variant"): 3 = the round-1 kernel (default: 42 us at C3); 0 / 1 / 2 = restructured variants
-                              // (gathers hoisted above the stores; measured 132 - 164 us, profiles/r02_raster.md) kept for A/B only
+int g_gather_variant = 3;     // read_set_option("gather_variant"): 3 = the production kernel (default); 0 / 1 / 2 = restructured variants
+                              // (gathers hoisted above the stores; measured slower, not re-measured on H100) kept for A/B only
 
 struct FusedArgs {
     const float *tex;
@@ -191,9 +191,8 @@ __global__ void __launch_bounds__(256, V == 1 ? 4 : 1) pyramid_resolve_gather_ke
         // level 3: horizontal lane ^ 2, vertical lane ^ 16
         unsigned long long m3 = umin64(m2, shfl_xor64(m2, 2));
         m3 = umin64(m3, shfl_xor64(m3, 16));
-        // ALL descriptor reads of the block are issued before the first store (round-2 ncu: 14.5 warps stalled on long
-        // scoreboard per issue - the level-1..3 gathers used to wait behind the level-0 stores, up to five serial DRAM round
-        // trips per block; now it is two: keys, then descriptors)
+        // ALL descriptor reads of the block are issued before the first store (the level-1..3 gathers would otherwise wait
+        // behind the level-0 stores: up to five serial DRAM round trips per block; this way it is two: keys, then descriptors)
         const bool p1 = (row & 1) == 0, p2 = p1 && (row & 2) == 0 && (lane & 1) == 0, p3 = lane == 0;
         if (V == 0) {           // round-1 order: every gather next to its store
             TO *o0 = static_cast<TO *>(a.out[0]);

@@ -46,7 +46,7 @@ __global__ void gather_backward_sparse_kernel(const float *__restrict__ go, cons
 
 // one thread per point; D <= 16.  D == 8 (the reference's descriptor size) takes a fully unrolled path: the point's 2 + 2 + 8 loads
 // (gradient row, square_avg row, 8 channel-major parameter words) are all in flight before the first use - the generic loop below
-// made 16 dependent DRAM round trips per touched point and ran slower than the DENSE torch optimizer (0.85 vs 0.50 ms at 5M points).
+// made 16 dependent DRAM round trips per touched point and ran slower than the DENSE torch optimizer.
 __global__ void sparse_rmsprop_kernel(float *__restrict__ param_cn, float *__restrict__ shadow_nd, float *__restrict__ grad_nd,
                                       unsigned char *__restrict__ touched, float *__restrict__ square_avg, int *__restrict__ last_step,
                                       long long N, int D, int step, float lr, float alpha, float eps, float weight_decay)

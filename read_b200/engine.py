@@ -21,8 +21,8 @@ class _Layer:
 
 
 class UNetEngine:
-    """Static-shape executor.  ``precision``: 'bf16' (tcgen05 tensor cores where supported) or 'fp32'
-    (CUDA-core parity mode).  ``conv_impl``: 'auto' (tcgen05 everywhere it applies) | 'tma_only' (tcgen05 TMA kernel
+    """Static-shape executor.  ``precision``: 'bf16' (wgmma tensor-core kernels where supported) or 'fp32'
+    (CUDA-core parity mode).  ``conv_impl``: 'auto' (tensor cores everywhere they apply) | 'tma_only' (TMA-fed wgmma kernel
     for the stride-1 layers, CUDA cores for the rest) | 'generic' (CUDA-core kernel everywhere)."""
 
     def __init__(self, state_dict, B, H, W, device, precision="bf16", conv_impl="auto", use_graph=True,
@@ -51,10 +51,9 @@ class UNetEngine:
         # pyramid levels depend only on the net's inputs and are first consumed deep in the encoder, and each of their launches is a few
         # tiles per SM - mostly pipeline fill and drain.  With the option they run on a second stream on SIDE_CTAS SMs while the main
         # chain (the half-resolution SCM block, the first conv) runs on the rest; one event joins them before the first consumer; both
-        # chains are captured into the same CUDA graph.  Measured at C3 (scripts/ab_side.py, ABAB of whole-net graph replays,
-        # identical output): 5.84 ms without, 6.31 / 6.12 / 6.06 ms with 16 / 24 / 32 side SMs - the cross-stream graph edges cost the
-        # programmatic-dependent-launch overlap of ~10 launches and the main chain loses more on its smaller grids than the side
-        # chain hides.  Kept as a documented negative result.
+        # chains are captured into the same CUDA graph.  Off because the cross-stream graph edges cost the programmatic-dependent-
+        # launch overlap of ~10 launches and the main chain loses more on its smaller grids than the side chain hides (the whole-net
+        # graph replay was slower with the option on; not re-measured on H100).  Output is identical either way.
         self.side_chain = os.environ.get("READ_B200_SIDE_CHAIN", "0") == "1" and type(self) is UNetEngine
         self._side_stream = None
         self.graph = None
@@ -137,7 +136,7 @@ class UNetEngine:
 
         kind = "generic"
         if raw or addin is not None:
-            d.impl = L.CONV_TCGEN05          # validation: these only exist on the tcgen05 TMA kernel
+            d.impl = L.CONV_TCGEN05          # validation: these only exist on the TMA-fed kernel
             assert self.bf16 and lib.read_conv_tc_supported(ctypes.byref(d)), prefix
             kind = "tma"
         elif self.bf16 and self.conv_impl != "generic":
@@ -230,7 +229,7 @@ class UNetEngine:
         next finer term; the sources at or above the output resolution are TMA sources (identity / traversal-stride) of
         the final launch.  The reference order cat[res1, res2, res3, z] fixes the weight column ranges."""
         prefix = f"AFFs.{idx}.conv.0"
-        # measured at C3: the split pays for the full-resolution head (0.35 -> 0.25 ms); at half resolution it is a wash
+        # the split pays for the full-resolution head (8x fewer MACs there); at half resolution the saving does not cover the extra launches
         chain_ok = self.bf16 and self.conv_impl == "auto" and c == self.base
         if chain_ok:
             coarse = [(i, t, f) for i, (t, mode, f) in enumerate(srcs) if mode == "up"]
@@ -402,8 +401,8 @@ class UNetEngine:
         return len(self.ops)
 
     def impl_histogram(self):
-        names = {L.CONV_GENERIC: "generic", L.CONV_TCGEN05: "tcgen05", L.CONV_TCGEN05_GATHER: "tcgen05_gather"}
-        h = {"tcgen05": 0, "tcgen05_gather": 0, "generic": 0}
+        names = {L.CONV_GENERIC: "generic", L.CONV_TCGEN05: "wgmma_tma", L.CONV_TCGEN05_GATHER: "wgmma_gather"}
+        h = {"wgmma_tma": 0, "wgmma_gather": 0, "generic": 0}
         for ly in self.layers:
             h[names[ly.impl]] += 1
         return h
@@ -438,7 +437,7 @@ class StripEngine(UNetEngine):
 
     def __init__(self, state_dict, H, W, device, rank, world, group=None, precision="bf16", use_graph=True):
         from . import strips
-        assert precision == "bf16", "the strip engine runs the production (tcgen05) path"
+        assert precision == "bf16", "the strip engine runs the production (tensor-core) path"
         self.rank, self.world, self.group = rank, world, group
         self.H_full = H
         _, H_local, self.h_top, self.h_bot = strips.strip_rows(H, world, rank, 0)

@@ -1,4 +1,4 @@
-"""Drop-in for ``READ.gl.myrender.MyRender`` (src/READ/gl/myrender.py:12-43), B200-native.
+"""Drop-in for ``READ.gl.myrender.MyRender`` (src/READ/gl/myrender.py:12-43), on the H100 kernels.
 
 Differences in HOW (not WHAT): the point clouds are uploaded once in ``update_ds`` and stay resident in HBM
 (the reference re-uploads N*12 bytes per level per call, pcpr_cuda.cpp:29); all L levels and all views of a

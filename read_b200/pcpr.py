@@ -6,7 +6,7 @@
 Same contract: inputs may live on CPU or CUDA (they are moved, pcpr_cuda.cpp:29-30), they must be float and
 contiguous (RuntimeError otherwise, pcpr_cuda.cpp:17-21,32-34), results are CPU float tensors
 ``[index[B,h,w], depth[B,h,w]]`` (point_render.cu:196-199).  ``block_size`` is accepted and ignored (the
-B200 kernel picks its own persistent launch shape).  Output is deterministic: min depth, ties -> lowest id,
+kernel picks its own persistent launch shape).  Output is deterministic: min depth, ties -> lowest id,
 empty -> 0 — the sequential semantics of DepthProject, which the reference kernel only approximates under
 contention (SURVEY.md §8 a3'').
 """

@@ -1,4 +1,4 @@
-"""Drop-in for ``READ.pipelines.ogl.TexturePipeline`` (READ/pipelines/ogl.py:58-154) over the B200 kernels.
+"""Drop-in for ``READ.pipelines.ogl.TexturePipeline`` (READ/pipelines/ogl.py:58-154) over the H100 kernels.
 
 Use ``--pipeline read_b200.pipeline.TexturePipeline`` with the reference's train.py (the plugin is located by dotted path,
 READ/utils/train.py:148-154), or shadow ``READ.pipelines.ogl`` (INTEGRATION.md).  The plugin contract train.py / viewer.py rely

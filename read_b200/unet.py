@@ -6,7 +6,7 @@ reference checkpoint works with ``strict=True``.  The module tree is generated f
 hand-written block classes; it only HOLDS parameters.
 
 Inference (``torch.no_grad()`` + ``.eval()`` on a CUDA device) runs on ``engine.UNetEngine``: 99 fused
-gated-conv kernel launches (tcgen05 tensor cores for the dominant 3x3 layers) replayed as one CUDA graph.
+gated-conv kernel launches (wgmma tensor-core kernels for the dominant 3x3 layers) replayed as one CUDA graph.
 There is no CPU path: inference on a CPU tensor raises.
 
 Training (autograd enabled) is routed through torch's own conv/batch-norm operators on the same parameters —
@@ -162,7 +162,7 @@ class UNet(nn.Module):
         if needs_autograd or self.training or getattr(self, '_is_replica', False):
             return self._forward_torch(inputs)
         if not x.is_cuda:
-            raise RuntimeError("read_b200.UNet: inference needs CUDA tensors on a B200 (no CPU fallback)")
+            raise RuntimeError("read_b200.UNet: inference needs CUDA tensors on an H100 (no CPU fallback)")
         B, _, H, W = x.shape
         eng = self.engine(B, H, W, x.device)
         eng.set_inputs_nchw(inputs[:4])

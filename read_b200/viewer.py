@@ -54,7 +54,7 @@ class FrameRenderer:
         self.model.to(self.device).eval()
         # camera upload: a ring of pinned 4x4 staging buffers.  A pageable ``.to(device)`` blocks the host until the copy has run,
         # and the copy is queued behind the previous frame's kernels - the host could not enqueue frame i+1 while frame i renders
-        # and the GPU idled for the host-side work of every frame (0.3 ms at C3).
+        # and the GPU idled for the host-side work of every frame.
         self._cam_host = [torch.empty((1, 4, 4), dtype=torch.float32).pin_memory() for _ in range(4)]
         self._cam_used = [None] * 4
         self._cam_i = 0

@@ -1,5 +1,5 @@
 """ABAB of an engine-construction environment switch on whole-net CUDA-graph replays (C3 shapes) plus per-layer in-sequence times.
-   python scripts/ab_env.py READ_B200_ALT_ORDER 0 1      |      python scripts/ab_env.py opt:tc_pair 1 2"""
+   python scripts/ab_env.py READ_B200_ALT_ORDER 0 1      |      python scripts/ab_env.py opt:tc_pdl 1 0"""
 import os, sys
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -15,7 +15,7 @@ feats = [torch.rand((1, 8, H >> l, W >> l), generator=g) for l in range(4)]
 
 
 def mk(v):
-    if VAR.startswith("opt:"):               # a read_set_option read at plan creation, e.g. opt:tc_pair
+    if VAR.startswith("opt:"):               # a read_set_option, e.g. opt:tc_pdl
         L.check(L.load().read_set_option(VAR[4:].encode(), int(v)))
     else:
         os.environ[VAR] = v

@@ -1,5 +1,5 @@
-"""Summarise an .ncu-rep (captured with --set full) into a small markdown table for profiles/.
-    python scripts/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r01_xxx.md "title"
+"""Summarise an .ncu-rep (captured with --set full) into a small markdown table.
+    python scripts/ncu_summary.py prof.ncu-rep summary.md "title"
 """
 import csv
 import io

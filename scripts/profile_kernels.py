@@ -1,7 +1,7 @@
 """Launch each hot kernel of the C3 workload exactly once (eagerly, no CUDA graph) so that
-`ncu --set full -k regex:...` captures one instance of each.  Usage on the GPU box:
+`ncu --set full -k regex:...` captures one instance of each.  Usage:
     ncu --set full --clock-control none --import-source on -k regex:"raster_project|gather_kernel|gated_conv" \
-        -o gpurun_out/prof_r1 python scripts/profile_kernels.py
+        -o prof python scripts/profile_kernels.py
 """
 import os
 import sys

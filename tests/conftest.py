@@ -8,11 +8,10 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-HAVE_REFERENCE = os.path.isdir("/root/reference/READ")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -1,12 +1,12 @@
 """Generate the committed golden fixtures by running THE REFERENCE'S OWN Python modules.
 
-Run once in the build container (needs /root/reference; it does not exist on the GPU box):
+Run once where a checkout of the reference exists (READ_REFERENCE_ROOT, default /root/reference); CPU only:
 
     python tests/golden/make_golden.py
 
 For each case: a small seeded scene + cameras -> index maps from the sequential z-buffer oracle (the
 reference's rasterizer is CUDA-only and cannot execute here) -> the reference's PointTexture / NetAndTexture /
-UNet (imported from /root/reference, top-level copies, `imageio` stubbed — SURVEY.md §8c) -> RGB.
+UNet (imported from the reference checkout, top-level copies, `imageio` stubbed — SURVEY.md §8c) -> RGB.
 Weights come from read_b200.synth.synth_state_dict(seed) loaded into the reference UNet with strict=True, so
 the fixture stores only a seed + a checksum instead of 120 MB of parameters.
 """
@@ -19,7 +19,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ.get("READ_REFERENCE_ROOT", "/root/reference"))
 sys.modules.setdefault("imageio", types.ModuleType("imageio"))
 
 from READ.models.unet import UNet as RefUNet                      # noqa: E402

@@ -110,7 +110,7 @@ def _desc_1x1(cout, srcs, out_mode=None, addin=False):
 
 
 def test_tc_supported_predicate_for_concat_raw_and_addin():
-    """Which layers the tcgen05 TMA kernel accepts (host-side predicate only): 1x1 virtual concats of identity /
+    """Which layers the TMA-fed wgmma kernel accepts (host-side predicate only): 1x1 virtual concats of identity /
     nearest-down sources in 32-channel granules, RAW terms and add-ins for Cout 16 / 32 / 64, stride-2 3x3 / 4x4."""
     lib = _lib.load()
     ID, DOWN, UP = _lib.SRC_IDENTITY, _lib.SRC_NEAREST_DOWN, _lib.SRC_NEAREST_UP

@@ -218,7 +218,7 @@ def test_tcgen05_matches_torch(case):
     kw = dict(kw)
     r = run_conv(srcs, cout, k, kw.pop("stride", 1), elu, True, TC, **kw)
     got, want = r[0], r[1]
-    assert torch.isfinite(got).all(), "tcgen05 kernel left outputs unwritten (NaN sentinel)"
+    assert torch.isfinite(got).all(), "TMA kernel left outputs unwritten (NaN sentinel)"
     # bf16 operands are exact in the reference (weights/inputs pre-rounded), accumulation fp32 on both sides:
     # error = output bf16 rounding + approx ex2/tanh (~1e-3 abs)
     tol = 2 ** -8 * float(want.abs().max()) + 4e-3
@@ -235,7 +235,7 @@ GATHER_CASES = [c for c in GENERIC_CASES if not c[6].get("mul")] + [
     ("3x3 s2 128->256", [(128, 16, 16, "id", 1)], 256, 3, 2, True, {"out2": True}),
     ("4x4 s2 256->128", [(256, 16, 16, "id", 1)], 128, 4, 2, True, {}),
     ("many tiles (phases wrap), s2", [(32, 256, 320, "id", 1)], 64, 3, 2, True, {}),
-    # persistence: 17+ tiles per CTA so every ring (stages, TMEM accumulators, epilogue dealing) wraps several times
+    # persistence: 17+ tiles per CTA so every ring (A stages, streamed weight stages, barrier phases) wraps several times
     ("persistent 1x1 32->32 + residual, 2560 tiles", [(32, 512, 640, "id", 1)], 32, 1, 1, True, {"residual": True}),
     ("persistent 3x3 8->32, 2 k-blocks per tile, 2560 tiles", [(8, 512, 640, "id", 1)], 32, 3, 1, True, {}),
     ("persistent concat 32+32 -> 64 1x1, 2560 tiles", [(32, 512, 640, "id", 1), (32, 256, 320, "up", 2)], 64, 1, 1, False, {}),
@@ -300,7 +300,7 @@ def _pack_tc(lib, dsc, wf, wm, d):
 
 
 def _run_1x1(srcs_nchw, modes, cout, elu, raw, addin_nchw, seed):
-    """1x1 gated conv on the tcgen05 TMA kernel with RAW output and/or an add-in; returns (got NCHW, want NCHW)."""
+    """1x1 gated conv on the TMA-fed wgmma kernel with RAW output and/or an add-in; returns (got NCHW, want NCHW)."""
     lib, d = L.load(), dev()
     g = torch.Generator().manual_seed(seed)
     xs = [x.to(torch.bfloat16).float() for x in srcs_nchw]
@@ -378,7 +378,7 @@ def test_tcgen05_addin_gated_matches_torch(cout):
     assert float((got - want).abs().max()) < tol
 
 
-# ---------------------------------------------------------------- CTA-pair kernel (conv_tc2.cu: tcgen05.mma.cta_group::2)
+# ---------------------------------------------------------------- TMA kernel: small-channel, wide and persistent shapes
 PAIR_CASES = [
     ("C32 16x32 exact tiles (2 pairs)", [(32, 16, 32, "id", 1)], 32, 3, True, {}),
     ("C32 ragged 19x23, odd tile count", [(32, 19, 23, "id", 1)], 32, 3, False, {"residual": True}),
@@ -389,7 +389,7 @@ PAIR_CASES = [
     ("C64 -> 32 channels, no activation", [(64, 20, 24, "id", 1)], 32, 3, False, {}),
     ("persistent C32, 2560 tiles (17 pairs per cluster: rings wrap)", [(32, 512, 640, "id", 1)], 32, 3, True, {"residual": True}),
     ("persistent C64 + residual, 1280 tiles", [(64, 256, 640, "id", 1)], 64, 3, False, {"residual": True}),
-    # streamed-weight variant (conv_tc2.cu gated_conv_tc2s_kernel): K chunks of 64 channels, 256-column n tiles
+    # streamed weights: K chunks of 64 channels, several n tiles
     ("wide C128 24x40 (2 K chunks)", [(128, 24, 40, "id", 1)], 128, 3, True, {}),
     ("wide C128 ragged, odd tile count + residual", [(128, 19, 23, "id", 1)], 128, 3, False, {"residual": True}),
     ("wide C256 (4 K chunks, 2 n tiles)", [(256, 17, 24, "id", 1)], 256, 3, True, {}),
@@ -403,24 +403,17 @@ PAIR_CASES = [
 
 @pytest.mark.parametrize("case", PAIR_CASES, ids=[c[0] for c in PAIR_CASES])
 def test_tcgen05_cta_pair_matches_torch_and_the_single_cta_kernel(case):
-    """cta_group::2 variant: same tolerance as the single-CTA kernel against torch; the resident-weight kernel is bit-identical to
-    it (same K order), the streamed-weight one accumulates the taps in a different order (within one bf16 ulp of it)."""
-    lib = L.load()
+    """The shapes the CTA-pair kernels of the Blackwell build served (ragged tiles, tiles spanning images, resident and streamed
+    weights, several n tiles, persistent grids whose rings wrap many times) now run on the TMA kernel: same tolerance against torch
+    as the other TMA-kernel cases, and within one bf16 ulp of the gather kernel on the same inputs (the two kernels accumulate
+    the K dimension in different orders)."""
     _, srcs, cout, k, elu, kw = case
-    try:
-        L.check(lib.read_set_option(b"tc_pair", 2))                      # every eligible layer, C=32 included
-        got, want = run_conv(srcs, cout, k, 1, elu, True, TC, **kw)[:2]
-        L.check(lib.read_set_option(b"tc_pair", 0))
-        base = run_conv(srcs, cout, k, 1, elu, True, TC, **kw)[0]
-    finally:
-        L.check(lib.read_set_option(b"tc_pair", 1))
-    assert torch.isfinite(got).all(), "pair kernel left outputs unwritten (NaN sentinel)"
+    got, want = run_conv(srcs, cout, k, 1, elu, True, TC, **kw)[:2]
+    other = run_conv(srcs, cout, k, 1, elu, True, GATHER, **kw)[0]
+    assert torch.isfinite(got).all(), "kernel left outputs unwritten (NaN sentinel)"
     tol = 2 ** -8 * float(want.abs().max()) + 4e-3
     assert float((got - want).abs().max()) < tol
-    if case[0].startswith(("wide", "persistent wide")):
-        assert float((got - base).abs().max()) <= 2 ** -7 * float(want.abs().max())
-    else:
-        assert torch.equal(got, base)
+    assert float((got - other).abs().max()) <= 2 ** -7 * float(want.abs().max())
 
 
 ORDER_CASES = [c for c in TC_CASES if not c[0].startswith("persistent C")][:24] + PAIR_CASES
@@ -429,18 +422,12 @@ ORDER_CASES = [c for c in TC_CASES if not c[0].startswith("persistent C")][:24] 
 @pytest.mark.parametrize("case", ORDER_CASES, ids=[f"{i}: {c[0]}" for i, c in enumerate(ORDER_CASES)])
 def test_reversed_tile_order_is_bit_identical(case):
     """read_conv_plan_set_tile_order(plan, 1) walks the tiles bottom-up (the engine alternates the direction between consecutive
-    layers for L2 reuse): same output bit for bit on every TMA kernel - single-CTA, CTA pair (odd tile counts: the phantom tile moves to
-    the other end) and streamed-weight pair."""
-    lib = L.load()
+    layers for L2 reuse): same output bit for bit on the TMA kernel, resident and streamed weights alike."""
     _, srcs, cout, k, elu, kw = case
     kw = dict(kw)
     stride = kw.pop("stride", 1)
-    try:
-        L.check(lib.read_set_option(b"tc_pair", 2))                      # pair kernels wherever they apply
-        fwd = run_conv(srcs, cout, k, stride, elu, True, TC, **kw)
-        rev = run_conv(srcs, cout, k, stride, elu, True, TC, reversed_order=True, **kw)
-    finally:
-        L.check(lib.read_set_option(b"tc_pair", 1))
+    fwd = run_conv(srcs, cout, k, stride, elu, True, TC, **kw)
+    rev = run_conv(srcs, cout, k, stride, elu, True, TC, reversed_order=True, **kw)
     assert torch.isfinite(rev[0]).all(), "outputs left unwritten (NaN sentinel)"
     assert torch.equal(fwd[0], rev[0])
     if kw.get("out2"):

@@ -115,7 +115,7 @@ def test_c3_window_1024x512_net_vs_oracle(oracle_mod, synth_sd, c3_scene):
 
 
 def test_c3_full_frame_bf16_vs_fp32_engine(synth_sd):
-    """The headline frame itself (1920x1088, B = 1): tcgen05 bf16 engine (CUDA graph) vs the fp32 CUDA-core engine on the same
+    """The headline frame itself (1920x1088, B = 1): wgmma bf16 engine (CUDA graph) vs the fp32 CUDA-core engine on the same
     feature pyramid.  The fp32 engine is pinned to the oracle / the reference fixtures at small sizes and on the C2 / C3-window
     cases above; here it carries that pin to the full frame (every persistent CTA walks 110 full-resolution tiles)."""
     W, H = 1920, 1088

@@ -1,30 +1,28 @@
-"""-m gpu: the UNMODIFIED reference CUDA extension (oracle/_ref/pcpr*.so, compiled from the reference's own
-sources by oracle/build_ref.py) against the oracle and against our kernel (SURVEY.md §8c(3)).
+"""-m gpu: the UNMODIFIED reference CUDA rasterizer (pcpr.forward, compiled from the reference's own sources by
+oracle/build_ref.py) against the oracle and against our kernel (SURVEY.md §8c(3)), through its outputs on the two scenes below
+as recorded by tests/golden/make_ref_pcpr_golden.py.
 
 The reference kernel is nondeterministic under pixel contention (its lock drops contended writes), so:
   * on a collision-free scene (at most one point per pixel) all three must agree exactly;
   * on a dense scene the reference may only be WORSE than the true z-buffer: ref_depth >= oracle_depth wherever
     both are non-empty, and it never invents coverage.
 """
+import os
+
 import numpy as np
 import pytest
-import torch
 
+from conftest import GOLDEN
 from gpu_util import render_gpu, scene_and_cams
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def ref_pcpr():
-    from oracle import build_ref
-    m = build_ref.load()
-    if m is None:
-        pytest.skip("oracle/_ref/pcpr*.so not built (only possible where /root/reference exists)")
-    return m
+def _ref(name):
+    return np.load(os.path.join(GOLDEN, name + ".npz"))
 
 
-def test_collision_free_scene_all_three_agree(oracle_mod, ref_pcpr):
+def test_collision_free_scene_all_three_agree(oracle_mod):
     W, H = 64, 48
     ys, xs = np.mgrid[0:H, 0:W]
     # one point per pixel centre (identity matrix: u = W(x+1)/2), random depths, shuffled ids
@@ -36,24 +34,23 @@ def test_collision_free_scene_all_three_agree(oracle_mod, ref_pcpr):
     xyz = np.concatenate([np.full((1, 3), 9, np.float32), xyz])       # id 0 off-screen ("0 denotes empty")
     M = np.eye(4, dtype=np.float32)[None]
     oi, od = oracle_mod.pcpr_forward(xyz, M, W, H)
-    ri, rd = ref_pcpr.forward(torch.from_numpy(xyz), torch.from_numpy(M), W, H, 512)
+    g = _ref("ref_pcpr_collision_free")
+    ri, rd = g["index"], g["depth"]
     gi, gd, _ = render_gpu(xyz, M, W, H, 1)
     assert (oi != 0).all()
-    np.testing.assert_array_equal(ri.numpy(), oi)
-    np.testing.assert_array_equal(rd.numpy(), od)
+    np.testing.assert_array_equal(ri, oi)
+    np.testing.assert_array_equal(rd, od)
     np.testing.assert_array_equal(gi[0], oi)
     np.testing.assert_array_equal(gd[0], od)
 
 
-def test_dense_scene_reference_is_never_better_than_the_zbuffer(oracle_mod, ref_pcpr):
+def test_dense_scene_reference_is_never_better_than_the_zbuffer(oracle_mod):
     xyz, M = scene_and_cams(300_000, 128, 96, [0], depth=60.0)
     oi, od = oracle_mod.pcpr_forward(xyz, M, 128, 96)
-    ri, rd = ref_pcpr.forward(torch.from_numpy(xyz), torch.from_numpy(M), 128, 96, 512)
-    ri, rd = ri.numpy(), rd.numpy()
+    rd = _ref("ref_pcpr_dense")["depth"]
     assert ((rd == 0) >= (od == 0)).all()                  # reference covers no pixel the z-buffer leaves empty
     both = (rd != 0) & (od != 0)
     assert (rd[both] >= od[both]).all()
-    frac_equal = float((ri == oi).mean())
-    print(f"reference kernel agrees with the sequential z-buffer on {100 * frac_equal:.2f}% of pixels")
+    print(f"reference depth equals the sequential z-buffer on {100 * float((rd == od).mean()):.2f}% of pixels")
     gi, gd, _ = render_gpu(xyz, M, 128, 96, 1)
     np.testing.assert_array_equal(gi[0], oi)               # ours is exact

@@ -51,11 +51,11 @@ def test_engine_bf16_within_stated_tolerance(synth_sd, name, conv_impl):
     out, eng = _engine_out(synth_sd, _golden_feats(g), "bf16", conv_impl)
     hist = eng.impl_histogram()
     if conv_impl == "auto":
-        assert hist["tcgen05"] >= 70 and hist["generic"] == 0, hist   # every layer on tensor cores
+        assert hist["wgmma_tma"] >= 70 and hist["generic"] == 0, hist   # every layer on tensor cores
     elif conv_impl == "tma_only":
-        assert hist["tcgen05"] >= 70 and hist["tcgen05_gather"] == 0, hist
+        assert hist["wgmma_tma"] >= 70 and hist["wgmma_gather"] == 0, hist
     else:
-        assert hist["tcgen05"] == 0 and hist["tcgen05_gather"] == 0
+        assert hist["wgmma_tma"] == 0 and hist["wgmma_gather"] == 0
     want = torch.from_numpy(g["out"])
     err = float((out - want).abs().max())
     assert err < TOL_BF16, err

@@ -1,5 +1,5 @@
 """Oracle vs the committed golden fixtures (generated from the reference's own Python modules by
-tests/golden/make_golden.py).  CPU only; travels to the GPU box."""
+tests/golden/make_golden.py).  CPU only."""
 import numpy as np
 import pytest
 import torch

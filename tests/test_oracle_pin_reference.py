@@ -1,82 +1,67 @@
-"""Pin the oracle's torch restatement to the reference's real modules (only where /root/reference exists,
-i.e. in the build container; skipped on the GPU box)."""
-import sys
-import types
+"""Pin the oracle's torch restatement and our UNet to the reference's real modules, through their outputs recorded by
+tests/golden/make_ref_modules_golden.py (the reference's UNet / PointTexture run on the same seeded inputs and weights)."""
+import os
 
 import numpy as np
-import pytest
 import torch
 
-from conftest import HAVE_REFERENCE
-from read_b200 import synth
-
-pytestmark = pytest.mark.skipif(not HAVE_REFERENCE, reason="/root/reference not present")
+from conftest import GOLDEN
 
 
-def _ref():
-    if "/root/reference" not in sys.path:
-        sys.path.insert(0, "/root/reference")
-    sys.modules.setdefault("imageio", types.ModuleType("imageio"))
-    from READ.models.unet import UNet
-    from READ.models.texture import PointTexture
-    from READ.models.compose import NetAndTexture
-    return UNet, PointTexture, NetAndTexture
+def _golden():
+    return np.load(os.path.join(GOLDEN, "ref_modules.npz"))
+
+
+def _ref_layout():
+    """{state_dict key: (shape, dtype name)} of the reference UNet."""
+    g = _golden()
+    return {str(k): (tuple(int(d) for d in s if d >= 0), str(t)) for k, s, t in zip(g["sd_keys"], g["sd_shapes"], g["sd_dtypes"])}
 
 
 def test_state_dict_keys_identical_to_reference(synth_sd):
-    UNet, _, _ = _ref()
-    ref_sd = UNet().state_dict()
-    assert set(ref_sd) == set(synth_sd)
-    for k, v in ref_sd.items():
-        assert tuple(v.shape) == tuple(synth_sd[k].shape), k
+    ref = _ref_layout()
+    assert set(ref) == set(synth_sd)
+    for k, (shape, _) in ref.items():
+        assert tuple(shape) == tuple(synth_sd[k].shape), k
     from read_b200.unet import UNet as OurUNet
     ours = OurUNet().state_dict()
-    assert list(sorted(ours)) == list(sorted(ref_sd))
-    for k, v in ref_sd.items():
-        assert tuple(v.shape) == tuple(ours[k].shape) and v.dtype == ours[k].dtype, k
-    OurUNet().load_state_dict(ref_sd, strict=True)
+    assert list(sorted(ours)) == list(sorted(ref))
+    for k, (shape, dtype) in ref.items():
+        assert tuple(shape) == tuple(ours[k].shape) and dtype == str(ours[k].dtype), k
+    OurUNet().load_state_dict({k: torch.zeros(shape, dtype=getattr(torch, dt.split(".")[1])) for k, (shape, dt) in ref.items()},
+                              strict=True)
 
 
 def test_unet_oracle_equals_reference_module(synth_sd):
     from oracle import unet_ref
-    UNet, _, _ = _ref()
-    net = UNet()
-    net.load_state_dict(synth_sd, strict=True)
-    net.eval()
     g = torch.Generator().manual_seed(7)
     H, W = 32, 48
     xs = [torch.rand((2, 8, H >> l, W >> l), generator=g) for l in range(5)]
+    want = torch.from_numpy(_golden()["unet_out"])
     with torch.no_grad():
-        want = net(*xs)
         got = unet_ref.unet_forward(synth_sd, xs)
     assert float((want - got).abs().max()) < 2e-5
 
 
 def test_gather_oracle_equals_reference_module():
     from oracle import unet_ref
-    _, PointTexture, _ = _ref()
+    gd = _golden()
     g = torch.Generator().manual_seed(3)
-    tex = PointTexture(8, 500, init_method='rand')
     ids = torch.randint(0, 500, (3, 1, 9, 7), generator=g).float()
-    with torch.no_grad():
-        want = tex(ids)
-    got = unet_ref.point_texture(tex.texture_.detach(), ids)
-    assert torch.equal(want, got)
+    got = unet_ref.point_texture(torch.from_numpy(gd["texture"]), ids)
+    assert torch.equal(torch.from_numpy(gd["gathered"]), got)
 
 
 def test_training_forward_of_our_unet_equals_reference(synth_sd):
     """The library (autograd) path of read_b200.unet.UNet must agree with the reference on CPU."""
-    UNet, _, _ = _ref()
     from read_b200.unet import UNet as OurUNet
-    ref, ours = UNet(), OurUNet()
-    ref.load_state_dict(synth_sd)
+    ours = OurUNet()
     ours.load_state_dict(synth_sd)
-    ref.eval()
     ours.eval()
     g = torch.Generator().manual_seed(11)
     xs = [torch.rand((1, 8, 32 >> l, 32 >> l), generator=g) for l in range(4)]
-    want = ref(*xs)
+    want = torch.from_numpy(_golden()["train_out"])
     got = ours(*xs)                      # grad enabled -> torch path
-    assert float((want - got).abs().max()) < 2e-5
+    assert float((want - got.detach()).abs().max()) < 2e-5
     got.sum().backward()
     assert ours.get_submodule("feat_extract.0").block["conv_f"].weight.grad is not None

@@ -1,7 +1,7 @@
-"""The built library really contains the Blackwell instructions DESIGN.md claims (checked on the SASS of libread_b200.so, no GPU needed):
-tcgen05.mma (UTCHMMA, and its cta_group::2 form in the CTA-pair kernels), TMEM loads (LDTM), TMA tile loads / stores (UTMALDG / UTMASTG),
-the multicast commit of the pair kernels (UTCBAR.2CTA.MULTICAST) and the bulk copy of the streaming rasterizer (UBLKCP); and that the
-work-skipping diagnostic knobs are absent from the shipped build.  Mnemonics as listed in /opt/skills/guides/B200_PROFILING.md."""
+"""The built library really contains the Hopper instructions DESIGN.md claims (checked on the SASS of libread_b200.so, no GPU needed):
+warpgroup MMAs (HGMMA) fed by ldmatrix (LDSM), TMA tile loads (UTMALDG), the cp.async-gathered A operand of the gather kernel
+(LDGSTS) and the bulk copy of the streaming rasterizer (UBLKCP); and that the work-skipping diagnostic knobs are absent from the
+shipped build."""
 import collections
 import os
 import re
@@ -44,28 +44,15 @@ def _has(counter, prefix):
     return sum(n for op, n in counter.items() if op.startswith(prefix))
 
 
-def test_single_cta_conv_kernels_use_tcgen05_tmem_and_tma(sass):
+def test_conv_kernels_use_wgmma_and_tma(sass):
     for name, ops in _kernels(sass, "gated_conv_tc_kernel").items():
-        assert _has(ops, "UTCHMMA") > 0 and _has(ops, "LDTM") > 0 and _has(ops, "UTMALDG") > 0, name
-        assert _has(ops, "UTCHMMA.2CTA") == 0, name
-    lean = {k: v for k, v in _kernels(sass, "gated_conv_tc_kernel").items() if "ELi640E" in k}
-    assert lean and all(_has(v, "UTMASTG") > 0 for v in lean.values()), "lean epilogues stage their items for TMA stores"
-
-
-def test_cta_pair_kernels_use_cta_group_2(sass):
-    for needle in ("gated_conv_tc2_kernel", "gated_conv_tc2s_kernel"):
-        for name, ops in _kernels(sass, needle).items():
-            assert _has(ops, "UTCHMMA.2CTA") > 0, name                       # tcgen05.mma.cta_group::2
-            assert _has(ops, "UTCHMMA") == _has(ops, "UTCHMMA.2CTA"), name    # ... and nothing else
-            assert _has(ops, "UTMALDG.4D.2CTA") > 0 and _has(ops, "UTMALDG.2D.2CTA") > 0, name
-            assert _has(ops, "UTCBAR.2CTA.MULTICAST") > 0, name               # one commit releases both CTAs
-            assert _has(ops, "LDTM") > 0, name
-    assert all(_has(v, "UTMASTG") > 0 for v in _kernels(sass, "gated_conv_tc2_kernel").values())
+        assert _has(ops, "HGMMA") > 0 and _has(ops, "LDSM") > 0 and _has(ops, "UTMALDG") > 0, name
+        assert _has(ops, "SYNCS") > 0, name                                  # mbarrier rings between producer and consumers
 
 
 def test_gather_kernel_and_rasterizer(sass):
     for name, ops in _kernels(sass, "gated_conv_tc_gather_kernel").items():
-        assert _has(ops, "UTCHMMA") > 0 and _has(ops, "LDTM") > 0 and _has(ops, "LDGSTS") > 0, name     # cp.async-gathered A operand
+        assert _has(ops, "HGMMA") > 0 and _has(ops, "LDSM") > 0 and _has(ops, "LDGSTS") > 0, name     # cp.async-gathered A operand
     for name, ops in _kernels(sass, "raster_stream_kernel").items():
         assert _has(ops, "UBLKCP") > 0 and _has(ops, "SYNCS") > 0, name        # cp.async.bulk ring + mbarriers
         assert _has(ops, "RED") + _has(ops, "ATOM") > 0, name                 # 64-bit min into the packed z-buffer
