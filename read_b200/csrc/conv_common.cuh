@@ -34,7 +34,8 @@ __device__ __forceinline__ float gate_fast(float f, float m, float scale, float 
 // least 0.5/d away from an integer, far more than the fp32 rounding error.
 __device__ __forceinline__ int fdiv_small(int x, float inv_d) { return (int)(((float)x + 0.5f) * inv_d); }
 
-// Epilogue of the wgmma kernels, straight from the accumulator registers.  Accumulator layout of wgmma m64nN (fp32): register
+// Epilogue parameters of the wgmma kernels and the register epilogue of the gather kernel and of the TMA kernel's final NCHW
+// layer (the TMA kernel's NHWC layers go through shared memory, conv_tc.cu: epilogue_smem).  Accumulator layout of wgmma m64nN (fp32): register
 // 4*j + 2*i + c of lane l holds row (l >> 2) + 8*i of the warp's 16 rows, column 8*j + 2*(l & 3) + c.  Columns [0, N/2) are
 // conv_f, [N/2, N) conv_m of the same output channels; a thread therefore owns both gates of two adjacent channels.
 struct EpiArgs {
@@ -57,9 +58,9 @@ __device__ __forceinline__ float2 bf16x2_val(uint32_t u) { return make_float2(__
 template <int N>
 constexpr int e_nj() { return N / 16; }   // 8-column groups per gate
 
-// Both rows of the thread: pixels (b, y[i], x[i]), output channels nt * N/2 + ...  Every global load of the epilogue (residual,
-// FAM multiplier, add-in) is issued before the first store: the stores may alias them as far as the compiler knows, so loads
-// interleaved with stores would each pay a full memory latency.
+// Both rows of the thread: pixels (b, y[i], x[i]), output channels nt * N/2 + ...  (no RAW output, no add-in: those layers run
+// on the TMA kernel).  Every global load of a column chunk (residual, FAM multiplier) is issued before its first store: the
+// stores may alias them as far as the compiler knows, so loads interleaved with stores would each pay a full memory latency.
 template <int N>
 __device__ __forceinline__ void epilogue_tile(const float (&d)[N / 2], int lane, int b, const int (&y)[2], const int (&x)[2],
                                               const bool (&inside)[2], int nt, const EpiArgs &e)
@@ -68,40 +69,12 @@ __device__ __forceinline__ void epilogue_tile(const float (&d)[N / 2], int lane,
     constexpr int NJ = e_nj<N>();
     const int q2 = 2 * (lane & 3);
     long long pix[2];
-    const __nv_bfloat16 *ap[2];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        pix[i] = ((long long)b * e.H + y[i]) * e.W + x[i];
-        ap[i] = (e.addin && inside[i]) ? e.addin + (((long long)b * e.addin_H + (y[i] >> 1)) * e.addin_W + (x[i] >> 1)) * N : nullptr;
-    }
-    if (e.raw) {
-#pragma unroll
-        for (int j0 = 0; j0 < N / 8; j0 += 4) {
-            uint32_t av[2][4];
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj)
-                    av[i][jj] = (ap[i] && j0 + jj < N / 8) ? *reinterpret_cast<const uint32_t *>(ap[i] + 8 * (j0 + jj) + q2) : 0u;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                if (!inside[i]) continue;
-                __nv_bfloat16 *op = static_cast<__nv_bfloat16 *>(e.out) + pix[i] * N;
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) {
-                    const int j = j0 + jj;
-                    if (j >= N / 8) break;
-                    const float2 a2 = bf16x2_val(av[i][jj]);
-                    *reinterpret_cast<uint32_t *>(op + 8 * j + q2) = bf16x2_bits(d[4 * j + 2 * i] + a2.x, d[4 * j + 2 * i + 1] + a2.y);
-                }
-            }
-        }
-        return;
-    }
+    for (int i = 0; i < 2; ++i) pix[i] = ((long long)b * e.H + y[i]) * e.W + x[i];
 #pragma unroll
     for (int j0 = 0; j0 < NJ; j0 += (N <= 64 ? 1 : 4)) {
-        constexpr int JC = N <= 64 ? 1 : 4;    // the N <= 64 kernels run two CTAs per SM (96 registers): one column group per chunk
-        uint32_t rv[2][JC], mv[2][JC], af[2][JC], am[2][JC];
+        constexpr int JC = N <= 64 ? 1 : 4;    // the N <= 64 instances run two CTAs per SM (register bound): one column group per chunk
+        uint32_t rv[2][JC], mv[2][JC];
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -112,8 +85,6 @@ __device__ __forceinline__ void epilogue_tile(const float (&d)[N / 2], int lane,
                 const long long o = pix[i] * e.Cout + co;
                 rv[i][jj] = (ok && e.residual) ? __ldg(reinterpret_cast<const unsigned int *>(e.residual + o)) : 0u;
                 mv[i][jj] = (ok && e.out2) ? __ldg(reinterpret_cast<const unsigned int *>(e.out2_mul + o)) : 0u;
-                af[i][jj] = (ap[i] && j0 + jj < NJ) ? *reinterpret_cast<const uint32_t *>(ap[i] + col) : 0u;
-                am[i][jj] = (ap[i] && j0 + jj < NJ) ? *reinterpret_cast<const uint32_t *>(ap[i] + HALF + col) : 0u;
             }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -125,9 +96,8 @@ __device__ __forceinline__ void epilogue_tile(const float (&d)[N / 2], int lane,
                 const int col = 8 * j + q2;
                 const int co = nt * HALF + col;
                 if (co >= e.Cout) continue;
-                const float2 fa = bf16x2_val(af[i][jj]), ma = bf16x2_val(am[i][jj]);
-                const float f0 = d[4 * j + 2 * i] + fa.x, f1 = d[4 * j + 2 * i + 1] + fa.y;
-                const float m0 = d[4 * (j + NJ) + 2 * i] + ma.x, m1 = d[4 * (j + NJ) + 2 * i + 1] + ma.y;
+                const float f0 = d[4 * j + 2 * i], f1 = d[4 * j + 2 * i + 1];
+                const float m0 = d[4 * (j + NJ) + 2 * i], m1 = d[4 * (j + NJ) + 2 * i + 1];
                 const float4 p0 = e.par[co], p1 = e.par[co + 1];
                 float y0, y1;
                 if (e.elu) {

@@ -15,12 +15,15 @@
 //               When the whole layer fits (<= 144 KB: the C=32 and C=64 layers) the weights are loaded ONCE per CTA and stay
 //               resident in shared memory; otherwise they stream through their own mbarrier ring.
 //   D           fp32 in registers: two consumer warpgroups, each owning 64 pixels (8 rows) of the tile.
-//   epilogue    bias, ELU, sigmoid gate, BN affine, residual add, bf16 pack -> global, straight from the accumulators
-//               (optionally a second output y*z for the following FAM, unet.py:115).
+//   epilogue    bias, ELU, sigmoid gate, BN affine, residual add, bf16 pack (optionally a second output y*z for the following
+//               FAM, unet.py:115) through an epilogue stage in shared memory: the producer TMA-loads the tile's residual / FAM
+//               multiplier / add-in into the stage, each consumer warpgroup overwrites them in place with its 64 output pixels
+//               and TMA-stores the result (clipped at the image edge).  Only the final NCHW fp32 layer stores from registers.
 //
 // Warp roles (288 threads, persistent over tiles): warps 0..7 = two consumer warpgroups (wgmma + epilogue), warp 8 = TMA
-// producer, which runs ahead through the A (and streamed B) rings while the consumers compute.  Layers with N <= 64 whose
-// weights and four A stages fit half the shared-memory budget run two CTAs per SM: one CTA's epilogue overlaps the other's MMAs.
+// producer, which runs ahead through the A (and streamed B) rings and the epilogue ring while the consumers compute.  Layers
+// with N <= 64 whose weights, three A stages and two epilogue stages fit half the shared-memory budget run two CTAs per SM:
+// one CTA's epilogue overlaps the other's MMAs.
 //
 // Stride 2 (3x3 / 4x4, pad 1): input column 2x + kx - 1 is an EVEN column for kx odd and an ODD one for kx even, so a stage
 // holds four phase tiles E/O x E/O, each loaded by one TMA with traversal stride 2 in x and y (tile[j][i] = in(sx + 2i, sy + 2j),
@@ -38,18 +41,24 @@ constexpr int TC_TW = 8, TC_TH = 16;          // 128-pixel M tile: 16 rows of 8 
 constexpr int TC_THREADS = 288;               // two consumer warpgroups + one producer warp
 constexpr int TC_PRODUCER_WARP = 8;
 constexpr int TC_MAX_STAGES = 16;
-constexpr uint32_t TC_SMEM_BUDGET = 200 * 1024;
-constexpr uint32_t TC_SMEM_BUDGET_SMALL_N = 100 * 1024;   // N <= 64: two CTAs per SM
+// H100 shared memory: at most 227 KB per CTA, 228 KB per SM of which the hardware reserves 1 KB per resident CTA
+constexpr uint32_t TC_SMEM_PER_CTA = 227 * 1024, TC_SMEM_PER_SM = 228 * 1024;
 __host__ __device__ constexpr int tc_ctas_per_sm(int n_tile) { return n_tile <= 64 ? 2 : 1; }
 constexpr uint32_t TC_RESIDENT_MAX = 144 * 1024;
 // barrier slots (uint64 each)
-constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_BRES = 64, BAR_PARAMS = 66;
+constexpr int TC_E_STAGES = 2;                 // epilogue stages
+constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_BRES = 64, BAR_EFULL = 66,
+              BAR_EEMPTY = BAR_EFULL + TC_E_STAGES, BAR_PARAMS = BAR_EEMPTY + TC_E_STAGES;
 constexpr uint32_t TC_CONSUMER_WARPS = 8;
 
 // activation tensor maps: one per source of a virtual concat (1x1 convs: torch.cat along channels, unet.py:88,105,263;
 // a nearest-DOWN resampled source is a traversal-stride load of the full-resolution tensor)
+// The epilogue's maps (NHWC outputs only): residual and out2_mul are loaded as the tile's 16 rows x 8 pixels, the add-in as the
+// nearest-x2 source region of 8 rows x 4 pixels; out and out2 are stored per warpgroup, 8 rows x 8 pixels.  Channels come in
+// blocks of at most 64 (128-byte rows, the widest swizzle).
 struct TcMaps {
     CUtensorMap a[READ_MAX_SRC];
+    CUtensorMap res, mul, add, out, out2;
 };
 
 struct TcArgs {
@@ -70,6 +79,8 @@ struct TcArgs {
     int pdl;                               // launched with programmatic stream serialization (griddepcontrol in the kernel)
     int ctas_per_sm;                       // 2: the layer fits half the shared-memory budget and its kernel instance two CTAs' registers
     int rev_total;                         // 0, or the number of work units: unit t is mapped to rev_total - 1 - t (read_conv_plan_set_tile_order)
+    uint32_t e_bytes, e_region_off;        // one epilogue stage (out | out2 | add-in regions), byte offset of the epilogue ring
+    uint32_t e_out2_off, e_add_off, e_tx_bytes;   // region offsets inside a stage, bytes the producer loads into one stage
     const float *bias_f, *bias_m, *scale, *shift;
     EpiArgs epi;
 };
@@ -90,6 +101,76 @@ __device__ __forceinline__ TileCoord decode_tile(int t, const TcArgs &a)
     return c;
 }
 
+// Byte offset of channel c of pixel p in an epilogue region of P pixels: blocks of CB channels, each P rows of 2*CB bytes with
+// the TMA swizzle of that row length.  Reads and writes in the accumulator layout (8 pixels x 4 channel pairs per warp access)
+// touch 32 distinct banks.
+template <int CB, int P>
+__device__ __forceinline__ uint32_t epi_off(int p, int c)
+{
+    return (uint32_t)(c / CB) * (P * 2u * CB) + swz((uint32_t)p * (2u * CB) + (uint32_t)(c % CB) * 2u, 2u * CB);
+}
+
+// Epilogue of one warp's 16 pixels (tile rows r0, r0 + 1) from the accumulators (layout: conv_common.cuh, epilogue_tile) into
+// the epilogue stage st: the out region [128 px][N/2 channels] (RAW: [128 px][N]) holds the residual when there is one and
+// receives the output in place, the out2 region likewise holds out2_mul and receives out2, the add-in region [32 px][N] holds
+// the nearest-x2 source of the tile.  The arithmetic is epilogue_tile's.
+template <int N>
+__device__ __forceinline__ void epilogue_smem(const float (&d)[N / 2], uint8_t *st, int lane, int r0, int nt, const float4 *par,
+                                              const TcArgs &a)
+{
+    constexpr int HALF = N / 2, NJ = e_nj<N>();
+    constexpr int CBA = N < 64 ? N : 64;                    // add-in channel block
+    const EpiArgs &e = a.epi;
+    const int q2 = 2 * (lane & 3), px = lane >> 2;
+    auto ld = [&](uint32_t off) { return bf16x2_val(*reinterpret_cast<const uint32_t *>(st + off)); };
+    auto stw = [&](uint32_t off, uint32_t v) { *reinterpret_cast<uint32_t *>(st + off) = v; };
+    const float2 zero = make_float2(0.f, 0.f);
+    if (e.raw) {
+        constexpr int CB = N < 64 ? N : 64;
+#pragma unroll
+        for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int r = r0 + i, c = 8 * j + q2;
+                const float2 a2 = e.addin ? ld(a.e_add_off + epi_off<CBA, 32>((r >> 1) * (TC_TW / 2) + (px >> 1), c)) : zero;
+                stw(epi_off<CB, 128>(r * TC_TW + px, c), bf16x2_bits(d[4 * j + 2 * i] + a2.x, d[4 * j + 2 * i + 1] + a2.y));
+            }
+        return;
+    }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int r = r0 + i, col = 8 * j + q2, co = nt * HALF + col;
+            float2 fa = zero, ma = zero;
+            if (e.addin) {
+                const int pa = (r >> 1) * (TC_TW / 2) + (px >> 1);
+                fa = ld(a.e_add_off + epi_off<CBA, 32>(pa, col));
+                ma = ld(a.e_add_off + epi_off<CBA, 32>(pa, HALF + col));
+            }
+            const float f0 = d[4 * j + 2 * i] + fa.x, f1 = d[4 * j + 2 * i + 1] + fa.y;
+            const float m0 = d[4 * (j + NJ) + 2 * i] + ma.x, m1 = d[4 * (j + NJ) + 2 * i + 1] + ma.y;
+            const float4 p0 = par[co], p1 = par[co + 1];
+            float y0, y1;
+            if (e.elu) {
+                y0 = gate_fast<true>(f0 + p0.x, m0 + p0.y, p0.z, p0.w);
+                y1 = gate_fast<true>(f1 + p1.x, m1 + p1.y, p1.z, p1.w);
+            } else {
+                y0 = gate_fast<false>(f0 + p0.x, m0 + p0.y, p0.z, p0.w);
+                y1 = gate_fast<false>(f1 + p1.x, m1 + p1.y, p1.z, p1.w);
+            }
+            const uint32_t o = epi_off<HALF, 128>(r * TC_TW + px, col);
+            const float2 rs = e.residual ? ld(o) : zero;
+            const uint32_t pk = bf16x2_bits(y0 + rs.x, y1 + rs.y);
+            stw(o, pk);
+            if (e.out2) {
+                const float2 ys = bf16x2_val(pk);                // the stored (rounded) activation
+                const float2 mm = ld(a.e_out2_off + o);
+                stw(a.e_out2_off + o, bf16x2_bits(ys.x * mm.x, ys.y * mm.y));
+            }
+        }
+}
+
 // ------------------------------------------------------------------ the kernel
 // KS = filter size, STR = stride, KKN = 16-element K steps per K chunk (cin_blk / 16), N = n_tile (wgmma N).  Filter size and
 // stride are compile-time so that the tap loop unrolls into constant shared-memory offsets.
@@ -103,11 +184,12 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
 
     constexpr int ntaps = KS * KS;
     const uint32_t b_region = smem_base + a.b_region_off;
-    const uint32_t b_region_bytes = a.b_resident ? (uint32_t)(ntaps * a.kchunks) * a.b_bytes : (uint32_t)a.b_stages * a.b_bytes;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.b_region_off + b_region_bytes);
+    const uint32_t e_region = smem_base + a.e_region_off;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + TC_E_STAGES * a.e_bytes);
     const uint32_t bar0 = s_u32(bars);
     const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY;
     const uint32_t bfull0 = bar0 + 8 * BAR_BFULL, bempty0 = bar0 + 8 * BAR_BEMPTY, bres = bar0 + 8 * BAR_BRES;
+    const uint32_t efull0 = bar0 + 8 * BAR_EFULL, eempty0 = bar0 + 8 * BAR_EEMPTY;
     float4 *s_par = reinterpret_cast<float4 *>(bars + BAR_PARAMS);
 
     const int lane = threadIdx.x & 31;
@@ -118,11 +200,20 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
     if (warp == TC_PRODUCER_WARP && lane == 0) {
         for (int i = 0; i < a.n_src; ++i) tma_prefetch_desc(&tm.a[i]);
         tma_prefetch_desc(&tmB);
+        if (N > 16) {
+            if (a.epi.residual) tma_prefetch_desc(&tm.res);
+            if (a.epi.out2) tma_prefetch_desc(&tm.mul);
+            if (a.epi.addin) tma_prefetch_desc(&tm.add);
+        }
         for (int s = 0; s < TC_MAX_STAGES; ++s) {
             mbar_init(afull0 + 8 * s, 1);
             mbar_init(aempty0 + 8 * s, TC_CONSUMER_WARPS);
             mbar_init(bfull0 + 8 * s, 1);
             mbar_init(bempty0 + 8 * s, TC_CONSUMER_WARPS);
+        }
+        for (int s = 0; s < TC_E_STAGES; ++s) {
+            mbar_init(efull0 + 8 * s, 1);
+            mbar_init(eempty0 + 8 * s, 2);          // one arrival per consumer warpgroup
         }
         mbar_init(bres, 1);
         mbar_fence_init();
@@ -141,7 +232,7 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
         }
         __syncwarp();
         if (a.pdl) pdl_wait();        // activations come from the previous kernel; the (static) weights above do not
-        uint32_t as = 0, aph = 0, bs = 0, bph = 0;
+        uint32_t as = 0, aph = 0, bs = 0, bph = 0, es = 0, eph = 0;
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const TileCoord tc_ = decode_tile(t, a);
             const int x0 = tc_.tx * TC_TW - a.pad, y0 = tc_.ty * TC_TH - a.pad;
@@ -180,6 +271,22 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
                     }
                 }
             }
+            if (N > 16) {
+                // the tile's epilogue operands, after its A chunks: a stage is freed only when the epilogue of the tile
+                // after its own starts, and the next tile's A loads must not wait for that
+                mbar_wait(eempty0 + 8 * es, eph ^ 1u);
+                if (elect_one()) {
+                    const uint32_t full = efull0 + 8 * es, dst = e_region + es * a.e_bytes;
+                    mbar_arrive_expect_tx(full, a.e_tx_bytes);       // 0 bytes (a plain arrival) when the epilogue loads nothing
+                    const int ex = tc_.tx * TC_TW, ey = tc_.ty * TC_TH, c0 = tc_.nt * (N / 2);
+                    if (a.epi.residual) tma_load_4d(&tm.res, full, dst, c0, ex, ey, tc_.b);
+                    if (a.epi.out2) tma_load_4d(&tm.mul, full, dst + a.e_out2_off, c0, ex, ey, tc_.b);
+                    if (a.epi.addin)
+                        for (int c = 0; c < N; c += 64) tma_load_4d(&tm.add, full, dst + a.e_add_off + 64u * c, c, ex >> 1, ey >> 1, tc_.b);
+                }
+                __syncwarp();
+                if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
+            }
         }
         return;
     }
@@ -192,9 +299,11 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
     const int lr = 64 * wg + 16 * wiw + (lane & 7) + 8 * ((lane >> 3) & 1);
     const uint32_t a_base = (uint32_t)((lr >> 3) * HALO_W + (lr & 7)) * row_bytes;   // tap (0, 0) of this lane's pixel
     const uint32_t khalf = (uint32_t)(lane >> 4) * 16u;
-    if (a.pdl) pdl_wait();        // residual / add-in / FAM-multiplier tensors come from earlier kernels
+    if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
     if (a.b_resident) mbar_wait(bres, 0);
-    uint32_t as = 0, aph = 0, bs = 0, bph = 0;
+    uint32_t as = 0, aph = 0, bs = 0, bph = 0, es = 0, eph = 0;
+    const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
+    int e_pend = -1;                               // stage whose stores the issuer has not yet seen read
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const TileCoord tc_ = decode_tile(t, a);
         float acc[N / 2];
@@ -248,13 +357,42 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
             }
             if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
         }
-        EpiArgs e = a.epi;
-        e.par = s_par;
-        const int x0 = tc_.tx * TC_TW + (lane >> 2), y0 = tc_.ty * TC_TH + 8 * wg + 2 * wiw;
-        const int xs[2] = {x0, x0}, ys[2] = {y0, y0 + 1};
-        const bool in[2] = {x0 < a.W && y0 < a.H, x0 < a.W && y0 + 1 < a.H};
-        epilogue_tile<N>(acc, lane, tc_.b, ys, xs, in, tc_.nt, e);
+        if constexpr (N == 16) {     // the final layer (Cout <= 8): fp32 NCHW, stored from the registers
+            EpiArgs e = a.epi;
+            e.par = s_par;
+            const int x0 = tc_.tx * TC_TW + (lane >> 2), y0 = tc_.ty * TC_TH + 8 * wg + 2 * wiw;
+            const int xs[2] = {x0, x0}, ys[2] = {y0, y0 + 1};
+            const bool in[2] = {x0 < a.W && y0 < a.H, x0 < a.W && y0 + 1 < a.H};
+            epilogue_tile<N>(acc, lane, tc_.b, ys, xs, in, tc_.nt, e);
+        } else {
+            if (issuer && e_pend >= 0) {
+                bulk_wait_group_read<0>();
+                mbar_arrive(eempty0 + 8 * e_pend);
+            }
+            mbar_wait(efull0 + 8 * es, eph);
+            epilogue_smem<N>(acc, smem_al + a.e_region_off + es * a.e_bytes, lane, 8 * wg + 2 * wiw, tc_.nt, s_par, a);
+            fence_proxy_async_smem();
+            named_bar_sync(1 + wg, 128);
+            if (issuer) {
+                const uint32_t st = e_region + es * a.e_bytes;
+                const int ex = tc_.tx * TC_TW, ey = tc_.ty * TC_TH + 8 * wg;
+                if (ey < a.H) {          // the TMA unit clips the rest of the box at the image edge
+                    if (a.epi.raw) {
+                        constexpr int CB = N < 64 ? N : 64;
+#pragma unroll
+                        for (int c = 0; c < N; c += CB) tma_store_4d(&tm.out, st + 256u * c + 128u * CB * wg, c, ex, ey, tc_.b);
+                    } else {
+                        tma_store_4d(&tm.out, st + 64u * N * wg, tc_.nt * (N / 2), ex, ey, tc_.b);
+                        if (a.epi.out2) tma_store_4d(&tm.out2, st + a.e_out2_off + 64u * N * wg, tc_.nt * (N / 2), ex, ey, tc_.b);
+                    }
+                }
+                bulk_commit_group();
+            }
+            e_pend = (int)es;
+            if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
+        }
     }
+    if (issuer) bulk_wait_group<0>();     // the stores have read shared memory and written the outputs before the CTA retires
 }
 
 // ------------------------------------------------------------------ weight packing
@@ -412,6 +550,8 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     RB_CHECK_ARG((reinterpret_cast<uintptr_t>(d.out) & 15) == 0, "wgmma conv: output must be 16B aligned");
     RB_CHECK_ARG(d.residual == nullptr || (reinterpret_cast<uintptr_t>(d.residual) & 15) == 0, "wgmma conv: residual must be 16B aligned");
     RB_CHECK_ARG(d.addin == nullptr || (reinterpret_cast<uintptr_t>(d.addin) & 15) == 0, "wgmma conv: addin must be 16B aligned");
+    RB_CHECK_ARG(d.out2 == nullptr || ((reinterpret_cast<uintptr_t>(d.out2) | reinterpret_cast<uintptr_t>(d.out2_mul)) & 15) == 0,
+                 "wgmma conv: out2 and out2_mul must be 16B aligned");
     const long long tiles = (long long)((d.Wout + TC_TW - 1) / TC_TW) * ((d.Hout + TC_TH - 1) / TC_TH) * d.B * g.n_tiles;
     RB_CHECK_ARG(tiles < (1ll << 31), "wgmma conv: too many tiles");
     TcPlan *p = new (std::nothrow) TcPlan{};
@@ -456,6 +596,33 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
             return READ_ERR_CUDA;
         }
     }
+    // epilogue maps, NHWC bf16 {C, W, H, B}; boxes of at most 64 channels with the swizzle of their row length
+    const bool nchw = d.out_mode == READ_OUT_NCHW_F32, raw = d.out_mode == READ_OUT_RAW_NHWC;
+    auto enc_epi = [&](CUtensorMap *m, const void *ptr, int C, int W, int H, int bc, int bw, int bh, const char *what) {
+        cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)d.B};
+        cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+        cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)bw, (cuuint32_t)bh, 1};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        const CUtensorMapSwizzle esw = bc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (bc == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+        CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(ptr), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, esw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) set_error("wgmma conv: cuTensorMapEncodeTiled(%s) failed with %d", what, (int)r);
+        return r == CUDA_SUCCESS;
+    };
+    const int half = g.n_tile / 2;
+    if (!nchw) {
+        const int oc = raw ? g.n_tile : half;             // channels of one output pixel in the tile
+        const int ocb = oc < 64 ? oc : 64, acb = g.n_tile < 64 ? g.n_tile : 64;
+        bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH / 2, "out");
+        if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
+        if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
+        if (ok && d.residual) ok = enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "residual");
+        if (ok && d.addin) ok = enc_epi(&p->tmA.add, d.addin, g.n_tile, d.addin_W, d.addin_H, acb, TC_TW / 2, TC_TH / 2, "addin");
+        if (!ok) {
+            delete p;
+            return READ_ERR_CUDA;
+        }
+    }
     TcArgs &a = p->args;
     a.B = d.B; a.H = d.Hout; a.W = d.Wout; a.Cin = d.Cin; a.Cout = d.Cout; a.cout_pad = g.cout_pad;
     a.ksize = d.k; a.pad = d.pad;
@@ -485,29 +652,46 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
-    // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights + >= 4 A stages in half the budget
+    // epilogue stage: out region (128 pixels of the tile's output channels), out2 region, add-in region (32 pixels x N);
+    // every region is a multiple of 1 KB, so each keeps the 1 KB alignment of the swizzle patterns
+    if (!nchw) {
+        const uint32_t out_b = 128u * (raw ? 2u : 1u) * (uint32_t)g.n_tile;
+        const uint32_t out2_b = d.out2 ? 128u * (uint32_t)g.n_tile : 0u, add_b = d.addin ? 64u * (uint32_t)g.n_tile : 0u;
+        a.e_out2_off = out_b;
+        a.e_add_off = out_b + out2_b;
+        a.e_bytes = out_b + out2_b + add_b;
+        a.e_tx_bytes = (d.residual ? out_b : 0u) + out2_b + add_b;
+    }
+    const uint32_t e_ring = TC_E_STAGES * a.e_bytes;
+    // the rings get what a CTA may have minus the alignment pad, barriers and per-channel parameters (smem_bytes below)
+    const uint32_t fixed = 1024 + 8 * BAR_PARAMS + 16 * (uint32_t)g.cout_pad + 64;
+    const uint32_t budget_2 = TC_SMEM_PER_SM / 2 - 1024 - fixed, budget_1 = TC_SMEM_PER_CTA - fixed;
+    // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights, the epilogue ring and >= 3 A
+    // stages in half of the SM
     a.ctas_per_sm = (tc_ctas_per_sm(g.n_tile) > 1 && g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX &&
-                     total_b + 4 * a.a_bytes <= TC_SMEM_BUDGET_SMALL_N) ? 2 : 1;
-    const uint32_t budget = a.ctas_per_sm > 1 ? TC_SMEM_BUDGET_SMALL_N : TC_SMEM_BUDGET;
-    a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && total_b + 2 * a.a_bytes <= budget) ? 1 : 0;
+                     total_b + e_ring + 3 * a.a_bytes <= budget_2) ? 2 : 1;
+    const uint32_t budget = a.ctas_per_sm > 1 ? budget_2 : budget_1;
+    a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && total_b + e_ring + 2 * a.a_bytes <= budget) ? 1 : 0;
     uint32_t b_region_bytes;
     if (a.b_resident) {
-        int st = (int)((budget - total_b) / a.a_bytes);
+        int st = (int)((budget - total_b - e_ring) / a.a_bytes);
         a.a_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         a.b_stages = 0;
         b_region_bytes = total_b;
     } else {
         a.a_stages = 3;
-        if (3 * a.a_bytes + 2 * a.b_bytes > budget) {
-            set_error("wgmma conv: layer does not fit shared memory (A stage %u B, B tile %u B)", a.a_bytes, a.b_bytes);
+        if (3 * a.a_bytes + e_ring + 2 * a.b_bytes > budget) {
+            set_error("wgmma conv: layer does not fit shared memory (A stage %u B, B tile %u B, epilogue stage %u B)", a.a_bytes,
+                      a.b_bytes, a.e_bytes);
             delete p;
             return READ_ERR_UNSUPPORTED;
         }
-        int st = (int)((budget - 3 * a.a_bytes) / a.b_bytes);
+        int st = (int)((budget - 3 * a.a_bytes - e_ring) / a.b_bytes);
         a.b_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
     }
     a.b_region_off = (uint32_t)a.a_stages * a.a_bytes;
+    a.e_region_off = a.b_region_off + b_region_bytes;
     a.bias_f = d.bias_f; a.bias_m = d.bias_m; a.scale = d.bn_scale; a.shift = d.bn_shift;
     EpiArgs &e = a.epi;
     e.H = d.Hout; e.W = d.Wout; e.Cout = d.Cout;
@@ -521,7 +705,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     e.out = d.out;
     e.out2 = static_cast<__nv_bfloat16 *>(d.out2);
     e.addin_H = d.addin_H; e.addin_W = d.addin_W;
-    p->smem_bytes = 1024 + (size_t)a.b_region_off + b_region_bytes + 8 * BAR_PARAMS + 16 * (size_t)g.cout_pad + 64;
+    p->smem_bytes = (size_t)a.e_region_off + e_ring + fixed;
     *out = p;
     return READ_OK;
 }

@@ -106,6 +106,8 @@ __device__ __forceinline__ void bulk_wait_group()
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// barrier `id` (1..15; 0 is __syncthreads) over `n` threads, whole warps
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 // L2 prefetch of a 4-D box (no shared-memory destination, no barrier): warms L2 for a tile that will be loaded later
 __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap *tm, int c0, int c1, int c2, int c3)
 {
