@@ -157,7 +157,8 @@ enum { READ_ACT_F32 = 0, READ_ACT_BF16 = 1 };
 enum { READ_SRC_IDENTITY = 0, READ_SRC_NEAREST_DOWN = 1, READ_SRC_NEAREST_UP = 2, READ_SRC_BILINEAR_UP4 = 3 };
 enum { READ_OUT_NHWC = 0, READ_OUT_NCHW_F32 = 1,
        /* pre-activation accumulators [conv_f | conv_m] (no bias / activation / BN), NHWC with 2*Cout channels: one term of a
-        * 1x1 conv over a concat whose other sources live at a finer resolution (see `addin`) */
+        * 1x1 conv over a concat whose other sources live at a finer resolution (see `addin`); for a 3x3 stride-1 conv, plus an
+        * optional residual of the same [B,H,W,2*Cout] shape (training: recomputed [f | m], input gradients) */
        READ_OUT_RAW_NHWC = 2 };
 enum { READ_CONV_AUTO = 0, READ_CONV_GENERIC = 1, READ_CONV_TCGEN05 = 2, READ_CONV_TCGEN05_GATHER = 3 };
 
@@ -213,8 +214,13 @@ int read_pack_weights_tc_strided(const float *wf, const float *wm, int Cout, int
 int read_pack_weights_tc_for(const read_conv_desc *d, const float *wf, const float *wm, void *out_bf16, void *stream);
 int read_pack_weights_tc(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16,
                          void *stream);
+/* Filters of the input gradient of a stride-1 3x3 conv pair (wf, wm: [Cout][Cin][3][3] f32), packed for a RAW plan of the TMA-fed
+ * kernel with Cin' = 2*Cout, Cout' = Cin/2, k = 3: its input is [df | dm] in the column order of the forward RAW output (blocks of
+ * 2*min(Cout, 64) columns, the conv_f half of each block first), its RAW output [B,H,W,Cin] is dX (plus the plan's residual).
+ * Size: read_tc_weight_elems(Cin/2, 2*Cout, 3).  Cin % 32 == 0. */
+int read_pack_weights_tc_dgrad(const float *wf, const float *wm, int Cout, int Cin, void *out_bf16, void *stream);
 /* 1 if the TMA-fed wgmma kernel supports this layer (stride-1 k x k / stride-2 3x3, 4x4 single source; 1x1 virtual concat of
- * identity / nearest-down sources), else 0. */
+ * identity / nearest-down sources; RAW 3x3 stride 1 over one source, optionally with a [B,H,W,2*Cout] residual), else 0. */
 int read_conv_tc_supported(const read_conv_desc *d);
 /* Same for the wgmma kernel with a gathered A operand (any stride / concat / resampling, bf16 activations);
  * it has its own weight packing. */
@@ -303,6 +309,22 @@ int read_compact_touched(const float *grad_nd, const unsigned char *touched, int
                          int32_t *out_ids, float *out_grads, void *stream);
 int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int64_t N, float *grad_nd, unsigned char *touched,
                        void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Backward of the gated 3x3 stride-1 convs of the residual blocks (EBlock / DBlock, READ/models/unet.py:56-76), bf16 training with
+ * eval-mode BatchNorm (read_b200/blocks.py).  Activations NHWC bf16; [f | m] rows are in the forward RAW output's column order
+ * (see read_pack_weights_tc_dgrad).  Reductions ACCUMULATE (+=) into caller-zeroed fp32 buffers.
+ *   read_gate_backward : fm = pre-activation accumulators [P, 2C] (without bias), dy = gradient of the conv's output [P, C];
+ *                        dfm [P, 2C] = [df | dm] with dg = dy*bn_scale, df = dg*sigmoid(m)*A'(f), dm = dg*A(f)*sigmoid'(m);
+ *                        dbias_f/m = sum df / dm, dgamma = sum dy*(g - mean)*inv_std, dbeta = sum dy.  C = 16, 32, 48, 64, 128,
+ *                        192 or 256 (C <= 64 or C % 64 == 0: the channel counts that have the RAW column order)
+ *   read_conv3x3_wgrad : dwf / dwm [Cout][Cin][3][3] += sum over pixels of [df | dm] x im2col(x), x [B,H,W,Cin] with zero
+ *                        padding 1.  Cin % 32 == 0; Cout = 32, 64 or a multiple of 64
+ * ---------------------------------------------------------------------------------------- */
+int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                       const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
+                       float *dbias_m, float *dgamma, float *dbeta, void *stream);
+int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream);
 
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);

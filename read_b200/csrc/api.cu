@@ -79,7 +79,8 @@ static int validate_conv(const read_conv_desc &d)
     RB_CHECK_ARG(eh == d.Hout && ew == d.Wout, "conv: output is %dx%d, expected %dx%d", d.Hout, d.Wout, eh, ew);
     RB_CHECK_ARG(d.bias_f && d.bias_m && d.bn_scale && d.bn_shift && d.out, "conv: null parameter pointer");
     RB_CHECK_ARG(d.out_mode == READ_OUT_NHWC || d.out_mode == READ_OUT_NCHW_F32 || d.out_mode == READ_OUT_RAW_NHWC, "conv: bad out_mode");
-    RB_CHECK_ARG(d.out_mode != READ_OUT_RAW_NHWC || (d.residual == nullptr && d.out2 == nullptr), "conv: RAW output takes no residual / out2");
+    RB_CHECK_ARG(d.out_mode != READ_OUT_RAW_NHWC || d.out2 == nullptr, "conv: RAW output takes no out2");
+    RB_CHECK_ARG(d.out_mode != READ_OUT_RAW_NHWC || d.residual == nullptr || d.k == 3, "conv: RAW output takes a residual only for 3x3 convs");
     RB_CHECK_ARG(d.addin == nullptr || (d.addin_H == (d.Hout + 1) / 2 && d.addin_W == (d.Wout + 1) / 2),
                  "conv: addin must be [B, ceil(Hout/2), ceil(Wout/2), 2*Cout]");
     RB_CHECK_ARG((d.out_mode != READ_OUT_RAW_NHWC && d.addin == nullptr) || d.impl == READ_CONV_TCGEN05,

@@ -1,0 +1,274 @@
+// Backward of the gated 3x3 stride-1 convs inside the residual blocks (EBlock / DBlock, READ/models/unet.py:56-76) for bf16
+// training (read_b200/blocks.py: ResStackFn).  Per conv, last to first:
+//   gate backward    one elementwise pass over dY and the recomputed pre-activation [f | m] -> [df | dm] (bf16) and the fp32
+//                    per-channel sums dbias_f, dbias_m, dgamma, dbeta of the eval-mode BatchNorm
+//   input gradient   the TMA wgmma conv kernel in RAW mode over [df | dm] with flipped, transposed filters
+//                    (conv_tc.cu: read_pack_weights_tc_dgrad); the ResBlock skip enters through its residual operand
+//   weight gradient  dW[2C][9][Cin] = sum over pixels of [df | dm]^T x im2col(x): the tensor-core kernel of this file
+// Both kernels read [f | m] / [df | dm] rows in the column order of the forward RAW output: blocks of 2*half columns
+// (half = min(C, 64), the forward plan's n_tile / 2), the conv_f half of a block first.
+#include "common.cuh"
+#include "conv_common.cuh"
+#include "ptx.cuh"
+
+namespace rb {
+
+__device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2 * half + co % half; }
+
+// ------------------------------------------------------------------ gate backward
+// y = scale * A(f + b_f) * sigmoid(m + b_m) + shift, scale = gamma * inv_std, shift = beta - mean * scale:
+//   dg = dy * scale, df = dg * sigmoid * A', dm = dg * A * sigmoid * (1 - sigmoid),
+//   dgamma = sum dy * (g - mean) * inv_std, dbeta = sum dy.
+// A thread owns 8 channels (one 16-byte vector) of one pixel per step and keeps its channel group across pixels; its sums are
+// reduced per CTA in shared memory and leave with one atomic per channel and CTA.
+constexpr int GB_THREADS = 256, GB_MAX_C = 256;
+
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+                const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+                float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta)
+{
+    __shared__ float red[4][GB_MAX_C];
+    for (int i = threadIdx.x; i < 4 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
+    __syncthreads();
+    const int G = C / 8, ppb = GB_THREADS / G;
+    const int cg = threadIdx.x % G, co0 = 8 * cg, fcol = fm_col(co0, half);
+    float bf[8], bm[8], sc[8], mu[8], is[8];
+    float s_bf[8], s_bm[8], s_g[8], s_b[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        bf[j] = bias_f[co0 + j]; bm[j] = bias_m[co0 + j]; sc[j] = scale[co0 + j]; mu[j] = mean[co0 + j]; is[j] = inv_std[co0 + j];
+        s_bf[j] = s_bm[j] = s_g[j] = s_b[j] = 0.f;
+    }
+    if (threadIdx.x < ppb * G) {
+        for (long long p = blockIdx.x * (long long)ppb + threadIdx.x / G; p < P; p += (long long)gridDim.x * ppb) {
+            const uint4 vy = *reinterpret_cast<const uint4 *>(dy + p * C + co0);
+            const uint4 vf = *reinterpret_cast<const uint4 *>(fm + p * 2 * C + fcol);
+            const uint4 vm = *reinterpret_cast<const uint4 *>(fm + p * 2 * C + fcol + half);
+            const uint32_t wy[4] = {vy.x, vy.y, vy.z, vy.w}, wf[4] = {vf.x, vf.y, vf.z, vf.w}, wm[4] = {vm.x, vm.y, vm.z, vm.w};
+            uint32_t odf[4], odm[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const float2 y2 = bf16x2_val(wy[q]), f2 = bf16x2_val(wf[q]), m2 = bf16x2_val(wm[q]);
+                float df[2], dm[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int j = 2 * q + h;
+                    const float y = h ? y2.y : y2.x;
+                    const float f = (h ? f2.y : f2.x) + bf[j], m = (h ? m2.y : m2.x) + bm[j];
+                    const float s = 1.f / (1.f + expf(-m));
+                    float A = f, Ad = 1.f;
+                    if (ELU && f <= 0.f) { A = expm1f(f); Ad = A + 1.f; }
+                    const float g = A * s, dg = y * sc[j];
+                    df[h] = dg * s * Ad;
+                    dm[h] = dg * A * s * (1.f - s);
+                    s_bf[j] += df[h];
+                    s_bm[j] += dm[h];
+                    s_g[j] = fmaf(y, (g - mu[j]) * is[j], s_g[j]);
+                    s_b[j] += y;
+                }
+                odf[q] = bf16x2_bits(df[0], df[1]);
+                odm[q] = bf16x2_bits(dm[0], dm[1]);
+            }
+            *reinterpret_cast<uint4 *>(dfm + p * 2 * C + fcol) = make_uint4(odf[0], odf[1], odf[2], odf[3]);
+            *reinterpret_cast<uint4 *>(dfm + p * 2 * C + fcol + half) = make_uint4(odm[0], odm[1], odm[2], odm[3]);
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            atomicAdd(&red[0][co0 + j], s_bf[j]);
+            atomicAdd(&red[1][co0 + j], s_bm[j]);
+            atomicAdd(&red[2][co0 + j], s_g[j]);
+            atomicAdd(&red[3][co0 + j], s_b[j]);
+        }
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < C; c += GB_THREADS) {
+        atomicAdd(dbf + c, red[0][c]);
+        atomicAdd(dbm + c, red[1][c]);
+        atomicAdd(dgamma + c, red[2][c]);
+        atomicAdd(dbeta + c, red[3][c]);
+    }
+}
+
+// ------------------------------------------------------------------ weight gradient
+// GEMM  dW[M = 2C columns of [df | dm]][N = 9 taps x Cin] += A[M][K = pixels] * B[K][N], bf16 in, fp32 accumulators in
+// registers (mma.sync m16n8k16).  A CTA owns a 64-column x 32-input-channel block for all 9 taps and walks a strided share of
+// the image's 32-pixel row segments (split K): per segment it loads the [32 px][64] slice of [df | dm] and the [3 rows][34 px][32]
+// halo of x once (cp.async, double-buffered, zero-filled outside the image, which is the forward conv's zero padding) and
+// reads every tap's B operand out of that halo with ldmatrix.trans at a shifted pixel offset.  Split-K partials leave through fp32
+// atomics into the torch-layout gradients [C][Cin][3][3].
+// Warps: 8 = 2 (32 columns each) x 4 (8 input channels each); a warp holds 2 x 9 m16n8 tiles = 72 accumulators per thread.
+constexpr int WG_THREADS = 256, WG_PX = 32, WG_M = 64, WG_N = 32, WG_HALO = WG_PX + 2;
+constexpr uint32_t WG_A_BYTES = WG_PX * WG_M * 2;                  // 128-byte rows
+constexpr uint32_t WG_X_BYTES = 3 * WG_HALO * WG_N * 2;            // 64-byte rows
+constexpr uint32_t WG_STAGE = WG_A_BYTES + WG_X_BYTES;             // a multiple of 128 bytes
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4])
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
+{
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+__global__ void __launch_bounds__(WG_THREADS)
+wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
+             int half, float *__restrict__ dwf, float *__restrict__ dwm)
+{
+    __shared__ __align__(128) uint8_t sm[2 * WG_STAGE];
+    const int m0 = blockIdx.y * WG_M, n0 = blockIdx.z * WG_N;
+    const int segs = (W + WG_PX - 1) / WG_PX;
+    const long long chunks = (long long)B * H * segs;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int wm = warp & 1, wq = warp >> 1;
+    const uint32_t s0 = s_u32(sm);
+    const int twoC = 2 * C;
+
+    auto load = [&](long long ch, int st) {
+        const int seg = (int)(ch % segs);
+        const long long r = ch / segs;
+        const int y = (int)(r % H), b = (int)(r / H), x0 = seg * WG_PX;
+        const uint32_t base = s0 + (uint32_t)st * WG_STAGE;
+        {   // [df | dm]: 32 pixels x 8 16-byte chunks, one per thread
+            const int k = tid >> 3, q = tid & 7;
+            const bool ok = x0 + k < W;
+            const __nv_bfloat16 *src = ok ? dfm + (((long long)b * H + y) * W + x0 + k) * twoC + m0 + 8 * q : dfm;
+            cp_async16(base + swz((uint32_t)k * 128u + 16u * q, 128u), src, ok);
+        }
+        for (int i = tid; i < 3 * WG_HALO * 4; i += WG_THREADS) {   // x halo: rows y-1..y+1, pixels x0-1..x0+32, 4 chunks
+            const int hp = i >> 2, q = i & 3;
+            const int gy = y + hp / WG_HALO - 1, gx = x0 + hp % WG_HALO - 1;
+            const bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
+            const __nv_bfloat16 *src = ok ? x + (((long long)b * H + gy) * W + gx) * Cin + n0 + 8 * q : x;
+            cp_async16(base + WG_A_BYTES + swz((uint32_t)hp * 64u + 16u * q, 64u), src, ok);
+        }
+    };
+
+    float acc[2][9][4];
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int t = 0; t < 9; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[mi][t][i] = 0.f;
+
+    const int j = lane >> 3;
+    int st = 0;
+    if (blockIdx.x < chunks) load(blockIdx.x, 0);
+    cp_async_commit();
+    for (long long ch = blockIdx.x; ch < chunks; ch += gridDim.x) {
+        if (ch + gridDim.x < chunks) load(ch + gridDim.x, st ^ 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        const uint32_t sa = s0 + (uint32_t)st * WG_STAGE, sx = sa + WG_A_BYTES;
+        // A fragments (columns x pixels) of the warp's two m16 tiles and the segment's two k16 steps, from the [pixel][column] tile
+        uint32_t af[2][2][4];
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                const int k = 16 * ks + (lane & 7) + 8 * (j >> 1);
+                const int col = 32 * wm + 16 * mi + 8 * (j & 1);
+                ldmatrix_x4_trans(sa + swz((uint32_t)k * 128u + (uint32_t)col * 2u, 128u), af[mi][ks]);
+            }
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+            // B fragments of both k16 steps: matrix j = pixels 8j..8j+7 of the segment, read at halo (ky, pixel + kx)
+            const int hp = (tap / 3) * WG_HALO + tap % 3 + 8 * j + (lane & 7);
+            uint32_t bfr[4];
+            ldmatrix_x4_trans(sx + swz((uint32_t)hp * 64u + 16u * wq, 64u), bfr);
+#pragma unroll
+            for (int mi = 0; mi < 2; ++mi) {
+                mma_16816(acc[mi][tap], af[mi][0], bfr[0], bfr[1]);
+                mma_16816(acc[mi][tap], af[mi][1], bfr[2], bfr[3]);
+            }
+        }
+        __syncthreads();
+        st ^= 1;
+    }
+    cp_async_wait<0>();
+
+    // accumulator (row g [+8], columns 2t, 2t+1) -> dW[o][ci][ky][kx] of conv_f or conv_m
+    const int g = lane >> 2, t4 = lane & 3;
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int col = m0 + 32 * wm + 16 * mi + g + 8 * (i >> 1);
+            const int ci = n0 + 8 * wq + 2 * t4 + (i & 1);
+            const int rr = col % (2 * half);
+            const int o = (col / (2 * half)) * half + rr % half;
+            float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * 9;
+#pragma unroll
+            for (int tap = 0; tap < 9; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
+        }
+}
+
+}  // namespace rb
+
+using namespace rb;
+
+extern "C" {
+
+int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                       const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
+                       float *dbias_m, float *dgamma, float *dbeta, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && dbias_f && dbias_m && dgamma && dbeta,
+                 "gate_backward: null pointer");
+    // the [f | m] column order (blocks of 2*min(C, 64)) exists only for C <= 64 or C % 64 == 0, as in the forward RAW plan
+    RB_CHECK_ARG(C >= 16 && C <= GB_MAX_C && C % 16 == 0 && (C <= 64 || C % 64 == 0) && pixels >= 0,
+                 "gate_backward: C must be 16, 32, 48, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
+                 "gate_backward: tensors must be 16B aligned");
+    if (pixels == 0) return READ_OK;
+    const int half = C < 64 ? C : 64, ppb = GB_THREADS / (C / 8);
+    long long blocks = (pixels + ppb - 1) / ppb;
+    if (blocks > 8ll * num_sms()) blocks = 8ll * num_sms();
+    auto k = elu ? gate_bwd_kernel<true> : gate_bwd_kernel<false>;
+    k<<<(unsigned)blocks, GB_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, half, bias_f, bias_m, bn_scale, bn_mean,
+        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream)
+{
+    RB_CHECK_ARG(dfm && x && dwf && dwm, "conv3x3_wgrad: null pointer");
+    RB_CHECK_ARG(B >= 1 && H >= 1 && W >= 1, "conv3x3_wgrad: bad shape");
+    RB_CHECK_ARG(Cout % 32 == 0 && Cin % 32 == 0 && Cout > 0 && Cin > 0 && (Cout <= 64 || Cout % 64 == 0),
+                 "conv3x3_wgrad: Cin must be a multiple of 32 and Cout 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x)) & 15) == 0,
+                 "conv3x3_wgrad: tensors must be 16B aligned");
+    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
+    const int mb = 2 * Cout / WG_M, nb = Cin / WG_N;
+    long long s = (2ll * num_sms() + mb * nb - 1) / (mb * nb);
+    if (s > chunks) s = chunks;
+    RB_CHECK_ARG(s <= 0x7FFFFFFF && nb <= 65535 && mb <= 65535, "conv3x3_wgrad: too large");
+    wgrad_kernel<<<dim3((unsigned)s, mb, nb), WG_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+}  // extern "C"

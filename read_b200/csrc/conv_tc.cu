@@ -126,6 +126,7 @@ __device__ __forceinline__ void epilogue_smem(const float (&d)[N / 2], uint8_t *
     auto stw = [&](uint32_t off, uint32_t v) { *reinterpret_cast<uint32_t *>(st + off) = v; };
     const float2 zero = make_float2(0.f, 0.f);
     if (e.raw) {
+        // the out region holds the tile's residual when there is one (RAW 3x3: input gradient of a ResBlock, conv_bwd.cu)
         constexpr int CB = N < 64 ? N : 64;
 #pragma unroll
         for (int j = 0; j < N / 8; ++j)
@@ -133,7 +134,9 @@ __device__ __forceinline__ void epilogue_smem(const float (&d)[N / 2], uint8_t *
             for (int i = 0; i < 2; ++i) {
                 const int r = r0 + i, c = 8 * j + q2;
                 const float2 a2 = e.addin ? ld(a.e_add_off + epi_off<CBA, 32>((r >> 1) * (TC_TW / 2) + (px >> 1), c)) : zero;
-                stw(epi_off<CB, 128>(r * TC_TW + px, c), bf16x2_bits(d[4 * j + 2 * i] + a2.x, d[4 * j + 2 * i + 1] + a2.y));
+                const uint32_t o = epi_off<CB, 128>(r * TC_TW + px, c);
+                const float2 rs = e.residual ? ld(o) : zero;
+                stw(o, bf16x2_bits(d[4 * j + 2 * i] + a2.x + rs.x, d[4 * j + 2 * i + 1] + a2.y + rs.y));
             }
         return;
     }
@@ -279,7 +282,14 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
                     const uint32_t full = efull0 + 8 * es, dst = e_region + es * a.e_bytes;
                     mbar_arrive_expect_tx(full, a.e_tx_bytes);       // 0 bytes (a plain arrival) when the epilogue loads nothing
                     const int ex = tc_.tx * TC_TW, ey = tc_.ty * TC_TH, c0 = tc_.nt * (N / 2);
-                    if (a.epi.residual) tma_load_4d(&tm.res, full, dst, c0, ex, ey, tc_.b);
+                    if (a.epi.residual) {
+                        if (a.epi.raw) {             // RAW rows of N channels, in blocks of at most 64 like the stores
+                            constexpr int CB = N < 64 ? N : 64;
+                            for (int c = 0; c < N; c += CB) tma_load_4d(&tm.res, full, dst + 256u * c, tc_.nt * N + c, ex, ey, tc_.b);
+                        } else {
+                            tma_load_4d(&tm.res, full, dst, c0, ex, ey, tc_.b);
+                        }
+                    }
                     if (a.epi.out2) tma_load_4d(&tm.mul, full, dst + a.e_out2_off, c0, ex, ey, tc_.b);
                     if (a.epi.addin)
                         for (int c = 0; c < N; c += 64) tma_load_4d(&tm.add, full, dst + a.e_add_off + 64u * c, c, ex >> 1, ey >> 1, tc_.b);
@@ -380,7 +390,7 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
                     if (a.epi.raw) {
                         constexpr int CB = N < 64 ? N : 64;
 #pragma unroll
-                        for (int c = 0; c < N; c += CB) tma_store_4d(&tm.out, st + 256u * c + 128u * CB * wg, c, ex, ey, tc_.b);
+                        for (int c = 0; c < N; c += CB) tma_store_4d(&tm.out, st + 256u * c + 128u * CB * wg, tc_.nt * N + c, ex, ey, tc_.b);
                     } else {
                         tma_store_4d(&tm.out, st + 64u * N * wg, tc_.nt * (N / 2), ex, ey, tc_.b);
                         if (a.epi.out2) tma_store_4d(&tm.out2, st + a.e_out2_off + 64u * N * wg, tc_.nt * (N / 2), ex, ey, tc_.b);
@@ -419,6 +429,31 @@ __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__rest
         const int ky = tap / k, kx = tap % k;
         const float *w = is_m ? wm : wf;
         out[i] = __float2bfloat16_rn((co < Cout && c < Cin) ? w[(((long long)co * Cin + c) * k + ky) * k + kx] : 0.f);
+    }
+}
+
+// Input gradient of a stride-1 3x3 conv pair (conv_f, conv_m: [Cout][Cin][3][3]) as a RAW plan of the same kernel: a 3x3 conv of
+// [df | dm] (2*Cout channels, in the column order of the forward RAW output: blocks of n_tile_f columns, conv_f half then conv_m
+// half) with the filters flipped in space and transposed, dX[n] = sum_{tap, c} dfm[c] * w[o(c)][n][2-ky][2-kx].  The plan's N
+// columns are the Cin input channels in order, so its RAW output is dX itself.
+__global__ void pack_tc_dgrad_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int Cin, int half_f,
+                                     int cin_blk, int kchunks, __nv_bfloat16 *__restrict__ out)
+{
+    const long long total = 9ll * kchunks * Cin * cin_blk;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int kk = (int)(i % cin_blk);
+        long long r = i / cin_blk;
+        const int n = (int)(r % Cin);
+        r /= Cin;
+        const int kc = (int)(r % kchunks);
+        const int tap = (int)(r / kchunks);
+        const int c = kc * cin_blk + kk;                         // column of [df | dm]
+        const int rr = c % (2 * half_f);
+        const int o = (c / (2 * half_f)) * half_f + rr % half_f;
+        const float *w = rr >= half_f ? wm : wf;
+        const int ky = 2 - tap / 3, kx = 2 - tap % 3;
+        out[i] = __float2bfloat16_rn(c < 2 * Cout ? w[(((long long)o * Cin + n) * 3 + ky) * 3 + kx] : 0.f);
     }
 }
 
@@ -494,7 +529,12 @@ bool tc_supported(const read_conv_desc &d)
     } else if (d.out_mode != READ_OUT_NHWC && d.out_mode != READ_OUT_RAW_NHWC) {
         return false;
     }
-    if (d.out_mode == READ_OUT_RAW_NHWC || d.addin != nullptr) {
+    if (d.out_mode == READ_OUT_RAW_NHWC && d.k == 3) {
+        // accumulators of a 3x3 stride-1 conv over one tensor, optionally plus a residual of the output's [B, H, W, 2*Cout]
+        // shape: the training path's recomputed [f | m] and ResBlock input gradients (read_b200/blocks.py)
+        if (d.stride != 1 || d.n_src != 1 || d.addin != nullptr || d.out2 != nullptr) return false;
+        if ((long long)d.B * d.Hout * d.Wout * 2 * d.Cout >= (1ll << 31)) return false;
+    } else if (d.out_mode == READ_OUT_RAW_NHWC || d.addin != nullptr) {
         // terms of a 1x1 conv over a multi-resolution concat: served by the lean epilogue (Cout 16 / 32 / 64)
         if (d.k != 1 || d.stride != 1) return false;
         if (!(d.Cout == 16 || d.Cout == 32 || d.Cout == 64)) return false;
@@ -616,7 +656,9 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH / 2, "out");
         if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
         if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
-        if (ok && d.residual) ok = enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "residual");
+        if (ok && d.residual)
+            ok = raw ? enc_epi(&p->tmA.res, d.residual, 2 * d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH, "residual")
+                     : enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "residual");
         if (ok && d.addin) ok = enc_epi(&p->tmA.add, d.addin, g.n_tile, d.addin_W, d.addin_H, acb, TC_TW / 2, TC_TH / 2, "addin");
         if (!ok) {
             delete p;
@@ -811,6 +853,21 @@ int read_pack_weights_tc_strided(const float *wf, const float *wm, int Cout, int
                                  void *stream)
 {
     return pack_tc_impl(wf, wm, Cout, Cin, k, stride, 64, out_bf16, stream);
+}
+
+int read_pack_weights_tc_dgrad(const float *wf, const float *wm, int Cout, int Cin, void *out_bf16, void *stream)
+{
+    TcGeom gf, gd;
+    RB_CHECK_ARG(wf && wm && out_bf16, "pack_tc_dgrad: null pointer");
+    RB_CHECK_ARG(Cin % 32 == 0 && tc_geom(Cin, Cout, 1, &gf) && tc_geom(2 * Cout, Cin / 2, 1, &gd) && gd.cout_pad == Cin / 2,
+                 "pack_tc_dgrad: unsupported channel counts %d -> %d", Cin, Cout);
+    const long long total = 9ll * gd.kchunks * gd.cin_blk * Cin;
+    long long blocks = (total + 255) / 256;
+    if (blocks > 65535) blocks = 65535;
+    pack_tc_dgrad_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, gf.n_tile / 2, gd.cin_blk,
+                                                                             gd.kchunks, (__nv_bfloat16 *)out_bf16);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 }  // extern "C"

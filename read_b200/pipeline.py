@@ -44,6 +44,8 @@ _CLI = (
     ('--texture_activation', dict(type=str, default='none'), True),
     ('--n_points', dict(type=int, default=0, help='this is for inference'), True),
     ('--dense_texture_optimizer', dict(action='store_true', help='torch.optim.RMSprop over all points instead of the sparse kernel'), False),
+    ('--net_train_precision', dict(type=str, default='fp32', choices=['fp32', 'bf16'],
+                                   help="bf16: train the net's residual blocks on the wgmma kernels (UNet.train_precision)"), False),
 )
 
 
@@ -115,6 +117,7 @@ class TexturePipeline(Pipeline):
             args.input_channels = [args.descriptor_size] * getattr(args, 'num_mipmap', 5)
         self.args = args
         self.net = get_net(args.input_channels, args)
+        self.net.train_precision = getattr(args, 'net_train_precision', 'fp32')
         if getattr(args, 'inference', False):
             self.textures = {0: get_texture(args.descriptor_size, args.n_points, args)}
         else:

@@ -10,8 +10,9 @@ gated-conv kernel launches (wgmma tensor-core kernels for the dominant 3x3 layer
 There is no CPU path: inference on a CPU tensor raises.
 
 Training (autograd enabled) is routed through torch's own conv/batch-norm operators on the same parameters —
-a LIBRARY path (cuDNN), kept so that the reference's train.py keeps working; it is not the product hot path
-(DESIGN.md "out of scope this round": conv backward kernels).
+a LIBRARY path (cuDNN), kept so that the reference's train.py keeps working.  ``train_precision = 'bf16'`` moves the 8
+residual block stacks (64 of the 99 convs) onto the wgmma kernels, forward and backward (read_b200/blocks.py); the
+default ``'fp32'`` keeps every layer on torch.
 """
 import threading
 
@@ -19,7 +20,10 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import blocks
 from .engine import UNetEngine
+
+TRAIN_PRECISIONS = ('fp32', 'bf16')
 
 
 def layer_table(base=32, num_res=4):
@@ -96,6 +100,8 @@ class UNet(nn.Module):
             m = GatedConv(cin, cout, k, stride, elu)
             _attach(self, prefix, m)
         self.precision = 'bf16'          # 'bf16' (tensor cores) | 'fp32' (CUDA-core parity mode)
+        # training (autograd) path: 'fp32' = torch operators everywhere | 'bf16' = residual block stacks on the wgmma kernels
+        self.train_precision = 'fp32'
         self.conv_impl = 'auto'
         self.use_graph = True
         self._engines = {}
@@ -175,11 +181,16 @@ class UNet(nn.Module):
         """Library (cuDNN/autograd) evaluation of unet.py:202-285 on the same parameters; training only."""
         c = self._c
         x, x_2, x_4, x_8 = inputs[:4]
+        tp = getattr(self, 'train_precision', 'fp32')       # modules pickled before the attribute existed
+        if tp not in TRAIN_PRECISIONS:
+            raise ValueError(f"read_b200.UNet: train_precision must be one of {TRAIN_PRECISIONS}, got {tp!r}")
 
         def res(p, t):
             return c(p + ".main.1", c(p + ".main.0", t)) + t
 
         def blk(p, t):
+            if tp == 'bf16':
+                return blocks.res_stack(self, p, t)
             for i in range(self.num_res):
                 t = res(f"{p}.layers.{i}", t)
             return t

@@ -1,0 +1,189 @@
+"""C5 training step (8 crops of 256x256 per step, 5M points, L1 loss, backward through the net and the descriptor gather, Adam on
+the net, sparse RMSprop on the descriptors) with the net's residual block stacks trained in fp32 (torch operators, cuDNN) and in
+bf16 (wgmma kernels, UNet.train_precision = 'bf16'), alternating in one process so that clock drift hits both alike.
+   python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--out result.json]
+Prints the card's name and power limit, per precision the step time and the share of the net's forward + backward in it, the time
+to re-pack the 64 block convs' filters (done on every bf16 step), and per stack shape the time of each backward kernel."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from read_b200 import synth, ops, blocks, _lib as L, train as rtrain          # noqa: E402
+from read_b200.unet import UNet                                                # noqa: E402
+from read_b200.texture import PointTexture                                     # noqa: E402
+from read_b200.compose import NetAndTexture                                    # noqa: E402
+
+N, W, H, BC, LEVELS = 5_000_000, 256, 256, 8, 4
+
+
+def ev():
+    return torch.cuda.Event(enable_timing=True)
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True).stdout.strip()
+    return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q}
+
+
+def make_model(sd, tp, dev):
+    tex = PointTexture(8, N, init_method='zeros')
+    with torch.no_grad():
+        tex.texture_.copy_(torch.rand((1, 8, N), generator=torch.Generator().manual_seed(synth.SEED)))
+    net = UNet()
+    net.load_state_dict(sd, strict=True)
+    net.train_precision = tp
+    model = NetAndTexture(net, {0: tex}, 1)
+    model.load_textures(0)
+    model.to(dev).eval()                        # eval-mode BatchNorm, as the reference trains
+    return dict(net=net, tex=tex, model=model, opt_net=torch.optim.Adam(net.parameters(), lr=1e-4),
+                opt_tex=rtrain.SparseRMSprop(tex, lr=1e-1))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(0)
+    L.require_device(0)
+    xyz = torch.from_numpy(synth.street_scene(N)).to(dev)
+    store = ops.SortedPoints(xyz)
+    pyr = ops.Pyramid(BC, W, H, LEVELS, dev)
+    rng = np.random.default_rng(synth.SEED)
+    n_mats = 3 + args.steps
+    mats = torch.stack([torch.from_numpy(synth.total_matrix(*synth.crop_cameras(W, H, rng.integers(0, 64, BC), rng)))
+                        for _ in range(n_mats)]).to(dev)
+    target = torch.rand((BC, 3, H, W), generator=torch.Generator().manual_seed(7)).to(dev)
+    keys = ["uv_1d_p1"] + [f"uv_1d_p1_ds{l}" for l in range(1, LEVELS)]
+    ids0 = torch.zeros(BC, dtype=torch.long)
+    sd = synth.synth_state_dict(synth.SEED)
+    runs = {tp: make_model(sd, tp, dev) for tp in ("fp32", "bf16")}
+
+    def step(r, m, marks=None):
+        e = [ev() for _ in range(4)] if marks is not None else None
+        if e: e[0].record()
+        pyr.clear()
+        ops.raster_project_sorted(pyr, store, m)
+        ops.raster_derive(pyr)
+        inputs = {k: ops.zbuf_resolve(pyr, l, want_depth=False)[0].unsqueeze(1) for l, k in enumerate(keys)}
+        inputs["id"] = ids0
+        if e: e[1].record()
+        loss = F.l1_loss(r["model"](inputs), target)
+        loss.backward()
+        if e: e[2].record()
+        r["opt_net"].step()
+        r["opt_tex"].step()
+        r["opt_net"].zero_grad(set_to_none=True)
+        if marks is not None:
+            e[3].record()
+            marks.append(e)
+        return loss
+
+    first_loss = {}
+    for tp, r in runs.items():                     # warm-up (and the loss of both precisions on the same first crops)
+        first_loss[tp] = float(step(r, mats[0]).detach())
+        for s in range(1, 3):
+            step(r, mats[s])
+    torch.cuda.synchronize()
+    ms = {tp: [] for tp in runs}
+    share = {tp: [] for tp in runs}
+    for _ in range(args.rounds):
+        for tp, r in runs.items():
+            torch.cuda.synchronize()
+            a, b = ev(), ev()
+            a.record()
+            for s in range(args.steps):
+                step(r, mats[3 + s])
+            b.record()
+            torch.cuda.synchronize()
+            ms[tp].append(a.elapsed_time(b) / args.steps)
+            marks = []
+            for s in range(3):
+                step(r, mats[3 + s], marks)
+            torch.cuda.synchronize()
+            net_ms = sum(e[1].elapsed_time(e[2]) for e in marks) / len(marks)
+            tot_ms = sum(e[0].elapsed_time(e[3]) for e in marks) / len(marks)
+            share[tp].append({"net_fwd_bwd_ms": net_ms, "step_ms": tot_ms, "share": net_ms / tot_ms})
+
+    # filter re-packing of the 64 block convs (what every bf16 step does before its first block launch)
+    net = runs["bf16"]["net"]
+    mods = [m for p in [f"Encoder.{i}" for i in range(4)] + [f"Decoder.{i}" for i in range(4)] for m in blocks.stack_convs(net, p)]
+    pack = []
+    for _ in range(5):
+        a, b = ev(), ev()
+        a.record()
+        for m in mods:
+            blocks.FoldedConv(m, *blocks.stack_params([m]))
+        b.record()
+        torch.cuda.synchronize()
+        pack.append(a.elapsed_time(b))
+
+    # backward kernels of one conv per stack shape at C5 (B = 8): RAW recompute, gate backward, weight gradient, input gradient
+    lib = L.load()
+    kern = []
+    for C, S in ((32, 256), (64, 128), (128, 64), (256, 32)):
+        m = next(mm for mm in mods if mm.block['conv_f'].weight.shape[0] == C)
+        fc = blocks.FoldedConv(m, *blocks.stack_params([m]))
+        x = torch.randn((BC, S, S, C), device=dev).bfloat16()
+        dy = torch.randn((BC, S, S, C), device=dev).bfloat16()
+        fm = torch.empty((BC, S, S, 2 * C), device=dev, dtype=torch.bfloat16)
+        dfm = torch.empty_like(fm)
+        red = torch.zeros((4, C), device=dev)
+        dwf, dwm = torch.zeros_like(fc.wf), torch.zeros_like(fc.wm)
+        st = L.stream_ptr()
+        P = BC * S * S
+        fns = {
+            "raw_recompute": lambda: blocks._launch(lib, x, C, fc.w_tc, fc.par, fc.elu, L.OUT_RAW_NHWC, fm),
+            "gate_backward": lambda: L.check(lib.read_gate_backward(dy.data_ptr(), fm.data_ptr(), P, C, 1, fc.bf.data_ptr(), fc.bm.data_ptr(),
+                                                                    fc.scale.data_ptr(), fc.mean.data_ptr(), fc.inv.data_ptr(), dfm.data_ptr(),
+                                                                    red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st)),
+            "wgrad": lambda: L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x.data_ptr(), BC, S, S, C, C, dwf.data_ptr(), dwm.data_ptr(), st)),
+            "dgrad": lambda: blocks.dgrad(dfm, fc, residual=dy),
+        }
+        row = {"C": C, "HxW": f"{S}x{S}", "B": BC}
+        for name, fn in fns.items():
+            for _ in range(3):
+                fn()
+            torch.cuda.synchronize()
+            a, b = ev(), ev()
+            a.record()
+            for _ in range(20):
+                fn()
+            b.record()
+            torch.cuda.synchronize()
+            row[name + "_us"] = a.elapsed_time(b) / 20 * 1e3
+        flops = 2.0 * 2 * C * 9 * C * P
+        row["wgrad_tflops"] = flops / (row["wgrad_us"] * 1e-6) / 1e12
+        row["wgrad_min_bytes"] = P * 3 * C * 2            # [df | dm] and x read once
+        row["wgrad_gbs"] = row["wgrad_min_bytes"] / (row["wgrad_us"] * 1e-6) / 1e9
+        kern.append(row)
+
+    res = {"card": card(), "steps": args.steps, "rounds": args.rounds, "crops_per_step": BC, "size": f"{W}x{H}", "n_points": N,
+           "ms_per_step": ms, "net_fwd_bwd_per_step": share, "first_loss": first_loss,
+           "bf16_filter_repack_ms_per_step": pack, "backward_kernels": kern}
+    for tp in runs:
+        med = sorted(ms[tp])[len(ms[tp]) // 2]
+        sh = sorted(share[tp], key=lambda x: x["share"])[len(share[tp]) // 2]
+        print(f"{tp}: {med:.2f} ms/step (rounds {', '.join(f'{v:.2f}' for v in ms[tp])}), net fwd+bwd {sh['net_fwd_bwd_ms']:.2f} ms "
+              f"of a {sh['step_ms']:.2f} ms profiled step = {100 * sh['share']:.1f} %")
+    print(f"card: {res['card']}")
+    print(f"first-step loss fp32 {first_loss['fp32']:.6f} bf16 {first_loss['bf16']:.6f}; filter re-pack {sorted(pack)[2]:.3f} ms/step")
+    for row in kern:
+        print(json.dumps(row))
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        json.dump(res, open(args.out, "w"), indent=1)
+
+
+if __name__ == "__main__":
+    main()
