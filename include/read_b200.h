@@ -311,20 +311,26 @@ int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int
                        void *stream);
 
 /* ------------------------------------------------------------------------------------------
- * Backward of the gated 3x3 stride-1 convs of the residual blocks (EBlock / DBlock, READ/models/unet.py:56-76), bf16 training with
- * eval-mode BatchNorm (read_b200/blocks.py).  Activations NHWC bf16; [f | m] rows are in the forward RAW output's column order
- * (see read_pack_weights_tc_dgrad).  Reductions ACCUMULATE (+=) into caller-zeroed fp32 buffers.
- *   read_gate_backward : fm = pre-activation accumulators [P, 2C] (without bias), dy = gradient of the conv's output [P, C];
- *                        dfm [P, 2C] = [df | dm] with dg = dy*bn_scale, df = dg*sigmoid(m)*A'(f), dm = dg*A(f)*sigmoid'(m);
- *                        dbias_f/m = sum df / dm, dgamma = sum dy*(g - mean)*inv_std, dbeta = sum dy.  C = 16, 32, 48, 64, 128,
- *                        192 or 256 (C <= 64 or C % 64 == 0: the channel counts that have the RAW column order)
- *   read_conv3x3_wgrad : dwf / dwm [Cout][Cin][3][3] += sum over pixels of [df | dm] x im2col(x), x [B,H,W,Cin] with zero
- *                        padding 1.  Cin % 32 == 0; Cout = 32, 64 or a multiple of 64
+ * Backward of the gated 3x3 stride-1 convs (the residual blocks EBlock / DBlock, READ/models/unet.py:56-76, and the single convs
+ * feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge), bf16 training with eval-mode BatchNorm (read_b200/blocks.py).
+ * Activations NHWC bf16; [f | m] rows are in the forward RAW output's column order (see read_pack_weights_tc_dgrad).  Reductions
+ * ACCUMULATE (+=) into caller-zeroed fp32 buffers.
+ *   read_gate_backward      : fm = pre-activation accumulators [P, 2C] (without bias), dy = gradient of the conv's output [P, C];
+ *                             dfm [P, 2C] = [df | dm] with dg = dy*bn_scale, df = dg*sigmoid(m)*A'(f), dm = dg*A(f)*sigmoid'(m);
+ *                             dbias_f/m = sum df / dm, dgamma = sum dy*(g - mean)*inv_std, dbeta = sum dy.  C = 16, 32, 48, 64,
+ *                             128, 192 or 256 (C <= 64 or C % 64 == 0: the channel counts that have the RAW column order); the RGB
+ *                             output conv (C = 3) is run padded to C = 16 by the caller
+ *   read_conv3x3_wgrad      : dwf / dwm [Cout][Cin][3][3] += sum over pixels of [df | dm] x im2col(x), x [B,H,W,Cin] with zero
+ *                             padding 1.  Cin = 8, 16 or a multiple of 32; Cout = 16, 32, 64 or a multiple of 64
+ *   read_conv3x3_dgrad_cin8 : input gradient dx [B,H,W,8] (bf16, overwritten) of a conv with Cin = 8 (the descriptor pyramid), from
+ *                             dfm [B,H,W,2*Cout] and the fp32 filters wf / wm [Cout][8][3][3].  Cout = 16, 32 or 64.  The input
+ *                             gradient of wider inputs is a RAW plan with read_pack_weights_tc_dgrad filters
  * ---------------------------------------------------------------------------------------- */
 int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                        const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
                        float *dbias_m, float *dgamma, float *dbeta, void *stream);
 int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream);
+int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, int B, int H, int W, int Cout, void *dx, void *stream);
 
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);

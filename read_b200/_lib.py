@@ -98,6 +98,7 @@ _SIGS = {
     "read_gate_backward": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                    c_vp]),
     "read_conv3x3_wgrad": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "read_conv3x3_dgrad_cin8": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_conv_tc_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_conv_tcg_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_tcg_weight_elems": (c_i64, [c_int, c_int, c_int]),

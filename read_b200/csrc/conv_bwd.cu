@@ -1,9 +1,10 @@
-// Backward of the gated 3x3 stride-1 convs inside the residual blocks (EBlock / DBlock, READ/models/unet.py:56-76) for bf16
-// training (read_b200/blocks.py: ResStackFn).  Per conv, last to first:
+// Backward of the gated 3x3 stride-1 convs (the residual blocks EBlock / DBlock, READ/models/unet.py:56-76, and the single convs
+// around them) for bf16 training (read_b200/blocks.py: ResStackFn, GatedConvFn).  Per conv, last to first:
 //   gate backward    one elementwise pass over dY and the recomputed pre-activation [f | m] -> [df | dm] (bf16) and the fp32
 //                    per-channel sums dbias_f, dbias_m, dgamma, dbeta of the eval-mode BatchNorm
 //   input gradient   the TMA wgmma conv kernel in RAW mode over [df | dm] with flipped, transposed filters
-//                    (conv_tc.cu: read_pack_weights_tc_dgrad); the ResBlock skip enters through its residual operand
+//                    (conv_tc.cu: read_pack_weights_tc_dgrad); the ResBlock skip enters through its residual operand.  An
+//                    8-channel input (the descriptor pyramid) has its own kernel in this file (dgrad_cin8_kernel)
 //   weight gradient  dW[2C][9][Cin] = sum over pixels of [df | dm]^T x im2col(x): the tensor-core kernel of this file
 // Both kernels read [f | m] / [df | dm] rows in the column order of the forward RAW output: blocks of 2*half columns
 // (half = min(C, 64), the forward plan's n_tile / 2), the conv_f half of a block first.
@@ -100,6 +101,8 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
 // reads every tap's B operand out of that halo with ldmatrix.trans at a shifted pixel offset.  Split-K partials leave through fp32
 // atomics into the torch-layout gradients [C][Cin][3][3].
 // Warps: 8 = 2 (32 columns each) x 4 (8 input channels each); a warp holds 2 x 9 m16n8 tiles = 72 accumulators per thread.
+// Narrow convs (Cin = 8 or 16: the descriptor pyramid; 2C = 32 columns: the RGB output conv padded to C = 16) run in one
+// partial block: its loads are zero-filled beyond Cin and beyond 2C, and only real (column, channel) pairs are stored.
 constexpr int WG_THREADS = 256, WG_PX = 32, WG_M = 64, WG_N = 32, WG_HALO = WG_PX + 2;
 constexpr uint32_t WG_A_BYTES = WG_PX * WG_M * 2;                  // 128-byte rows
 constexpr uint32_t WG_X_BYTES = 3 * WG_HALO * WG_N * 2;            // 64-byte rows
@@ -149,14 +152,14 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
         const uint32_t base = s0 + (uint32_t)st * WG_STAGE;
         {   // [df | dm]: 32 pixels x 8 16-byte chunks, one per thread
             const int k = tid >> 3, q = tid & 7;
-            const bool ok = x0 + k < W;
+            const bool ok = x0 + k < W && m0 + 8 * q < twoC;
             const __nv_bfloat16 *src = ok ? dfm + (((long long)b * H + y) * W + x0 + k) * twoC + m0 + 8 * q : dfm;
             cp_async16(base + swz((uint32_t)k * 128u + 16u * q, 128u), src, ok);
         }
         for (int i = tid; i < 3 * WG_HALO * 4; i += WG_THREADS) {   // x halo: rows y-1..y+1, pixels x0-1..x0+32, 4 chunks
             const int hp = i >> 2, q = i & 3;
             const int gy = y + hp / WG_HALO - 1, gx = x0 + hp % WG_HALO - 1;
-            const bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
+            const bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W && n0 + 8 * q < Cin;
             const __nv_bfloat16 *src = ok ? x + (((long long)b * H + gy) * W + gx) * Cin + n0 + 8 * q : x;
             cp_async16(base + WG_A_BYTES + swz((uint32_t)hp * 64u + 16u * q, 64u), src, ok);
         }
@@ -215,12 +218,102 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
         for (int i = 0; i < 4; ++i) {
             const int col = m0 + 32 * wm + 16 * mi + g + 8 * (i >> 1);
             const int ci = n0 + 8 * wq + 2 * t4 + (i & 1);
+            if (col >= twoC || ci >= Cin) continue;
             const int rr = col % (2 * half);
             const int o = (col / (2 * half)) * half + rr % half;
             float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * 9;
 #pragma unroll
             for (int tap = 0; tap < 9; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
         }
+}
+
+// ------------------------------------------------------------------ input gradient of an 8-channel input
+// The convs that read the descriptor pyramid (feat_extract.0, SCM*.main.0: Cin = 8, C = 16 / 32 / 64) need
+//   dX[p][n] = sum over taps (ty, tx) and columns k of [df | dm] of dfm[p + (ty - 1, tx - 1)][k] * w_k[n][2 - ty][2 - tx],
+// an implicit GEMM with N = 8: exactly one mma.sync m16n8k16 tile, where the TMA kernel's smallest N is 16.  A persistent CTA
+// converts the flipped, transposed filters to bf16 in shared memory once ([tap][n][k]), then walks a strided share of the
+// image's 64-pixel row segments: per segment it loads the 3-row [df | dm] halo (cp.async, zero-filled outside the image, which
+// is the transposed conv's zero padding) and each warp computes 16 pixels x 8 channels over all 9 taps.  Shared-memory rows
+// are padded by 16 bytes, so the ldmatrix reads of A and the 32-bit reads of B touch 32 distinct banks.
+constexpr int DG8_THREADS = 128, DG8_PX = 64, DG8_HALO = DG8_PX + 2;
+
+__host__ __device__ constexpr uint32_t dg8_row_bytes(int K2) { return (uint32_t)K2 * 2u + 16u; }
+__host__ __device__ constexpr uint32_t dg8_smem_bytes(int K2) { return (9u * 8u + 3u * DG8_HALO) * dg8_row_bytes(K2); }
+
+template <int K2>       // columns of [df | dm] = 2C
+__global__ void __launch_bounds__(DG8_THREADS)
+dgrad_cin8_kernel(const __nv_bfloat16 *__restrict__ dfm, const float *__restrict__ wf, const float *__restrict__ wm, int B, int H,
+                  int W, __nv_bfloat16 *__restrict__ dx)
+{
+    extern __shared__ __align__(16) uint8_t dg_sm[];
+    constexpr uint32_t ROW = dg8_row_bytes(K2);
+    constexpr int HALF = K2 / 2 < 64 ? K2 / 2 : 64;          // the RAW column order's block: 2*HALF columns, conv_f half first
+    const uint32_t sw = s_u32(dg_sm), sx = sw + 9u * 8u * ROW;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int i = tid; i < 9 * 8 * K2; i += DG8_THREADS) {
+        const int k = i % K2, n = (i / K2) % 8, tap = i / (8 * K2);
+        const int rr = k % (2 * HALF), o = (k / (2 * HALF)) * HALF + rr % HALF;
+        const float *w = rr >= HALF ? wm : wf;
+        const int ky = 2 - tap / 3, kx = 2 - tap % 3;
+        *reinterpret_cast<__nv_bfloat16 *>(dg_sm + (tap * 8 + n) * ROW + 2 * k) = __float2bfloat16_rn(w[((o * 8 + n) * 3 + ky) * 3 + kx]);
+    }
+    const int segs = (W + DG8_PX - 1) / DG8_PX;
+    const long long chunks = (long long)B * H * segs;
+    const int pr = 16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1);   // this lane's ldmatrix row: pixel of the segment
+    const uint32_t a_lane = sx + (uint32_t)pr * ROW + (uint32_t)(lane >> 4) * 16u;
+    const uint32_t b_lane = sw + (uint32_t)(lane >> 2) * ROW + 4u * (lane & 3);
+    const int g = lane >> 2, t4 = lane & 3;
+    for (long long ch = blockIdx.x; ch < chunks; ch += gridDim.x) {
+        const int seg = (int)(ch % segs);
+        const long long r = ch / segs;
+        const int y = (int)(r % H), b = (int)(r / H), x0 = seg * DG8_PX;
+        __syncthreads();                      // the previous segment's halo is read (and, the first time, the filters stored)
+        for (int i = tid; i < 3 * DG8_HALO * (K2 / 8); i += DG8_THREADS) {
+            const int hp = i / (K2 / 8), q = i % (K2 / 8);
+            const int gy = y + hp / DG8_HALO - 1, gx = x0 + hp % DG8_HALO - 1;
+            const bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
+            const __nv_bfloat16 *src = ok ? dfm + (((long long)b * H + gy) * W + gx) * K2 + 8 * q : dfm;
+            cp_async16(sx + (uint32_t)hp * ROW + 16u * q, src, ok);
+        }
+        cp_async_commit();
+        cp_async_wait<0>();
+        __syncthreads();
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+            const uint32_t a_tap = a_lane + (uint32_t)((tap / 3) * DG8_HALO + tap % 3) * ROW, b_tap = b_lane + tap * 8u * ROW;
+#pragma unroll
+            for (int ks = 0; ks < K2 / 16; ++ks) {
+                uint32_t af[4], b0, b1;
+                ldmatrix_x4(a_tap + 32u * ks, af);
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b0) : "r"(b_tap + 32u * ks));
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b1) : "r"(b_tap + 32u * ks + 16u));
+                mma_16816(acc, af, b0, b1);
+            }
+        }
+        // accumulator rows g, g + 8 = pixels, columns 2t, 2t + 1 = input channels
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int px = x0 + 16 * warp + g + 8 * i;
+            if (px < W)
+                *reinterpret_cast<uint32_t *>(dx + (((long long)b * H + y) * W + px) * 8 + 2 * t4) = bf16x2_bits(acc[2 * i], acc[2 * i + 1]);
+        }
+    }
+}
+
+template <int K2>
+static int launch_dgrad_cin8(const void *dfm, const float *wf, const float *wm, int B, int H, int W, void *dx, cudaStream_t st)
+{
+    constexpr uint32_t smem = dg8_smem_bytes(K2);
+    RB_CUDA(cudaFuncSetAttribute(dgrad_cin8_kernel<K2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const long long chunks = (long long)B * H * ((W + DG8_PX - 1) / DG8_PX);
+    long long per_sm = (200u * 1024u) / smem;              // CTAs that fit one SM's shared memory
+    if (per_sm > 8) per_sm = 8;
+    long long grid = per_sm * num_sms();
+    if (grid > chunks) grid = chunks;
+    dgrad_cin8_kernel<K2><<<(unsigned)grid, DG8_THREADS, smem, st>>>((const __nv_bfloat16 *)dfm, wf, wm, B, H, W, (__nv_bfloat16 *)dx);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 }  // namespace rb
@@ -256,12 +349,14 @@ int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int 
 {
     RB_CHECK_ARG(dfm && x && dwf && dwm, "conv3x3_wgrad: null pointer");
     RB_CHECK_ARG(B >= 1 && H >= 1 && W >= 1, "conv3x3_wgrad: bad shape");
-    RB_CHECK_ARG(Cout % 32 == 0 && Cin % 32 == 0 && Cout > 0 && Cin > 0 && (Cout <= 64 || Cout % 64 == 0),
-                 "conv3x3_wgrad: Cin must be a multiple of 32 and Cout 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    RB_CHECK_ARG((Cin == 8 || Cin == 16 || (Cin % 32 == 0 && Cin > 0)) &&
+                     (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
+                 "conv3x3_wgrad: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin,
+                 Cout);
     RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x)) & 15) == 0,
                  "conv3x3_wgrad: tensors must be 16B aligned");
     const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
-    const int mb = 2 * Cout / WG_M, nb = Cin / WG_N;
+    const int mb = (2 * Cout + WG_M - 1) / WG_M, nb = (Cin + WG_N - 1) / WG_N;
     long long s = (2ll * num_sms() + mb * nb - 1) / (mb * nb);
     if (s > chunks) s = chunks;
     RB_CHECK_ARG(s <= 0x7FFFFFFF && nb <= 65535 && mb <= 65535, "conv3x3_wgrad: too large");
@@ -269,6 +364,19 @@ int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int 
         (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
     RB_LAUNCH_CHECK();
     return READ_OK;
+}
+
+int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, int B, int H, int W, int Cout, void *dx, void *stream)
+{
+    RB_CHECK_ARG(dfm && wf && wm && dx, "conv3x3_dgrad_cin8: null pointer");
+    RB_CHECK_ARG(B >= 1 && H >= 1 && W >= 1, "conv3x3_dgrad_cin8: bad shape");
+    RB_CHECK_ARG(Cout == 16 || Cout == 32 || Cout == 64, "conv3x3_dgrad_cin8: Cout must be 16, 32 or 64 (got %d)", Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0,
+                 "conv3x3_dgrad_cin8: tensors must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (Cout == 16) return launch_dgrad_cin8<32>(dfm, wf, wm, B, H, W, dx, st);
+    if (Cout == 32) return launch_dgrad_cin8<64>(dfm, wf, wm, B, H, W, dx, st);
+    return launch_dgrad_cin8<128>(dfm, wf, wm, B, H, W, dx, st);
 }
 
 }  // extern "C"

@@ -10,9 +10,11 @@ gated-conv kernel launches (wgmma tensor-core kernels for the dominant 3x3 layer
 There is no CPU path: inference on a CPU tensor raises.
 
 Training (autograd enabled) is routed through torch's own conv/batch-norm operators on the same parameters —
-a LIBRARY path (cuDNN), kept so that the reference's train.py keeps working.  ``train_precision = 'bf16'`` moves the 8
-residual block stacks (64 of the 99 convs) onto the wgmma kernels, forward and backward (read_b200/blocks.py); the
-default ``'fp32'`` keeps every layer on torch.
+a LIBRARY path (cuDNN), kept so that the reference's train.py keeps working.  ``train_precision = 'bf16'`` moves the 78
+gated 3x3 stride-1 convs onto the wgmma kernels, forward and backward (read_b200/blocks.py): the 8 residual block stacks
+(64 convs) and the 14 single convs feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1 and FAM*.merge.  The other 21
+convs (the 1x1 convs and the stride-2 3x3 / 4x4 convs), FAM's product and sum, the interpolations and the concats stay on
+torch.  The default ``'fp32'`` keeps every layer on torch.
 """
 import threading
 
@@ -100,7 +102,7 @@ class UNet(nn.Module):
             m = GatedConv(cin, cout, k, stride, elu)
             _attach(self, prefix, m)
         self.precision = 'bf16'          # 'bf16' (tensor cores) | 'fp32' (CUDA-core parity mode)
-        # training (autograd) path: 'fp32' = torch operators everywhere | 'bf16' = residual block stacks on the wgmma kernels
+        # training (autograd) path: 'fp32' = torch operators everywhere | 'bf16' = the 78 gated 3x3 stride-1 convs on the wgmma kernels
         self.train_precision = 'fp32'
         self.conv_impl = 'auto'
         self.use_graph = True
@@ -185,6 +187,12 @@ class UNet(nn.Module):
         if tp not in TRAIN_PRECISIONS:
             raise ValueError(f"read_b200.UNet: train_precision must be one of {TRAIN_PRECISIONS}, got {tp!r}")
 
+        def c3(name, t):
+            # the gated 3x3 stride-1 convs outside the blocks: feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge
+            if tp == 'bf16':
+                return blocks.gated_conv(self.get_submodule(name), t)
+            return c(name, t)
+
         def res(p, t):
             return c(p + ".main.1", c(p + ".main.0", t)) + t
 
@@ -196,19 +204,19 @@ class UNet(nn.Module):
             return t
 
         def scm(p, t):
-            y = c(p + ".main.3", c(p + ".main.2", c(p + ".main.1", c(p + ".main.0", t))))
+            y = c(p + ".main.3", c3(p + ".main.2", c(p + ".main.1", c3(p + ".main.0", t))))
             return c(p + ".conv", torch.cat([t, y], 1))
 
         def fam(p, a, b):
-            return a + c(p + ".merge", a * b)
+            return a + c3(p + ".merge", a * b)
 
         def aff(i, *xs):
-            return c(f"AFFs.{i}.conv.1", c(f"AFFs.{i}.conv.0", torch.cat(xs, 1)))
+            return c3(f"AFFs.{i}.conv.1", c(f"AFFs.{i}.conv.0", torch.cat(xs, 1)))
 
         up4 = lambda t: F.interpolate(t, scale_factor=4, mode='bilinear', align_corners=False)
         nn_ = lambda t, s: F.interpolate(t, scale_factor=s)
         z2, z4, z8 = scm("SCM2", x_2), scm("SCM1", x_4), scm("SCM0", x_8)
-        res1 = blk("Encoder.0", c("feat_extract.0", x))
+        res1 = blk("Encoder.0", c3("feat_extract.0", x))
         res2 = blk("Encoder.1", fam("FAM2", c("feat_extract.1", res1), z2))
         res3 = blk("Encoder.2", fam("FAM1", c("feat_extract.2", res2), z4))
         z = blk("Encoder.3", fam("FAM0", c("feat_extract.6", res3), z8))
@@ -219,4 +227,4 @@ class UNet(nn.Module):
         z = blk("Decoder.1", c("Convs.0", torch.cat([up4(c("feat_extract.7", z)), r3], 1)))
         z = blk("Decoder.2", c("Convs.1", torch.cat([up4(c("feat_extract.3", z)), r2], 1)))
         z = blk("Decoder.3", c("Convs.2", torch.cat([up4(c("feat_extract.4", z)), r1], 1)))
-        return c("feat_extract.5", z)
+        return c3("feat_extract.5", z)

@@ -3,7 +3,10 @@ the net, sparse RMSprop on the descriptors) with the net's residual block stacks
 bf16 (wgmma kernels, UNet.train_precision = 'bf16'), alternating in one process so that clock drift hits both alike.
    python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--out result.json]
 Prints the card's name and power limit, per precision the step time and the share of the net's forward + backward in it, the time
-to re-pack the 64 block convs' filters (done on every bf16 step), and per stack shape the time of each backward kernel."""
+to re-pack the 64 block convs' filters (done on every bf16 step), per stack shape the time of each backward kernel, the same for
+the new shapes of the 14 single gated 3x3 convs (8-channel inputs, the RGB conv padded to C = 16) with the 8-channel input gradient
+timed against the alternative of zero-padding the input and filters to 32 channels, and the forward + backward time of those 14
+convs at their C5 shapes in each precision."""
 import argparse
 import json
 import os
@@ -168,9 +171,91 @@ def main():
         row["wgrad_gbs"] = row["wgrad_min_bytes"] / (row["wgrad_us"] * 1e-6) / 1e9
         kern.append(row)
 
+    # the new shapes of the 14 single convs at C5: (layer, Cin, C as launched, ELU, resolution)
+    single = []
+    for name, cin, C, elu, S in (("feat_extract.0", 8, 32, True, 256), ("feat_extract.5", 32, 16, False, 256),
+                                 ("SCM2.main.0", 8, 16, True, 128), ("SCM1.main.0", 8, 32, True, 64), ("SCM0.main.0", 8, 64, True, 32)):
+        m = net.get_submodule(name)
+        fc = blocks.FoldedConv(m, *blocks.stack_params([m]), cout=C)
+        x = torch.rand((BC, S, S, cin), device=dev).bfloat16()
+        dy = torch.randn((BC, S, S, C), device=dev).bfloat16()
+        fm = torch.empty((BC, S, S, 2 * C), device=dev, dtype=torch.bfloat16)
+        dfm = torch.randn((BC, S, S, 2 * C), device=dev).bfloat16()
+        red = torch.zeros((4, C), device=dev)
+        dwf, dwm = torch.zeros_like(fc.wf), torch.zeros_like(fc.wm)
+        st = L.stream_ptr()
+        P = BC * S * S
+        fns = {
+            "raw_recompute": lambda: blocks._launch(lib, x, C, fc.w_tc, fc.par, fc.elu, L.OUT_RAW_NHWC, fm),
+            "gate_backward": lambda: L.check(lib.read_gate_backward(dy.data_ptr(), fm.data_ptr(), P, C, int(elu), fc.bf.data_ptr(),
+                                                                    fc.bm.data_ptr(), fc.scale.data_ptr(), fc.mean.data_ptr(),
+                                                                    fc.inv.data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
+                                                                    red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st)),
+            "wgrad": lambda: L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x.data_ptr(), BC, S, S, C, cin, dwf.data_ptr(),
+                                                            dwm.data_ptr(), st)),
+            "dgrad": lambda: blocks.dgrad(dfm, fc),
+        }
+        if cin == 8:
+            # the alternative: the input and the filters zero-padded to 32 channels, the TMA kernel's RAW dgrad (N = 32), and
+            # the padded input's copy that the weight gradient would then read
+            zpad = lambda t: torch.cat([t, t.new_zeros(t.shape[:1] + (24,) + t.shape[2:])], 1)
+            fc32 = blocks.FoldedConv(m, zpad(m.block['conv_f'].weight), m.block['conv_f'].bias, zpad(m.block['conv_m'].weight),
+                                     m.block['conv_m'].bias, m.block['norm'].weight, m.block['norm'].bias, cout=C)
+            fns["dgrad_padded32"] = lambda: blocks.dgrad(dfm, fc32)
+            fns["pad_input_to_32"] = lambda: F.pad(x, (0, 24))
+        row = {"layer": name, "Cin": cin, "C": C, "HxW": f"{S}x{S}", "B": BC}
+        for kname, fn in fns.items():
+            for _ in range(3):
+                fn()
+            torch.cuda.synchronize()
+            a, b = ev(), ev()
+            a.record()
+            for _ in range(20):
+                fn()
+            b.record()
+            torch.cuda.synchronize()
+            row[kname + "_us"] = a.elapsed_time(b) / 20 * 1e3
+        single.append(row)
+
+    # forward + backward of the 14 single convs at their C5 shapes, fp32 (torch / cuDNN) against bf16 (GatedConvFn)
+    shapes = [("feat_extract.0", 256), ("feat_extract.5", 256)] + \
+             [(f"SCM{i}.main.{j}", 32 << i) for i in range(3) for j in (0, 2)] + \
+             [(f"AFFs.{i}.conv.1", 256 >> i) for i in range(3)] + [(f"FAM{i}.merge", 32 << i) for i in range(3)]
+    assert len(shapes) == 14
+    singles_ms = {}
+    for tp in ("fp32", "bf16"):
+        case = []
+        for name, S in shapes:
+            m = runs[tp]["net"].get_submodule(name)
+            cin = m.block['conv_f'].weight.shape[1]
+            x = torch.rand((BC, cin, S, S), device=dev, requires_grad=True)
+            gy = torch.randn((BC, m.block['conv_f'].weight.shape[0], S, S), device=dev)
+            case.append((m, x, gy))
+
+        def run_all():
+            for m, x, gy in case:
+                y = blocks.gated_conv(m, x) if tp == "bf16" else m(x)
+                y.backward(gy)
+        for _ in range(3):
+            run_all()
+        torch.cuda.synchronize()
+        vals = []
+        for _ in range(args.rounds):
+            a, b = ev(), ev()
+            a.record()
+            for _ in range(5):
+                run_all()
+            b.record()
+            torch.cuda.synchronize()
+            vals.append(a.elapsed_time(b) / 5)
+        singles_ms[tp] = vals
+    for tp in runs:
+        runs[tp]["opt_net"].zero_grad(set_to_none=True)
+
     res = {"card": card(), "steps": args.steps, "rounds": args.rounds, "crops_per_step": BC, "size": f"{W}x{H}", "n_points": N,
            "ms_per_step": ms, "net_fwd_bwd_per_step": share, "first_loss": first_loss,
-           "bf16_filter_repack_ms_per_step": pack, "backward_kernels": kern}
+           "bf16_filter_repack_ms_per_step": pack, "backward_kernels": kern, "single_conv_kernels": single,
+           "single_convs_fwd_bwd_ms_per_step": singles_ms}
     for tp in runs:
         med = sorted(ms[tp])[len(ms[tp]) // 2]
         sh = sorted(share[tp], key=lambda x: x["share"])[len(share[tp]) // 2]
@@ -178,8 +263,10 @@ def main():
               f"of a {sh['step_ms']:.2f} ms profiled step = {100 * sh['share']:.1f} %")
     print(f"card: {res['card']}")
     print(f"first-step loss fp32 {first_loss['fp32']:.6f} bf16 {first_loss['bf16']:.6f}; filter re-pack {sorted(pack)[2]:.3f} ms/step")
-    for row in kern:
+    for row in kern + single:
         print(json.dumps(row))
+    for tp, v in singles_ms.items():
+        print(f"14 single 3x3 convs fwd+bwd at C5, {tp}: {sorted(v)[len(v) // 2]:.2f} ms/step (rounds {', '.join(f'{x:.2f}' for x in v)})")
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         json.dump(res, open(args.out, "w"), indent=1)
