@@ -219,8 +219,15 @@ int read_pack_weights_tc(const float *wf, const float *wm, int Cout, int Cin, in
  * 2*min(Cout, 64) columns, the conv_f half of each block first), its RAW output [B,H,W,Cin] is dX (plus the plan's residual).
  * Size: read_tc_weight_elems(Cin/2, 2*Cout, 3).  Cin % 32 == 0. */
 int read_pack_weights_tc_dgrad(const float *wf, const float *wm, int Cout, int Cin, void *out_bf16, void *stream);
+/* Filters of the input gradient of input channels c0 .. c0 + cn - 1 of a 1x1 conv pair (wf, wm: [Cout][Cin] f32): one source of a
+ * concat, or a 128-channel slice of a wider input.  Packed for a RAW 1x1 plan with Cin' = 2*Cout (its input is [df | dm] in the
+ * RAW column order) and Cout' = max(cn, 32) / 2: its RAW output [B,H,W,max(cn, 32)] is dX of those channels, the columns beyond
+ * cn zero (cn = 16 is padded to the plans' smallest N tile).  Size: read_tc_weight_elems(max(cn, 32) / 2, 2*Cout, 1).
+ * cn = 16, 32, 64 or 128; Cout = 16, 32, 48, 64 or a multiple of 64. */
+int read_pack_weights_tc_dgrad1x1(const float *wf, const float *wm, int Cout, int Cin, int c0, int cn, void *out_bf16, void *stream);
 /* 1 if the TMA-fed wgmma kernel supports this layer (stride-1 k x k / stride-2 3x3, 4x4 single source; 1x1 virtual concat of
- * identity / nearest-down sources; RAW 3x3 stride 1 over one source, optionally with a [B,H,W,2*Cout] residual), else 0. */
+ * identity / nearest-down sources; RAW 3x3 stride 1 over one source, optionally with a [B,H,W,2*Cout] residual; RAW stride-2
+ * 3x3 / 4x4 without a residual; RAW 1x1 at Cout 16 / 32 / 64), else 0. */
 int read_conv_tc_supported(const read_conv_desc *d);
 /* Same for the wgmma kernel with a gathered A operand (any stride / concat / resampling, bf16 activations);
  * it has its own weight packing. */
@@ -311,8 +318,10 @@ int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int
                        void *stream);
 
 /* ------------------------------------------------------------------------------------------
- * Backward of the gated 3x3 stride-1 convs (the residual blocks EBlock / DBlock, READ/models/unet.py:56-76, and the single convs
- * feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge), bf16 training with eval-mode BatchNorm (read_b200/blocks.py).
+ * Backward of the gated convs, bf16 training with eval-mode BatchNorm (read_b200/blocks.py): the 3x3 stride-1 convs (the residual
+ * blocks EBlock / DBlock, READ/models/unet.py:56-76, and the single convs feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1,
+ * FAM*.merge) and, under train_precision 'bf16_all', the 1x1 convs (Convs.*, AFFs.*.conv.0, SCM*.main.1 / .3, SCM*.conv) and the
+ * stride-2 3x3 / 4x4 convs (feat_extract.1 / .2 / .3 / .4 / .6 / .7).
  * Activations NHWC bf16; [f | m] rows are in the forward RAW output's column order (see read_pack_weights_tc_dgrad).  Reductions
  * ACCUMULATE (+=) into caller-zeroed fp32 buffers.
  *   read_gate_backward      : fm = pre-activation accumulators [P, 2C] (without bias), dy = gradient of the conv's output [P, C];
@@ -325,12 +334,23 @@ int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int
  *   read_conv3x3_dgrad_cin8 : input gradient dx [B,H,W,8] (bf16, overwritten) of a conv with Cin = 8 (the descriptor pyramid), from
  *                             dfm [B,H,W,2*Cout] and the fp32 filters wf / wm [Cout][8][3][3].  Cout = 16, 32 or 64.  The input
  *                             gradient of wider inputs is a RAW plan with read_pack_weights_tc_dgrad filters
+ *   read_conv_wgrad         : read_conv3x3_wgrad for k x k stride s: 1x1 and 3x3 stride 1, 3x3 and 4x4 stride 2 (pad 1, the input
+ *                             exactly twice the output: Hin == 2*Hout, Win == 2*Wout).  dwf / dwm [Cout][Cin][k][k], x [B,Hin,Win,Cin],
+ *                             dfm [B,Hout,Wout,2*Cout]; same channel rules
+ *   read_pack_weights_dgrad_s2 : the filters of read_conv_dgrad_s2: [k*k][Cin][2*Cout] bf16, the 2*Cout columns in the RAW order
+ *   read_conv_dgrad_s2      : input gradient dx [B,2*Hout,2*Wout,Cin] (bf16, overwritten) of a stride-2 pad-1 3x3 / 4x4 conv from
+ *                             dfm [B,Hout,Wout,2*Cout].  Cin a multiple of 32; Cout 16, 32, 64 or a multiple of 64.  The input
+ *                             gradient of a 1x1 conv is a RAW 1x1 plan with read_pack_weights_tc_dgrad1x1 filters
  * ---------------------------------------------------------------------------------------- */
 int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                        const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
                        float *dbias_m, float *dgamma, float *dbeta, void *stream);
 int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream);
 int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, int B, int H, int W, int Cout, void *dx, void *stream);
+int read_conv_wgrad(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
+                    int stride, float *dwf, float *dwm, void *stream);
+int read_pack_weights_dgrad_s2(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16, void *stream);
+int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wout, int Cout, int Cin, int k, void *dx, void *stream);
 
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);

@@ -95,10 +95,14 @@ _SIGS = {
     "read_pack_weights_tc_strided": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_pack_weights_tc_for": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "read_pack_weights_tc_dgrad": (c_int, [c_vp, c_vp, c_int, c_int, c_vp, c_vp]),
+    "read_pack_weights_tc_dgrad1x1": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_gate_backward": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                    c_vp]),
     "read_conv3x3_wgrad": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "read_conv3x3_dgrad_cin8": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "read_conv_wgrad": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "read_pack_weights_dgrad_s2": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp]),
+    "read_conv_dgrad_s2": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_conv_tc_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_conv_tcg_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_tcg_weight_elems": (c_i64, [c_int, c_int, c_int]),

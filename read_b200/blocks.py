@@ -1,7 +1,8 @@
 """bf16 training of the gated 3x3 stride-1 convs (READ/models/unet.py:22-53) on the wgmma kernels.
 
 ``UNet.train_precision = 'bf16'`` sends 78 of the net's 99 convs here; the other 21 (the 1x1 and stride-2 convs), the
-interpolations, concats and FAM products / sums stay on torch operators in the same autograd graph.
+interpolations, concats and FAM products / sums stay on torch operators in the same autograd graph.  ``'bf16_all'`` also sends
+those 21 convs here (``MultiSourceConvFn``, at the end of this file).
 * ``ResStackFn``: each of the 8 residual block stacks (Encoder.0-3, Decoder.0-3: 4 ResBlocks = 8 convs at constant C, 64 convs).
 * ``GatedConvFn``: one conv with an optional residual, for the 14 single convs feat_extract.0 (8 -> 32), feat_extract.5 (32 -> 3,
   the RGB output, run padded to C = 16), SCM*.main.0 (8 -> 16 / 32 / 64), SCM*.main.2, AFFs.*.conv.1 and FAM*.merge.
@@ -43,17 +44,27 @@ def fm_columns(C):
     return torch.where(r < half, blk * half + r, C + blk * half + r - half)
 
 
-def _launch(lib, src, cout, w_tc, par, elu, out_mode, out, residual=None):
-    """One 3x3 stride-1 launch of the TMA wgmma kernel over the NHWC bf16 tensor ``src``; par = (bias_f, bias_m, scale, shift)."""
-    B, H, W, cin = src.shape
+def _desc(srcs, cout, k=3, stride=1):
+    """Descriptor of a k x k conv (pad (k - 1) // 2) over the NHWC bf16 tensors ``srcs`` (a virtual concat when there are several)."""
+    B, H, W, _ = srcs[0].shape
     d = L.ReadConvDesc()
-    d.act_dtype, d.n_src = L.ACT_BF16, 1
-    d.src[0].ptr = src.data_ptr()
-    d.src[0].C, d.src[0].H, d.src[0].W = cin, H, W
-    d.src[0].mode, d.src[0].factor = L.SRC_IDENTITY, 1
-    d.B, d.Hin, d.Win, d.Cin = B, H, W, cin
-    d.Hout, d.Wout, d.Cout = H, W, cout
-    d.k, d.stride, d.pad, d.elu = 3, 1, 1, int(elu)
+    d.act_dtype, d.n_src = L.ACT_BF16, len(srcs)
+    for i, s in enumerate(srcs):
+        d.src[i].ptr = s.data_ptr()
+        d.src[i].C, d.src[i].H, d.src[i].W = s.shape[3], H, W
+        d.src[i].mode, d.src[i].factor = L.SRC_IDENTITY, 1
+    pad = (k - 1) // 2
+    d.B, d.Hin, d.Win, d.Cin = B, H, W, sum(s.shape[3] for s in srcs)
+    d.Hout, d.Wout, d.Cout = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, cout
+    d.k, d.stride, d.pad = k, stride, pad
+    return d
+
+
+def _launch(lib, src, cout, w_tc, par, elu, out_mode, out, residual=None, k=3, stride=1):
+    """One launch of the TMA wgmma kernel over the NHWC bf16 tensor ``src`` (or a list of them: a 1x1 conv's virtual concat), a
+    3x3 stride-1 conv unless ``k`` / ``stride`` say otherwise; par = (bias_f, bias_m, scale, shift)."""
+    d = _desc(src if isinstance(src, (list, tuple)) else [src], cout, k, stride)
+    d.elu = int(elu)
     d.bias_f, d.bias_m, d.bn_scale, d.bn_shift = (t.data_ptr() for t in par)
     d.w_tc, d.impl = w_tc.data_ptr(), L.CONV_TCGEN05
     d.out, d.out_mode = out.data_ptr(), out_mode
@@ -70,9 +81,12 @@ def _launch(lib, src, cout, w_tc, par, elu, out_mode, out, residual=None):
 class FoldedConv:
     """One GatedConv's live parameters for this step: folded eval-mode BatchNorm and the bf16 filters of the forward conv (also
     used for the RAW recompute) and of the input gradient.  ``cout`` > the conv's C pads it with zero filters, biases and BatchNorm
-    scale / shift (the RGB output conv, C = 3, runs as C = 16): the padded channels compute 0 and get 0 gradients."""
+    scale / shift (the RGB output conv, C = 3, runs as C = 16; SCM*.main.3, C = 56 / 120 / 248, as 64 / 128 / 256): the padded
+    channels compute 0 and get 0 gradients.  A 1x1 or stride-2 conv (k in {1, 3, 4}, stride in {1, 2}) packs its forward filters
+    for the launch over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks); its input-gradient filters are
+    packed in backward (dgrad_s2_filters, dgrad_1x1)."""
 
-    def __init__(self, mod, wf, bf, wm, bm, gamma, beta, cout=None):
+    def __init__(self, mod, wf, bf, wm, bm, gamma, beta, cout=None, srcs=None):
         lib, st = L.load(), L.stream_ptr()
         norm = mod.block['norm']
         cin = wf.shape[1]
@@ -84,9 +98,14 @@ class FoldedConv:
         scale = gamma.detach().float() * inv
         self.mean, self.inv = pad(norm.running_mean), pad(inv)
         self.scale, self.shift = pad(scale), pad(beta.detach().float() - norm.running_mean.detach().float() * scale)
-        self.w_tc = torch.empty(lib.read_tc_weight_elems(C, cin, 3), dtype=torch.bfloat16, device=wf.device)
-        L.check(lib.read_pack_weights_tc(self.wf.data_ptr(), self.wm.data_ptr(), C, cin, 3, self.w_tc.data_ptr(), st))
+        self.k, self.stride = mod.k, mod.stride
+        self.w_tc = torch.empty(lib.read_tc_weight_elems(C, cin, mod.k), dtype=torch.bfloat16, device=wf.device)
         self.w_dgrad = None                  # an 8-channel input's gradient kernel reads wf / wm itself
+        if (mod.k, mod.stride) != (3, 1):
+            L.check(lib.read_pack_weights_tc_for(ctypes.byref(_desc(srcs, C, mod.k, mod.stride)), self.wf.data_ptr(),
+                                                 self.wm.data_ptr(), self.w_tc.data_ptr(), st))
+            return
+        L.check(lib.read_pack_weights_tc(self.wf.data_ptr(), self.wm.data_ptr(), C, cin, 3, self.w_tc.data_ptr(), st))
         if cin != 8:
             self.w_dgrad = torch.empty(lib.read_tc_weight_elems(cin // 2, 2 * C, 3), dtype=torch.bfloat16, device=wf.device)
             L.check(lib.read_pack_weights_tc_dgrad(self.wf.data_ptr(), self.wm.data_ptr(), C, cin, self.w_dgrad.data_ptr(), st))
@@ -266,3 +285,153 @@ def gated_conv(mod, x, residual=None):
         raise ValueError(f"read_b200: gated_conv runs 3x3 stride-1 convs only (got k={mod.k}, stride={mod.stride})")
     _check_eval([mod])
     return GatedConvFn.apply(x, residual, mod, *stack_params([mod]))
+
+
+# ------------------------------------------------------------------ the 1x1 and stride-2 convs ('bf16_all')
+GEOMETRIES = ((1, 1), (3, 2), (4, 2))        # (k, stride) of the convs MultiSourceConvFn runs
+
+
+def padded_channels(c):
+    """The channel count a conv with C = c runs at: 16, 32, 64 or a multiple of 64 (the counts the gate backward, the weight
+    gradient and the RAW 1x1 plans take)."""
+    return 16 if c <= 16 else 32 if c <= 32 else 64 * ((c + 63) // 64)
+
+
+def recompute_fm(lib, srcs, c):
+    """[f | m] (RAW column order) of the FoldedConv ``c`` over the NHWC sources.  A RAW 1x1 plan takes at most 64 output channels
+    (one N tile), so a wider 1x1 conv is recomputed per 64-channel block with that block's filters: block b of the RAW order is
+    [f | m] of channels 64b .. 64b + 63."""
+    d = _desc(srcs, c.C, c.k, c.stride)
+    B, H, W = d.B, d.Hout, d.Wout
+    zeros = torch.zeros(c.C, dtype=torch.float32, device=srcs[0].device)  # a RAW launch reads no epilogue parameters
+    if c.k != 1 or c.C <= 64:
+        fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=srcs[0].device)
+        _launch(lib, srcs, c.C, c.w_tc, (zeros,) * 4, False, L.OUT_RAW_NHWC, fm, k=c.k, stride=c.stride)
+        return fm
+    blocks_ = []
+    w = torch.empty(lib.read_tc_weight_elems(64, d.Cin, 1), dtype=torch.bfloat16, device=srcs[0].device)
+    d64 = _desc(srcs, 64, 1, 1)
+    for b in range(c.C // 64):
+        L.check(lib.read_pack_weights_tc_for(ctypes.byref(d64), c.wf[64 * b: 64 * b + 64].data_ptr(),
+                                             c.wm[64 * b: 64 * b + 64].data_ptr(), w.data_ptr(), L.stream_ptr()))
+        out = torch.empty((B, H, W, 128), dtype=torch.bfloat16, device=srcs[0].device)
+        _launch(lib, srcs, 64, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
+        blocks_.append(out)
+    return torch.cat(blocks_, -1)
+
+
+def dgrad_s2_filters(c):
+    """The flipped-by-phase filters [k*k][Cin][2C] (bf16) of the stride-2 input-gradient kernel for the FoldedConv ``c``."""
+    lib = L.load()
+    cin = c.wf.shape[1]
+    w = torch.empty((c.k * c.k, cin, 2 * c.C), dtype=torch.bfloat16, device=c.wf.device)
+    L.check(lib.read_pack_weights_dgrad_s2(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, c.k, w.data_ptr(), L.stream_ptr()))
+    return w
+
+
+def dgrad_1x1(dfm, c, c0, cs):
+    """Input gradient [B,H,W,cs] (bf16) of input channels c0 .. c0 + cs - 1 of the 1x1 FoldedConv ``c``: RAW 1x1 plans over
+    [df | dm] with transposed filters, one per 128 channels (the plans' widest N tile); 16 channels run padded to 32."""
+    lib, st = L.load(), L.stream_ptr()
+    B, H, W, _ = dfm.shape
+    cin = c.wf.shape[1]
+    parts = []
+    for a in range(c0, c0 + cs, 128):
+        cn = min(128, c0 + cs - a)
+        n_out = max(cn, 32)
+        w = torch.empty(lib.read_tc_weight_elems(n_out // 2, 2 * c.C, 1), dtype=torch.bfloat16, device=dfm.device)
+        L.check(lib.read_pack_weights_tc_dgrad1x1(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, a, cn, w.data_ptr(), st))
+        out = torch.empty((B, H, W, n_out), dtype=torch.bfloat16, device=dfm.device)
+        zeros = torch.zeros(n_out // 2, dtype=torch.float32, device=dfm.device)
+        _launch(lib, dfm, n_out // 2, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
+        parts.append(out if cn == n_out else out[..., :cn])
+    return parts[0] if len(parts) == 1 else torch.cat(parts, -1)
+
+
+class MultiSourceConvFn(torch.autograd.Function):
+    """The gated 1x1 or stride-2 3x3 / 4x4 conv ``mod`` over the NCHW f32 tensors ``xs`` (a 1x1 conv reads several as a virtual
+    concat along channels); ``params`` = (conv_f.weight, conv_f.bias, conv_m.weight, conv_m.bias, norm.weight, norm.bias).  A conv
+    whose C is not 16, 32, 64 or a multiple of 64 runs padded (padded_channels)."""
+
+    @staticmethod
+    def forward(ctx, mod, n_src, *args):
+        xs, params = args[:n_src], args[n_src:]
+        _check_cuda(xs[0])
+        lib = L.load()
+        cout = params[0].shape[0]
+        ts = [ops.nchw_to_nhwc(x.detach().float().contiguous(), True) for x in xs]
+        conv = FoldedConv(mod, *params, cout=padded_channels(cout), srcs=ts)
+        d = _desc(ts, conv.C, mod.k, mod.stride)
+        y = torch.empty((d.B, d.Hout, d.Wout, conv.C), dtype=torch.bfloat16, device=ts[0].device)
+        _launch(lib, ts, conv.C, conv.w_tc, conv.par, conv.elu, L.OUT_NHWC, y, k=mod.k, stride=mod.stride)
+        ctx.conv, ctx.cout, ctx.n_src = conv, cout, n_src
+        ctx.save_for_backward(*ts, *params)            # the parameters: an in-place update before backward raises
+        y = ops.nhwc_to_nchw(y)
+        return y if cout == conv.C else y[:, :cout].contiguous()
+
+    @staticmethod
+    def backward(ctx, gout):
+        lib, st = L.load(), L.stream_ptr()
+        n_src, c, cout = ctx.n_src, ctx.conv, ctx.cout
+        ts = ctx.saved_tensors[:n_src]
+        need = ctx.needs_input_grad[2:]                                    # the sources, then the 6 parameters
+        C, dev = c.C, ts[0].device
+        B, Hin, Win, _ = ts[0].shape
+        gp = gout.float()
+        if cout < C:
+            gp = torch.cat([gp, gp.new_zeros((B, C - cout) + tuple(gp.shape[2:]))], 1)  # the padded channels' gradient is 0
+        g = ops.nchw_to_nhwc(gp.contiguous(), True)
+        Hout, Wout = g.shape[1], g.shape[2]
+        fm = recompute_fm(lib, ts, c)
+        dfm = torch.empty_like(fm)
+        red = torch.zeros((4, C), dtype=torch.float32, device=dev)        # dbias_f, dbias_m, dgamma, dbeta
+        L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), B * Hout * Wout, C, int(c.elu), c.bf.data_ptr(),
+                                       c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
+                                       red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
+        del fm
+        dwf = dwm = None
+        if need[n_src] or need[n_src + 2]:                                 # not for a frozen net
+            kk = (c.k, c.k)
+            dws = [(torch.zeros((C, t.shape[3]) + kk, device=dev), torch.zeros((C, t.shape[3]) + kk, device=dev)) for t in ts]
+            for t, (wf_s, wm_s) in zip(ts, dws):
+                L.check(lib.read_conv_wgrad(dfm.data_ptr(), t.data_ptr(), B, Hin, Win, Hout, Wout, C, t.shape[3], c.k, c.stride,
+                                            wf_s.data_ptr(), wm_s.data_ptr(), st))
+            dwf = torch.cat([w[0] for w in dws], 1) if n_src > 1 else dws[0][0]
+            dwm = torch.cat([w[1] for w in dws], 1) if n_src > 1 else dws[0][1]
+        dxs = [None] * n_src
+        c0 = 0
+        for i, t in enumerate(ts):
+            cs = t.shape[3]
+            if need[i]:
+                if c.stride == 2:
+                    dx = torch.empty_like(t)
+                    L.check(lib.read_conv_dgrad_s2(dfm.data_ptr(), dgrad_s2_filters(c).data_ptr(), B, Hout, Wout, C, cs, c.k,
+                                                   dx.data_ptr(), st))
+                else:
+                    dx = dgrad_1x1(dfm, c, c0, cs)
+                dxs[i] = ops.nhwc_to_nchw(dx.contiguous())
+            c0 += cs
+        grads = [dwf, red[0], dwm, red[1], red[2], red[3]]
+        grads = [gr[:cout] if gr is not None and need[n_src + j] else None for j, gr in enumerate(grads)]
+        return (None, None, *dxs, *grads)
+
+
+def gated_conv_srcs(mod, xs, name=None):
+    """bf16 forward of the gated 1x1 or stride-2 conv ``mod`` (a GatedConv) over the NCHW tensors ``xs`` on the wgmma kernels,
+    differentiable through MultiSourceConvFn.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels);
+    a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors."""
+    label = name or f"GatedConv(k={mod.k}, stride={mod.stride})"
+    xs = list(xs)
+    if (mod.k, mod.stride) not in GEOMETRIES:
+        raise ValueError(f"read_b200: {label}: gated_conv_srcs runs 1x1 and stride-2 3x3 / 4x4 convs (got k={mod.k}, "
+                         f"stride={mod.stride}); a 3x3 stride-1 conv goes through gated_conv")
+    if len(xs) > 1 and (mod.k != 1 or any(x.shape[1] % 32 for x in xs)):
+        raise ValueError(f"read_b200: {label}: only a 1x1 conv reads several sources, each a multiple of 32 channels "
+                         f"(got {[x.shape[1] for x in xs]})")
+    if len(xs) > 4:
+        raise ValueError(f"read_b200: {label}: at most 4 sources (got {len(xs)})")
+    if mod.stride == 2 and (xs[0].shape[2] % 2 or xs[0].shape[3] % 2):
+        raise ValueError(f"read_b200: {label}: a stride-2 conv needs an even input height and width (got "
+                         f"{xs[0].shape[2]}x{xs[0].shape[3]})")
+    _check_eval([mod])
+    return MultiSourceConvFn.apply(mod, len(xs), *xs, *stack_params([mod]))

@@ -6,6 +6,9 @@
 //                    (conv_tc.cu: read_pack_weights_tc_dgrad); the ResBlock skip enters through its residual operand.  An
 //                    8-channel input (the descriptor pyramid) has its own kernel in this file (dgrad_cin8_kernel)
 //   weight gradient  dW[2C][9][Cin] = sum over pixels of [df | dm]^T x im2col(x): the tensor-core kernel of this file
+// The 1x1 and stride-2 3x3 / 4x4 convs of train_precision 'bf16_all' (blocks.py: MultiSourceConvFn) use the same gate backward,
+// the weight-gradient kernel's other instances (read_conv_wgrad) and, for a stride-2 conv, the input-gradient kernel
+// dgrad_s2_kernel of this file; a 1x1 conv's input gradient is a RAW 1x1 plan of the TMA kernel.
 // Both kernels read [f | m] / [df | dm] rows in the column order of the forward RAW output: blocks of 2*half columns
 // (half = min(C, 64), the forward plan's n_tile / 2), the conv_f half of a block first.
 #include "common.cuh"
@@ -103,10 +106,18 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
 // Warps: 8 = 2 (32 columns each) x 4 (8 input channels each); a warp holds 2 x 9 m16n8 tiles = 72 accumulators per thread.
 // Narrow convs (Cin = 8 or 16: the descriptor pyramid; 2C = 32 columns: the RGB output conv padded to C = 16) run in one
 // partial block: its loads are zero-filled beyond Cin and beyond 2C, and only real (column, channel) pairs are stored.
-constexpr int WG_THREADS = 256, WG_PX = 32, WG_M = 64, WG_N = 32, WG_HALO = WG_PX + 2;
+// The kernel is a template over the filter size KS and the stride (pad (KS - 1) / 2 rounded up: 0 for 1x1, 1 otherwise):
+// 32 output pixels read the x halo of KR filter rows x (STRIDE * 31 + KS) input pixels, tap (ky, kx) of output pixel p sits at
+// halo pixel STRIDE * p + kx.  A CTA holds the taps of KR filter rows; a 4x4 filter is split into two groups of two rows over
+// blockIdx.z (16 taps would take 128 accumulators per thread), the other sizes keep all rows (KR = KS).
+constexpr int WG_THREADS = 256, WG_PX = 32, WG_M = 64, WG_N = 32;
 constexpr uint32_t WG_A_BYTES = WG_PX * WG_M * 2;                  // 128-byte rows
-constexpr uint32_t WG_X_BYTES = 3 * WG_HALO * WG_N * 2;            // 64-byte rows
-constexpr uint32_t WG_STAGE = WG_A_BYTES + WG_X_BYTES;             // a multiple of 128 bytes
+__host__ __device__ constexpr int wg_halo(int KS, int STRIDE) { return STRIDE * (WG_PX - 1) + KS; }
+__host__ __device__ constexpr uint32_t wg_x_bytes(int KS, int STRIDE, int KR)          // 64-byte rows, rounded up to 128 bytes
+{
+    return ((uint32_t)KR * wg_halo(KS, STRIDE) * WG_N * 2u + 127u) & ~127u;
+}
+__host__ __device__ constexpr uint32_t wg_stage(int KS, int STRIDE, int KR) { return WG_A_BYTES + wg_x_bytes(KS, STRIDE, KR); }
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
 {
@@ -132,12 +143,17 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4],
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// H, W: the output (= [df | dm]) size; the input x is [B][STRIDE * H][STRIDE * W][Cin] (the callers check Hin == STRIDE * Hout).
+template <int KS, int STRIDE, int KR>
 __global__ void __launch_bounds__(WG_THREADS)
 wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
              int half, float *__restrict__ dwf, float *__restrict__ dwm)
 {
-    __shared__ __align__(128) uint8_t sm[2 * WG_STAGE];
-    const int m0 = blockIdx.y * WG_M, n0 = blockIdx.z * WG_N;
+    constexpr int HALO = wg_halo(KS, STRIDE), TAPS = KR * KS, GROUPS = KS / KR, PAD = KS == 1 ? 0 : 1;
+    constexpr uint32_t STAGE = wg_stage(KS, STRIDE, KR);
+    __shared__ __align__(128) uint8_t sm[2 * STAGE];
+    const int ky0 = (blockIdx.z % GROUPS) * KR;
+    const int m0 = blockIdx.y * WG_M, n0 = (blockIdx.z / GROUPS) * WG_N;
     const int segs = (W + WG_PX - 1) / WG_PX;
     const long long chunks = (long long)B * H * segs;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -149,27 +165,27 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
         const int seg = (int)(ch % segs);
         const long long r = ch / segs;
         const int y = (int)(r % H), b = (int)(r / H), x0 = seg * WG_PX;
-        const uint32_t base = s0 + (uint32_t)st * WG_STAGE;
+        const uint32_t base = s0 + (uint32_t)st * STAGE;
         {   // [df | dm]: 32 pixels x 8 16-byte chunks, one per thread
             const int k = tid >> 3, q = tid & 7;
             const bool ok = x0 + k < W && m0 + 8 * q < twoC;
             const __nv_bfloat16 *src = ok ? dfm + (((long long)b * H + y) * W + x0 + k) * twoC + m0 + 8 * q : dfm;
             cp_async16(base + swz((uint32_t)k * 128u + 16u * q, 128u), src, ok);
         }
-        for (int i = tid; i < 3 * WG_HALO * 4; i += WG_THREADS) {   // x halo: rows y-1..y+1, pixels x0-1..x0+32, 4 chunks
+        for (int i = tid; i < KR * HALO * 4; i += WG_THREADS) {   // x halo: KR filter rows x HALO pixels, 4 chunks
             const int hp = i >> 2, q = i & 3;
-            const int gy = y + hp / WG_HALO - 1, gx = x0 + hp % WG_HALO - 1;
-            const bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W && n0 + 8 * q < Cin;
-            const __nv_bfloat16 *src = ok ? x + (((long long)b * H + gy) * W + gx) * Cin + n0 + 8 * q : x;
+            const int gy = STRIDE * y + ky0 + hp / HALO - PAD, gx = STRIDE * x0 + hp % HALO - PAD;
+            const bool ok = gy >= 0 && gy < STRIDE * H && gx >= 0 && gx < STRIDE * W && n0 + 8 * q < Cin;
+            const __nv_bfloat16 *src = ok ? x + (((long long)b * (STRIDE * H) + gy) * (STRIDE * W) + gx) * Cin + n0 + 8 * q : x;
             cp_async16(base + WG_A_BYTES + swz((uint32_t)hp * 64u + 16u * q, 64u), src, ok);
         }
     };
 
-    float acc[2][9][4];
+    float acc[2][TAPS][4];
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-        for (int t = 0; t < 9; ++t)
+        for (int t = 0; t < TAPS; ++t)
 #pragma unroll
             for (int i = 0; i < 4; ++i) acc[mi][t][i] = 0.f;
 
@@ -182,7 +198,7 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
         cp_async_commit();
         cp_async_wait<1>();
         __syncthreads();
-        const uint32_t sa = s0 + (uint32_t)st * WG_STAGE, sx = sa + WG_A_BYTES;
+        const uint32_t sa = s0 + (uint32_t)st * STAGE, sx = sa + WG_A_BYTES;
         // A fragments (columns x pixels) of the warp's two m16 tiles and the segment's two k16 steps, from the [pixel][column] tile
         uint32_t af[2][2][4];
 #pragma unroll
@@ -194,9 +210,9 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
                 ldmatrix_x4_trans(sa + swz((uint32_t)k * 128u + (uint32_t)col * 2u, 128u), af[mi][ks]);
             }
 #pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-            // B fragments of both k16 steps: matrix j = pixels 8j..8j+7 of the segment, read at halo (ky, pixel + kx)
-            const int hp = (tap / 3) * WG_HALO + tap % 3 + 8 * j + (lane & 7);
+        for (int tap = 0; tap < TAPS; ++tap) {
+            // B fragments of both k16 steps: matrix j = pixels 8j..8j+7 of the segment, read at halo (ky, STRIDE * pixel + kx)
+            const int hp = (tap / KS) * HALO + tap % KS + STRIDE * (8 * j + (lane & 7));
             uint32_t bfr[4];
             ldmatrix_x4_trans(sx + swz((uint32_t)hp * 64u + 16u * wq, 64u), bfr);
 #pragma unroll
@@ -221,10 +237,25 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
             if (col >= twoC || ci >= Cin) continue;
             const int rr = col % (2 * half);
             const int o = (col / (2 * half)) * half + rr % half;
-            float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * 9;
+            float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * (KS * KS) + ky0 * KS;
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
+            for (int tap = 0; tap < TAPS; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
         }
+}
+
+template <int KS, int STRIDE, int KR>
+static int launch_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm,
+                        cudaStream_t st)
+{
+    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
+    const int mb = (2 * Cout + WG_M - 1) / WG_M, nz = ((Cin + WG_N - 1) / WG_N) * (KS / KR);
+    long long s = (2ll * num_sms() + mb * nz - 1) / (mb * nz);
+    if (s > chunks) s = chunks;
+    RB_CHECK_ARG(s <= 0x7FFFFFFF && nz <= 65535 && mb <= 65535, "conv_wgrad: too large");
+    wgrad_kernel<KS, STRIDE, KR><<<dim3((unsigned)s, mb, nz), WG_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 // ------------------------------------------------------------------ input gradient of an 8-channel input
@@ -316,6 +347,157 @@ static int launch_dgrad_cin8(const void *dfm, const float *wf, const float *wm, 
     return READ_OK;
 }
 
+// ------------------------------------------------------------------ input gradient of a stride-2 conv
+// A stride-2 pad-1 conv (3x3 / 4x4) reads input pixel i = 2o - 1 + k with tap k of output pixel o, so its input gradient is a
+// transposed conv: input pixel i = 2a + p receives dfm[o] * w[k] for every k = 2(a - o) + p + 1 in [0, KS), i.e. from output
+// pixel o = a + (p + 1 - k) / 2 with k of the parity of p + 1 (p = 0: k = 1 [, 3]; p = 1: k = 0, 2).  Rows and columns are
+// independent, so per input row the kernel needs at most two rows of [df | dm] (slot s: filter row ky = 2s + 1 - p) and per
+// column phase at most two filter columns.  A CTA (4 warps) owns one input row, a 64-pixel segment of it (32 pixels of each
+// column phase) and 32 input channels: warp w computes the 16 pixels 16 * (w >> 1) + 0..15 of column phase w & 1 with
+// mma.sync m16n8k16 (bf16 in, fp32 accumulators), K = the 2C columns of [df | dm] in chunks of 32 times its <= 4 taps.  Per chunk
+// a stage holds the two 34-pixel [df | dm] rows and the row phase's <= 8 taps of the packed filters ([tap][Cin][2C] bf16,
+// read_pack_weights_dgrad_s2), loaded with cp.async (zero-filled outside the output image: the conv's zero padding), double
+// buffered across the CTA's sequence of (row segment, chunk) items.  The interleaved NHWC dx is written straight from the
+// accumulators.  64-byte shared-memory rows with the 64-byte swizzle: the ldmatrix reads touch 32 distinct banks.
+constexpr int DS_THREADS = 128, DS_PX = 64, DS_OX = DS_PX / 2 + 2, DS_K = 32, DS_N = 32;
+constexpr uint32_t DS_A_BYTES = 2u * DS_OX * DS_K * 2u;             // two [df | dm] rows
+constexpr uint32_t DS_B_BYTES = 8u * DS_N * DS_K * 2u;              // <= 2 filter rows x 4 filter columns
+constexpr uint32_t DS_STAGE = DS_A_BYTES + DS_B_BYTES;
+
+template <int KS>
+__global__ void __launch_bounds__(DS_THREADS)
+dgrad_s2_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ wt, int B, int Ho, int Wo, int K2,
+                int Cin, __nv_bfloat16 *__restrict__ dx)
+{
+    __shared__ __align__(128) uint8_t sm[2 * DS_STAGE];
+    const int Hi = 2 * Ho, Wi = 2 * Wo;
+    const int n0 = blockIdx.y * DS_N;
+    const int segs = (Wi + DS_PX - 1) / DS_PX, kchunks = K2 / DS_K;
+    const long long rows = (long long)B * Hi * segs;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int px = warp & 1, grp = warp >> 1;
+    const uint32_t s0 = s_u32(sm);
+
+    auto load = [&](long long rw, int kc, int st) {
+        const int seg = (int)(rw % segs);
+        const long long r = rw / segs;
+        const int i = (int)(r % Hi), b = (int)(r / Hi);
+        const int py = i & 1, a = i >> 1, c0 = seg * (DS_PX / 2);
+        const uint32_t base = s0 + (uint32_t)st * DS_STAGE;
+        for (int q = tid; q < 2 * DS_OX * 4; q += DS_THREADS) {      // [df | dm] rows: slot s = filter row 2s + 1 - py
+            const int hp = q >> 2, ch = q & 3, s = hp / DS_OX, ox = c0 - 1 + hp % DS_OX;
+            const int ky = 2 * s + 1 - py, oy = a + (py + 1 - ky) / 2;
+            const bool ok = ky < KS && oy >= 0 && oy < Ho && ox >= 0 && ox < Wo;
+            const __nv_bfloat16 *src = ok ? dfm + (((long long)b * Ho + oy) * Wo + ox) * K2 + kc * DS_K + 8 * ch : dfm;
+            cp_async16(base + swz((uint32_t)hp * 64u + 16u * ch, 64u), src, ok);
+        }
+        for (int q = tid; q < 2 * KS * DS_N * 4; q += DS_THREADS) {  // filters: [slot s][kx][n][k]
+            const int row = q >> 2, ch = q & 3, t = row / DS_N, n = row % DS_N, ky = 2 * (t / KS) + 1 - py, kx = t % KS;
+            const bool ok = ky < KS;
+            const __nv_bfloat16 *src = ok ? wt + ((long long)(ky * KS + kx) * Cin + n0 + n) * K2 + kc * DS_K + 8 * ch : wt;
+            cp_async16(base + DS_A_BYTES + swz((uint32_t)row * 64u + 16u * ch, 64u), src, ok);
+        }
+    };
+
+    const int arow = (lane & 7) + 8 * ((lane >> 3) & 1);              // this lane's ldmatrix row of the A tile: pixel
+    const uint32_t a_k = (uint32_t)(lane >> 4) * 16u;
+    const int brow = (lane & 7) + 8 * (lane >> 4);                    // ... of the B tiles: input channel
+    const uint32_t b_k = (uint32_t)((lane >> 3) & 1) * 16u;
+    const int g = lane >> 2, t4 = lane & 3;
+    float acc[4][4];
+    long long rw = blockIdx.x;
+    int kc = 0, st = 0;
+    if (rw < rows) load(rw, 0, 0);
+    cp_async_commit();
+    while (rw < rows) {
+        long long nrw = rw;
+        int nkc = kc + 1;
+        if (nkc == kchunks) { nkc = 0; nrw += gridDim.x; }
+        if (nrw < rows) load(nrw, nkc, st ^ 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        if (kc == 0) {
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
+        }
+        const long long r = rw / segs;
+        const int py = (int)(r % Hi) & 1;
+        const uint32_t sa = s0 + (uint32_t)st * DS_STAGE, sb = sa + DS_A_BYTES;
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            if (2 * s + 1 - py >= KS) continue;                           // 3x3, even rows: one filter row
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                const int kx = 2 * u + 1 - px;
+                if (kx >= KS) continue;                                   // 3x3, even columns: one filter column
+                const int hp = s * DS_OX + 16 * grp + 1 + (px + 1 - kx) / 2 + arow;     // dfm pixel c + (px + 1 - kx) / 2
+                const uint32_t bt = sb + (uint32_t)(s * KS + kx) * DS_N * 64u;
+#pragma unroll
+                for (int ks = 0; ks < DS_K / 16; ++ks) {
+                    uint32_t af[4];
+                    ldmatrix_x4(sa + swz((uint32_t)hp * 64u + 32u * ks + a_k, 64u), af);
+#pragma unroll
+                    for (int np = 0; np < 2; ++np) {
+                        uint32_t bf[4];
+                        ldmatrix_x4(bt + swz((uint32_t)(16 * np + brow) * 64u + 32u * ks + b_k, 64u), bf);
+                        mma_16816(acc[2 * np], af, bf[0], bf[1]);
+                        mma_16816(acc[2 * np + 1], af, bf[2], bf[3]);
+                    }
+                }
+            }
+        }
+        if (kc == kchunks - 1) {
+            // accumulator rows g, g + 8 = the warp's pixels, columns 2t, 2t + 1 = input channels of an n8 tile
+            const int seg = (int)(rw % segs), i = (int)(r % Hi), b = (int)(r / Hi);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int j = seg * DS_PX + 2 * (16 * grp + g + 8 * h) + px;
+                if (j >= Wi) continue;
+                __nv_bfloat16 *o = dx + (((long long)b * Hi + i) * Wi + j) * Cin + n0 + 2 * t4;
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+                    *reinterpret_cast<uint32_t *>(o + 8 * nt) = bf16x2_bits(acc[nt][2 * h], acc[nt][2 * h + 1]);
+            }
+        }
+        __syncthreads();
+        st ^= 1;
+        rw = nrw;
+        kc = nkc;
+    }
+    cp_async_wait<0>();
+}
+
+// wt[ky * KS + kx][n][c] = w(c)[o(c)][n][ky][kx] in bf16: c = a column of [df | dm] in the RAW column order (blocks of 2*half)
+__global__ void pack_dgrad_s2_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int Cin, int KS, int half,
+                                     __nv_bfloat16 *__restrict__ out)
+{
+    const long long total = (long long)KS * KS * Cin * 2 * Cout;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % (2 * Cout));
+        const long long r = i / (2 * Cout);
+        const int n = (int)(r % Cin), tap = (int)(r / Cin);
+        const int rr = c % (2 * half), o = (c / (2 * half)) * half + rr % half;
+        out[i] = __float2bfloat16_rn((rr >= half ? wm : wf)[((long long)o * Cin + n) * KS * KS + tap]);
+    }
+}
+
+template <int KS>
+static int launch_dgrad_s2(const void *dfm, const void *wt, int B, int Ho, int Wo, int Cout, int Cin, void *dx, cudaStream_t st)
+{
+    const long long rows = (long long)B * (2 * Ho) * ((2 * Wo + DS_PX - 1) / DS_PX);
+    const int nb = Cin / DS_N;
+    long long grid = (6ll * num_sms() + nb - 1) / nb;                 // 41.5 KB of shared memory: 5 CTAs per SM
+    if (grid > rows) grid = rows;
+    RB_CHECK_ARG(grid <= 0x7FFFFFFF && nb <= 65535, "conv_dgrad_s2: too large");
+    dgrad_s2_kernel<KS><<<dim3((unsigned)grid, nb), DS_THREADS, 0, st>>>((const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)wt, B, Ho,
+                                                                        Wo, 2 * Cout, Cin, (__nv_bfloat16 *)dx);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -360,7 +542,7 @@ int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int 
     long long s = (2ll * num_sms() + mb * nb - 1) / (mb * nb);
     if (s > chunks) s = chunks;
     RB_CHECK_ARG(s <= 0x7FFFFFFF && nb <= 65535 && mb <= 65535, "conv3x3_wgrad: too large");
-    wgrad_kernel<<<dim3((unsigned)s, mb, nb), WG_THREADS, 0, (cudaStream_t)stream>>>(
+    wgrad_kernel<3, 1, 3><<<dim3((unsigned)s, mb, nb), WG_THREADS, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
     RB_LAUNCH_CHECK();
     return READ_OK;
@@ -377,6 +559,61 @@ int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, i
     if (Cout == 16) return launch_dgrad_cin8<32>(dfm, wf, wm, B, H, W, dx, st);
     if (Cout == 32) return launch_dgrad_cin8<64>(dfm, wf, wm, B, H, W, dx, st);
     return launch_dgrad_cin8<128>(dfm, wf, wm, B, H, W, dx, st);
+}
+
+static bool wgrad_channels_ok(int Cout, int Cin)
+{
+    return (Cin == 8 || Cin == 16 || (Cin % 32 == 0 && Cin > 0)) && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0)));
+}
+
+int read_conv_wgrad(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
+                    int stride, float *dwf, float *dwm, void *stream)
+{
+    RB_CHECK_ARG(dfm && x && dwf && dwm, "conv_wgrad: null pointer");
+    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_wgrad: bad shape");
+    RB_CHECK_ARG((stride == 1 && (k == 1 || k == 3)) || (stride == 2 && (k == 3 || k == 4)),
+                 "conv_wgrad: k=%d stride=%d is not one of 1x1 / 3x3 stride 1, 3x3 / 4x4 stride 2", k, stride);
+    RB_CHECK_ARG(Hin == stride * Hout && Win == stride * Wout,
+                 "conv_wgrad: input %dx%d does not match output %dx%d at stride %d (stride 2 needs an even input)", Hin, Win, Hout,
+                 Wout, stride);
+    RB_CHECK_ARG(wgrad_channels_ok(Cout, Cin),
+                 "conv_wgrad: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x)) & 15) == 0,
+                 "conv_wgrad: tensors must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (k == 1) return launch_wgrad<1, 1, 1>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
+    if (stride == 1) return launch_wgrad<3, 1, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
+    if (k == 3) return launch_wgrad<3, 2, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
+    return launch_wgrad<4, 2, 2>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
+}
+
+int read_pack_weights_dgrad_s2(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16, void *stream)
+{
+    RB_CHECK_ARG(wf && wm && out_bf16, "pack_dgrad_s2: null pointer");
+    RB_CHECK_ARG(k == 3 || k == 4, "pack_dgrad_s2: k must be 3 or 4 (got %d)", k);
+    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
+                 "pack_dgrad_s2: Cin must be a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    const long long total = (long long)k * k * Cin * 2 * Cout;
+    long long blocks = (total + 255) / 256;
+    if (blocks > 65535) blocks = 65535;
+    pack_dgrad_s2_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, k, Cout < 64 ? Cout : 64,
+                                                                             (__nv_bfloat16 *)out_bf16);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wout, int Cout, int Cin, int k, void *dx, void *stream)
+{
+    RB_CHECK_ARG(dfm && wt && dx, "conv_dgrad_s2: null pointer");
+    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_dgrad_s2: bad shape");
+    RB_CHECK_ARG(k == 3 || k == 4, "conv_dgrad_s2: k must be 3 or 4 (got %d)", k);
+    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
+                 "conv_dgrad_s2: Cin must be a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(wt) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0,
+                 "conv_dgrad_s2: tensors must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (k == 3) return launch_dgrad_s2<3>(dfm, wt, B, Hout, Wout, Cout, Cin, dx, st);
+    return launch_dgrad_s2<4>(dfm, wt, B, Hout, Wout, Cout, Cin, dx, st);
 }
 
 }  // extern "C"

@@ -435,25 +435,27 @@ __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__rest
 // Input gradient of a stride-1 3x3 conv pair (conv_f, conv_m: [Cout][Cin][3][3]) as a RAW plan of the same kernel: a 3x3 conv of
 // [df | dm] (2*Cout channels, in the column order of the forward RAW output: blocks of n_tile_f columns, conv_f half then conv_m
 // half) with the filters flipped in space and transposed, dX[n] = sum_{tap, c} dfm[c] * w[o(c)][n][2-ky][2-kx].  The plan's N
-// columns are the Cin input channels in order, so its RAW output is dX itself.
-__global__ void pack_tc_dgrad_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int Cin, int half_f,
-                                     int cin_blk, int kchunks, __nv_bfloat16 *__restrict__ out)
+// columns are the Cin input channels in order, so its RAW output is dX itself.  k = 1 packs the input gradient of the input
+// channels c0 .. c0 + cn - 1 of a 1x1 conv (one source of a concat) as a RAW 1x1 plan with n_out >= cn columns, the columns
+// beyond cn zero filters.
+__global__ void pack_tc_dgrad_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int Cin, int k, int half_f,
+                                     int cin_blk, int kchunks, int c0, int cn, int n_out, __nv_bfloat16 *__restrict__ out)
 {
-    const long long total = 9ll * kchunks * Cin * cin_blk;
+    const long long total = (long long)k * k * kchunks * n_out * cin_blk;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         const int kk = (int)(i % cin_blk);
         long long r = i / cin_blk;
-        const int n = (int)(r % Cin);
-        r /= Cin;
+        const int n = (int)(r % n_out);
+        r /= n_out;
         const int kc = (int)(r % kchunks);
         const int tap = (int)(r / kchunks);
         const int c = kc * cin_blk + kk;                         // column of [df | dm]
         const int rr = c % (2 * half_f);
         const int o = (c / (2 * half_f)) * half_f + rr % half_f;
         const float *w = rr >= half_f ? wm : wf;
-        const int ky = 2 - tap / 3, kx = 2 - tap % 3;
-        out[i] = __float2bfloat16_rn(c < 2 * Cout ? w[(((long long)o * Cin + n) * 3 + ky) * 3 + kx] : 0.f);
+        const int ky = k - 1 - tap / k, kx = k - 1 - tap % k;
+        out[i] = __float2bfloat16_rn(c < 2 * Cout && n < cn ? w[(((long long)o * Cin + c0 + n) * k + ky) * k + kx] : 0.f);
     }
 }
 
@@ -529,10 +531,14 @@ bool tc_supported(const read_conv_desc &d)
     } else if (d.out_mode != READ_OUT_NHWC && d.out_mode != READ_OUT_RAW_NHWC) {
         return false;
     }
-    if (d.out_mode == READ_OUT_RAW_NHWC && d.k == 3) {
+    if (d.out_mode == READ_OUT_RAW_NHWC && d.k == 3 && d.stride == 1) {
         // accumulators of a 3x3 stride-1 conv over one tensor, optionally plus a residual of the output's [B, H, W, 2*Cout]
         // shape: the training path's recomputed [f | m] and ResBlock input gradients (read_b200/blocks.py)
-        if (d.stride != 1 || d.n_src != 1 || d.addin != nullptr || d.out2 != nullptr) return false;
+        if (d.n_src != 1 || d.addin != nullptr || d.out2 != nullptr) return false;
+        if ((long long)d.B * d.Hout * d.Wout * 2 * d.Cout >= (1ll << 31)) return false;
+    } else if (d.out_mode == READ_OUT_RAW_NHWC && d.stride == 2) {
+        // the recomputed [f | m] of a stride-2 3x3 / 4x4 conv (bf16 training): no epilogue operands
+        if (d.residual != nullptr || d.addin != nullptr || d.out2 != nullptr) return false;
         if ((long long)d.B * d.Hout * d.Wout * 2 * d.Cout >= (1ll << 31)) return false;
     } else if (d.out_mode == READ_OUT_RAW_NHWC || d.addin != nullptr) {
         // terms of a 1x1 conv over a multi-resolution concat: served by the lean epilogue (Cout 16 / 32 / 64)
@@ -864,8 +870,29 @@ int read_pack_weights_tc_dgrad(const float *wf, const float *wm, int Cout, int C
     const long long total = 9ll * gd.kchunks * gd.cin_blk * Cin;
     long long blocks = (total + 255) / 256;
     if (blocks > 65535) blocks = 65535;
-    pack_tc_dgrad_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, gf.n_tile / 2, gd.cin_blk,
-                                                                             gd.kchunks, (__nv_bfloat16 *)out_bf16);
+    pack_tc_dgrad_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, 3, gf.n_tile / 2, gd.cin_blk,
+                                                                             gd.kchunks, 0, Cin, Cin, (__nv_bfloat16 *)out_bf16);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_pack_weights_tc_dgrad1x1(const float *wf, const float *wm, int Cout, int Cin, int c0, int cn, void *out_bf16, void *stream)
+{
+    TcGeom gd;
+    RB_CHECK_ARG(wf && wm && out_bf16, "pack_tc_dgrad1x1: null pointer");
+    RB_CHECK_ARG(Cout % 16 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0),
+                 "pack_tc_dgrad1x1: Cout must be 16, 32, 48, 64 or a multiple of 64 (got %d)", Cout);
+    RB_CHECK_ARG((cn == 16 || cn == 32 || cn == 64 || cn == 128) && c0 >= 0 && c0 + cn <= Cin,
+                 "pack_tc_dgrad1x1: input channels %d..%d of %d: the slice must lie in the input and hold 16, 32, 64 or 128 channels",
+                 c0, c0 + cn - 1, Cin);
+    const int n_out = cn < 32 ? 32 : cn;                  // N = 16 is below the RAW plans' smallest N tile: zero filters pad it
+    RB_CHECK_ARG(tc_geom(2 * Cout, n_out / 2, 1, &gd) && gd.n_tiles == 1, "pack_tc_dgrad1x1: unsupported channel counts %d -> %d",
+                 Cin, Cout);
+    const long long total = (long long)gd.kchunks * gd.cin_blk * n_out;
+    long long blocks = (total + 255) / 256;
+    if (blocks > 65535) blocks = 65535;
+    pack_tc_dgrad_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, 1, Cout < 64 ? Cout : 64, gd.cin_blk,
+                                                                             gd.kchunks, c0, cn, n_out, (__nv_bfloat16 *)out_bf16);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

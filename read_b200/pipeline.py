@@ -44,8 +44,9 @@ _CLI = (
     ('--texture_activation', dict(type=str, default='none'), True),
     ('--n_points', dict(type=int, default=0, help='this is for inference'), True),
     ('--dense_texture_optimizer', dict(action='store_true', help='torch.optim.RMSprop over all points instead of the sparse kernel'), False),
-    ('--net_train_precision', dict(type=str, default='fp32', choices=['fp32', 'bf16'],
-                                   help="bf16: train the net's residual blocks on the wgmma kernels (UNet.train_precision)"), False),
+    ('--net_train_precision', dict(type=str, default='fp32', choices=['fp32', 'bf16', 'bf16_all'],
+                                   help="bf16: train the net's 3x3 stride-1 convs on the wgmma kernels; bf16_all: every conv "
+                                        "(UNet.train_precision)"), False),
 )
 
 

@@ -14,7 +14,9 @@ a LIBRARY path (cuDNN), kept so that the reference's train.py keeps working.  ``
 gated 3x3 stride-1 convs onto the wgmma kernels, forward and backward (read_b200/blocks.py): the 8 residual block stacks
 (64 convs) and the 14 single convs feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1 and FAM*.merge.  The other 21
 convs (the 1x1 convs and the stride-2 3x3 / 4x4 convs), FAM's product and sum, the interpolations and the concats stay on
-torch.  The default ``'fp32'`` keeps every layer on torch.
+torch.  ``'bf16_all'`` also moves those 21 convs onto the wgmma kernels (blocks.gated_conv_srcs), so every conv of the net trains
+there; FAM's product and sum, the interpolations, the concats that include an 8-channel source, the loss and the optimizers stay
+on torch.  The default ``'fp32'`` keeps every layer on torch.
 """
 import threading
 
@@ -25,7 +27,7 @@ import torch.nn.functional as F
 from . import blocks
 from .engine import UNetEngine
 
-TRAIN_PRECISIONS = ('fp32', 'bf16')
+TRAIN_PRECISIONS = ('fp32', 'bf16', 'bf16_all')
 
 
 def layer_table(base=32, num_res=4):
@@ -103,6 +105,7 @@ class UNet(nn.Module):
             _attach(self, prefix, m)
         self.precision = 'bf16'          # 'bf16' (tensor cores) | 'fp32' (CUDA-core parity mode)
         # training (autograd) path: 'fp32' = torch operators everywhere | 'bf16' = the 78 gated 3x3 stride-1 convs on the wgmma kernels
+        # | 'bf16_all' = all 99 convs on the wgmma kernels
         self.train_precision = 'fp32'
         self.conv_impl = 'auto'
         self.use_graph = True
@@ -187,44 +190,52 @@ class UNet(nn.Module):
         if tp not in TRAIN_PRECISIONS:
             raise ValueError(f"read_b200.UNet: train_precision must be one of {TRAIN_PRECISIONS}, got {tp!r}")
 
+        bf16 = tp in ('bf16', 'bf16_all')
+
         def c3(name, t):
             # the gated 3x3 stride-1 convs outside the blocks: feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge
-            if tp == 'bf16':
+            if bf16:
                 return blocks.gated_conv(self.get_submodule(name), t)
             return c(name, t)
+
+        def c1(name, *ts):
+            # the 1x1 and stride-2 convs; a 1x1 conv's sources are concatenated along channels (virtually under 'bf16_all')
+            if tp == 'bf16_all':
+                return blocks.gated_conv_srcs(self.get_submodule(name), ts, name)
+            return c(name, ts[0] if len(ts) == 1 else torch.cat(ts, 1))
 
         def res(p, t):
             return c(p + ".main.1", c(p + ".main.0", t)) + t
 
         def blk(p, t):
-            if tp == 'bf16':
+            if bf16:
                 return blocks.res_stack(self, p, t)
             for i in range(self.num_res):
                 t = res(f"{p}.layers.{i}", t)
             return t
 
         def scm(p, t):
-            y = c(p + ".main.3", c3(p + ".main.2", c(p + ".main.1", c3(p + ".main.0", t))))
-            return c(p + ".conv", torch.cat([t, y], 1))
+            y = c1(p + ".main.3", c3(p + ".main.2", c1(p + ".main.1", c3(p + ".main.0", t))))
+            return c1(p + ".conv", torch.cat([t, y], 1))      # torch's concat: the 8-channel source is not 32-channel granular
 
         def fam(p, a, b):
             return a + c3(p + ".merge", a * b)
 
         def aff(i, *xs):
-            return c3(f"AFFs.{i}.conv.1", c(f"AFFs.{i}.conv.0", torch.cat(xs, 1)))
+            return c3(f"AFFs.{i}.conv.1", c1(f"AFFs.{i}.conv.0", *xs))
 
         up4 = lambda t: F.interpolate(t, scale_factor=4, mode='bilinear', align_corners=False)
         nn_ = lambda t, s: F.interpolate(t, scale_factor=s)
         z2, z4, z8 = scm("SCM2", x_2), scm("SCM1", x_4), scm("SCM0", x_8)
         res1 = blk("Encoder.0", c3("feat_extract.0", x))
-        res2 = blk("Encoder.1", fam("FAM2", c("feat_extract.1", res1), z2))
-        res3 = blk("Encoder.2", fam("FAM1", c("feat_extract.2", res2), z4))
-        z = blk("Encoder.3", fam("FAM0", c("feat_extract.6", res3), z8))
+        res2 = blk("Encoder.1", fam("FAM2", c1("feat_extract.1", res1), z2))
+        res3 = blk("Encoder.2", fam("FAM1", c1("feat_extract.2", res2), z4))
+        z = blk("Encoder.3", fam("FAM0", c1("feat_extract.6", res3), z8))
         r1 = aff(0, res1, nn_(res2, 2), nn_(res3, 4), nn_(z, 8))
         r2 = aff(1, nn_(res1, 0.5), res2, nn_(res3, 2), nn_(z, 4))
         r3 = aff(2, nn_(res1, 0.25), nn_(res2, 0.5), res3, nn_(z, 2))
         z = blk("Decoder.0", z)
-        z = blk("Decoder.1", c("Convs.0", torch.cat([up4(c("feat_extract.7", z)), r3], 1)))
-        z = blk("Decoder.2", c("Convs.1", torch.cat([up4(c("feat_extract.3", z)), r2], 1)))
-        z = blk("Decoder.3", c("Convs.2", torch.cat([up4(c("feat_extract.4", z)), r1], 1)))
+        z = blk("Decoder.1", c1("Convs.0", up4(c1("feat_extract.7", z)), r3))
+        z = blk("Decoder.2", c1("Convs.1", up4(c1("feat_extract.3", z)), r2))
+        z = blk("Decoder.3", c1("Convs.2", up4(c1("feat_extract.4", z)), r1))
         return c3("feat_extract.5", z)

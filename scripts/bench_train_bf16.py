@@ -1,12 +1,15 @@
 """C5 training step (8 crops of 256x256 per step, 5M points, L1 loss, backward through the net and the descriptor gather, Adam on
-the net, sparse RMSprop on the descriptors) with the net's residual block stacks trained in fp32 (torch operators, cuDNN) and in
-bf16 (wgmma kernels, UNet.train_precision = 'bf16'), alternating in one process so that clock drift hits both alike.
+the net, sparse RMSprop on the descriptors) with the net trained in fp32 (torch operators, cuDNN), in bf16 (the 78 gated 3x3
+stride-1 convs on the wgmma kernels, UNet.train_precision = 'bf16') and in bf16_all (all 99 convs), alternating in one process
+so that clock drift hits all alike.
    python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--out result.json]
 Prints the card's name and power limit, per precision the step time and the share of the net's forward + backward in it, the time
 to re-pack the 64 block convs' filters (done on every bf16 step), per stack shape the time of each backward kernel, the same for
 the new shapes of the 14 single gated 3x3 convs (8-channel inputs, the RGB conv padded to C = 16) with the 8-channel input gradient
 timed against the alternative of zero-padding the input and filters to 32 channels, and the forward + backward time of those 14
-convs at their C5 shapes in each precision."""
+convs at their C5 shapes in each precision; then for the 21 1x1 / stride-2 convs of 'bf16_all' their forward + backward time at
+C5 in fp32 and in bf16_all, per conv the time of each backward piece (RAW recompute, gate backward, weight gradient, input
+gradient), and the activation bytes each precision saves for their backward."""
 import argparse
 import json
 import os
@@ -70,7 +73,7 @@ def main():
     keys = ["uv_1d_p1"] + [f"uv_1d_p1_ds{l}" for l in range(1, LEVELS)]
     ids0 = torch.zeros(BC, dtype=torch.long)
     sd = synth.synth_state_dict(synth.SEED)
-    runs = {tp: make_model(sd, tp, dev) for tp in ("fp32", "bf16")}
+    runs = {tp: make_model(sd, tp, dev) for tp in ("fp32", "bf16", "bf16_all")}
 
     def step(r, m, marks=None):
         e = [ev() for _ in range(4)] if marks is not None else None
@@ -252,21 +255,125 @@ def main():
     for tp in runs:
         runs[tp]["opt_net"].zero_grad(set_to_none=True)
 
+    # the 21 1x1 / stride-2 convs at C5: (layer, sources' (channels, resolution)); forward + backward in fp32 (torch, the concat
+    # on torch) against bf16_all (MultiSourceConvFn, a virtual concat), and per conv the backward's pieces
+    new_convs = [("feat_extract.1", [(32, 256)]), ("feat_extract.2", [(64, 128)]), ("feat_extract.6", [(128, 64)]),
+                 ("feat_extract.7", [(256, 32)]), ("feat_extract.3", [(128, 64)]), ("feat_extract.4", [(64, 128)]),
+                 ("Convs.0", [(128, 64)] * 2), ("Convs.1", [(64, 128)] * 2), ("Convs.2", [(32, 256)] * 2)] + \
+                [(f"AFFs.{i}.conv.0", [(c, 256 >> i) for c in (32, 64, 128, 256)]) for i in range(3)] + \
+                [(f"SCM{i}.{n}", [(c << (2 - i), 32 << i)]) for i in range(3) for n, c in (("main.1", 16), ("main.3", 32), ("conv", 64))]
+    assert len(new_convs) == 21
+    saved_bytes = {"fp32_conv_inputs": 0, "bf16_all_sources": 0}
+    new_ms, new_kern = {}, []
+    for tp in ("fp32", "bf16_all"):
+        case = []
+        for name, srcs in new_convs:
+            m = runs[tp]["net"].get_submodule(name)
+            xs = [torch.rand((BC, c, S, S), device=dev, requires_grad=True) for c, S in srcs]
+            S = srcs[0][1] // m.stride
+            gy = torch.randn((BC, m.block['conv_f'].weight.shape[0], S, S), device=dev)
+            case.append((name, m, xs, gy))
+            if tp == "fp32":
+                saved_bytes["fp32_conv_inputs"] += sum(x.numel() for x in xs) * 4
+                saved_bytes["bf16_all_sources"] += sum(x.numel() for x in xs) * 2
+
+        def run_all():
+            for name, m, xs, gy in case:
+                y = blocks.gated_conv_srcs(m, xs, name) if tp == "bf16_all" else m(torch.cat(xs, 1) if len(xs) > 1 else xs[0])
+                y.backward(gy)
+        for _ in range(3):
+            run_all()
+        torch.cuda.synchronize()
+        vals = []
+        for _ in range(args.rounds):
+            a, b = ev(), ev()
+            a.record()
+            for _ in range(5):
+                run_all()
+            b.record()
+            torch.cuda.synchronize()
+            vals.append(a.elapsed_time(b) / 5)
+        new_ms[tp] = vals
+        if tp != "bf16_all":
+            continue
+        for name, m, xs, gy in case:
+            ts = [ops.nchw_to_nhwc(x.detach(), True) for x in xs]
+            C = blocks.padded_channels(m.block['conv_f'].weight.shape[0])
+            fc = blocks.FoldedConv(m, *blocks.stack_params([m]), cout=C, srcs=ts)
+            fm = blocks.recompute_fm(lib, ts, fc)
+            B_, Ho, Wo, _ = fm.shape
+            Hi, Wi = ts[0].shape[1:3]
+            dy = torch.randn((B_, Ho, Wo, C), device=dev).bfloat16()
+            dfm = torch.randn_like(fm)
+            red = torch.zeros((4, C), device=dev)
+            dwf, dwm = torch.zeros_like(fc.wf), torch.zeros_like(fc.wm)
+            st = L.stream_ptr()
+            P = B_ * Ho * Wo
+
+            def wgrad():
+                for t in ts:
+                    L.check(lib.read_conv_wgrad(dfm.data_ptr(), t.data_ptr(), B_, Hi, Wi, Ho, Wo, C, t.shape[3], fc.k, fc.stride,
+                                                dwf.data_ptr(), dwm.data_ptr(), st))
+
+            def dgrad():
+                if fc.stride == 2:
+                    dx = torch.empty_like(ts[0])
+                    L.check(lib.read_conv_dgrad_s2(dfm.data_ptr(), blocks.dgrad_s2_filters(fc).data_ptr(), B_, Ho, Wo, C,
+                                                   ts[0].shape[3], fc.k, dx.data_ptr(), st))
+                    return
+                c0 = 0
+                for t in ts:
+                    blocks.dgrad_1x1(dfm, fc, c0, t.shape[3])
+                    c0 += t.shape[3]
+            fns = {
+                "raw_recompute": lambda: blocks.recompute_fm(lib, ts, fc),
+                "gate_backward": lambda: L.check(lib.read_gate_backward(dy.data_ptr(), fm.data_ptr(), P, C, int(fc.elu), fc.bf.data_ptr(),
+                                                                        fc.bm.data_ptr(), fc.scale.data_ptr(), fc.mean.data_ptr(),
+                                                                        fc.inv.data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
+                                                                        red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st)),
+                "wgrad": wgrad,
+                "dgrad": dgrad,
+            }
+            row = {"layer": name, "sources": [t.shape[3] for t in ts], "C": C, "k": fc.k, "stride": fc.stride,
+                   "in": f"{Hi}x{Wi}", "out": f"{Ho}x{Wo}", "B": BC}
+            for kname, fn in fns.items():
+                for _ in range(3):
+                    fn()
+                torch.cuda.synchronize()
+                a, b = ev(), ev()
+                a.record()
+                for _ in range(20):
+                    fn()
+                b.record()
+                torch.cuda.synchronize()
+                row[kname + "_us"] = a.elapsed_time(b) / 20 * 1e3
+            flops = 2.0 * 2 * C * fc.k * fc.k * sum(t.shape[3] for t in ts) * P     # one GEMM of the conv pair
+            row["wgrad_tflops"] = flops / (row["wgrad_us"] * 1e-6) / 1e12
+            row["dgrad_tflops"] = flops / (row["dgrad_us"] * 1e-6) / 1e12
+            new_kern.append(row)
+    for tp in runs:
+        runs[tp]["opt_net"].zero_grad(set_to_none=True)
+
     res = {"card": card(), "steps": args.steps, "rounds": args.rounds, "crops_per_step": BC, "size": f"{W}x{H}", "n_points": N,
            "ms_per_step": ms, "net_fwd_bwd_per_step": share, "first_loss": first_loss,
            "bf16_filter_repack_ms_per_step": pack, "backward_kernels": kern, "single_conv_kernels": single,
-           "single_convs_fwd_bwd_ms_per_step": singles_ms}
+           "single_convs_fwd_bwd_ms_per_step": singles_ms, "new_convs_fwd_bwd_ms_per_step": new_ms, "new_conv_kernels": new_kern,
+           "new_convs_saved_bytes_per_step": saved_bytes}
     for tp in runs:
         med = sorted(ms[tp])[len(ms[tp]) // 2]
         sh = sorted(share[tp], key=lambda x: x["share"])[len(share[tp]) // 2]
         print(f"{tp}: {med:.2f} ms/step (rounds {', '.join(f'{v:.2f}' for v in ms[tp])}), net fwd+bwd {sh['net_fwd_bwd_ms']:.2f} ms "
               f"of a {sh['step_ms']:.2f} ms profiled step = {100 * sh['share']:.1f} %")
     print(f"card: {res['card']}")
-    print(f"first-step loss fp32 {first_loss['fp32']:.6f} bf16 {first_loss['bf16']:.6f}; filter re-pack {sorted(pack)[2]:.3f} ms/step")
-    for row in kern + single:
+    print(f"first-step loss fp32 {first_loss['fp32']:.6f} bf16 {first_loss['bf16']:.6f} bf16_all {first_loss['bf16_all']:.6f}; "
+          f"filter re-pack {sorted(pack)[2]:.3f} ms/step")
+    for row in kern + single + new_kern:
         print(json.dumps(row))
     for tp, v in singles_ms.items():
         print(f"14 single 3x3 convs fwd+bwd at C5, {tp}: {sorted(v)[len(v) // 2]:.2f} ms/step (rounds {', '.join(f'{x:.2f}' for x in v)})")
+    for tp, v in new_ms.items():
+        print(f"21 1x1 / stride-2 convs fwd+bwd at C5, {tp}: {sorted(v)[len(v) // 2]:.2f} ms/step (rounds {', '.join(f'{x:.2f}' for x in v)})")
+    print(f"activations saved for the 21 convs' backward at C5: {saved_bytes}")
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         json.dump(res, open(args.out, "w"), indent=1)
