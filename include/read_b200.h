@@ -352,6 +352,35 @@ int read_conv_wgrad(const void *dfm, const void *x, int B, int Hin, int Win, int
 int read_pack_weights_dgrad_s2(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16, void *stream);
 int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wout, int Cout, int Cin, int k, void *dx, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Train-mode BatchNorm of the gated convs (read_b200/blocks.py, batch_stats=True), torch.nn.BatchNorm2d's semantics: the conv runs
+ * with an identity epilogue (bn_scale 1, bn_shift 0, no residual) and writes g [P, C] (NHWC bf16); then
+ *   read_bn_batch_stats     : per-channel mean and biased variance var of g over the P pixels; writes mean, inv_std = 1/sqrt(var+eps),
+ *                             var (optional, may be NULL), scale = gamma*inv_std, shift = beta - mean*scale, and updates in place
+ *                             running_mean = (1-momentum)*running_mean + momentum*mean and running_var likewise with the unbiased
+ *                             var*P/(P-1).  Channels >= n_real are padding (g == 0): scale = shift = 0 and no running update; gamma,
+ *                             beta, running_* have n_real entries.  workspace: read_bn_workspace_bytes(C) bytes, 16B aligned,
+ *                             uninitialised, used by one call at a time.  Deterministic run to run
+ *   read_bn_apply           : y = bf16(g*scale + shift [+ residual]); residual (optional) [P, C] bf16; y may be g
+ *   read_bn_backward_reduce : sum_dy += sum dy, sum_dy_xhat += sum dy*(g - mean)*inv_std (= dbeta, dgamma) with g recomputed from the
+ *                             RAW [f | m] and the biases (caller-zeroed fp32 [C])
+ *   read_gate_backward_batch_stats : read_gate_backward with the batch-statistics terms: dg = scale*(dy - sum_dy/P
+ *                             - xhat*sum_dy_xhat/P); writes dfm, accumulates dbias_f / dbias_m (dgamma / dbeta are the two sums)
+ * C = 16, 32, 64 or a multiple of 64 up to 256; pixels >= 2; activations 16B aligned.
+ * ---------------------------------------------------------------------------------------- */
+int64_t read_bn_workspace_bytes(int C);
+int read_bn_batch_stats(const void *g, int64_t pixels, int C, int n_real, const float *gamma, const float *beta, float eps,
+                        float momentum, float *running_mean, float *running_var, float *mean, float *inv_std, float *var,
+                        float *scale, float *shift, void *workspace, void *stream);
+int read_bn_apply(const void *g, int64_t pixels, int C, const float *scale, const float *shift, const void *residual, void *y,
+                  void *stream);
+int read_bn_backward_reduce(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                            const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat, void *stream);
+int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                   const float *bias_m, const float *bn_scale, const float *bn_mean, const float *bn_inv_std,
+                                   const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
+                                   void *stream);
+
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);
 

@@ -19,10 +19,19 @@ gradients; weight gradient (tensor-core kernel, fp32 atomics into the torch-layo
 input gradient = RAW launch of the TMA kernel over [df | dm] with flipped, transposed filters, the ResBlock skip added through its
 residual operand, or for an 8-channel input (the descriptor pyramid) the dedicated dgrad_cin8 kernel.
 
-BatchNorm is eval-mode (running statistics, as the reference trains: eval_in_train), folded into scale / shift like the inference
-engine.  Filters are re-packed from the live fp32 parameters on every call.
+BatchNorm is per conv, from the mode of that conv's norm at forward time:
+* eval mode (running statistics, as the reference trains with eval_in_train): folded into scale / shift like the inference engine,
+  the residual added in the conv's epilogue;
+* train mode (the reference's default training, the net in train()), with ``batch_stats=True``: torch.nn.BatchNorm2d's train-mode
+  semantics.  The conv launch writes g = A(f + b_f) * sigmoid(m + b_m) with an identity epilogue; csrc/bn_train.cu computes the
+  batch mean / variance over the B * H_out * W_out pixels, the folded scale / shift and the in-place running-statistics update on the
+  device, then y = g * scale + shift [+ residual].  Backward adds the terms through the statistics (read_bn_backward_reduce, then
+  read_gate_backward_batch_stats).  Without ``batch_stats`` a train-mode norm raises, as before.
+The packed bf16 filters are cached per module and weight version (_packed): an optimizer step re-packs them, repeated calls with
+the same weights (the per-item loop of training in train()) do not.
 """
 import ctypes
+import weakref
 
 import torch
 
@@ -78,41 +87,148 @@ def _launch(lib, src, cout, w_tc, par, elu, out_mode, out, residual=None, k=3, s
         lib.read_conv_plan_destroy(plan)
 
 
+# packed filters per GatedConv: module -> (key, dict of filters); see _packed
+_FILTERS = weakref.WeakKeyDictionary()
+cache_filters = True        # False: pack on every call (measurement of the cache, scripts/bench_train_bf16.py)
+
+
+def clear_filter_cache():
+    _FILTERS.clear()
+
+
+def filter_key(mod, wf, wm, C, srcs=None):
+    """What the packed filters of ``mod`` depend on: the identity, storage and in-place version of both weights (an optimizer step
+    bumps the version), the padded channel count and a concat's source channel split."""
+    return (id(wf), wf.data_ptr(), wf._version, id(wm), wm.data_ptr(), wm._version, C, str(wf.device),
+            None if srcs is None else tuple(s.shape[3] for s in srcs))
+
+
+def _packed(mod, wf, wm, C, srcs):
+    """The fp32 filters padded to C channels and the bf16 forward (and 3x3 input-gradient) filters of ``mod``, from the cache when
+    the weights are unchanged.  The dict also holds the filters backward packs lazily (dgrad_s2_filters, recompute_fm,
+    dgrad_1x1); entries are only ever added, and a new weight version starts a new dict, so a FoldedConv of an earlier forward
+    keeps the filters it was built with.  Writes that bypass the version counter (through ``.data``) are not seen."""
+    key = filter_key(mod, wf, wm, C, srcs)
+    ent = _FILTERS.get(mod) if cache_filters else None
+    if ent is not None and ent[0] == key:
+        return ent[1]
+    lib, st = L.load(), L.stream_ptr()
+    cin = wf.shape[1]
+    pad = lambda t: _pad_rows(t.detach().float(), C).contiguous()
+    pk = {'wf': pad(wf), 'wm': pad(wm), 'w_dgrad': None}       # an 8-channel input's gradient kernel reads wf / wm itself
+    pk['w_tc'] = torch.empty(lib.read_tc_weight_elems(C, cin, mod.k), dtype=torch.bfloat16, device=wf.device)
+    if (mod.k, mod.stride) != (3, 1):
+        L.check(lib.read_pack_weights_tc_for(ctypes.byref(_desc(srcs, C, mod.k, mod.stride)), pk['wf'].data_ptr(),
+                                             pk['wm'].data_ptr(), pk['w_tc'].data_ptr(), st))
+    else:
+        L.check(lib.read_pack_weights_tc(pk['wf'].data_ptr(), pk['wm'].data_ptr(), C, cin, 3, pk['w_tc'].data_ptr(), st))
+        if cin != 8:
+            pk['w_dgrad'] = torch.empty(lib.read_tc_weight_elems(cin // 2, 2 * C, 3), dtype=torch.bfloat16, device=wf.device)
+            L.check(lib.read_pack_weights_tc_dgrad(pk['wf'].data_ptr(), pk['wm'].data_ptr(), C, cin, pk['w_dgrad'].data_ptr(), st))
+    if (mod.k, mod.stride) != (3, 1):
+        # the backward's filters too, so that a backward packs nothing (its launches are the same on every call)
+        c = _Filters(pk, C, mod.k, mod.stride)
+        if mod.stride == 2:
+            dgrad_s2_filters(c)
+        else:
+            if C > 64:
+                _fm64_filters(lib, srcs, c)
+            c0 = 0
+            for s in srcs:
+                for a in range(c0, c0 + s.shape[3], 128):
+                    _dgrad1x1_filters(lib, c, a, min(128, c0 + s.shape[3] - a), wf.device)
+                c0 += s.shape[3]
+    if cache_filters:
+        _FILTERS[mod] = (key, pk)
+    return pk
+
+
+class _Filters:
+    """The attributes of a FoldedConv the filter packers read."""
+
+    def __init__(self, pk, C, k, stride):
+        self.pk, self.wf, self.wm, self.C, self.k, self.stride = pk, pk['wf'], pk['wm'], C, k, stride
+
+
 class FoldedConv:
-    """One GatedConv's live parameters for this step: folded eval-mode BatchNorm and the bf16 filters of the forward conv (also
-    used for the RAW recompute) and of the input gradient.  ``cout`` > the conv's C pads it with zero filters, biases and BatchNorm
-    scale / shift (the RGB output conv, C = 3, runs as C = 16; SCM*.main.3, C = 56 / 120 / 248, as 64 / 128 / 256): the padded
-    channels compute 0 and get 0 gradients.  A 1x1 or stride-2 conv (k in {1, 3, 4}, stride in {1, 2}) packs its forward filters
-    for the launch over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks); its input-gradient filters are
-    packed in backward (dgrad_s2_filters, dgrad_1x1)."""
+    """One GatedConv's live parameters for this step: its BatchNorm and the bf16 filters of the forward conv (also used for the RAW
+    recompute) and of the input gradient.  ``cout`` > the conv's C pads it with zero filters, biases and BatchNorm scale / shift
+    (the RGB output conv, C = 3, runs as C = 16; SCM*.main.3, C = 56 / 120 / 248, as 64 / 128 / 256): the padded channels compute
+    0 and get 0 gradients.  A 1x1 or stride-2 conv (k in {1, 3, 4}, stride in {1, 2}) packs its forward filters for the launch
+    over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks); its input-gradient filters are packed in
+    backward (dgrad_s2_filters, dgrad_1x1).
+    An eval-mode norm is folded into scale / shift from its running statistics.  A train-mode norm (``batch``) runs the forward
+    launch with the identity epilogue ``fwd_par``; mean / inv / scale / shift are then filled by bn_forward from the batch."""
 
     def __init__(self, mod, wf, bf, wm, bm, gamma, beta, cout=None, srcs=None):
-        lib, st = L.load(), L.stream_ptr()
         norm = mod.block['norm']
-        cin = wf.shape[1]
         C = cout or wf.shape[0]
         pad = lambda t: _pad_rows(t.detach().float(), C).contiguous()
         self.C, self.elu = C, bool(mod.elu)
-        self.wf, self.wm, self.bf, self.bm = pad(wf), pad(wm), pad(bf), pad(bm)
-        inv = torch.rsqrt(norm.running_var.detach().float() + norm.eps)
-        scale = gamma.detach().float() * inv
-        self.mean, self.inv = pad(norm.running_mean), pad(inv)
-        self.scale, self.shift = pad(scale), pad(beta.detach().float() - norm.running_mean.detach().float() * scale)
+        self.bf, self.bm = pad(bf), pad(bm)
         self.k, self.stride = mod.k, mod.stride
-        self.w_tc = torch.empty(lib.read_tc_weight_elems(C, cin, mod.k), dtype=torch.bfloat16, device=wf.device)
-        self.w_dgrad = None                  # an 8-channel input's gradient kernel reads wf / wm itself
-        if (mod.k, mod.stride) != (3, 1):
-            L.check(lib.read_pack_weights_tc_for(ctypes.byref(_desc(srcs, C, mod.k, mod.stride)), self.wf.data_ptr(),
-                                                 self.wm.data_ptr(), self.w_tc.data_ptr(), st))
-            return
-        L.check(lib.read_pack_weights_tc(self.wf.data_ptr(), self.wm.data_ptr(), C, cin, 3, self.w_tc.data_ptr(), st))
-        if cin != 8:
-            self.w_dgrad = torch.empty(lib.read_tc_weight_elems(cin // 2, 2 * C, 3), dtype=torch.bfloat16, device=wf.device)
-            L.check(lib.read_pack_weights_tc_dgrad(self.wf.data_ptr(), self.wm.data_ptr(), C, cin, self.w_dgrad.data_ptr(), st))
+        self.batch = norm.training
+        if self.batch:
+            dev = wf.device
+            self.norm, self.n_real = norm, wf.shape[0]
+            self.gamma, self.beta = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
+            self.mean, self.inv, self.scale, self.shift = torch.empty((4, C), dtype=torch.float32, device=dev).unbind(0)
+            self.fwd_par = (self.bf, self.bm, torch.ones(C, device=dev), torch.zeros(C, device=dev))
+        else:
+            inv = torch.rsqrt(norm.running_var.detach().float() + norm.eps)
+            scale = gamma.detach().float() * inv
+            self.mean, self.inv = pad(norm.running_mean), pad(inv)
+            self.scale, self.shift = pad(scale), pad(beta.detach().float() - norm.running_mean.detach().float() * scale)
+            self.fwd_par = self.par
+        self.pk = _packed(mod, wf, wm, C, srcs)
+        self.wf, self.wm, self.w_tc, self.w_dgrad = self.pk['wf'], self.pk['wm'], self.pk['w_tc'], self.pk['w_dgrad']
 
     @property
     def par(self):
         return (self.bf, self.bm, self.scale, self.shift)
+
+
+def bn_forward(lib, c, g, residual=None):
+    """Train-mode BatchNorm of the FoldedConv ``c`` over its identity-epilogue output ``g`` (NHWC bf16, C channels), in place:
+    batch statistics, running-statistics update and y = g * scale + shift [+ residual]."""
+    st, n = L.stream_ptr(), c.norm
+    P = g.numel() // c.C
+    ws = torch.empty(lib.read_bn_workspace_bytes(c.C), dtype=torch.uint8, device=g.device)
+    L.check(lib.read_bn_batch_stats(g.data_ptr(), P, c.C, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps, n.momentum,
+                                    n.running_mean.data_ptr(), n.running_var.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), None,
+                                    c.scale.data_ptr(), c.shift.data_ptr(), ws.data_ptr(), st))
+    n.num_batches_tracked.add_(1)              # torch's own op: bumps the version UNet._weights_version sums
+    L.check(lib.read_bn_apply(g.data_ptr(), P, c.C, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual), g.data_ptr(), st))
+
+
+def conv_forward(lib, src, c, out, residual=None):
+    """Forward of the FoldedConv ``c`` over ``src`` into ``out`` (NHWC bf16): one launch with the folded BatchNorm and the residual
+    in its epilogue, or for a train-mode norm the identity-epilogue launch followed by bn_forward."""
+    if not c.batch:
+        _launch(lib, src, c.C, c.w_tc, c.par, c.elu, L.OUT_NHWC, out, residual, k=c.k, stride=c.stride)
+        return
+    _launch(lib, src, c.C, c.w_tc, c.fwd_par, c.elu, L.OUT_NHWC, out, k=c.k, stride=c.stride)
+    bn_forward(lib, c, out, residual)
+
+
+def gate_backward(lib, g, fm, c, dfm):
+    """[df | dm] (into ``dfm``, RAW column order) and [dbias_f, dbias_m, dgamma, dbeta] (fp32 [4, C]) of the FoldedConv ``c`` from
+    its output gradient ``g`` and the recomputed [f | m]; a train-mode norm adds the terms through the batch statistics."""
+    st = L.stream_ptr()
+    P = g.numel() // c.C
+    red = torch.zeros((4, c.C), dtype=torch.float32, device=g.device)  # dbias_f, dbias_m, dgamma, dbeta
+    if c.batch:
+        L.check(lib.read_bn_backward_reduce(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
+                                            c.mean.data_ptr(), c.inv.data_ptr(), red[3].data_ptr(), red[2].data_ptr(), st))
+        L.check(lib.read_gate_backward_batch_stats(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(),
+                                                   c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
+                                                   red[3].data_ptr(), red[2].data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
+                                                   red[1].data_ptr(), st))
+        return red
+    L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
+                                   c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
+                                   red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
+    return red
 
 
 def dgrad(dfm, conv, residual=None):
@@ -152,9 +268,9 @@ class ResStackFn(torch.autograd.Function):
         saved = []
         for r in range(0, len(convs), 2):
             h = torch.empty_like(t)
-            _launch(lib, t, C, convs[r].w_tc, convs[r].par, convs[r].elu, L.OUT_NHWC, h)
+            conv_forward(lib, t, convs[r], h)
             y = torch.empty_like(t)
-            _launch(lib, h, C, convs[r + 1].w_tc, convs[r + 1].par, convs[r + 1].elu, L.OUT_NHWC, y, residual=t)
+            conv_forward(lib, h, convs[r + 1], y, residual=t)
             saved += [t, h]
             t = y
         ctx.convs, ctx.n_inputs = convs, len(saved)
@@ -179,10 +295,7 @@ class ResStackFn(torch.autograd.Function):
             if i % 2 == 1:
                 g_block = g                                               # gradient of this ResBlock's output
             _launch(lib, x_in, C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-            red = torch.zeros((4, C), dtype=torch.float32, device=dev)   # dbias_f, dbias_m, dgamma, dbeta
-            L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), B * H * W, C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                           c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
-                                           red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
+            red = gate_backward(lib, g, fm, c, dfm)                       # dbias_f, dbias_m, dgamma, dbeta
             dwf = dwm = None
             if ctx.needs_input_grad[2 + 6 * i] or ctx.needs_input_grad[4 + 6 * i]:    # not for a frozen net
                 dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
@@ -201,9 +314,10 @@ def stack_convs(net, prefix):
     return [net.get_submodule(f"{prefix}.layers.{i}.main.{j}") for i in range(net.num_res) for j in (0, 1)]
 
 
-def res_stack(net, prefix, x):
+def res_stack(net, prefix, x, batch_stats=False):
     """bf16 forward of one EBlock / DBlock of ``net`` on the wgmma kernels, differentiable through ResStackFn."""
-    return stack_forward(stack_convs(net, prefix), x)
+    names = [f"{prefix}.layers.{i}.main.{j}" for i in range(net.num_res) for j in (0, 1)]
+    return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=names)
 
 
 def stack_params(mods):
@@ -221,9 +335,37 @@ def _check_eval(mods):
                            "mode (the reference trains with eval-mode BatchNorm)")
 
 
-def stack_forward(mods, x):
-    """The ResBlocks t -> t + mods[2r+1](mods[2r](t)) applied to x in turn, bf16 on the wgmma kernels."""
-    _check_eval(mods)
+def _label(mod, name):
+    return name or f"GatedConv(k={mod.k}, stride={mod.stride})"
+
+
+def check_norms(mods, batch_stats, pixels, names=None):
+    """Without ``batch_stats`` every norm must be in eval mode (RuntimeError).  With it, a train-mode norm must be one the batch
+    statistics kernels implement (momentum set, running statistics tracked, affine) and the conv must have at least 2 output
+    pixels (``pixels`` = B * H_out * W_out; torch raises for 1 too); otherwise a ValueError names the layer."""
+    if not batch_stats:
+        _check_eval(mods)
+        return
+    for i, m in enumerate(mods):
+        n = m.block['norm']
+        if not n.training:
+            continue
+        label = _label(m, names[i] if names else None)
+        if n.momentum is None:
+            raise ValueError(f"read_b200: {label}: train-mode BatchNorm with momentum=None (cumulative moving average) is not "
+                             "supported on the bf16 path")
+        if not n.track_running_stats or not n.affine:
+            raise ValueError(f"read_b200: {label}: train-mode BatchNorm needs track_running_stats=True and affine=True on the "
+                             f"bf16 path (got track_running_stats={n.track_running_stats}, affine={n.affine})")
+        if pixels < 2:
+            raise ValueError(f"read_b200: {label}: train-mode BatchNorm needs more than 1 value per channel (got B * H * W = "
+                             f"{pixels})")
+
+
+def stack_forward(mods, x, batch_stats=False, names=None):
+    """The ResBlocks t -> t + mods[2r+1](mods[2r](t)) applied to x in turn, bf16 on the wgmma kernels.  ``batch_stats``: a conv
+    whose norm is in train mode normalises with batch statistics (else such a conv raises); ``names`` label the convs in errors."""
+    check_norms(mods, batch_stats, x.shape[0] * x.shape[2] * x.shape[3], names)
     return ResStackFn.apply(x, list(mods), *stack_params(mods))
 
 
@@ -243,7 +385,7 @@ class GatedConvFn(torch.autograd.Function):
         B, H, W, _ = t.shape
         r = None if residual is None else ops.nchw_to_nhwc(residual.detach().float().contiguous(), True)
         y = torch.empty((B, H, W, conv.C), dtype=torch.bfloat16, device=t.device)
-        _launch(lib, t, conv.C, conv.w_tc, conv.par, conv.elu, L.OUT_NHWC, y, residual=r)
+        conv_forward(lib, t, conv, y, residual=r)
         ctx.conv, ctx.cout = conv, cout
         ctx.save_for_backward(t, *params)              # the parameters: an in-place update before backward raises
         y = ops.nhwc_to_nchw(y)
@@ -263,10 +405,7 @@ class GatedConvFn(torch.autograd.Function):
         fm = torch.empty((B, H, W, 2 * C), dtype=torch.bfloat16, device=dev)
         dfm = torch.empty_like(fm)
         _launch(lib, x_in, C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-        red = torch.zeros((4, C), dtype=torch.float32, device=dev)       # dbias_f, dbias_m, dgamma, dbeta
-        L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), B * H * W, C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                       c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
-                                       red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
+        red = gate_backward(lib, g, fm, c, dfm)                           # dbias_f, dbias_m, dgamma, dbeta
         dwf = dwm = None
         if need[3] or need[5]:                                            # not for a frozen net
             dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
@@ -278,12 +417,13 @@ class GatedConvFn(torch.autograd.Function):
         return (dx, gout if need[1] else None, None, *grads)
 
 
-def gated_conv(mod, x, residual=None):
+def gated_conv(mod, x, residual=None, batch_stats=False, name=None):
     """bf16 forward of the gated 3x3 stride-1 conv ``mod`` (a GatedConv) on the wgmma kernels, plus ``residual`` (NCHW, the
-    output's shape) when given, differentiable through GatedConvFn."""
+    output's shape) when given, differentiable through GatedConvFn.  ``batch_stats``: a train-mode norm normalises with batch
+    statistics (else it raises); ``name`` labels the layer in errors."""
     if mod.k != 3 or mod.stride != 1:
         raise ValueError(f"read_b200: gated_conv runs 3x3 stride-1 convs only (got k={mod.k}, stride={mod.stride})")
-    _check_eval([mod])
+    check_norms([mod], batch_stats, x.shape[0] * x.shape[2] * x.shape[3], [name])
     return GatedConvFn.apply(x, residual, mod, *stack_params([mod]))
 
 
@@ -309,38 +449,60 @@ def recompute_fm(lib, srcs, c):
         _launch(lib, srcs, c.C, c.w_tc, (zeros,) * 4, False, L.OUT_RAW_NHWC, fm, k=c.k, stride=c.stride)
         return fm
     blocks_ = []
-    w = torch.empty(lib.read_tc_weight_elems(64, d.Cin, 1), dtype=torch.bfloat16, device=srcs[0].device)
-    d64 = _desc(srcs, 64, 1, 1)
-    for b in range(c.C // 64):
-        L.check(lib.read_pack_weights_tc_for(ctypes.byref(d64), c.wf[64 * b: 64 * b + 64].data_ptr(),
-                                             c.wm[64 * b: 64 * b + 64].data_ptr(), w.data_ptr(), L.stream_ptr()))
+    for w in _fm64_filters(lib, srcs, c):
         out = torch.empty((B, H, W, 128), dtype=torch.bfloat16, device=srcs[0].device)
         _launch(lib, srcs, 64, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
         blocks_.append(out)
     return torch.cat(blocks_, -1)
 
 
+def _fm64_filters(lib, srcs, c):
+    """The forward filters of each 64-channel block of a 1x1 FoldedConv wider than 64 (recompute_fm), packed once per entry."""
+    ws = c.pk.get('fm64')
+    if ws is None:
+        d64 = _desc(srcs, 64, 1, 1)
+        ws = [torch.empty(lib.read_tc_weight_elems(64, d64.Cin, 1), dtype=torch.bfloat16, device=c.wf.device)
+              for _ in range(c.C // 64)]
+        for b, w in enumerate(ws):
+            L.check(lib.read_pack_weights_tc_for(ctypes.byref(d64), c.wf[64 * b: 64 * b + 64].data_ptr(),
+                                                 c.wm[64 * b: 64 * b + 64].data_ptr(), w.data_ptr(), L.stream_ptr()))
+        c.pk['fm64'] = ws
+    return ws
+
+
+def _dgrad1x1_filters(lib, c, a, cn, device):
+    """The transposed filters of the RAW 1x1 input-gradient plan for input channels a .. a + cn - 1 (dgrad_1x1)."""
+    w = c.pk.get(('d1x1', a, cn))
+    if w is None:
+        n_out = max(cn, 32)
+        w = torch.empty(lib.read_tc_weight_elems(n_out // 2, 2 * c.C, 1), dtype=torch.bfloat16, device=device)
+        L.check(lib.read_pack_weights_tc_dgrad1x1(c.wf.data_ptr(), c.wm.data_ptr(), c.C, c.wf.shape[1], a, cn, w.data_ptr(),
+                                                  L.stream_ptr()))
+        c.pk[('d1x1', a, cn)] = w
+    return w
+
+
 def dgrad_s2_filters(c):
     """The flipped-by-phase filters [k*k][Cin][2C] (bf16) of the stride-2 input-gradient kernel for the FoldedConv ``c``."""
-    lib = L.load()
-    cin = c.wf.shape[1]
-    w = torch.empty((c.k * c.k, cin, 2 * c.C), dtype=torch.bfloat16, device=c.wf.device)
-    L.check(lib.read_pack_weights_dgrad_s2(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, c.k, w.data_ptr(), L.stream_ptr()))
+    w = c.pk.get('s2')
+    if w is None:
+        cin = c.wf.shape[1]
+        w = torch.empty((c.k * c.k, cin, 2 * c.C), dtype=torch.bfloat16, device=c.wf.device)
+        L.check(L.load().read_pack_weights_dgrad_s2(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, c.k, w.data_ptr(), L.stream_ptr()))
+        c.pk['s2'] = w
     return w
 
 
 def dgrad_1x1(dfm, c, c0, cs):
     """Input gradient [B,H,W,cs] (bf16) of input channels c0 .. c0 + cs - 1 of the 1x1 FoldedConv ``c``: RAW 1x1 plans over
     [df | dm] with transposed filters, one per 128 channels (the plans' widest N tile); 16 channels run padded to 32."""
-    lib, st = L.load(), L.stream_ptr()
+    lib = L.load()
     B, H, W, _ = dfm.shape
-    cin = c.wf.shape[1]
     parts = []
     for a in range(c0, c0 + cs, 128):
         cn = min(128, c0 + cs - a)
         n_out = max(cn, 32)
-        w = torch.empty(lib.read_tc_weight_elems(n_out // 2, 2 * c.C, 1), dtype=torch.bfloat16, device=dfm.device)
-        L.check(lib.read_pack_weights_tc_dgrad1x1(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, a, cn, w.data_ptr(), st))
+        w = _dgrad1x1_filters(lib, c, a, cn, dfm.device)
         out = torch.empty((B, H, W, n_out), dtype=torch.bfloat16, device=dfm.device)
         zeros = torch.zeros(n_out // 2, dtype=torch.float32, device=dfm.device)
         _launch(lib, dfm, n_out // 2, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
@@ -363,7 +525,7 @@ class MultiSourceConvFn(torch.autograd.Function):
         conv = FoldedConv(mod, *params, cout=padded_channels(cout), srcs=ts)
         d = _desc(ts, conv.C, mod.k, mod.stride)
         y = torch.empty((d.B, d.Hout, d.Wout, conv.C), dtype=torch.bfloat16, device=ts[0].device)
-        _launch(lib, ts, conv.C, conv.w_tc, conv.par, conv.elu, L.OUT_NHWC, y, k=mod.k, stride=mod.stride)
+        conv_forward(lib, ts, conv, y)
         ctx.conv, ctx.cout, ctx.n_src = conv, cout, n_src
         ctx.save_for_backward(*ts, *params)            # the parameters: an in-place update before backward raises
         y = ops.nhwc_to_nchw(y)
@@ -384,10 +546,7 @@ class MultiSourceConvFn(torch.autograd.Function):
         Hout, Wout = g.shape[1], g.shape[2]
         fm = recompute_fm(lib, ts, c)
         dfm = torch.empty_like(fm)
-        red = torch.zeros((4, C), dtype=torch.float32, device=dev)        # dbias_f, dbias_m, dgamma, dbeta
-        L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), B * Hout * Wout, C, int(c.elu), c.bf.data_ptr(),
-                                       c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
-                                       red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
+        red = gate_backward(lib, g, fm, c, dfm)                            # dbias_f, dbias_m, dgamma, dbeta
         del fm
         dwf = dwm = None
         if need[n_src] or need[n_src + 2]:                                 # not for a frozen net
@@ -416,10 +575,11 @@ class MultiSourceConvFn(torch.autograd.Function):
         return (None, None, *dxs, *grads)
 
 
-def gated_conv_srcs(mod, xs, name=None):
+def gated_conv_srcs(mod, xs, name=None, batch_stats=False):
     """bf16 forward of the gated 1x1 or stride-2 conv ``mod`` (a GatedConv) over the NCHW tensors ``xs`` on the wgmma kernels,
     differentiable through MultiSourceConvFn.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels);
-    a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors."""
+    a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors.  ``batch_stats``: a
+    train-mode norm normalises with batch statistics (else it raises)."""
     label = name or f"GatedConv(k={mod.k}, stride={mod.stride})"
     xs = list(xs)
     if (mod.k, mod.stride) not in GEOMETRIES:
@@ -433,5 +593,6 @@ def gated_conv_srcs(mod, xs, name=None):
     if mod.stride == 2 and (xs[0].shape[2] % 2 or xs[0].shape[3] % 2):
         raise ValueError(f"read_b200: {label}: a stride-2 conv needs an even input height and width (got "
                          f"{xs[0].shape[2]}x{xs[0].shape[3]})")
-    _check_eval([mod])
+    pixels = xs[0].shape[0] * (xs[0].shape[2] // mod.stride) * (xs[0].shape[3] // mod.stride)
+    check_norms([mod], batch_stats, pixels, [label])
     return MultiSourceConvFn.apply(mod, len(xs), *xs, *stack_params([mod]))

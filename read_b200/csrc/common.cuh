@@ -15,6 +15,8 @@ void set_error(const char *fmt, ...);
 extern std::atomic<long long> g_launches;
 inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int num_sms();
+// channel counts of the train-mode BatchNorm entry points (bn_train.cu, conv_bwd.cu): the gate backward's, without 48
+inline bool bn_channels_ok(int C) { return C == 16 || C == 32 || C == 64 || (C % 64 == 0 && C > 0 && C <= 256); }
 
 #define RB_CHECK_ARG(cond, ...)                        \
     do {                                               \

@@ -25,14 +25,20 @@ __device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2
 //   dgamma = sum dy * (g - mean) * inv_std, dbeta = sum dy.
 // A thread owns 8 channels (one 16-byte vector) of one pixel per step and keeps its channel group across pixels; its sums are
 // reduced per CTA in shared memory and leave with one atomic per channel and CTA.
+// BATCH: train-mode BatchNorm (mean / inv_std are this batch's statistics over the P pixels).  Its backward adds the terms through
+// the statistics: dg = scale * (dy - sum_dy / P - xhat * sum_dy_xhat / P) = scale * dy + k1 * (g - mean) + k0 with
+// k1 = -scale * inv_std * sum_dy_xhat / P, k0 = -scale * sum_dy / P; the two sums (= dgamma, dbeta) come from bn_bwd_reduce_kernel,
+// so this instance accumulates no dgamma / dbeta.  BATCH = false compiles to the eval-mode kernel unchanged (the appended
+// parameters are never read).
 constexpr int GB_THREADS = 256, GB_MAX_C = 256;
 
-template <bool ELU>
+template <bool ELU, bool BATCH>
 __global__ void __launch_bounds__(GB_THREADS)
 gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
                 const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
                 const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
-                float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta)
+                float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
+                const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
 {
     __shared__ float red[4][GB_MAX_C];
     for (int i = threadIdx.x; i < 4 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
@@ -41,10 +47,16 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
     const int cg = threadIdx.x % G, co0 = 8 * cg, fcol = fm_col(co0, half);
     float bf[8], bm[8], sc[8], mu[8], is[8];
     float s_bf[8], s_bm[8], s_g[8], s_b[8];
+    float k1[8], k0[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         bf[j] = bias_f[co0 + j]; bm[j] = bias_m[co0 + j]; sc[j] = scale[co0 + j]; mu[j] = mean[co0 + j]; is[j] = inv_std[co0 + j];
         s_bf[j] = s_bm[j] = s_g[j] = s_b[j] = 0.f;
+        if constexpr (BATCH) {
+            const float rp = 1.f / (float)P;
+            k1[j] = -sc[j] * is[j] * sum_dy_xhat[co0 + j] * rp;
+            k0[j] = -sc[j] * sum_dy[co0 + j] * rp;
+        }
     }
     if (threadIdx.x < ppb * G) {
         for (long long p = blockIdx.x * (long long)ppb + threadIdx.x / G; p < P; p += (long long)gridDim.x * ppb) {
@@ -65,13 +77,18 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
                     const float s = 1.f / (1.f + expf(-m));
                     float A = f, Ad = 1.f;
                     if (ELU && f <= 0.f) { A = expm1f(f); Ad = A + 1.f; }
-                    const float g = A * s, dg = y * sc[j];
+                    const float g = A * s;
+                    float dg;
+                    if constexpr (BATCH) dg = fmaf(y, sc[j], fmaf(k1[j], g - mu[j], k0[j]));
+                    else dg = y * sc[j];
                     df[h] = dg * s * Ad;
                     dm[h] = dg * A * s * (1.f - s);
                     s_bf[j] += df[h];
                     s_bm[j] += dm[h];
-                    s_g[j] = fmaf(y, (g - mu[j]) * is[j], s_g[j]);
-                    s_b[j] += y;
+                    if constexpr (!BATCH) {
+                        s_g[j] = fmaf(y, (g - mu[j]) * is[j], s_g[j]);
+                        s_b[j] += y;
+                    }
                 }
                 odf[q] = bf16x2_bits(df[0], df[1]);
                 odm[q] = bf16x2_bits(dm[0], dm[1]);
@@ -83,16 +100,75 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
         for (int j = 0; j < 8; ++j) {
             atomicAdd(&red[0][co0 + j], s_bf[j]);
             atomicAdd(&red[1][co0 + j], s_bm[j]);
-            atomicAdd(&red[2][co0 + j], s_g[j]);
-            atomicAdd(&red[3][co0 + j], s_b[j]);
+            if constexpr (!BATCH) {
+                atomicAdd(&red[2][co0 + j], s_g[j]);
+                atomicAdd(&red[3][co0 + j], s_b[j]);
+            }
         }
     }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += GB_THREADS) {
         atomicAdd(dbf + c, red[0][c]);
         atomicAdd(dbm + c, red[1][c]);
-        atomicAdd(dgamma + c, red[2][c]);
-        atomicAdd(dbeta + c, red[3][c]);
+        if constexpr (!BATCH) {
+            atomicAdd(dgamma + c, red[2][c]);
+            atomicAdd(dbeta + c, red[3][c]);
+        }
+    }
+}
+
+// ------------------------------------------------------------------ train-mode BatchNorm: backward reduction
+// sum_dy += sum dy, sum_dy_xhat += sum dy * (g - mean) * inv_std over the P pixels, with g = A(f + b_f) * sigmoid(m + b_m)
+// recomputed from the RAW [f | m] (mean / inv_std: the batch statistics of the forward).  These are dbeta and dgamma, and the
+// two terms the corrected gate backward (gate_bwd_kernel<ELU, true>) needs.  Same thread layout and reduction as the gate backward.
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                     const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
+                     const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
+{
+    __shared__ float red[2][GB_MAX_C];
+    for (int i = threadIdx.x; i < 2 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
+    __syncthreads();
+    const int G = C / 8, ppb = GB_THREADS / G;
+    const int cg = threadIdx.x % G, co0 = 8 * cg, fcol = fm_col(co0, half);
+    float bf[8], bm[8], mu[8], is[8], s_b[8], s_g[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        bf[j] = bias_f[co0 + j]; bm[j] = bias_m[co0 + j]; mu[j] = mean[co0 + j]; is[j] = inv_std[co0 + j];
+        s_b[j] = s_g[j] = 0.f;
+    }
+    if (threadIdx.x < ppb * G) {
+        for (long long p = blockIdx.x * (long long)ppb + threadIdx.x / G; p < P; p += (long long)gridDim.x * ppb) {
+            const uint4 vy = *reinterpret_cast<const uint4 *>(dy + p * C + co0);
+            const uint4 vf = *reinterpret_cast<const uint4 *>(fm + p * 2 * C + fcol);
+            const uint4 vm = *reinterpret_cast<const uint4 *>(fm + p * 2 * C + fcol + half);
+            const uint32_t wy[4] = {vy.x, vy.y, vy.z, vy.w}, wf[4] = {vf.x, vf.y, vf.z, vf.w}, wm[4] = {vm.x, vm.y, vm.z, vm.w};
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const float2 y2 = bf16x2_val(wy[q]), f2 = bf16x2_val(wf[q]), m2 = bf16x2_val(wm[q]);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int j = 2 * q + h;
+                    const float y = h ? y2.y : y2.x;
+                    const float f = (h ? f2.y : f2.x) + bf[j], m = (h ? m2.y : m2.x) + bm[j];
+                    const float s = 1.f / (1.f + expf(-m));
+                    const float A = (ELU && f <= 0.f) ? expm1f(f) : f;
+                    s_g[j] = fmaf(y, (A * s - mu[j]) * is[j], s_g[j]);
+                    s_b[j] += y;
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            atomicAdd(&red[0][co0 + j], s_b[j]);
+            atomicAdd(&red[1][co0 + j], s_g[j]);
+        }
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < C; c += GB_THREADS) {
+        atomicAdd(sum_dy + c, red[0][c]);
+        atomicAdd(sum_dy_xhat + c, red[1][c]);
     }
 }
 
@@ -519,10 +595,54 @@ int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, in
     const int half = C < 64 ? C : 64, ppb = GB_THREADS / (C / 8);
     long long blocks = (pixels + ppb - 1) / ppb;
     if (blocks > 8ll * num_sms()) blocks = 8ll * num_sms();
-    auto k = elu ? gate_bwd_kernel<true> : gate_bwd_kernel<false>;
+    auto k = elu ? gate_bwd_kernel<true, false> : gate_bwd_kernel<false, false>;
     k<<<(unsigned)blocks, GB_THREADS, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, half, bias_f, bias_m, bn_scale, bn_mean,
-        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta);
+        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, nullptr, nullptr);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+static long long gate_grid(int64_t pixels, int C)
+{
+    const int ppb = GB_THREADS / (C / 8);
+    long long blocks = (pixels + ppb - 1) / ppb;
+    return blocks > 8ll * num_sms() ? 8ll * num_sms() : blocks;
+}
+
+int read_bn_backward_reduce(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                            const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat, "bn_backward_reduce: null pointer");
+    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
+    RB_CHECK_ARG(pixels >= 2, "bn_backward_reduce: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm)) & 15) == 0,
+                 "bn_backward_reduce: tensors must be 16B aligned");
+    auto k = elu ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>;
+    k<<<(unsigned)gate_grid(pixels, C), GB_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        bn_inv_std, sum_dy, sum_dy_xhat);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                   const float *bias_m, const float *bn_scale, const float *bn_mean, const float *bn_inv_std,
+                                   const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
+                                   void *stream)
+{
+    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat && dbias_f &&
+                     dbias_m,
+                 "gate_backward_batch_stats: null pointer");
+    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    RB_CHECK_ARG(pixels >= 2, "gate_backward_batch_stats: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
+                 "gate_backward_batch_stats: tensors must be 16B aligned");
+    auto k = elu ? gate_bwd_kernel<true, true> : gate_bwd_kernel<false, true>;
+    k<<<(unsigned)gate_grid(pixels, C), GB_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
+        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, nullptr, nullptr, sum_dy, sum_dy_xhat);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

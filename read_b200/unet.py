@@ -191,17 +191,20 @@ class UNet(nn.Module):
             raise ValueError(f"read_b200.UNet: train_precision must be one of {TRAIN_PRECISIONS}, got {tp!r}")
 
         bf16 = tp in ('bf16', 'bf16_all')
+        # a conv whose BatchNorm is in train mode (the net in train()) normalises with batch statistics on our kernels, like
+        # torch's BatchNorm2d; the keyword is passed only when some norm trains, so an eval-mode net calls res_stack as before
+        bs = {'batch_stats': True} if bf16 and any(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)) else {}
 
         def c3(name, t):
             # the gated 3x3 stride-1 convs outside the blocks: feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge
             if bf16:
-                return blocks.gated_conv(self.get_submodule(name), t)
+                return blocks.gated_conv(self.get_submodule(name), t, name=name, **bs)
             return c(name, t)
 
         def c1(name, *ts):
             # the 1x1 and stride-2 convs; a 1x1 conv's sources are concatenated along channels (virtually under 'bf16_all')
             if tp == 'bf16_all':
-                return blocks.gated_conv_srcs(self.get_submodule(name), ts, name)
+                return blocks.gated_conv_srcs(self.get_submodule(name), ts, name, **bs)
             return c(name, ts[0] if len(ts) == 1 else torch.cat(ts, 1))
 
         def res(p, t):
@@ -209,7 +212,7 @@ class UNet(nn.Module):
 
         def blk(p, t):
             if bf16:
-                return blocks.res_stack(self, p, t)
+                return blocks.res_stack(self, p, t, **bs)
             for i in range(self.num_res):
                 t = res(f"{p}.layers.{i}", t)
             return t

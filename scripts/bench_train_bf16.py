@@ -2,7 +2,11 @@
 the net, sparse RMSprop on the descriptors) with the net trained in fp32 (torch operators, cuDNN), in bf16 (the 78 gated 3x3
 stride-1 convs on the wgmma kernels, UNet.train_precision = 'bf16') and in bf16_all (all 99 convs), alternating in one process
 so that clock drift hits all alike.
-   python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--out result.json]
+   python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--batchnorm running|batch] [--out result.json]
+--batchnorm batch puts the model in train() (the reference's default training: train-mode BatchNorm with batch statistics, and
+NetAndTexture's per-item loop, B = 1 per net call) and then reports, instead of the eval-mode sections below, the step time per
+precision, the time and bytes of the batch-statistics kernels at the C5 shapes, and the kernel launches per step with and without
+the packed-filter cache (read_b200/blocks.py).  The default, running, is the eval-mode measurement:
 Prints the card's name and power limit, per precision the step time and the share of the net's forward + backward in it, the time
 to re-pack the 64 block convs' filters (done on every bf16 step), per stack shape the time of each backward kernel, the same for
 the new shapes of the 14 single gated 3x3 convs (8-channel inputs, the RGB conv padded to C = 16) with the 8-channel input gradient
@@ -39,7 +43,7 @@ def card():
     return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q}
 
 
-def make_model(sd, tp, dev):
+def make_model(sd, tp, dev, batch=False):
     tex = PointTexture(8, N, init_method='zeros')
     with torch.no_grad():
         tex.texture_.copy_(torch.rand((1, 8, N), generator=torch.Generator().manual_seed(synth.SEED)))
@@ -48,7 +52,8 @@ def make_model(sd, tp, dev):
     net.train_precision = tp
     model = NetAndTexture(net, {0: tex}, 1)
     model.load_textures(0)
-    model.to(dev).eval()                        # eval-mode BatchNorm, as the reference trains
+    model.to(dev)
+    model.train(batch)                          # running: eval-mode BatchNorm (eval_in_train); batch: the reference's default
     return dict(net=net, tex=tex, model=model, opt_net=torch.optim.Adam(net.parameters(), lr=1e-4),
                 opt_tex=rtrain.SparseRMSprop(tex, lr=1e-1))
 
@@ -57,8 +62,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--batchnorm", choices=("running", "batch"), default="running")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    batch = args.batchnorm == "batch"
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
     L.require_device(0)
@@ -66,14 +73,14 @@ def main():
     store = ops.SortedPoints(xyz)
     pyr = ops.Pyramid(BC, W, H, LEVELS, dev)
     rng = np.random.default_rng(synth.SEED)
-    n_mats = 3 + args.steps
+    n_mats = 3 + max(args.steps, 3)                 # 3 warm-up crops, then one per timed step and at least the 3 profiled ones
     mats = torch.stack([torch.from_numpy(synth.total_matrix(*synth.crop_cameras(W, H, rng.integers(0, 64, BC), rng)))
                         for _ in range(n_mats)]).to(dev)
     target = torch.rand((BC, 3, H, W), generator=torch.Generator().manual_seed(7)).to(dev)
     keys = ["uv_1d_p1"] + [f"uv_1d_p1_ds{l}" for l in range(1, LEVELS)]
     ids0 = torch.zeros(BC, dtype=torch.long)
     sd = synth.synth_state_dict(synth.SEED)
-    runs = {tp: make_model(sd, tp, dev) for tp in ("fp32", "bf16", "bf16_all")}
+    runs = {tp: make_model(sd, tp, dev, batch) for tp in ("fp32", "bf16", "bf16_all")}
 
     def step(r, m, marks=None):
         e = [ev() for _ in range(4)] if marks is not None else None
@@ -120,6 +127,9 @@ def main():
             net_ms = sum(e[1].elapsed_time(e[2]) for e in marks) / len(marks)
             tot_ms = sum(e[0].elapsed_time(e[3]) for e in marks) / len(marks)
             share[tp].append({"net_fwd_bwd_ms": net_ms, "step_ms": tot_ms, "share": net_ms / tot_ms})
+
+    if batch:
+        return report_batch(args, runs, ms, share, first_loss, step, mats, dev)
 
     # filter re-packing of the 64 block convs (what every bf16 step does before its first block launch)
     net = runs["bf16"]["net"]
@@ -374,6 +384,87 @@ def main():
     for tp, v in new_ms.items():
         print(f"21 1x1 / stride-2 convs fwd+bwd at C5, {tp}: {sorted(v)[len(v) // 2]:.2f} ms/step (rounds {', '.join(f'{x:.2f}' for x in v)})")
     print(f"activations saved for the 21 convs' backward at C5: {saved_bytes}")
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        json.dump(res, open(args.out, "w"), indent=1)
+
+
+def report_batch(args, runs, ms, share, first_loss, step, mats, dev):
+    """--batchnorm batch: step times, the batch-statistics kernels at the C5 shapes (one net call = one 256x256 crop, so the
+    stacks run at P = 65536 / 16384 / 4096 / 1024 pixels with C = 32 / 64 / 128 / 256) and the launches per step."""
+    lib = L.load()
+    launches = {}
+    for tp in ("bf16", "bf16_all"):
+        for cached in (True, False):
+            blocks.cache_filters = cached
+            blocks.clear_filter_cache()
+            step(runs[tp], mats[-1])                                          # fills the cache (or not)
+            torch.cuda.synchronize()
+            n0 = ops.launch_count()
+            step(runs[tp], mats[-2])
+            torch.cuda.synchronize()
+            launches[f"{tp}, filter cache {'on' if cached else 'off'}"] = ops.launch_count() - n0
+    blocks.cache_filters = True
+    torch.cuda.synchronize()
+    n0 = ops.launch_count()
+    step(runs["fp32"], mats[-1])
+    torch.cuda.synchronize()
+    launches["fp32 (library kernels only: raster, gather, descriptors)"] = ops.launch_count() - n0
+
+    kern = []
+    reps = 50
+    for C, side in ((32, 256), (64, 128), (128, 64), (256, 32)):
+        P = side * side
+        g = torch.randn((P, C), device=dev).bfloat16()
+        fm = torch.randn((P, 2 * C), device=dev).bfloat16()
+        dy = torch.randn((P, C), device=dev).bfloat16()
+        dfm, y = torch.empty_like(fm), torch.empty_like(g)
+        v = torch.rand((10, C), device=dev) + 0.5
+        red = torch.zeros((4, C), device=dev)
+        ws = torch.empty(lib.read_bn_workspace_bytes(C), dtype=torch.uint8, device=dev)
+        st = L.stream_ptr()
+        p = [t.data_ptr() for t in v]
+        fns = {
+            "bn_stats": (lambda: L.check(lib.read_bn_batch_stats(g.data_ptr(), P, C, C, p[0], p[1], 1e-5, 0.1, p[2], p[3], p[4],
+                                                                 p[5], None, p[6], p[7], ws.data_ptr(), st)), P * C * 2),
+            "bn_apply": (lambda: L.check(lib.read_bn_apply(g.data_ptr(), P, C, p[6], p[7], None, y.data_ptr(), st)), 2 * P * C * 2),
+            "bn_backward_reduce": (lambda: L.check(lib.read_bn_backward_reduce(dy.data_ptr(), fm.data_ptr(), P, C, 1, p[0], p[1],
+                                                                               p[4], p[5], red[3].data_ptr(), red[2].data_ptr(),
+                                                                               st)), 3 * P * C * 2),
+            "gate_backward_batch_stats": (lambda: L.check(lib.read_gate_backward_batch_stats(
+                dy.data_ptr(), fm.data_ptr(), P, C, 1, p[0], p[1], p[6], p[4], p[5], red[3].data_ptr(), red[2].data_ptr(),
+                dfm.data_ptr(), red[0].data_ptr(), red[1].data_ptr(), st)), 5 * P * C * 2),
+        }
+        for name, (fn, nbytes) in fns.items():
+            for _ in range(5):
+                fn()
+            rounds = []
+            for _ in range(3):
+                a, b = ev(), ev()
+                a.record()
+                for _ in range(reps):
+                    fn()
+                b.record()
+                torch.cuda.synchronize()
+                rounds.append(a.elapsed_time(b) * 1e3 / reps)
+            us = sorted(rounds)[1]
+            kern.append({"kernel": name, "C": C, "pixels": P, "us": round(us, 2), "rounds_us": [round(x, 2) for x in rounds],
+                         "bytes": nbytes, "share_of_3.35TB/s": round(nbytes / (us * 1e-6) / 3.35e12, 3)})
+
+    res = {"card": card(), "batchnorm": "batch", "steps": args.steps, "rounds": args.rounds, "crops_per_step": BC,
+           "size": f"{W}x{H}", "n_points": N, "ms_per_step": ms, "net_fwd_bwd_per_step": share, "first_loss": first_loss,
+           "launches_per_step": launches, "batch_stats_kernels": kern}
+    print(f"card: {res['card']}")
+    for tp in runs:
+        med = sorted(ms[tp])[len(ms[tp]) // 2]
+        sh = sorted(share[tp], key=lambda x: x["share"])[len(share[tp]) // 2]
+        print(f"{tp} (train mode): {med:.2f} ms/step (rounds {', '.join(f'{v:.2f}' for v in ms[tp])}), net fwd+bwd "
+              f"{sh['net_fwd_bwd_ms']:.2f} ms of a {sh['step_ms']:.2f} ms profiled step")
+    print("first-step loss " + ", ".join(f"{tp} {v:.6f}" for tp, v in first_loss.items()))
+    for k, v in launches.items():
+        print(f"library kernel launches per step, {k}: {v}")
+    for row in kern:
+        print(json.dumps(row))
     if args.out:
         os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
         json.dump(res, open(args.out, "w"), indent=1)
