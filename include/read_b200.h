@@ -381,6 +381,34 @@ int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixel
                                    const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
                                    void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Per-item train-mode BatchNorm (read_b200/blocks.py, UNet.train_batchnorm = 'per_item'): a call of `items` batch items, item i
+ * being the `pixels` rows [i*pixels, (i+1)*pixels) of g / dy / fm, each normalised with its own statistics.  mean, inv_std, scale,
+ * shift, sum_dy and sum_dy_xhat are fp32 [items, C]; the rest is as in the call-wide entry points above.
+ *   read_bn_batch_stats_items : item i's mean / inv_std / scale / shift are bit-identical to read_bn_batch_stats on its rows alone;
+ *                               the running statistics are updated once per item, in item order, bit-identical to `items` calls
+ *                               of read_bn_batch_stats in a row.  workspace: read_bn_workspace_bytes_items(items, C) bytes
+ *   read_bn_apply_items       : y = bf16(g*scale_i + shift_i [+ residual]) with the scale / shift of the pixel's item
+ *   read_bn_backward_reduce_items : the two sums per (item, channel) into caller-zeroed [items, C]; dbeta / dgamma are their sums
+ *                               over items
+ *   read_gate_backward_batch_stats_items : the corrected gate backward with item i's sums and `pixels`; dbias_f / dbias_m
+ *                               accumulate over all items
+ * items in 1..65535, pixels (per item) >= 2.
+ * ---------------------------------------------------------------------------------------- */
+int64_t read_bn_workspace_bytes_items(int items, int C);
+int read_bn_batch_stats_items(const void *g, int items, int64_t pixels, int C, int n_real, const float *gamma, const float *beta,
+                              float eps, float momentum, float *running_mean, float *running_var, float *mean, float *inv_std,
+                              float *scale, float *shift, void *workspace, void *stream);
+int read_bn_apply_items(const void *g, int items, int64_t pixels, int C, const float *scale, const float *shift, const void *residual,
+                        void *y, void *stream);
+int read_bn_backward_reduce_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu, const float *bias_f,
+                                  const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy,
+                                  float *sum_dy_xhat, void *stream);
+int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                         const float *bias_f, const float *bias_m, const float *bn_scale, const float *bn_mean,
+                                         const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
+                                         float *dbias_f, float *dbias_m, void *stream);
+
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);
 

@@ -110,6 +110,13 @@ _SIGS = {
     "read_bn_backward_reduce": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "read_gate_backward_batch_stats": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                c_vp, c_vp]),
+    "read_bn_workspace_bytes_items": (c_i64, [c_int, c_int]),
+    "read_bn_batch_stats_items": (c_int, [c_vp, c_int, c_i64, c_int, c_int, c_vp, c_vp, ctypes.c_float, ctypes.c_float, c_vp, c_vp,
+                                          c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_bn_apply_items": (c_int, [c_vp, c_int, c_i64, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_bn_backward_reduce_items": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_gate_backward_batch_stats_items": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                     c_vp, c_vp, c_vp, c_vp]),
     "read_conv_tc_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_conv_tcg_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_tcg_weight_elems": (c_i64, [c_int, c_int, c_int]),

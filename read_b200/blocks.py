@@ -27,6 +27,9 @@ BatchNorm is per conv, from the mode of that conv's norm at forward time:
   batch mean / variance over the B * H_out * W_out pixels, the folded scale / shift and the in-place running-statistics update on the
   device, then y = g * scale + shift [+ residual].  Backward adds the terms through the statistics (read_bn_backward_reduce, then
   read_gate_backward_batch_stats).  Without ``batch_stats`` a train-mode norm raises, as before.
+  With ``per_item`` as well (UNet.train_batchnorm = 'per_item'), each batch item is normalised with the statistics of its own
+  H_out * W_out pixels, and the running statistics are updated once per item in item order: one batched call computes what B
+  calls of one item each would.  The statistics are [items, C] and the *_items entry points take them.
 The packed bf16 filters are cached per module and weight version (_packed): an optimizer step re-packs them, repeated calls with
 the same weights (the per-item loop of training in train()) do not.
 """
@@ -158,9 +161,10 @@ class FoldedConv:
     over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks); its input-gradient filters are packed in
     backward (dgrad_s2_filters, dgrad_1x1).
     An eval-mode norm is folded into scale / shift from its running statistics.  A train-mode norm (``batch``) runs the forward
-    launch with the identity epilogue ``fwd_par``; mean / inv / scale / shift are then filled by bn_forward from the batch."""
+    launch with the identity epilogue ``fwd_par``; mean / inv / scale / shift are then filled by bn_forward from the batch, per
+    batch item ([items, C]) when ``items`` is given (per-item statistics), else per channel ([C])."""
 
-    def __init__(self, mod, wf, bf, wm, bm, gamma, beta, cout=None, srcs=None):
+    def __init__(self, mod, wf, bf, wm, bm, gamma, beta, cout=None, srcs=None, items=None):
         norm = mod.block['norm']
         C = cout or wf.shape[0]
         pad = lambda t: _pad_rows(t.detach().float(), C).contiguous()
@@ -168,11 +172,13 @@ class FoldedConv:
         self.bf, self.bm = pad(bf), pad(bm)
         self.k, self.stride = mod.k, mod.stride
         self.batch = norm.training
+        self.items = items if self.batch else None
         if self.batch:
             dev = wf.device
             self.norm, self.n_real = norm, wf.shape[0]
             self.gamma, self.beta = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-            self.mean, self.inv, self.scale, self.shift = torch.empty((4, C), dtype=torch.float32, device=dev).unbind(0)
+            shape = (4, C) if items is None else (4, items, C)
+            self.mean, self.inv, self.scale, self.shift = torch.empty(shape, dtype=torch.float32, device=dev).unbind(0)
             self.fwd_par = (self.bf, self.bm, torch.ones(C, device=dev), torch.zeros(C, device=dev))
         else:
             inv = torch.rsqrt(norm.running_var.detach().float() + norm.eps)
@@ -192,6 +198,9 @@ def bn_forward(lib, c, g, residual=None):
     """Train-mode BatchNorm of the FoldedConv ``c`` over its identity-epilogue output ``g`` (NHWC bf16, C channels), in place:
     batch statistics, running-statistics update and y = g * scale + shift [+ residual]."""
     st, n = L.stream_ptr(), c.norm
+    if c.items is not None:
+        _bn_forward_items(lib, c, g, residual)
+        return
     P = g.numel() // c.C
     ws = torch.empty(lib.read_bn_workspace_bytes(c.C), dtype=torch.uint8, device=g.device)
     L.check(lib.read_bn_batch_stats(g.data_ptr(), P, c.C, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps, n.momentum,
@@ -199,6 +208,20 @@ def bn_forward(lib, c, g, residual=None):
                                     c.scale.data_ptr(), c.shift.data_ptr(), ws.data_ptr(), st))
     n.num_batches_tracked.add_(1)              # torch's own op: bumps the version UNet._weights_version sums
     L.check(lib.read_bn_apply(g.data_ptr(), P, c.C, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual), g.data_ptr(), st))
+
+
+def _bn_forward_items(lib, c, g, residual):
+    """bn_forward with per-item statistics: item i of ``g`` ([items, H, W, C]) with its own; the running statistics are updated
+    once per item, in item order, and num_batches_tracked advances by the number of items, as that many single-item calls would."""
+    st, n = L.stream_ptr(), c.norm
+    items, P = g.shape[0], g.shape[1] * g.shape[2]
+    ws = torch.empty(lib.read_bn_workspace_bytes_items(items, c.C), dtype=torch.uint8, device=g.device)
+    L.check(lib.read_bn_batch_stats_items(g.data_ptr(), items, P, c.C, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps,
+                                          n.momentum, n.running_mean.data_ptr(), n.running_var.data_ptr(), c.mean.data_ptr(),
+                                          c.inv.data_ptr(), c.scale.data_ptr(), c.shift.data_ptr(), ws.data_ptr(), st))
+    n.num_batches_tracked.add_(items)
+    L.check(lib.read_bn_apply_items(g.data_ptr(), items, P, c.C, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual),
+                                    g.data_ptr(), st))
 
 
 def conv_forward(lib, src, c, out, residual=None):
@@ -217,6 +240,18 @@ def gate_backward(lib, g, fm, c, dfm):
     st = L.stream_ptr()
     P = g.numel() // c.C
     red = torch.zeros((4, c.C), dtype=torch.float32, device=g.device)  # dbias_f, dbias_m, dgamma, dbeta
+    if c.items is not None:
+        items, P = g.shape[0], g.shape[1] * g.shape[2]
+        sums = torch.zeros((2, items, c.C), dtype=torch.float32, device=g.device)     # sum dy, sum dy * xhat per item
+        L.check(lib.read_bn_backward_reduce_items(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
+                                                  c.bm.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), sums[0].data_ptr(),
+                                                  sums[1].data_ptr(), st))
+        L.check(lib.read_gate_backward_batch_stats_items(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
+                                                         c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
+                                                         sums[0].data_ptr(), sums[1].data_ptr(), dfm.data_ptr(),
+                                                         red[0].data_ptr(), red[1].data_ptr(), st))
+        red[3], red[2] = sums[0].sum(0), sums[1].sum(0)
+        return red
     if c.batch:
         L.check(lib.read_bn_backward_reduce(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
                                             c.mean.data_ptr(), c.inv.data_ptr(), red[3].data_ptr(), red[2].data_ptr(), st))
@@ -260,9 +295,13 @@ class ResStackFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, mods, *params):
+        return ResStackFn._forward(ctx, x, mods, params, None)
+
+    @staticmethod
+    def _forward(ctx, x, mods, params, items):
         _check_cuda(x)
         lib = L.load()
-        convs = [FoldedConv(m, *params[6 * i: 6 * i + 6]) for i, m in enumerate(mods)]   # packed before the first conv launch
+        convs = [FoldedConv(m, *params[6 * i: 6 * i + 6], items=items) for i, m in enumerate(mods)]   # packed before the first launch
         t = ops.nchw_to_nhwc(x.detach().float().contiguous(), True)
         C = t.shape[3]
         saved = []
@@ -309,14 +348,24 @@ class ResStackFn(torch.autograd.Function):
         return (dx, None, *grads)
 
 
+class ResStackItemsFn(ResStackFn):
+    """ResStackFn with per-item statistics for its train-mode norms (each batch item normalised with its own)."""
+
+    @staticmethod
+    def forward(ctx, x, mods, *params):
+        return ResStackFn._forward(ctx, x, mods, params, x.shape[0])
+
+
 def stack_convs(net, prefix):
     """The 8 GatedConvs of the stack ``prefix`` (e.g. 'Encoder.0') in forward order."""
     return [net.get_submodule(f"{prefix}.layers.{i}.main.{j}") for i in range(net.num_res) for j in (0, 1)]
 
 
-def res_stack(net, prefix, x, batch_stats=False):
+def res_stack(net, prefix, x, batch_stats=False, per_item=False):
     """bf16 forward of one EBlock / DBlock of ``net`` on the wgmma kernels, differentiable through ResStackFn."""
     names = [f"{prefix}.layers.{i}.main.{j}" for i in range(net.num_res) for j in (0, 1)]
+    if per_item:
+        return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=names, per_item=True)
     return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=names)
 
 
@@ -339,10 +388,11 @@ def _label(mod, name):
     return name or f"GatedConv(k={mod.k}, stride={mod.stride})"
 
 
-def check_norms(mods, batch_stats, pixels, names=None):
+def check_norms(mods, batch_stats, pixels, names=None, per_item=False):
     """Without ``batch_stats`` every norm must be in eval mode (RuntimeError).  With it, a train-mode norm must be one the batch
     statistics kernels implement (momentum set, running statistics tracked, affine) and the conv must have at least 2 output
-    pixels (``pixels`` = B * H_out * W_out; torch raises for 1 too); otherwise a ValueError names the layer."""
+    pixels (``pixels`` = B * H_out * W_out, or H_out * W_out per item with ``per_item``; torch raises for 1 too); otherwise a
+    ValueError names the layer."""
     if not batch_stats:
         _check_eval(mods)
         return
@@ -358,15 +408,16 @@ def check_norms(mods, batch_stats, pixels, names=None):
             raise ValueError(f"read_b200: {label}: train-mode BatchNorm needs track_running_stats=True and affine=True on the "
                              f"bf16 path (got track_running_stats={n.track_running_stats}, affine={n.affine})")
         if pixels < 2:
-            raise ValueError(f"read_b200: {label}: train-mode BatchNorm needs more than 1 value per channel (got B * H * W = "
-                             f"{pixels})")
+            got = f"H * W = {pixels} per item" if per_item else f"B * H * W = {pixels}"
+            raise ValueError(f"read_b200: {label}: train-mode BatchNorm needs more than 1 value per channel (got {got})")
 
 
-def stack_forward(mods, x, batch_stats=False, names=None):
+def stack_forward(mods, x, batch_stats=False, names=None, per_item=False):
     """The ResBlocks t -> t + mods[2r+1](mods[2r](t)) applied to x in turn, bf16 on the wgmma kernels.  ``batch_stats``: a conv
-    whose norm is in train mode normalises with batch statistics (else such a conv raises); ``names`` label the convs in errors."""
-    check_norms(mods, batch_stats, x.shape[0] * x.shape[2] * x.shape[3], names)
-    return ResStackFn.apply(x, list(mods), *stack_params(mods))
+    whose norm is in train mode normalises with batch statistics (else such a conv raises), each batch item with its own with
+    ``per_item``; ``names`` label the convs in errors."""
+    check_norms(mods, batch_stats, (1 if per_item else x.shape[0]) * x.shape[2] * x.shape[3], names, per_item)
+    return (ResStackItemsFn if per_item else ResStackFn).apply(x, list(mods), *stack_params(mods))
 
 
 class GatedConvFn(torch.autograd.Function):
@@ -375,10 +426,14 @@ class GatedConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, residual, mod, *params):
+        return GatedConvFn._forward(ctx, x, residual, mod, params, None)
+
+    @staticmethod
+    def _forward(ctx, x, residual, mod, params, items):
         _check_cuda(x)
         lib = L.load()
         cout = params[0].shape[0]
-        conv = FoldedConv(mod, *params, cout=max(cout, 16))
+        conv = FoldedConv(mod, *params, cout=max(cout, 16), items=items)
         if residual is not None and conv.C != cout:
             raise ValueError("read_b200: a residual needs C >= 16")
         t = ops.nchw_to_nhwc(x.detach().float().contiguous(), True)
@@ -417,14 +472,22 @@ class GatedConvFn(torch.autograd.Function):
         return (dx, gout if need[1] else None, None, *grads)
 
 
-def gated_conv(mod, x, residual=None, batch_stats=False, name=None):
+class GatedConvItemsFn(GatedConvFn):
+    """GatedConvFn with per-item statistics for a train-mode norm (each batch item normalised with its own)."""
+
+    @staticmethod
+    def forward(ctx, x, residual, mod, *params):
+        return GatedConvFn._forward(ctx, x, residual, mod, params, x.shape[0])
+
+
+def gated_conv(mod, x, residual=None, batch_stats=False, name=None, per_item=False):
     """bf16 forward of the gated 3x3 stride-1 conv ``mod`` (a GatedConv) on the wgmma kernels, plus ``residual`` (NCHW, the
     output's shape) when given, differentiable through GatedConvFn.  ``batch_stats``: a train-mode norm normalises with batch
-    statistics (else it raises); ``name`` labels the layer in errors."""
+    statistics (else it raises), each batch item with its own with ``per_item``; ``name`` labels the layer in errors."""
     if mod.k != 3 or mod.stride != 1:
         raise ValueError(f"read_b200: gated_conv runs 3x3 stride-1 convs only (got k={mod.k}, stride={mod.stride})")
-    check_norms([mod], batch_stats, x.shape[0] * x.shape[2] * x.shape[3], [name])
-    return GatedConvFn.apply(x, residual, mod, *stack_params([mod]))
+    check_norms([mod], batch_stats, (1 if per_item else x.shape[0]) * x.shape[2] * x.shape[3], [name], per_item)
+    return (GatedConvItemsFn if per_item else GatedConvFn).apply(x, residual, mod, *stack_params([mod]))
 
 
 # ------------------------------------------------------------------ the 1x1 and stride-2 convs ('bf16_all')
@@ -517,12 +580,16 @@ class MultiSourceConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, mod, n_src, *args):
+        return MultiSourceConvFn._forward(ctx, mod, n_src, args, False)
+
+    @staticmethod
+    def _forward(ctx, mod, n_src, args, per_item):
         xs, params = args[:n_src], args[n_src:]
         _check_cuda(xs[0])
         lib = L.load()
         cout = params[0].shape[0]
         ts = [ops.nchw_to_nhwc(x.detach().float().contiguous(), True) for x in xs]
-        conv = FoldedConv(mod, *params, cout=padded_channels(cout), srcs=ts)
+        conv = FoldedConv(mod, *params, cout=padded_channels(cout), srcs=ts, items=xs[0].shape[0] if per_item else None)
         d = _desc(ts, conv.C, mod.k, mod.stride)
         y = torch.empty((d.B, d.Hout, d.Wout, conv.C), dtype=torch.bfloat16, device=ts[0].device)
         conv_forward(lib, ts, conv, y)
@@ -575,11 +642,19 @@ class MultiSourceConvFn(torch.autograd.Function):
         return (None, None, *dxs, *grads)
 
 
-def gated_conv_srcs(mod, xs, name=None, batch_stats=False):
+class MultiSourceConvItemsFn(MultiSourceConvFn):
+    """MultiSourceConvFn with per-item statistics for a train-mode norm (each batch item normalised with its own)."""
+
+    @staticmethod
+    def forward(ctx, mod, n_src, *args):
+        return MultiSourceConvFn._forward(ctx, mod, n_src, args, True)
+
+
+def gated_conv_srcs(mod, xs, name=None, batch_stats=False, per_item=False):
     """bf16 forward of the gated 1x1 or stride-2 conv ``mod`` (a GatedConv) over the NCHW tensors ``xs`` on the wgmma kernels,
     differentiable through MultiSourceConvFn.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels);
     a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors.  ``batch_stats``: a
-    train-mode norm normalises with batch statistics (else it raises)."""
+    train-mode norm normalises with batch statistics (else it raises), each batch item with its own with ``per_item``."""
     label = name or f"GatedConv(k={mod.k}, stride={mod.stride})"
     xs = list(xs)
     if (mod.k, mod.stride) not in GEOMETRIES:
@@ -593,6 +668,6 @@ def gated_conv_srcs(mod, xs, name=None, batch_stats=False):
     if mod.stride == 2 and (xs[0].shape[2] % 2 or xs[0].shape[3] % 2):
         raise ValueError(f"read_b200: {label}: a stride-2 conv needs an even input height and width (got "
                          f"{xs[0].shape[2]}x{xs[0].shape[3]})")
-    pixels = xs[0].shape[0] * (xs[0].shape[2] // mod.stride) * (xs[0].shape[3] // mod.stride)
-    check_norms([mod], batch_stats, pixels, [label])
-    return MultiSourceConvFn.apply(mod, len(xs), *xs, *stack_params([mod]))
+    pixels = (1 if per_item else xs[0].shape[0]) * (xs[0].shape[2] // mod.stride) * (xs[0].shape[3] // mod.stride)
+    check_norms([mod], batch_stats, pixels, [label], per_item)
+    return (MultiSourceConvItemsFn if per_item else MultiSourceConvFn).apply(mod, len(xs), *xs, *stack_params([mod]))

@@ -11,7 +11,8 @@ Contract kept (what train.py, viewer.py and READ/gl/nn.py:76-129 rely on):
   ``return_input=True``, the LAST item's multi-scale net input, as the reference's loop leaves it).
 
 Eval-mode batches that share one texture run as ONE batched net pass (equivalent under eval-mode BatchNorm, SURVEY.md §8a
-"Batching"); in training mode the reference's per-item loop is kept, because BatchNorm statistics are per call there.
+"Batching"); in training mode the reference's per-item loop is kept, because BatchNorm statistics are per call there, unless the
+net normalises each item on its own (``UNet.train_batchnorm = 'per_item'``): then one batched pass computes what the loop does.
 
 Extra fast path (not in the reference): ``render(points, total_m, W, H)`` goes points -> packed z-buffer pyramid -> feature
 pyramid -> net without materialising index maps, including the viewer's ``supersampling`` and ``temporal_average`` options.
@@ -124,8 +125,10 @@ class NetAndTexture(nn.Module):
             if out is not None:
                 return out
         one_texture = len(set(texture_ids)) == 1
-        if one_texture and len(texture_ids) > 1 and not self.temporal_average and not self.net.training:
-            # eval-mode BatchNorm is per-pixel affine: B batch-1 passes == one batch-B pass
+        items_apart = not self.net.training or getattr(self.net, 'train_batchnorm', 'batch') == 'per_item'
+        if one_texture and len(texture_ids) > 1 and not self.temporal_average and items_apart:
+            # eval-mode BatchNorm is per-pixel affine, and per-item train-mode BatchNorm normalises each item with its own
+            # statistics: B batch-1 passes == one batch-B pass
             net_input = self._multiscale_input(self._texture(texture_ids[0]), maps)
             out = self.net(*net_input, **kwargs)
             net_input = [t[-1:] for t in net_input]              # the reference returns the last item's input

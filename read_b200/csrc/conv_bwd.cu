@@ -33,12 +33,12 @@ __device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2
 constexpr int GB_THREADS = 256, GB_MAX_C = 256;
 
 template <bool ELU, bool BATCH>
-__global__ void __launch_bounds__(GB_THREADS)
-gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
-                const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
-                float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
-                const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
+__device__ __forceinline__ void
+gate_bwd_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+              const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+              const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+              float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
+              const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
 {
     __shared__ float red[4][GB_MAX_C];
     for (int i = threadIdx.x; i < 4 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
@@ -117,15 +117,43 @@ gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__res
     }
 }
 
+template <bool ELU, bool BATCH>
+__global__ void __launch_bounds__(GB_THREADS)
+gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+                const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+                float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
+                const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
+{
+    gate_bwd_body<ELU, BATCH>(dy, fm, P, C, half, bias_f, bias_m, scale, mean, inv_std, dfm, dbf, dbm, dgamma, dbeta, sum_dy,
+                              sum_dy_xhat);
+}
+
+// Per-item train-mode BatchNorm (UNet.train_batchnorm = 'per_item'): item i = blockIdx.y is the P rows [i * P, (i + 1) * P) with
+// its own statistics (row i of the [items, C] scale / mean / inv_std / sums), so k1 / k0 come from item i's sums and P; dbias_f /
+// dbias_m accumulate over every item.
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+gate_bwd_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                      const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+                      const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+                      float *__restrict__ dbf, float *__restrict__ dbm, const float *__restrict__ sum_dy,
+                      const float *__restrict__ sum_dy_xhat)
+{
+    const long long it = blockIdx.y, o = it * C;
+    gate_bwd_body<ELU, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, scale + o, mean + o, inv_std + o,
+                             dfm + it * P * 2 * C, dbf, dbm, nullptr, nullptr, sum_dy + o, sum_dy_xhat + o);
+}
+
 // ------------------------------------------------------------------ train-mode BatchNorm: backward reduction
 // sum_dy += sum dy, sum_dy_xhat += sum dy * (g - mean) * inv_std over the P pixels, with g = A(f + b_f) * sigmoid(m + b_m)
 // recomputed from the RAW [f | m] (mean / inv_std: the batch statistics of the forward).  These are dbeta and dgamma, and the
 // two terms the corrected gate backward (gate_bwd_kernel<ELU, true>) needs.  Same thread layout and reduction as the gate backward.
 template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                     const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
-                     const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
+__device__ __forceinline__ void
+bn_bwd_reduce_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                   const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
+                   const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
 {
     __shared__ float red[2][GB_MAX_C];
     for (int i = threadIdx.x; i < 2 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
@@ -170,6 +198,28 @@ bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *
         atomicAdd(sum_dy + c, red[0][c]);
         atomicAdd(sum_dy_xhat + c, red[1][c]);
     }
+}
+
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                     const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
+                     const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
+{
+    bn_bwd_reduce_body<ELU>(dy, fm, P, C, half, bias_f, bias_m, mean, inv_std, sum_dy, sum_dy_xhat);
+}
+
+// per item: the sums of item blockIdx.y (its P rows, its mean / inv_std) into row blockIdx.y of [items, C]
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+bn_bwd_reduce_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C,
+                           int half, const float *__restrict__ bias_f, const float *__restrict__ bias_m,
+                           const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy,
+                           float *__restrict__ sum_dy_xhat)
+{
+    const long long it = blockIdx.y, o = it * C;
+    bn_bwd_reduce_body<ELU>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o, sum_dy + o,
+                            sum_dy_xhat + o);
 }
 
 // ------------------------------------------------------------------ weight gradient
@@ -643,6 +693,59 @@ int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixel
     k<<<(unsigned)gate_grid(pixels, C), GB_THREADS, 0, (cudaStream_t)stream>>>(
         (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
         bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, nullptr, nullptr, sum_dy, sum_dy_xhat);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+// CTAs per item of the per-item gate passes: the call's CTAs are capped as for a single call of all the items' pixels
+static long long gate_grid_items(int items, int64_t pixels, int C)
+{
+    const int ppb = GB_THREADS / (C / 8);
+    long long blocks = (pixels + ppb - 1) / ppb, cap = 8ll * num_sms() / items;
+    if (cap < 1) cap = 1;
+    return blocks > cap ? cap : blocks;
+}
+
+int read_bn_backward_reduce_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu, const float *bias_f,
+                                  const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy,
+                                  float *sum_dy_xhat, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat,
+                 "bn_backward_reduce_items: null pointer");
+    RB_CHECK_ARG(items >= 1 && items <= 65535, "bn_backward_reduce_items: items must lie in 1..65535 (got %d)", items);
+    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    RB_CHECK_ARG(pixels >= 2, "bn_backward_reduce_items: batch statistics need at least 2 pixels per item (got %lld)",
+                 (long long)pixels);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm)) & 15) == 0,
+                 "bn_backward_reduce_items: tensors must be 16B aligned");
+    auto k = elu ? bn_bwd_reduce_items_kernel<true> : bn_bwd_reduce_items_kernel<false>;
+    k<<<dim3((unsigned)gate_grid_items(items, pixels, C), (unsigned)items), GB_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        bn_inv_std, sum_dy, sum_dy_xhat);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                         const float *bias_f, const float *bias_m, const float *bn_scale, const float *bn_mean,
+                                         const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
+                                         float *dbias_f, float *dbias_m, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat && dbias_f &&
+                     dbias_m,
+                 "gate_backward_batch_stats_items: null pointer");
+    RB_CHECK_ARG(items >= 1 && items <= 65535, "gate_backward_batch_stats_items: items must lie in 1..65535 (got %d)", items);
+    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    RB_CHECK_ARG(pixels >= 2, "gate_backward_batch_stats_items: batch statistics need at least 2 pixels per item (got %lld)",
+                 (long long)pixels);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
+                 "gate_backward_batch_stats_items: tensors must be 16B aligned");
+    auto k = elu ? gate_bwd_items_kernel<true> : gate_bwd_items_kernel<false>;
+    k<<<dim3((unsigned)gate_grid_items(items, pixels, C), (unsigned)items), GB_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
+        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, sum_dy, sum_dy_xhat);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

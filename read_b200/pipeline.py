@@ -47,6 +47,10 @@ _CLI = (
     ('--net_train_precision', dict(type=str, default='fp32', choices=['fp32', 'bf16', 'bf16_all'],
                                    help="bf16: train the net's 3x3 stride-1 convs on the wgmma kernels; bf16_all: every conv "
                                         "(UNet.train_precision)"), False),
+    ('--net_train_batchnorm', dict(type=str, default='batch', choices=['batch', 'per_item'],
+                                   help="train-mode BatchNorm statistics over the whole net call (batch) or per crop (per_item: "
+                                        "the training batch runs as one net call, with the statistics of the per-crop loop; "
+                                        "UNet.train_batchnorm)"), False),
 )
 
 
@@ -119,6 +123,7 @@ class TexturePipeline(Pipeline):
         self.args = args
         self.net = get_net(args.input_channels, args)
         self.net.train_precision = getattr(args, 'net_train_precision', 'fp32')
+        self.net.train_batchnorm = getattr(args, 'net_train_batchnorm', 'batch')
         if getattr(args, 'inference', False):
             self.textures = {0: get_texture(args.descriptor_size, args.n_points, args)}
         else:

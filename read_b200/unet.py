@@ -17,6 +17,10 @@ convs (the 1x1 convs and the stride-2 3x3 / 4x4 convs), FAM's product and sum, t
 torch.  ``'bf16_all'`` also moves those 21 convs onto the wgmma kernels (blocks.gated_conv_srcs), so every conv of the net trains
 there; FAM's product and sum, the interpolations, the concats that include an 8-channel source, the loss and the optimizers stay
 on torch.  The default ``'fp32'`` keeps every layer on torch.
+
+``train_batchnorm`` chooses what a train-mode BatchNorm normalises over at every precision: ``'batch'`` (default,
+torch.nn.BatchNorm2d) the whole call, ``'per_item'`` each batch item on its own, with the running statistics updated once per item
+in item order, so one call of B items computes what B calls of one item each would (the reference's per-item training loop).
 """
 import threading
 
@@ -28,6 +32,7 @@ from . import blocks
 from .engine import UNetEngine
 
 TRAIN_PRECISIONS = ('fp32', 'bf16', 'bf16_all')
+TRAIN_BATCHNORMS = ('batch', 'per_item')
 
 
 def layer_table(base=32, num_res=4):
@@ -56,6 +61,17 @@ def layer_table(base=32, num_res=4):
                   (f"{name}.main.2", ch // 2, ch // 2, 3, 1, True), (f"{name}.main.3", ch // 2, ch - 8, 1, 1, True),
                   (f"{name}.conv", ch, ch, 1, 1, False)]
     return t
+
+
+def gated_conv_per_item(mod, x):
+    """GatedConv.forward on torch with a train-mode norm applied to each batch item on its own, in item order (UNet.train_batchnorm
+    = 'per_item'): each item's statistics and running-statistics update, num_batches_tracked advancing by B."""
+    b = mod.block
+    f = b['conv_f'](x)
+    if mod.elu:
+        f = F.elu(f)
+    g = f * torch.sigmoid(b['conv_m'](x))
+    return torch.cat([b['norm'](g[i:i + 1]) for i in range(g.shape[0])])
 
 
 class _Group(nn.Module):
@@ -107,6 +123,8 @@ class UNet(nn.Module):
         # training (autograd) path: 'fp32' = torch operators everywhere | 'bf16' = the 78 gated 3x3 stride-1 convs on the wgmma kernels
         # | 'bf16_all' = all 99 convs on the wgmma kernels
         self.train_precision = 'fp32'
+        # train-mode BatchNorm: 'batch' = statistics over the whole call | 'per_item' = each batch item with its own
+        self.train_batchnorm = 'batch'
         self.conv_impl = 'auto'
         self.use_graph = True
         self._engines = {}
@@ -179,21 +197,31 @@ class UNet(nn.Module):
         eng.set_inputs_nchw(inputs[:4])
         return eng.run().clone()
 
-    def _c(self, name, x):
-        return self.get_submodule(name)(x)
-
     def _forward_torch(self, inputs):
         """Library (cuDNN/autograd) evaluation of unet.py:202-285 on the same parameters; training only."""
-        c = self._c
         x, x_2, x_4, x_8 = inputs[:4]
         tp = getattr(self, 'train_precision', 'fp32')       # modules pickled before the attribute existed
         if tp not in TRAIN_PRECISIONS:
             raise ValueError(f"read_b200.UNet: train_precision must be one of {TRAIN_PRECISIONS}, got {tp!r}")
 
+        tb = getattr(self, 'train_batchnorm', 'batch')
+        if tb not in TRAIN_BATCHNORMS:
+            raise ValueError(f"read_b200.UNet: train_batchnorm must be one of {TRAIN_BATCHNORMS}, got {tb!r}")
+
         bf16 = tp in ('bf16', 'bf16_all')
+        trains = any(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d))
+        per_item = tb == 'per_item' and trains
         # a conv whose BatchNorm is in train mode (the net in train()) normalises with batch statistics on our kernels, like
         # torch's BatchNorm2d; the keyword is passed only when some norm trains, so an eval-mode net calls res_stack as before
-        bs = {'batch_stats': True} if bf16 and any(m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d)) else {}
+        bs = {'batch_stats': True} if bf16 and trains else {}
+        if per_item:
+            bs['per_item'] = True
+
+        def c(name, t):
+            m = self.get_submodule(name)
+            if per_item and m.block['norm'].training:
+                return gated_conv_per_item(m, t)
+            return m(t)
 
         def c3(name, t):
             # the gated 3x3 stride-1 convs outside the blocks: feat_extract.0 / .5, SCM*.main.0 / .2, AFFs.*.conv.1, FAM*.merge

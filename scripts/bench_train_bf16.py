@@ -2,7 +2,11 @@
 the net, sparse RMSprop on the descriptors) with the net trained in fp32 (torch operators, cuDNN), in bf16 (the 78 gated 3x3
 stride-1 convs on the wgmma kernels, UNet.train_precision = 'bf16') and in bf16_all (all 99 convs), alternating in one process
 so that clock drift hits all alike.
-   python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--batchnorm running|batch] [--out result.json]
+   python scripts/bench_train_bf16.py [--steps 10] [--rounds 3] [--batchnorm running|batch|per_item] [--out result.json]
+--batchnorm per_item also puts the model in train(), and alternates per precision NetAndTexture's per-item loop (8 net calls per
+step, UNet.train_batchnorm = 'batch') with one batched net call per step under UNet.train_batchnorm = 'per_item' (each crop
+normalised with its own statistics, as in the loop); it reports the step times, the launches per step and the per-item BatchNorm
+kernels at the C5 shapes of the stacks (8 crops per call).
 --batchnorm batch puts the model in train() (the reference's default training: train-mode BatchNorm with batch statistics, and
 NetAndTexture's per-item loop, B = 1 per net call) and then reports, instead of the eval-mode sections below, the step time per
 precision, the time and bytes of the batch-statistics kernels at the C5 shapes, and the kernel launches per step with and without
@@ -43,13 +47,14 @@ def card():
     return {"torch_name": torch.cuda.get_device_name(0), "nvidia_smi": q}
 
 
-def make_model(sd, tp, dev, batch=False):
+def make_model(sd, tp, dev, batch=False, per_item=False):
     tex = PointTexture(8, N, init_method='zeros')
     with torch.no_grad():
         tex.texture_.copy_(torch.rand((1, 8, N), generator=torch.Generator().manual_seed(synth.SEED)))
     net = UNet()
     net.load_state_dict(sd, strict=True)
     net.train_precision = tp
+    net.train_batchnorm = 'per_item' if per_item else 'batch'
     model = NetAndTexture(net, {0: tex}, 1)
     model.load_textures(0)
     model.to(dev)
@@ -62,10 +67,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--batchnorm", choices=("running", "batch"), default="running")
+    ap.add_argument("--batchnorm", choices=("running", "batch", "per_item"), default="running")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    batch = args.batchnorm == "batch"
+    batch = args.batchnorm in ("batch", "per_item")
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
     L.require_device(0)
@@ -80,7 +85,11 @@ def main():
     keys = ["uv_1d_p1"] + [f"uv_1d_p1_ds{l}" for l in range(1, LEVELS)]
     ids0 = torch.zeros(BC, dtype=torch.long)
     sd = synth.synth_state_dict(synth.SEED)
-    runs = {tp: make_model(sd, tp, dev, batch) for tp in ("fp32", "bf16", "bf16_all")}
+    if args.batchnorm == "per_item":                # the loop and the batched per-item call, alternating per precision
+        runs = {f"{tp} {how}": make_model(sd, tp, dev, True, how == "per_item") for tp in ("fp32", "bf16", "bf16_all")
+                for how in ("loop", "per_item")}
+    else:
+        runs = {tp: make_model(sd, tp, dev, batch) for tp in ("fp32", "bf16", "bf16_all")}
 
     def step(r, m, marks=None):
         e = [ev() for _ in range(4)] if marks is not None else None
@@ -128,6 +137,8 @@ def main():
             tot_ms = sum(e[0].elapsed_time(e[3]) for e in marks) / len(marks)
             share[tp].append({"net_fwd_bwd_ms": net_ms, "step_ms": tot_ms, "share": net_ms / tot_ms})
 
+    if args.batchnorm == "per_item":
+        return report_items(args, runs, ms, share, first_loss, step, mats, dev)
     if batch:
         return report_batch(args, runs, ms, share, first_loss, step, mats, dev)
 
@@ -463,6 +474,80 @@ def report_batch(args, runs, ms, share, first_loss, step, mats, dev):
     print("first-step loss " + ", ".join(f"{tp} {v:.6f}" for tp, v in first_loss.items()))
     for k, v in launches.items():
         print(f"library kernel launches per step, {k}: {v}")
+    for row in kern:
+        print(json.dumps(row))
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        json.dump(res, open(args.out, "w"), indent=1)
+
+
+def report_items(args, runs, ms, share, first_loss, step, mats, dev):
+    """--batchnorm per_item: step times of the loop and the batched per-item call, the launches per step, and the four per-item
+    BatchNorm kernels at the C5 shapes of the stacks with the 8 crops of a step in one call (P = 65536 / 16384 / 4096 / 1024
+    pixels per crop at C = 32 / 64 / 128 / 256)."""
+    lib = L.load()
+    launches = {}
+    for name, r in runs.items():
+        step(r, mats[-1])
+        torch.cuda.synchronize()
+        n0 = ops.launch_count()
+        step(r, mats[-2])
+        torch.cuda.synchronize()
+        launches[name] = ops.launch_count() - n0
+
+    kern = []
+    reps, items = 50, BC
+    for C, side in ((32, 256), (64, 128), (128, 64), (256, 32)):
+        P = side * side
+        g = torch.randn((items * P, C), device=dev).bfloat16()
+        fm = torch.randn((items * P, 2 * C), device=dev).bfloat16()
+        dy = torch.randn((items * P, C), device=dev).bfloat16()
+        dfm, y = torch.empty_like(fm), torch.empty_like(g)
+        v = torch.rand((6, C), device=dev) + 0.5                           # bias_f, bias_m, gamma, beta, running mean / var
+        it = torch.rand((6, items, C), device=dev) + 0.5                   # mean, inv_std, scale, shift, sum_dy, sum_dy_xhat
+        red = torch.zeros((2, C), device=dev)
+        ws = torch.empty(lib.read_bn_workspace_bytes_items(items, C), dtype=torch.uint8, device=dev)
+        st = L.stream_ptr()
+        p, q = [t.data_ptr() for t in v], [t.data_ptr() for t in it]
+        fns = {
+            "bn_stats_items": (lambda: L.check(lib.read_bn_batch_stats_items(
+                g.data_ptr(), items, P, C, C, p[2], p[3], 1e-5, 0.1, p[4], p[5], q[0], q[1], q[2], q[3], ws.data_ptr(), st)),
+                items * P * C * 2),
+            "bn_apply_items": (lambda: L.check(lib.read_bn_apply_items(g.data_ptr(), items, P, C, q[2], q[3], None, y.data_ptr(),
+                                                                       st)), 2 * items * P * C * 2),
+            "bn_backward_reduce_items": (lambda: L.check(lib.read_bn_backward_reduce_items(
+                dy.data_ptr(), fm.data_ptr(), items, P, C, 1, p[0], p[1], q[0], q[1], q[4], q[5], st)), 3 * items * P * C * 2),
+            "gate_backward_batch_stats_items": (lambda: L.check(lib.read_gate_backward_batch_stats_items(
+                dy.data_ptr(), fm.data_ptr(), items, P, C, 1, p[0], p[1], q[2], q[0], q[1], q[4], q[5], dfm.data_ptr(),
+                red[0].data_ptr(), red[1].data_ptr(), st)), 5 * items * P * C * 2),
+        }
+        for name, (fn, nbytes) in fns.items():
+            for _ in range(5):
+                fn()
+            rounds = []
+            for _ in range(3):
+                a, b = ev(), ev()
+                a.record()
+                for _ in range(reps):
+                    fn()
+                b.record()
+                torch.cuda.synchronize()
+                rounds.append(a.elapsed_time(b) * 1e3 / reps)
+            us = sorted(rounds)[1]
+            kern.append({"kernel": name, "C": C, "items": items, "pixels_per_item": P, "us": round(us, 2),
+                         "rounds_us": [round(x, 2) for x in rounds], "bytes": nbytes,
+                         "share_of_3.35TB/s": round(nbytes / (us * 1e-6) / 3.35e12, 3)})
+
+    res = {"card": card(), "batchnorm": "per_item", "steps": args.steps, "rounds": args.rounds, "crops_per_step": BC,
+           "size": f"{W}x{H}", "n_points": N, "ms_per_step": ms, "net_fwd_bwd_per_step": share, "first_loss": first_loss,
+           "launches_per_step": launches, "per_item_kernels": kern}
+    print(f"card: {res['card']}")
+    for name in runs:
+        med = sorted(ms[name])[len(ms[name]) // 2]
+        sh = sorted(share[name], key=lambda x: x["share"])[len(share[name]) // 2]
+        print(f"{name} (train mode): {med:.2f} ms/step (rounds {', '.join(f'{v:.2f}' for v in ms[name])}), net fwd+bwd "
+              f"{sh['net_fwd_bwd_ms']:.2f} ms of a {sh['step_ms']:.2f} ms profiled step, {launches[name]} library launches")
+    print("first-step loss " + ", ".join(f"{k} {v:.6f}" for k, v in first_loss.items()))
     for row in kern:
         print(json.dumps(row))
     if args.out:
