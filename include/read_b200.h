@@ -409,6 +409,33 @@ int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int ite
                                          const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
                                          float *dbias_f, float *dbias_m, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * VGG19 perceptual loss (read_b200/vgg_loss.py, the reference's READ/criterions/vgg_loss.py).  The convs are RAW 3x3 plans of the
+ * TMA-fed kernel (a plain conv of c filters = the gated pair of c/2 whose RAW column order is the natural channel order) and, for
+ * the image's input gradient, read_conv3x3_dgrad_cin8; these entry points are the glue around them.  A call holds n output images
+ * and n target images as ONE NHWC bf16 batch of 2n: images 0 .. n-1 the output, n .. 2n-1 the target.
+ *   read_vgg_workspace_bytes : bytes of the workspace read_vgg_post needs on a loss layer (16B aligned, one call at a time)
+ *   read_vgg_normalize   : input, target NCHW f32 [n,3,H,W] -> out [2n,H,W,8] bf16 = (x - mean[c]) / std[c] (channels 3..7 zero);
+ *                          mean, std f32 [3] device
+ *   read_vgg_post        : raw [2n,H,W,C] bf16 = a conv's RAW accumulators; y = ReLU(raw + bias[c]) for both halves.  term
+ *                          (nullable: not a loss layer): *term (double, device) += scale * sum |y_out - y_tgt|, deterministic (fixed
+ *                          combine order for a given shape).  code (nullable) int8 [n,H,W,C]: 0 where y_out = 0, else
+ *                          2 + sign(y_out - y_tgt) (2 off the loss layers).  out (nullable): pool = 0: y [2n,H,W,C] (may be raw);
+ *                          pool = 1: AvgPool2d(2, 2) of y, [2n,H/2,W/2,C] (floor).  C % 8 == 0
+ *   read_vgg_dgrad_in    : dy [n,H,W,C] bf16 = [code != 0] * (U + (code - 2) * g[0] * coef), U = up [n,H,W,C] (pool = 0) or the
+ *                          AvgPool2d(2, 2) backward of up [n,H/2,W/2,C] (pool = 1: up / 4, 0 on a dropped odd row / column), 0 when
+ *                          up is NULL; g f32 [1] device
+ *   read_vgg_image_grad  : dx [n,H,W,8] bf16 -> out [n,3,H,W] f32 = dx[c] / std[c] (channels 3..7 ignored)
+ * ---------------------------------------------------------------------------------------- */
+int64_t read_vgg_workspace_bytes(void);
+int read_vgg_normalize(const float *input, const float *target, int n, int H, int W, const float *mean, const float *std_, void *out,
+                       void *stream);
+int read_vgg_post(const void *raw, int n, int H, int W, int C, const float *bias, int pool, void *out, void *code, double *term,
+                  double scale, void *workspace, void *stream);
+int read_vgg_dgrad_in(const void *up, int pool, const void *code, int n, int H, int W, int C, const float *g, float coef, void *dy,
+                      void *stream);
+int read_vgg_image_grad(const void *dx, int n, int H, int W, const float *std_, float *out, void *stream);
+
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);
 
