@@ -426,6 +426,13 @@ int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int ite
  *                          AvgPool2d(2, 2) backward of up [n,H/2,W/2,C] (pool = 1: up / 4, 0 on a dropped odd row / column), 0 when
  *                          up is NULL; g f32 [1] device
  *   read_vgg_image_grad  : dx [n,H,W,8] bf16 -> out [n,3,H,W] f32 = dx[c] / std[c] (channels 3..7 ignored)
+ * partialconv=True: conv1_1 is a partial conv over the target's validity mask M [n,H,W] (1 where the target's channel sum
+ * > 1e-9, else 0; the same M for output b and target b).  With cnt = valid pixels of M's 3x3 window at a pixel (zero padding),
+ * upd = [cnt > 0] and ratio = upd * reciprocal(cnt) * 9 (fp32, torch's rounding of 9 / (cnt + 1e-8)):
+ *   read_vgg_normalize_masked  : as read_vgg_normalize, both halves times M; mask (out) uint8 [n,H,W] = M
+ *   read_vgg_post_partial      : as read_vgg_post with pool = 0 and y = ReLU((raw * ratio + bias[c]) * upd); mask uint8 [n,H,W]
+ *   read_vgg_dgrad_in_partial  : as read_vgg_dgrad_in with pool = 0, times ratio
+ *   read_vgg_image_grad_masked : as read_vgg_image_grad, times M
  * ---------------------------------------------------------------------------------------- */
 int64_t read_vgg_workspace_bytes(void);
 int read_vgg_normalize(const float *input, const float *target, int n, int H, int W, const float *mean, const float *std_, void *out,
@@ -435,6 +442,13 @@ int read_vgg_post(const void *raw, int n, int H, int W, int C, const float *bias
 int read_vgg_dgrad_in(const void *up, int pool, const void *code, int n, int H, int W, int C, const float *g, float coef, void *dy,
                       void *stream);
 int read_vgg_image_grad(const void *dx, int n, int H, int W, const float *std_, float *out, void *stream);
+int read_vgg_normalize_masked(const float *input, const float *target, int n, int H, int W, const float *mean, const float *std_,
+                              void *out, void *mask, void *stream);
+int read_vgg_post_partial(const void *raw, const void *mask, int n, int H, int W, int C, const float *bias, void *out, void *code,
+                          double *term, double scale, void *workspace, void *stream);
+int read_vgg_dgrad_in_partial(const void *up, const void *mask, const void *code, int n, int H, int W, int C, const float *g,
+                              float coef, void *dy, void *stream);
+int read_vgg_image_grad_masked(const void *dx, const void *mask, int n, int H, int W, const float *std_, float *out, void *stream);
 
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);

@@ -122,6 +122,10 @@ _SIGS = {
     "read_vgg_post": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, ctypes.c_double, c_vp, c_vp]),
     "read_vgg_dgrad_in": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_vp, ctypes.c_float, c_vp, c_vp]),
     "read_vgg_image_grad": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "read_vgg_normalize_masked": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_vgg_post_partial": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_vp, c_vp]),
+    "read_vgg_dgrad_in_partial": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, ctypes.c_float, c_vp, c_vp]),
+    "read_vgg_image_grad_masked": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "read_conv_tc_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_conv_tcg_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_tcg_weight_elems": (c_i64, [c_int, c_int, c_int]),

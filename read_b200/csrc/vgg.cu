@@ -10,6 +10,13 @@
 //                   the next conv's input gradient (read through the pool's backward: a quarter of the pooled gradient, 0 on the
 //                   dropped rows / columns), coef = 1 / numel of the layer's L1 term (0 off the loss layers)
 //   vgg_image_grad  NHWC bf16 8-channel input gradient -> NCHW f32 3 channels, divided by std
+// partialconv=True (the mask-aware loss) runs VGG's first conv as a partial convolution over the validity mask M of the target
+// (M = [sum of the target's channels > 1e-9]), the same M for both halves.  Four variants, each used at conv1_1 only:
+//   vgg_normalize_masked   vgg_normalize, both halves' channels times M, and M as one byte per pixel [n, H, W]
+//   vgg_post_partial       vgg_post (no pool) with y = ReLU((raw * ratio + bias) * upd): upd = [the 3x3 window of M holds a valid
+//                          pixel], ratio = upd * 9 / (valid pixels in it), both recomputed from the byte mask
+//   vgg_dgrad_in_partial   vgg_dgrad_in (no pool) times ratio
+//   vgg_image_grad_masked  vgg_image_grad times M
 #include "common.cuh"
 #include "conv_common.cuh"
 
@@ -42,6 +49,27 @@ static unsigned vg_blocks(long long units)
     return (unsigned)(b < 1 ? 1 : b > VG_MAX_CTAS ? VG_MAX_CTAS : b);
 }
 
+// Valid pixels in the 3x3 window at (y, x) of one H x W byte mask, zero padding outside: the partial conv's 0 .. 9 count
+__device__ __forceinline__ int vg_window(const uint8_t *__restrict__ m, int H, int W, int y, int x)
+{
+    int c = 0;
+#pragma unroll
+    for (int dy = -1; dy <= 1; ++dy) {
+        const int yy = y + dy;
+        if (yy < 0 || yy >= H) continue;
+#pragma unroll
+        for (int dx = -1; dx <= 1; ++dx) {
+            const int xx = x + dx;
+            if (xx >= 0 && xx < W) c += m[(long long)yy * W + xx];
+        }
+    }
+    return c;
+}
+
+// The partial conv's ratio 9 / (c + 1e-8) * clamp(c, 0, 1) as torch evaluates it in fp32: 1e-8 is below half an ulp of c >= 1, and
+// 9 / t is reciprocal(t) * 9, two roundings (it differs from a correctly rounded 9 / c at c = 5 and 7)
+__device__ __forceinline__ float vg_ratio(int c) { return c ? __fmul_rn(__frcp_rn((float)c), 9.f) : 0.f; }
+
 // ------------------------------------------------------------------ 1. normalise
 __global__ void __launch_bounds__(VG_THREADS)
 vgg_normalize_kernel(const float *__restrict__ in, const float *__restrict__ tgt, int n, int H, int W, const float *__restrict__ mean,
@@ -60,16 +88,43 @@ vgg_normalize_kernel(const float *__restrict__ in, const float *__restrict__ tgt
     }
 }
 
+// One thread per pixel of image b: reads the pixel of output b and of target b, writes both halves and the mask byte.
+__global__ void __launch_bounds__(VG_THREADS)
+vgg_normalize_masked_kernel(const float *__restrict__ in, const float *__restrict__ tgt, int n, int H, int W,
+                            const float *__restrict__ mean, const float *__restrict__ stdv, __nv_bfloat16 *__restrict__ out,
+                            uint8_t *__restrict__ mask)
+{
+    const long long HW = (long long)H * W, total = (long long)n * HW;
+    const float m0 = mean[0], m1 = mean[1], m2 = mean[2], s0 = stdv[0], s1 = stdv[1], s2 = stdv[2];
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long b = i / HW, p = i - b * HW;
+        const float *x = in + b * 3 * HW + p, *t = tgt + b * 3 * HW + p;
+        const float t0 = t[0], t1 = t[HW], t2 = t[2 * HW];
+        // target.sum(1) > 1e-9 in fp32
+        const float m = __fadd_rn(__fadd_rn(t0, t1), t2) > 1e-9f ? 1.f : 0.f;
+        // ((x - mean) / std) * M, each operation rounded as torch rounds it
+        const float x0 = __fmul_rn(__fdiv_rn(__fsub_rn(x[0], m0), s0), m), x1 = __fmul_rn(__fdiv_rn(__fsub_rn(x[HW], m1), s1), m),
+                    x2 = __fmul_rn(__fdiv_rn(__fsub_rn(x[2 * HW], m2), s2), m);
+        const float y0 = __fmul_rn(__fdiv_rn(__fsub_rn(t0, m0), s0), m), y1 = __fmul_rn(__fdiv_rn(__fsub_rn(t1, m1), s1), m),
+                    y2 = __fmul_rn(__fdiv_rn(__fsub_rn(t2, m2), s2), m);
+        *reinterpret_cast<uint4 *>(out + i * 8) = make_uint4(bf16x2_bits(x0, x1), bf16x2_bits(x2, 0.f), 0u, 0u);
+        *reinterpret_cast<uint4 *>(out + (total + i) * 8) = make_uint4(bf16x2_bits(y0, y1), bf16x2_bits(y2, 0.f), 0u, 0u);
+        mask[i] = (uint8_t)(m != 0.f);
+    }
+}
+
 // ------------------------------------------------------------------ 2. bias, ReLU, L1 term, backward code, pool
 // A work unit is 8 channels (16 bytes) of one P x P pixel block (P = 2 before a pool, else 1) of output image b and of target
 // image b + n.  Threads sum |y_out - y_tgt| in fp32; a CTA adds its threads' sums in double in a fixed tree, the last CTA to
 // finish (counter + fence) adds the CTAs' in CTA order and adds the result, times scale (1 / numel of the term), to *term.
-template <int P>
-__global__ void __launch_bounds__(VG_THREADS)
-vgg_post_kernel(const __nv_bfloat16 *raw, int n, int H, int W, int C, const float *__restrict__ bias, __nv_bfloat16 *out,
-                int8_t *__restrict__ code, double *__restrict__ term, double scale, double *__restrict__ part,
-                unsigned int *__restrict__ counter)
+// PARTIAL (P = 1 only): the partial conv of conv1_1 over the byte mask [n, H, W] before the ReLU, (raw * ratio + bias) * upd.
+template <int P, bool PARTIAL>
+__device__ __forceinline__ void vgg_post_body(const __nv_bfloat16 *raw, const uint8_t *__restrict__ mask, int n, int H, int W, int C,
+                                              const float *__restrict__ bias, __nv_bfloat16 *out, int8_t *__restrict__ code,
+                                              double *__restrict__ term, double scale, double *__restrict__ part,
+                                              unsigned int *__restrict__ counter)
 {
+    static_assert(!PARTIAL || P == 1, "the partial conv is VGG's first, which no pool follows");
     __shared__ double red[VG_THREADS];
     __shared__ bool last;
     const int G = C / 8;
@@ -100,11 +155,23 @@ vgg_post_kernel(const __nv_bfloat16 *raw, int n, int H, int W, int C, const floa
                 float fi[8], ft[8];
                 unpack8(ld8(raw + o), fi);
                 unpack8(ld8(raw + o + (long long)n * img), ft);
+                float ratio = 1.f;
+                bool upd = true;
+                if (PARTIAL) {
+                    const int c = vg_window(mask + (long long)b * H * W, H, W, y, x);
+                    upd = c != 0;
+                    ratio = vg_ratio(c);
+                }
                 uint32_t cw[2] = {0u, 0u};
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    fi[j] = fmaxf(fi[j] + bs[j], 0.f);
-                    ft[j] = fmaxf(ft[j] + bs[j], 0.f);
+                    if (PARTIAL) {
+                        fi[j] = upd ? fmaxf(fi[j] * ratio + bs[j], 0.f) : 0.f;
+                        ft[j] = upd ? fmaxf(ft[j] * ratio + bs[j], 0.f) : 0.f;
+                    } else {
+                        fi[j] = fmaxf(fi[j] + bs[j], 0.f);
+                        ft[j] = fmaxf(ft[j] + bs[j], 0.f);
+                    }
                     const float d = fi[j] - ft[j];
                     if (term) acc += fabsf(d);
                     const int s = term ? (d > 0.f) - (d < 0.f) : 0;
@@ -152,12 +219,31 @@ vgg_post_kernel(const __nv_bfloat16 *raw, int n, int H, int W, int C, const floa
     }
 }
 
-// ------------------------------------------------------------------ 3. gradient into a conv's RAW output
-template <bool POOL>
+template <int P>
 __global__ void __launch_bounds__(VG_THREADS)
-vgg_dgrad_in_kernel(const __nv_bfloat16 *__restrict__ up, const int8_t *__restrict__ code, int n, int H, int W, int C,
-                    const float *__restrict__ g, float coef, __nv_bfloat16 *__restrict__ dy)
+vgg_post_kernel(const __nv_bfloat16 *raw, int n, int H, int W, int C, const float *__restrict__ bias, __nv_bfloat16 *out,
+                int8_t *__restrict__ code, double *__restrict__ term, double scale, double *__restrict__ part,
+                unsigned int *__restrict__ counter)
 {
+    vgg_post_body<P, false>(raw, nullptr, n, H, W, C, bias, out, code, term, scale, part, counter);
+}
+
+__global__ void __launch_bounds__(VG_THREADS)
+vgg_post_partial_kernel(const __nv_bfloat16 *raw, const uint8_t *__restrict__ mask, int n, int H, int W, int C,
+                        const float *__restrict__ bias, __nv_bfloat16 *out, int8_t *__restrict__ code, double *__restrict__ term,
+                        double scale, double *__restrict__ part, unsigned int *__restrict__ counter)
+{
+    vgg_post_body<1, true>(raw, mask, n, H, W, C, bias, out, code, term, scale, part, counter);
+}
+
+// ------------------------------------------------------------------ 3. gradient into a conv's RAW output
+// PARTIAL (no pool): times the partial conv's ratio at the pixel, recomputed from the byte mask [n, H, W].
+template <bool POOL, bool PARTIAL>
+__device__ __forceinline__ void vgg_dgrad_in_body(const __nv_bfloat16 *__restrict__ up, const int8_t *__restrict__ code,
+                                                  const uint8_t *__restrict__ mask, int n, int H, int W, int C,
+                                                  const float *__restrict__ g, float coef, __nv_bfloat16 *__restrict__ dy)
+{
+    static_assert(!(PARTIAL && POOL), "the partial conv is VGG's first, which no pool follows");
     const int G = C / 8, Hu = POOL ? H / 2 : H, Wu = POOL ? W / 2 : W;
     const long long units = (long long)n * H * W * G;
     const float l1 = g[0] * coef;
@@ -185,8 +271,28 @@ vgg_dgrad_in_kernel(const __nv_bfloat16 *__restrict__ up, const int8_t *__restri
             const int c = (int)(((j < 4 ? cv.x : cv.y) >> (8 * (j % 4))) & 0xFFu);
             d[j] = c ? uf[j] + (float)(c - 2) * l1 : 0.f;
         }
+        if (PARTIAL) {
+            const float ratio = vg_ratio(vg_window(mask + (long long)b * H * W, H, W, y, x));
+#pragma unroll
+            for (int j = 0; j < 8; ++j) d[j] *= ratio;
+        }
         *reinterpret_cast<uint4 *>(dy + u * 8) = pack8(d);
     }
+}
+
+template <bool POOL>
+__global__ void __launch_bounds__(VG_THREADS)
+vgg_dgrad_in_kernel(const __nv_bfloat16 *__restrict__ up, const int8_t *__restrict__ code, int n, int H, int W, int C,
+                    const float *__restrict__ g, float coef, __nv_bfloat16 *__restrict__ dy)
+{
+    vgg_dgrad_in_body<POOL, false>(up, code, nullptr, n, H, W, C, g, coef, dy);
+}
+
+__global__ void __launch_bounds__(VG_THREADS)
+vgg_dgrad_in_partial_kernel(const __nv_bfloat16 *__restrict__ up, const int8_t *__restrict__ code, const uint8_t *__restrict__ mask,
+                            int n, int H, int W, int C, const float *__restrict__ g, float coef, __nv_bfloat16 *__restrict__ dy)
+{
+    vgg_dgrad_in_body<false, true>(up, code, mask, n, H, W, C, g, coef, dy);
 }
 
 // ------------------------------------------------------------------ 4. image gradient
@@ -203,6 +309,25 @@ vgg_image_grad_kernel(const __nv_bfloat16 *__restrict__ dx, int n, int H, int W,
         o[0] = __fdiv_rn(f[0], s0);
         o[HW] = __fdiv_rn(f[1], s1);
         o[2 * HW] = __fdiv_rn(f[2], s2);
+    }
+}
+
+__global__ void __launch_bounds__(VG_THREADS)
+vgg_image_grad_masked_kernel(const __nv_bfloat16 *__restrict__ dx, const uint8_t *__restrict__ mask, int n, int H, int W,
+                             const float *__restrict__ stdv, float *__restrict__ out)
+{
+    const long long HW = (long long)H * W, total = (long long)n * HW;
+    const float s0 = stdv[0], s1 = stdv[1], s2 = stdv[2];
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const long long b = i / HW, p = i - b * HW;
+        float f[8];
+        unpack8(ld8(dx + i * 8), f);
+        const float m = mask[i] ? 1.f : 0.f;
+        float *o = out + b * 3 * HW + p;
+        // (dx * M) / std, the backward of ((x - mean) / std) * M
+        o[0] = __fdiv_rn(__fmul_rn(f[0], m), s0);
+        o[HW] = __fdiv_rn(__fmul_rn(f[1], m), s1);
+        o[2 * HW] = __fdiv_rn(__fmul_rn(f[2], m), s2);
     }
 }
 
@@ -280,6 +405,62 @@ int read_vgg_image_grad(const void *dx, int n, int H, int W, const float *std_, 
     RB_CHECK_ARG(vg_aligned(dx, 16), "vgg_image_grad: input must be 16B aligned");
     vgg_image_grad_kernel<<<vg_blocks((long long)n * H * W), VG_THREADS, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)dx, n, H, W,
                                                                                                   std_, out);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_vgg_normalize_masked(const float *input, const float *target, int n, int H, int W, const float *mean, const float *std_,
+                              void *out, void *mask, void *stream)
+{
+    RB_CHECK_ARG(input && target && mean && std_ && out && mask, "vgg_normalize_masked: null pointer");
+    RB_CHECK_ARG(n > 0 && H > 0 && W > 0, "vgg_normalize_masked: empty batch (n = %d, %d x %d)", n, H, W);
+    RB_CHECK_ARG(vg_aligned(out, 16), "vgg_normalize_masked: output must be 16B aligned");
+    vgg_normalize_masked_kernel<<<vg_blocks((long long)n * H * W), VG_THREADS, 0, (cudaStream_t)stream>>>(
+        input, target, n, H, W, mean, std_, (__nv_bfloat16 *)out, (uint8_t *)mask);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_vgg_post_partial(const void *raw, const void *mask, int n, int H, int W, int C, const float *bias, void *out, void *code,
+                          double *term, double scale, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(raw && mask && bias, "vgg_post_partial: null pointer");
+    RB_CHECK_ARG(n > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "vgg_post_partial: bad shape (n = %d, %d x %d x %d)", n, H, W, C);
+    RB_CHECK_ARG(!term || workspace, "vgg_post_partial: a loss layer needs the workspace");
+    RB_CHECK_ARG(vg_aligned(raw, 16) && vg_aligned(out, 16) && vg_aligned(code, 8) && vg_aligned(workspace, 16),
+                 "vgg_post_partial: tensors must be 16B aligned (code 8B)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned int *counter = (unsigned int *)workspace;
+    double *part = workspace ? (double *)((char *)workspace + 256) : nullptr;
+    if (term) RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), st));
+    vgg_post_partial_kernel<<<vg_blocks((long long)n * H * W * (C / 8)), VG_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)raw, (const uint8_t *)mask, n, H, W, C, bias, (__nv_bfloat16 *)out, (int8_t *)code, term, scale, part,
+        counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_vgg_dgrad_in_partial(const void *up, const void *mask, const void *code, int n, int H, int W, int C, const float *g,
+                              float coef, void *dy, void *stream)
+{
+    RB_CHECK_ARG(mask && code && g && dy, "vgg_dgrad_in_partial: null pointer");
+    RB_CHECK_ARG(n > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "vgg_dgrad_in_partial: bad shape (n = %d, %d x %d x %d)", n, H, W,
+                 C);
+    RB_CHECK_ARG(vg_aligned(up, 16) && vg_aligned(code, 8) && vg_aligned(dy, 16),
+                 "vgg_dgrad_in_partial: tensors must be 16B aligned (code 8B)");
+    vgg_dgrad_in_partial_kernel<<<vg_blocks((long long)n * H * W * (C / 8)), VG_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)up, (const int8_t *)code, (const uint8_t *)mask, n, H, W, C, g, coef, (__nv_bfloat16 *)dy);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_vgg_image_grad_masked(const void *dx, const void *mask, int n, int H, int W, const float *std_, float *out, void *stream)
+{
+    RB_CHECK_ARG(dx && mask && std_ && out, "vgg_image_grad_masked: null pointer");
+    RB_CHECK_ARG(n > 0 && H > 0 && W > 0, "vgg_image_grad_masked: empty batch (n = %d, %d x %d)", n, H, W);
+    RB_CHECK_ARG(vg_aligned(dx, 16), "vgg_image_grad_masked: input must be 16B aligned");
+    vgg_image_grad_masked_kernel<<<vg_blocks((long long)n * H * W), VG_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)dx, (const uint8_t *)mask, n, H, W, std_, out);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

@@ -13,6 +13,12 @@ int8 code per element of the output half: the ReLU mask and the sign of f_in - f
 when a pool follows.  Backward, last conv to first: dY = mask * (upstream + sign * g / numel) (the pool's backward folded into the
 read of the upstream gradient), then the conv's input gradient: a RAW plan with read_pack_weights_tc_dgrad filters, or for the
 image (conv1_1, 3 channels run as 8) read_conv3x3_dgrad_cin8.  The packed filters are cached per module and device.
+
+partialconv=True is the mask-aware form: conv1_1 becomes a partial convolution (PartialConv2d) over the validity mask of the target
+(M = [sum of the target's channels > 1e-9], from the raw target, the same M for both images).  The forward then normalises with
+read_vgg_normalize_masked (both images times M, M saved as one byte per pixel) and runs conv1_1's post-conv pass as
+read_vgg_post_partial; backward multiplies conv1_1's dY by the partial conv's ratio (read_vgg_dgrad_in_partial) and the image
+gradient by M (read_vgg_image_grad_masked).  Nothing flows through the mask: it depends on the target only.
 """
 import os
 
@@ -45,10 +51,52 @@ def vgg19_modules():
     return out
 
 
+MASK_EPS = 1e-9                                  # a target pixel is valid where its channel sum exceeds this
+
+
+class PartialConv2d(nn.Conv2d):
+    """VGG's first conv as partialconv=True runs it: a partial convolution with one mask channel shared by all input channels
+    (Liu et al., "Image Inpainting for Irregular Holes Using Partial Convolutions", 2018).  With cnt the number of valid pixels
+    in each window of ``mask_in`` [B, 1, H, W] (zero padding), upd = clamp(cnt, 0, 1) and ratio = window size / (cnt + 1e-8) * upd:
+    out = (conv(input * mask_in) * ratio + bias) * upd.  The parameters are those of the plain conv it replaces (state_dict keys
+    ``weight`` / ``bias``); the mask gets no gradient.  Built with from_conv, so that the weights are shared, not copied."""
+
+    @classmethod
+    def from_conv(cls, conv):
+        p = cls(conv.in_channels, conv.out_channels, conv.kernel_size, stride=conv.stride, padding=conv.padding,
+                dilation=conv.dilation, groups=conv.groups, bias=conv.bias is not None, device='meta')
+        p.weight, p.bias = conv.weight, conv.bias
+        return p
+
+    def forward(self, input, mask_in):
+        with torch.no_grad():
+            ones = torch.ones((1, 1, *self.kernel_size), dtype=mask_in.dtype, device=mask_in.device)
+            cnt = F.conv2d(mask_in, ones, stride=self.stride, padding=self.padding, dilation=self.dilation)
+            upd = cnt.clamp(0, 1)
+            ratio = self.kernel_size[0] * self.kernel_size[1] / (cnt + 1e-8) * upd
+        out = F.conv2d(input * mask_in, self.weight, None, self.stride, self.padding, self.dilation, self.groups) * ratio
+        if self.bias is not None:
+            out = out + self.bias.view(1, -1, 1, 1)
+        return out * upd
+
+
+def partial_features(features):
+    """A new nn.Sequential of ``features``' modules with the first conv replaced by a PartialConv2d sharing its weight and bias:
+    the layout VGGLoss(partialconv=True, features=...) takes.  ``features`` itself is not modified."""
+    mods = list(features)
+    mods[0] = PartialConv2d.from_conv(mods[0])
+    return nn.Sequential(*mods)
+
+
+def target_mask(target):
+    """partialconv=True's validity mask [B, 1, H, W] of the raw target: 1 where the channels sum above MASK_EPS, else 0."""
+    return (target.sum(1, keepdim=True) > MASK_EPS).to(target.dtype)
+
+
 def check_layout(features):
     """Raise a ValueError unless ``features`` is an nn.Sequential in the layout of torchvision's vgg19().features: 37 modules,
     3x3 stride-1 pad-1 convs with bias at the VGG19 channel counts, ReLUs, and 2x2 pools (MaxPool2d, or the reference's
-    AvgPool2d(2, 2)) where the pools are."""
+    AvgPool2d(2, 2)) where the pools are.  The first conv may be a PartialConv2d (partialconv=True)."""
     if not isinstance(features, nn.Sequential):
         raise ValueError(f"read_b200.VGGLoss: features must be an nn.Sequential (got {type(features).__name__})")
     mods, want = list(features), vgg19_modules()
@@ -61,7 +109,7 @@ def check_layout(features):
             ok = (isinstance(m, (nn.MaxPool2d, nn.AvgPool2d)) and _pair(m.kernel_size) == (2, 2) and _pair(m.stride) == (2, 2)
                   and _pair(m.padding) == (0, 0) and not m.ceil_mode)
         else:
-            ok = (isinstance(m, nn.Conv2d) and type(m) is nn.Conv2d and (m.in_channels, m.out_channels) == w[1:]
+            ok = (type(m) in ((nn.Conv2d, PartialConv2d) if i == 0 else (nn.Conv2d,)) and (m.in_channels, m.out_channels) == w[1:]
                   and m.kernel_size == (3, 3) and m.stride == (1, 1) and m.padding == (1, 1) and m.dilation == (1, 1)
                   and m.groups == 1 and m.bias is not None and m.padding_mode == 'zeros')
         if not ok:
@@ -161,13 +209,17 @@ def normalization(net):
 
 def reference_loss(vgg19, mean, std, layers, input, target):
     """The reference's loop (vgg_loss.py:100-111) in torch, stopped after the last loss layer: DataParallel replicas, the float64
-    restatement of the tests and the torch arm of the benchmark."""
+    restatement of the tests and the torch arm of the benchmark.  A PartialConv2d runs over target_mask(target) for both images."""
+    mask = target_mask(target) if any(isinstance(m, PartialConv2d) for m in vgg19) else None
     x, y = (input - mean) / std, (target - mean) / std
     loss = 0
     for i, layer in enumerate(vgg19):
         if i > max(layers):
             break
-        x, y = layer(x), layer(y)
+        if isinstance(layer, PartialConv2d):
+            x, y = layer(x, mask), layer(y, mask)
+        else:
+            x, y = layer(x), layer(y)
         if i in layers:
             loss = loss + F.l1_loss(x, y)
     return loss
@@ -176,18 +228,26 @@ def reference_loss(vgg19, mean, std, layers, input, target):
 class VGGLoss(nn.Module):
     """Drop-in for READ.criterions.vgg_loss.VGGLoss: same constructor, buffers (mean_, std_), module list (vgg19, pools as
     AvgPool2d(2, 2)) and forward(input, target) -> scalar.  ``features``: VGG19's features (torchvision layout) to use instead of
-    the file ``net`` names.  partialconv=True is not supported."""
+    the file ``net`` names.  partialconv=True runs vgg19[0] as a PartialConv2d over the target's validity mask: loaded from the
+    file, the plain conv is wrapped as the reference does (same weight and bias Parameters).  ``features`` is used exactly as
+    given, never rewritten: its first conv must already be a PartialConv2d when partialconv=True (partial_features(features)
+    builds that layout) and a plain Conv2d otherwise."""
 
     def __init__(self, net='caffe', partialconv=False, optimized=False, save_dir='.cache/torch/models', features=None):
         super().__init__()
-        if partialconv:
-            raise ValueError("read_b200.VGGLoss: partialconv=True is not supported")
         if net not in ('caffe', 'pytorch'):
             raise ValueError(f"read_b200.VGGLoss: net must be 'caffe' or 'pytorch' (got {net!r})")
-        self.partialconv = False
-        if features is None:
+        self.partialconv = bool(partialconv)
+        loaded = features is None
+        if loaded:
             features = load_features(net, save_dir)
         check_layout(features)
+        if loaded and self.partialconv:
+            features = partial_features(features)
+        if self.partialconv != (type(features[0]) is PartialConv2d):
+            raise ValueError(f"read_b200.VGGLoss: partialconv={self.partialconv} but features[0] is a {type(features[0]).__name__}; "
+                             "features= is used as given, so pass vgg_loss.partial_features(features) with partialconv=True "
+                             "and a plain first conv without it")
         mean, std = normalization(net)
         self.register_buffer('mean_', mean)
         self.register_buffer('std_', std)
@@ -257,8 +317,8 @@ class VGGLoss(nn.Module):
 
 
 def _forward(mod, pk, input, target, chunks):
-    """The loss (f32 scalar) of input against target.  ``chunks`` (a list) receives, per chunk of image pairs, (b0, n, codes)
-    for backward; None saves nothing."""
+    """The loss (f32 scalar) of input against target.  ``chunks`` (a list) receives, per chunk of image pairs, (b0, n, codes,
+    mask) for backward, mask the chunk's byte mask [n, H, W] (None unless partialconv); None saves nothing."""
     lib, st = L.load(), L.stream_ptr()
     steps = mod.steps()
     B, _, H, W = input.shape
@@ -274,8 +334,14 @@ def _forward(mod, pk, input, target, chunks):
     for b0 in range(0, B, per):
         n = min(per, B - b0)
         x = torch.empty((2 * n, H, W, 8), dtype=torch.bfloat16, device=dev)
-        L.check(lib.read_vgg_normalize(inp[b0].data_ptr(), tgt[b0].data_ptr(), n, H, W, mean.data_ptr(), std.data_ptr(),
-                                       x.data_ptr(), st))
+        mask = None
+        if mod.partialconv:
+            mask = torch.empty((n, H, W), dtype=torch.uint8, device=dev)
+            L.check(lib.read_vgg_normalize_masked(inp[b0].data_ptr(), tgt[b0].data_ptr(), n, H, W, mean.data_ptr(), std.data_ptr(),
+                                                  x.data_ptr(), mask.data_ptr(), st))
+        else:
+            L.check(lib.read_vgg_normalize(inp[b0].data_ptr(), tgt[b0].data_ptr(), n, H, W, mean.data_ptr(), std.data_ptr(),
+                                           x.data_ptr(), st))
         codes, k = [], 0
         for i, (s, (h, w)) in enumerate(zip(steps, sizes)):
             raw = torch.empty((2 * n, h, w, s.cout), dtype=torch.bfloat16, device=dev)
@@ -288,12 +354,16 @@ def _forward(mod, pk, input, target, chunks):
                 x = raw                                                   # in place
             code = torch.empty((n, h, w, s.cout), dtype=torch.int8, device=dev) if chunks is not None else None
             term = terms[k].data_ptr() if s.loss else None
-            L.check(lib.read_vgg_post(raw.data_ptr(), n, h, w, s.cout, pk[i]['bias'].data_ptr(), int(s.pool), L.ptr(x),
-                                      L.ptr(code), term, 1.0 / (B * s.cout * h * w), ws.data_ptr(), st))
+            if i == 0 and mask is not None:
+                L.check(lib.read_vgg_post_partial(raw.data_ptr(), mask.data_ptr(), n, h, w, s.cout, pk[i]['bias'].data_ptr(),
+                                                  L.ptr(x), L.ptr(code), term, 1.0 / (B * s.cout * h * w), ws.data_ptr(), st))
+            else:
+                L.check(lib.read_vgg_post(raw.data_ptr(), n, h, w, s.cout, pk[i]['bias'].data_ptr(), int(s.pool), L.ptr(x),
+                                          L.ptr(code), term, 1.0 / (B * s.cout * h * w), ws.data_ptr(), st))
             k += s.loss
             codes.append(code)
         if chunks is not None:
-            chunks.append((b0, n, codes))
+            chunks.append((b0, n, codes, mask))
     return terms.sum().float()
 
 
@@ -319,14 +389,18 @@ class _VGGLossFn(torch.autograd.Function):
         g = gout.detach().float().reshape(1).contiguous()
         zeros = torch.zeros(256, dtype=torch.float32, device=dev)
         grad = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
-        for b0, n, codes in ctx.chunks:
+        for b0, n, codes, mask in ctx.chunks:
             up = None
             for i in reversed(range(len(steps))):
                 s, (h, w) = steps[i], sizes[i]
                 dy = torch.empty((n, h, w, s.cout), dtype=torch.bfloat16, device=dev)
                 coef = 1.0 / (B * s.cout * h * w) if s.loss else 0.0
-                L.check(lib.read_vgg_dgrad_in(L.ptr(up), int(s.pool), codes[i].data_ptr(), n, h, w, s.cout, g.data_ptr(), coef,
-                                              dy.data_ptr(), st))
+                if i == 0 and mask is not None:
+                    L.check(lib.read_vgg_dgrad_in_partial(L.ptr(up), mask.data_ptr(), codes[i].data_ptr(), n, h, w, s.cout,
+                                                          g.data_ptr(), coef, dy.data_ptr(), st))
+                else:
+                    L.check(lib.read_vgg_dgrad_in(L.ptr(up), int(s.pool), codes[i].data_ptr(), n, h, w, s.cout, g.data_ptr(),
+                                                  coef, dy.data_ptr(), st))
                 codes[i] = None
                 if i == 0:
                     up = torch.empty((n, h, w, 8), dtype=torch.bfloat16, device=dev)
@@ -335,6 +409,24 @@ class _VGGLossFn(torch.autograd.Function):
                 else:
                     up = torch.empty((n, h, w, s.cin), dtype=torch.bfloat16, device=dev)
                     blocks._launch(lib, dy, s.cin // 2, pk[i]['w_dgrad'], (zeros,) * 4, False, L.OUT_RAW_NHWC, up)
-            L.check(lib.read_vgg_image_grad(up.data_ptr(), n, H, W, ctx.std.data_ptr(), grad[b0].data_ptr(), st))
+            if mask is not None:
+                L.check(lib.read_vgg_image_grad_masked(up.data_ptr(), mask.data_ptr(), n, H, W, ctx.std.data_ptr(),
+                                                       grad[b0].data_ptr(), st))
+            else:
+                L.check(lib.read_vgg_image_grad(up.data_ptr(), n, H, W, ctx.std.data_ptr(), grad[b0].data_ptr(), st))
         ctx.chunks = None
         return grad, None, None, None
+
+
+class VGGLossMix(nn.Module):
+    """Drop-in for READ.criterions.vgg_loss.VGGLossMix: weight * l1(input, target) + (1 - weight) * l2(input, target), l1 and l2
+    VGGLoss() and VGGLoss(net='caffe') as the reference builds them (both 'caffe').  ``kwargs`` (save_dir, features) go to both."""
+
+    def __init__(self, weight=0.5, **kwargs):
+        super().__init__()
+        self.l1 = VGGLoss(**kwargs)
+        self.l2 = VGGLoss(net='caffe', **kwargs)
+        self.weight = weight
+
+    def forward(self, input, target):
+        return self.l1(input, target) * self.weight + self.l2(input, target) * (1 - self.weight)
