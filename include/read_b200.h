@@ -450,6 +450,56 @@ int read_vgg_dgrad_in_partial(const void *up, const void *mask, const void *code
                               float coef, void *dy, void *stream);
 int read_vgg_image_grad_masked(const void *dx, const void *mask, int n, int H, int W, const float *std_, float *out, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Deterministic training reductions (read_b200 picks them when torch.are_deterministic_algorithms_enabled()).  The entry points
+ * above add partial sums with fp32 atomics, so their last bits vary from run to run; these compute the same quantities with a fixed
+ * order of additions: the same inputs give the same bits on every call, on the same device and build.  Each takes a caller-owned
+ * workspace (16B aligned, uninitialised, used by one call at a time) of the size its *_workspace_bytes query returns (-1: shape not
+ * supported), and otherwise the arguments and accumulate (+=) semantics of its default form.
+ *
+ *   read_gather_backward_det / read_gather_backward_sparse_det : read_gather_backward / read_gather_backward_sparse.  Order: with
+ *       key[p] = clamp(id[p], 0, N-1) for the flat pixel p = (b*h + y)*w + x, the pixels are sorted stably by key (so each id's
+ *       pixels stay in ascending p).  The sorted sequence is cut into chunks of 128 positions.  Within a chunk, each run of equal
+ *       keys is summed in sorted order in fp32, starting from 0.  An id whose pixels all lie in one chunk gets that run sum; an id
+ *       whose pixels cross chunk boundaries gets its runs' sums added in chunk order (the first run's sum, + the next, ...).  That
+ *       sum is added once to row id (grad_tex_nd, or grad_nd with touched[id] = 1), per channel independently.
+ *       workspace: read_gather_backward_det_workspace_bytes(B, D, h, w, N); B*h*w < 2^31, N < 2^31
+ *   read_gate_backward_det, read_bn_backward_reduce_det, read_gate_backward_batch_stats_det, read_bn_backward_reduce_items_det,
+ *   read_gate_backward_batch_stats_items_det : the per-channel sums leave each CTA through the workspace (the CTA's threads added
+ *       in thread order) and the last CTA to finish adds the CTAs' rows in a fixed order.  workspace: read_gate_det_workspace_bytes
+ *       (items, C), items = 1 for the call-wide forms
+ *   read_conv_wgrad_det : read_conv_wgrad (and read_conv3x3_wgrad as k = 3, stride = 1).  Each split-K part of the pixels writes its
+ *       own copy of the gradients to the workspace; the copies are added in split order and then to dwf / dwm.  The number of
+ *       splits depends on the device's SM count.  workspace: read_conv_wgrad_det_workspace_bytes(B, Hout, Wout, Cout, Cin, k,
+ *       stride)
+ * ---------------------------------------------------------------------------------------- */
+int64_t read_gather_backward_det_workspace_bytes(int B, int D, int h, int w, int64_t N);
+int read_gather_backward_det(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                             void *workspace, void *stream);
+int read_gather_backward_sparse_det(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
+                                    unsigned char *touched, void *workspace, void *stream);
+int64_t read_gate_det_workspace_bytes(int items, int C);
+int read_gate_backward_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                           const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
+                           float *dbias_m, float *dgamma, float *dbeta, void *workspace, void *stream);
+int read_bn_backward_reduce_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat,
+                                void *workspace, void *stream);
+int read_gate_backward_batch_stats_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                       const float *bias_m, const float *bn_scale, const float *bn_mean, const float *bn_inv_std,
+                                       const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
+                                       void *workspace, void *stream);
+int read_bn_backward_reduce_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                      const float *bias_f, const float *bias_m, const float *bn_mean, const float *bn_inv_std,
+                                      float *sum_dy, float *sum_dy_xhat, void *workspace, void *stream);
+int read_gate_backward_batch_stats_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                             const float *bias_f, const float *bias_m, const float *bn_scale, const float *bn_mean,
+                                             const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
+                                             float *dbias_f, float *dbias_m, void *workspace, void *stream);
+int64_t read_conv_wgrad_det_workspace_bytes(int B, int Hout, int Wout, int Cout, int Cin, int k, int stride);
+int read_conv_wgrad_det(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
+                        int stride, float *dwf, float *dwm, void *workspace, void *stream);
+
 /* Counts kernels launched by this library since load (bench.py's gpu_launches claim). */
 int64_t read_launch_count(void);
 

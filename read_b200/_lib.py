@@ -126,6 +126,22 @@ _SIGS = {
     "read_vgg_post_partial": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_vp, c_vp]),
     "read_vgg_dgrad_in_partial": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, ctypes.c_float, c_vp, c_vp]),
     "read_vgg_image_grad_masked": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "read_gather_backward_det_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int, c_i64]),
+    "read_gather_backward_det": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
+    "read_gather_backward_sparse_det": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "read_gate_det_workspace_bytes": (c_i64, [c_int, c_int]),
+    "read_gate_backward_det": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                       c_vp, c_vp]),
+    "read_bn_backward_reduce_det": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_gate_backward_batch_stats_det": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                   c_vp, c_vp, c_vp, c_vp]),
+    "read_bn_backward_reduce_items_det": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                  c_vp]),
+    "read_gate_backward_batch_stats_items_det": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                         c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "read_conv_wgrad_det_workspace_bytes": (c_i64, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "read_conv_wgrad_det": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                                    c_vp]),
     "read_conv_tc_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_conv_tcg_supported": (c_int, [ctypes.POINTER(ReadConvDesc)]),
     "read_tcg_weight_elems": (c_i64, [c_int, c_int, c_int]),

@@ -240,6 +240,8 @@ def gate_backward(lib, g, fm, c, dfm):
     st = L.stream_ptr()
     P = g.numel() // c.C
     red = torch.zeros((4, c.C), dtype=torch.float32, device=g.device)  # dbias_f, dbias_m, dgamma, dbeta
+    if torch.are_deterministic_algorithms_enabled():
+        return _gate_backward_det(lib, g, fm, c, dfm, P, red, st)
     if c.items is not None:
         items, P = g.shape[0], g.shape[1] * g.shape[2]
         sums = torch.zeros((2, items, c.C), dtype=torch.float32, device=g.device)     # sum dy, sum dy * xhat per item
@@ -264,6 +266,55 @@ def gate_backward(lib, g, fm, c, dfm):
                                    c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
                                    red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
     return red
+
+
+def _gate_backward_det(lib, g, fm, c, dfm, P, red, st):
+    """gate_backward under torch.use_deterministic_algorithms(True): the same passes through the *_det entry points, whose sums
+    are combined in a fixed order."""
+    items = g.shape[0] if c.items is not None else 1
+    ws = ops.det_workspace(lib.read_gate_det_workspace_bytes(items, c.C), g.device, "gate backward")
+    if c.items is not None:
+        P = g.shape[1] * g.shape[2]
+        sums = torch.zeros((2, items, c.C), dtype=torch.float32, device=g.device)
+        L.check(lib.read_bn_backward_reduce_items_det(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
+                                                      c.bm.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), sums[0].data_ptr(),
+                                                      sums[1].data_ptr(), ws.data_ptr(), st))
+        L.check(lib.read_gate_backward_batch_stats_items_det(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu),
+                                                             c.bf.data_ptr(), c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(),
+                                                             c.inv.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(),
+                                                             dfm.data_ptr(), red[0].data_ptr(), red[1].data_ptr(), ws.data_ptr(),
+                                                             st))
+        red[3], red[2] = sums[0].sum(0), sums[1].sum(0)
+        return red
+    if c.batch:
+        L.check(lib.read_bn_backward_reduce_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
+                                                c.mean.data_ptr(), c.inv.data_ptr(), red[3].data_ptr(), red[2].data_ptr(),
+                                                ws.data_ptr(), st))
+        L.check(lib.read_gate_backward_batch_stats_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(),
+                                                       c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
+                                                       red[3].data_ptr(), red[2].data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
+                                                       red[1].data_ptr(), ws.data_ptr(), st))
+        return red
+    L.check(lib.read_gate_backward_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
+                                       c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
+                                       red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), ws.data_ptr(), st))
+    return red
+
+
+def conv_wgrad(lib, dfm, x, B, Hout, Wout, C, k, stride, dwf, dwm, st):
+    """dwf / dwm [C][Cin][k][k] += the weight gradient of a gated conv from [df | dm] [B,Hout,Wout,2C] and its input x
+    [B,stride*Hout,stride*Wout,Cin] (NHWC bf16); under torch.use_deterministic_algorithms(True) with the split-K partials added in
+    a fixed order."""
+    Hin, Win, Cin = x.shape[1], x.shape[2], x.shape[3]
+    if torch.are_deterministic_algorithms_enabled():
+        ws = ops.det_workspace(lib.read_conv_wgrad_det_workspace_bytes(B, Hout, Wout, C, Cin, k, stride), dfm.device, "conv wgrad")
+        L.check(lib.read_conv_wgrad_det(dfm.data_ptr(), x.data_ptr(), B, Hin, Win, Hout, Wout, C, Cin, k, stride, dwf.data_ptr(),
+                                        dwm.data_ptr(), ws.data_ptr(), st))
+    elif k == 3 and stride == 1:
+        L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x.data_ptr(), B, Hout, Wout, C, Cin, dwf.data_ptr(), dwm.data_ptr(), st))
+    else:
+        L.check(lib.read_conv_wgrad(dfm.data_ptr(), x.data_ptr(), B, Hin, Win, Hout, Wout, C, Cin, k, stride, dwf.data_ptr(),
+                                    dwm.data_ptr(), st))
 
 
 def dgrad(dfm, conv, residual=None):
@@ -338,7 +389,7 @@ class ResStackFn(torch.autograd.Function):
             dwf = dwm = None
             if ctx.needs_input_grad[2 + 6 * i] or ctx.needs_input_grad[4 + 6 * i]:    # not for a frozen net
                 dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
-                L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x_in.data_ptr(), B, H, W, C, C, dwf.data_ptr(), dwm.data_ptr(), st))
+                conv_wgrad(lib, dfm, x_in, B, H, W, C, 3, 1, dwf, dwm, st)
             grads[6 * i: 6 * i + 6] = [dwf, red[0], dwm, red[1], red[2], red[3]]
             if i > 0 or ctx.needs_input_grad[0]:
                 # the first conv of a ResBlock adds the gradient that reaches its input through the skip
@@ -464,8 +515,7 @@ class GatedConvFn(torch.autograd.Function):
         dwf = dwm = None
         if need[3] or need[5]:                                            # not for a frozen net
             dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
-            L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x_in.data_ptr(), B, H, W, C, x_in.shape[3], dwf.data_ptr(),
-                                           dwm.data_ptr(), st))
+            conv_wgrad(lib, dfm, x_in, B, H, W, C, 3, 1, dwf, dwm, st)
         dx = ops.nhwc_to_nchw(dgrad(dfm, c)) if need[0] else None
         grads = [dwf, red[0], dwm, red[1], red[2], red[3]]
         grads = [gr[:cout] if gr is not None and need[3 + k] else None for k, gr in enumerate(grads)]
@@ -605,7 +655,7 @@ class MultiSourceConvFn(torch.autograd.Function):
         ts = ctx.saved_tensors[:n_src]
         need = ctx.needs_input_grad[2:]                                    # the sources, then the 6 parameters
         C, dev = c.C, ts[0].device
-        B, Hin, Win, _ = ts[0].shape
+        B = ts[0].shape[0]
         gp = gout.float()
         if cout < C:
             gp = torch.cat([gp, gp.new_zeros((B, C - cout) + tuple(gp.shape[2:]))], 1)  # the padded channels' gradient is 0
@@ -620,8 +670,7 @@ class MultiSourceConvFn(torch.autograd.Function):
             kk = (c.k, c.k)
             dws = [(torch.zeros((C, t.shape[3]) + kk, device=dev), torch.zeros((C, t.shape[3]) + kk, device=dev)) for t in ts]
             for t, (wf_s, wm_s) in zip(ts, dws):
-                L.check(lib.read_conv_wgrad(dfm.data_ptr(), t.data_ptr(), B, Hin, Win, Hout, Wout, C, t.shape[3], c.k, c.stride,
-                                            wf_s.data_ptr(), wm_s.data_ptr(), st))
+                conv_wgrad(lib, dfm, t, B, Hout, Wout, C, c.k, c.stride, wf_s, wm_s, st)
             dwf = torch.cat([w[0] for w in dws], 1) if n_src > 1 else dws[0][0]
             dwm = torch.cat([w[1] for w in dws], 1) if n_src > 1 else dws[0][1]
         dxs = [None] * n_src

@@ -32,17 +32,78 @@ __device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2
 // parameters are never read).
 constexpr int GB_THREADS = 256, GB_MAX_C = 256;
 
-template <bool ELU, bool BATCH>
+// ---- deterministic reduction (DET instances, torch.use_deterministic_algorithms): no atomics on the sums.
+// A CTA adds the per-thread sums of channel c in thread order (threads c / 8, c / 8 + G, ...) and stores them as its row of the
+// caller's workspace part[cta][NS][C] (cta = blockIdx.y * gridDim.x + blockIdx.x); the last CTA to finish (counter + fence, the
+// counter zeroed by the entry point and again by that CTA) combines the rows in a fixed order, see gate_det_combine.
+__device__ __forceinline__ void gate_det_cta_sum(const float (&v)[8], int C, int G, int ppb, float *__restrict__ row)
+{
+    __shared__ float buf[GB_THREADS * 8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) buf[threadIdx.x * 8 + j] = v[j];
+    __syncthreads();
+    for (int c = threadIdx.x; c < C; c += GB_THREADS) {
+        float s = 0.f;
+        for (int r = 0; r < ppb; ++r) s += buf[(r * G + c / 8) * 8 + c % 8];
+        row[c] = s;
+    }
+    __syncthreads();
+}
+
+__device__ __forceinline__ bool gate_det_last(unsigned *counter)
+{
+    __shared__ bool last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(counter, 1u) == gridDim.x * gridDim.y - 1;
+    __syncthreads();
+    if (last) __threadfence();
+    return last;
+}
+
+// The last CTA: output e = (row r, sum k, channel c), r = an item when PER_ITEM (blockIdx.y's CTAs only), else 0 (every CTA).  Its
+// n CTA rows are split over `lanes` threads (lane l adds CTAs l, l + lanes, ... in order, lanes = GB_THREADS / outputs when there
+// are fewer outputs than threads, else 1) and the lanes' sums are added in lane order; the result is added to dst[k][r * C + c].
+template <int NS, bool PER_ITEM>
+__device__ __forceinline__ void gate_det_combine(const float *part, int C, float *d0, float *d1, float *d2, float *d3,
+                                                 unsigned *counter)
+{
+    __shared__ float lred[GB_THREADS];
+    const int gx = gridDim.x, rows = PER_ITEM ? gridDim.y : 1, n = PER_ITEM ? gx : gx * gridDim.y, O = rows * NS * C;
+    const int lanes = O < GB_THREADS ? GB_THREADS / O : 1;
+    for (int e0 = 0; e0 < O; e0 += GB_THREADS / lanes) {
+        const int e = e0 + threadIdx.x % (GB_THREADS / lanes), l = threadIdx.x / (GB_THREADS / lanes);
+        const int c = e % C, k = (e / C) % NS, r = e / (NS * C);
+        float s = 0.f;
+        if (e < O && l < lanes)
+            for (int i = l; i < n; i += lanes) s += __ldcg(part + ((long long)(r * gx + i) * NS + k) * C + c);
+        lred[threadIdx.x] = s;
+        __syncthreads();
+        if (threadIdx.x < GB_THREADS / lanes && e < O) {
+            float t = 0.f;
+            for (int q = 0; q < lanes; ++q) t += lred[q * (GB_THREADS / lanes) + threadIdx.x];
+            float *d = k == 0 ? d0 : k == 1 ? d1 : k == 2 ? d2 : d3;
+            d[(long long)r * C + c] += t;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *counter = 0u;
+}
+
+template <bool ELU, bool BATCH, bool DET = false>
 __device__ __forceinline__ void
 gate_bwd_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
               const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
               const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
               float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
-              const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
+              const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part = nullptr,
+              unsigned *__restrict__ counter = nullptr)
 {
     __shared__ float red[4][GB_MAX_C];
-    for (int i = threadIdx.x; i < 4 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
-    __syncthreads();
+    if constexpr (!DET) {
+        for (int i = threadIdx.x; i < 4 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
+        __syncthreads();
+    }
     const int G = C / 8, ppb = GB_THREADS / G;
     const int cg = threadIdx.x % G, co0 = 8 * cg, fcol = fm_col(co0, half);
     float bf[8], bm[8], sc[8], mu[8], is[8];
@@ -96,15 +157,29 @@ gate_bwd_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restr
             *reinterpret_cast<uint4 *>(dfm + p * 2 * C + fcol) = make_uint4(odf[0], odf[1], odf[2], odf[3]);
             *reinterpret_cast<uint4 *>(dfm + p * 2 * C + fcol + half) = make_uint4(odm[0], odm[1], odm[2], odm[3]);
         }
+        if constexpr (!DET) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            atomicAdd(&red[0][co0 + j], s_bf[j]);
-            atomicAdd(&red[1][co0 + j], s_bm[j]);
-            if constexpr (!BATCH) {
-                atomicAdd(&red[2][co0 + j], s_g[j]);
-                atomicAdd(&red[3][co0 + j], s_b[j]);
+            for (int j = 0; j < 8; ++j) {
+                atomicAdd(&red[0][co0 + j], s_bf[j]);
+                atomicAdd(&red[1][co0 + j], s_bm[j]);
+                if constexpr (!BATCH) {
+                    atomicAdd(&red[2][co0 + j], s_g[j]);
+                    atomicAdd(&red[3][co0 + j], s_b[j]);
+                }
             }
         }
+    }
+    if constexpr (DET) {
+        constexpr int NS = BATCH ? 2 : 4;
+        float *row = part + (long long)(blockIdx.y * gridDim.x + blockIdx.x) * NS * C;
+        gate_det_cta_sum(s_bf, C, G, ppb, row);
+        gate_det_cta_sum(s_bm, C, G, ppb, row + C);
+        if constexpr (!BATCH) {
+            gate_det_cta_sum(s_g, C, G, ppb, row + 2 * C);
+            gate_det_cta_sum(s_b, C, G, ppb, row + 3 * C);
+        }
+        if (gate_det_last(counter)) gate_det_combine<NS, false>(part, C, dbf, dbm, dgamma, dbeta, counter);
+        return;
     }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += GB_THREADS) {
@@ -149,15 +224,19 @@ gate_bwd_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 
 // sum_dy += sum dy, sum_dy_xhat += sum dy * (g - mean) * inv_std over the P pixels, with g = A(f + b_f) * sigmoid(m + b_m)
 // recomputed from the RAW [f | m] (mean / inv_std: the batch statistics of the forward).  These are dbeta and dgamma, and the
 // two terms the corrected gate backward (gate_bwd_kernel<ELU, true>) needs.  Same thread layout and reduction as the gate backward.
-template <bool ELU>
+// DET: the deterministic reduction above; PER_ITEM: the last CTA writes item r's sums to row r (sum_dy / sum_dy_xhat [items, C]).
+template <bool ELU, bool DET = false, bool PER_ITEM = false>
 __device__ __forceinline__ void
 bn_bwd_reduce_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
                    const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
-                   const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
+                   const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat,
+                   float *__restrict__ part = nullptr, unsigned *__restrict__ counter = nullptr)
 {
     __shared__ float red[2][GB_MAX_C];
-    for (int i = threadIdx.x; i < 2 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
-    __syncthreads();
+    if constexpr (!DET) {
+        for (int i = threadIdx.x; i < 2 * GB_MAX_C; i += GB_THREADS) (&red[0][0])[i] = 0.f;
+        __syncthreads();
+    }
     const int G = C / 8, ppb = GB_THREADS / G;
     const int cg = threadIdx.x % G, co0 = 8 * cg, fcol = fm_col(co0, half);
     float bf[8], bm[8], mu[8], is[8], s_b[8], s_g[8];
@@ -187,11 +266,20 @@ bn_bwd_reduce_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__
                 }
             }
         }
+        if constexpr (!DET) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            atomicAdd(&red[0][co0 + j], s_b[j]);
-            atomicAdd(&red[1][co0 + j], s_g[j]);
+            for (int j = 0; j < 8; ++j) {
+                atomicAdd(&red[0][co0 + j], s_b[j]);
+                atomicAdd(&red[1][co0 + j], s_g[j]);
+            }
         }
+    }
+    if constexpr (DET) {
+        float *row = part + (long long)(blockIdx.y * gridDim.x + blockIdx.x) * 2 * C;
+        gate_det_cta_sum(s_b, C, G, ppb, row);
+        gate_det_cta_sum(s_g, C, G, ppb, row + C);
+        if (gate_det_last(counter)) gate_det_combine<2, PER_ITEM>(part, C, sum_dy, sum_dy_xhat, nullptr, nullptr, counter);
+        return;
     }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += GB_THREADS) {
@@ -220,6 +308,58 @@ bn_bwd_reduce_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bflo
     const long long it = blockIdx.y, o = it * C;
     bn_bwd_reduce_body<ELU>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o, sum_dy + o,
                             sum_dy_xhat + o);
+}
+
+// Deterministic instances (torch.use_deterministic_algorithms): the bodies above with DET, the CTA partials in part / counter.
+// The per-item forms take the unshifted pointers: the body's last CTA combines every item (gate: into one dbias_f / dbias_m; BN
+// reduce: item r into row r).
+template <bool ELU, bool BATCH>
+__global__ void __launch_bounds__(GB_THREADS)
+gate_bwd_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                    const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+                    const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+                    float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
+                    const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part,
+                    unsigned *__restrict__ counter)
+{
+    gate_bwd_body<ELU, BATCH, true>(dy, fm, P, C, half, bias_f, bias_m, scale, mean, inv_std, dfm, dbf, dbm, dgamma, dbeta, sum_dy,
+                                    sum_dy_xhat, part, counter);
+}
+
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+gate_bwd_items_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                          const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
+                          const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
+                          float *__restrict__ dbf, float *__restrict__ dbm, const float *__restrict__ sum_dy,
+                          const float *__restrict__ sum_dy_xhat, float *__restrict__ part, unsigned *__restrict__ counter)
+{
+    const long long it = blockIdx.y, o = it * C;
+    gate_bwd_body<ELU, true, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, scale + o, mean + o,
+                                   inv_std + o, dfm + it * P * 2 * C, dbf, dbm, nullptr, nullptr, sum_dy + o, sum_dy_xhat + o, part,
+                                   counter);
+}
+
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+bn_bwd_reduce_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
+                         const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
+                         const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat,
+                         float *__restrict__ part, unsigned *__restrict__ counter)
+{
+    bn_bwd_reduce_body<ELU, true>(dy, fm, P, C, half, bias_f, bias_m, mean, inv_std, sum_dy, sum_dy_xhat, part, counter);
+}
+
+template <bool ELU>
+__global__ void __launch_bounds__(GB_THREADS)
+bn_bwd_reduce_items_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C,
+                               int half, const float *__restrict__ bias_f, const float *__restrict__ bias_m,
+                               const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy,
+                               float *__restrict__ sum_dy_xhat, float *__restrict__ part, unsigned *__restrict__ counter)
+{
+    const long long it = blockIdx.y, o = it * C;
+    bn_bwd_reduce_body<ELU, true, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o,
+                                        sum_dy, sum_dy_xhat, part, counter);
 }
 
 // ------------------------------------------------------------------ weight gradient
@@ -270,10 +410,12 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4],
 }
 
 // H, W: the output (= [df | dm]) size; the input x is [B][STRIDE * H][STRIDE * W][Cin] (the callers check Hin == STRIDE * Hout).
-template <int KS, int STRIDE, int KR>
-__global__ void __launch_bounds__(WG_THREADS)
-wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
-             int half, float *__restrict__ dwf, float *__restrict__ dwm)
+// DET (torch.use_deterministic_algorithms): instead of the atomics, split blockIdx.x stores its partial sums to its own copy of
+// the gradients, part[split][2][C][Cin][KS][KS] (conv_f, then conv_m); wgrad_split_sum_kernel adds the copies in split order.
+template <int KS, int STRIDE, int KR, bool DET>
+__device__ __forceinline__ void
+wgrad_body(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin, int half,
+           float *__restrict__ dwf, float *__restrict__ dwm, float *__restrict__ part)
 {
     constexpr int HALO = wg_halo(KS, STRIDE), TAPS = KR * KS, GROUPS = KS / KR, PAD = KS == 1 ? 0 : 1;
     constexpr uint32_t STAGE = wg_stage(KS, STRIDE, KR);
@@ -363,10 +505,75 @@ wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restr
             if (col >= twoC || ci >= Cin) continue;
             const int rr = col % (2 * half);
             const int o = (col / (2 * half)) * half + rr % half;
-            float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * (KS * KS) + ky0 * KS;
+            if constexpr (DET) {
+                const long long nw = (long long)C * Cin * (KS * KS);
+                float *dw = part + ((long long)blockIdx.x * 2 + (rr >= half)) * nw + ((long long)o * Cin + ci) * (KS * KS) + ky0 * KS;
 #pragma unroll
-            for (int tap = 0; tap < TAPS; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
+                for (int tap = 0; tap < TAPS; ++tap) dw[tap] = acc[mi][tap][i];
+            } else {
+                float *dw = (rr >= half ? dwm : dwf) + ((long long)o * Cin + ci) * (KS * KS) + ky0 * KS;
+#pragma unroll
+                for (int tap = 0; tap < TAPS; ++tap) atomicAdd(dw + tap, acc[mi][tap][i]);
+            }
         }
+}
+
+template <int KS, int STRIDE, int KR>
+__global__ void __launch_bounds__(WG_THREADS)
+wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
+             int half, float *__restrict__ dwf, float *__restrict__ dwm)
+{
+    wgrad_body<KS, STRIDE, KR, false>(dfm, x, B, H, W, C, Cin, half, dwf, dwm, nullptr);
+}
+
+template <int KS, int STRIDE, int KR>
+__global__ void __launch_bounds__(WG_THREADS)
+wgrad_det_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
+                 int half, float *__restrict__ part)
+{
+    wgrad_body<KS, STRIDE, KR, true>(dfm, x, B, H, W, C, Cin, half, nullptr, nullptr, part);
+}
+
+// dwf[e] / dwm[e] += the splits' copies of element e added in split order, from 0
+__global__ void wgrad_split_sum_kernel(const float *__restrict__ part, int splits, long long nw, float *__restrict__ dwf,
+                                       float *__restrict__ dwm)
+{
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < 2 * nw; e += (long long)gridDim.x * blockDim.x) {
+        float s = 0.f;
+        for (int k = 0; k < splits; ++k) s += __ldcg(part + k * 2 * nw + e);
+        (e < nw ? dwf : dwm)[e < nw ? e : e - nw] += s;
+    }
+}
+
+// the launch geometry of wgrad_kernel<KS, STRIDE, KR>: splits (blockIdx.x), column blocks, input-channel blocks x filter-row groups
+template <int KS, int KR>
+static void wgrad_grid(int B, int H, int W, int Cout, int Cin, long long &s, int &mb, int &nz)
+{
+    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
+    mb = (2 * Cout + WG_M - 1) / WG_M;
+    nz = ((Cin + WG_N - 1) / WG_N) * (KS / KR);
+    s = (2ll * num_sms() + mb * nz - 1) / (mb * nz);
+    if (s > chunks) s = chunks;
+}
+
+template <int KS, int STRIDE, int KR>
+static int launch_wgrad_det(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm,
+                            void *workspace, cudaStream_t st)
+{
+    long long s;
+    int mb, nz;
+    wgrad_grid<KS, KR>(B, H, W, Cout, Cin, s, mb, nz);
+    RB_CHECK_ARG(s <= 0x7FFFFFFF && nz <= 65535 && mb <= 65535, "conv_wgrad_det: too large");
+    float *part = (float *)workspace;
+    wgrad_det_kernel<KS, STRIDE, KR><<<dim3((unsigned)s, mb, nz), WG_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, part);
+    RB_LAUNCH_CHECK();
+    const long long nw = (long long)Cout * Cin * KS * KS;
+    long long blocks = (2 * nw + 255) / 256;
+    if (blocks > 16ll * num_sms()) blocks = 16ll * num_sms();
+    wgrad_split_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, (int)s, nw, dwf, dwm);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 template <int KS, int STRIDE, int KR>
@@ -837,6 +1044,176 @@ int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wou
     const cudaStream_t st = (cudaStream_t)stream;
     if (k == 3) return launch_dgrad_s2<3>(dfm, wt, B, Hout, Wout, Cout, Cin, dx, st);
     return launch_dgrad_s2<4>(dfm, wt, B, Hout, Wout, Cout, Cin, dx, st);
+}
+
+// ------------------------------------------------------------------ deterministic entry points
+// CTAs of the deterministic gate passes: at most 2 per SM (the last CTA reads every CTA's row), per item for the per-item forms
+static long long gate_det_grid(int items, int64_t pixels, int C)
+{
+    const int ppb = GB_THREADS / (C / 8);
+    long long blocks = (pixels + ppb - 1) / ppb, cap = 2ll * num_sms() / items;
+    if (cap < 1) cap = 1;
+    return blocks > cap ? cap : blocks;
+}
+
+static bool gate_det_ok(int C) { return C >= 16 && C <= GB_MAX_C && C % 16 == 0 && (C <= 64 || C % 64 == 0); }
+
+int64_t read_gate_det_workspace_bytes(int items, int C)
+{
+    if (!gate_det_ok(C) || items < 1 || items > 65535) return -1;
+    const long long ctas = items > 2ll * num_sms() ? items : 2ll * num_sms();
+    return 256 + ctas * 4 * C * (int64_t)sizeof(float);
+}
+
+#define GATE_DET_CHECKS(name, items, pixels, minpx, ...)                                                                        \
+    RB_CHECK_ARG(__VA_ARGS__, name ": null pointer");                                                                          \
+    RB_CHECK_ARG(items >= 1 && items <= 65535, name ": items must lie in 1..65535 (got %d)", items);                            \
+    RB_CHECK_ARG(pixels >= minpx, name ": needs at least %d pixels (got %lld)", minpx, (long long)pixels);                      \
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(workspace)) & \
+                  15) == 0,                                                                                                    \
+                 name ": tensors and workspace must be 16B aligned")
+
+int read_gate_backward_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
+                           const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
+                           float *dbias_m, float *dgamma, float *dbeta, void *workspace, void *stream)
+{
+    GATE_DET_CHECKS("gate_backward_det", 1, pixels, 0, dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std &&
+                                                           dbias_f && dbias_m && dgamma && dbeta && workspace);
+    RB_CHECK_ARG(gate_det_ok(C), "gate_backward_det: C must be 16, 32, 48, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_det: tensors must be 16B aligned");
+    if (pixels == 0) return READ_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? gate_bwd_det_kernel<true, false> : gate_bwd_det_kernel<false, false>;
+    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale, bn_mean,
+        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, nullptr, nullptr, (float *)((char *)workspace + 256),
+        counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_bn_backward_reduce_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat,
+                                void *workspace, void *stream)
+{
+    GATE_DET_CHECKS("bn_backward_reduce_det", 1, pixels, 2, dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy &&
+                                                                sum_dy_xhat && workspace);
+    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? bn_bwd_reduce_det_kernel<true> : bn_bwd_reduce_det_kernel<false>;
+    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        bn_inv_std, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256), counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_gate_backward_batch_stats_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
+                                       const float *bias_m, const float *bn_scale, const float *bn_mean, const float *bn_inv_std,
+                                       const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
+                                       void *workspace, void *stream)
+{
+    GATE_DET_CHECKS("gate_backward_batch_stats_det", 1, pixels, 2, dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean &&
+                                                                       bn_inv_std && sum_dy && sum_dy_xhat && dbias_f && dbias_m &&
+                                                                       workspace);
+    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_batch_stats_det: tensors must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? gate_bwd_det_kernel<true, true> : gate_bwd_det_kernel<false, true>;
+    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
+        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, nullptr, nullptr, sum_dy, sum_dy_xhat,
+        (float *)((char *)workspace + 256), counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_bn_backward_reduce_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                      const float *bias_f, const float *bias_m, const float *bn_mean, const float *bn_inv_std,
+                                      float *sum_dy, float *sum_dy_xhat, void *workspace, void *stream)
+{
+    GATE_DET_CHECKS("bn_backward_reduce_items_det", items, pixels, 2, dy && fm && bias_f && bias_m && bn_mean && bn_inv_std &&
+                                                                          sum_dy && sum_dy_xhat && workspace);
+    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_items_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? bn_bwd_reduce_items_det_kernel<true> : bn_bwd_reduce_items_det_kernel<false>;
+    k<<<dim3((unsigned)gate_det_grid(items, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        bn_inv_std, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256), counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_gate_backward_batch_stats_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
+                                             const float *bias_f, const float *bias_m, const float *bn_scale, const float *bn_mean,
+                                             const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
+                                             float *dbias_f, float *dbias_m, void *workspace, void *stream)
+{
+    GATE_DET_CHECKS("gate_backward_batch_stats_items_det", items, pixels, 2, dy && fm && dfm && bias_f && bias_m && bn_scale &&
+                                                                                 bn_mean && bn_inv_std && sum_dy && sum_dy_xhat &&
+                                                                                 dbias_f && dbias_m && workspace);
+    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_items_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
+                 GB_MAX_C, C);
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_batch_stats_items_det: tensors must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? gate_bwd_items_det_kernel<true> : gate_bwd_items_det_kernel<false>;
+    k<<<dim3((unsigned)gate_det_grid(items, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
+        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256),
+        counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+#undef GATE_DET_CHECKS
+
+static bool wgrad_geom_ok(int Hin, int Win, int Hout, int Wout, int k, int stride)
+{
+    return ((stride == 1 && (k == 1 || k == 3)) || (stride == 2 && (k == 3 || k == 4))) && Hin == stride * Hout &&
+           Win == stride * Wout;
+}
+
+int64_t read_conv_wgrad_det_workspace_bytes(int B, int Hout, int Wout, int Cout, int Cin, int k, int stride)
+{
+    if (B < 1 || Hout < 1 || Wout < 1 || !wgrad_channels_ok(Cout, Cin) || !wgrad_geom_ok(stride * Hout, stride * Wout, Hout, Wout, k, stride))
+        return -1;
+    long long s;
+    int mb, nz;
+    if (k == 4) wgrad_grid<4, 2>(B, Hout, Wout, Cout, Cin, s, mb, nz);
+    else if (k == 3) wgrad_grid<3, 3>(B, Hout, Wout, Cout, Cin, s, mb, nz);
+    else wgrad_grid<1, 1>(B, Hout, Wout, Cout, Cin, s, mb, nz);
+    return s * 2 * (int64_t)Cout * Cin * k * k * (int64_t)sizeof(float);
+}
+
+int read_conv_wgrad_det(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
+                        int stride, float *dwf, float *dwm, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(dfm && x && dwf && dwm && workspace, "conv_wgrad_det: null pointer");
+    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_wgrad_det: bad shape");
+    RB_CHECK_ARG(wgrad_geom_ok(Hin, Win, Hout, Wout, k, stride),
+                 "conv_wgrad_det: k=%d stride=%d input %dx%d output %dx%d is not 1x1 / 3x3 stride 1 or 3x3 / 4x4 stride 2 "
+                 "(input = stride x output)", k, stride, Hin, Win, Hout, Wout);
+    RB_CHECK_ARG(wgrad_channels_ok(Cout, Cin),
+                 "conv_wgrad_det: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
+                 "conv_wgrad_det: tensors and workspace must be 16B aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (k == 1) return launch_wgrad_det<1, 1, 1>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
+    if (stride == 1) return launch_wgrad_det<3, 1, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
+    if (k == 3) return launch_wgrad_det<3, 2, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
+    return launch_wgrad_det<4, 2, 2>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
 }
 
 }  // extern "C"

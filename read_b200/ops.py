@@ -229,14 +229,27 @@ def fused_resolve_supported(pyr, D=8):
 
 
 def gather_backward(grad_out, ids, N):
-    """grad_out [B,D,h,w] f32, ids [B,h,w] f32 -> grad [N,D] f32 (scatter-add)."""
+    """grad_out [B,D,h,w] f32, ids [B,h,w] f32 -> grad [N,D] f32 (scatter-add).  Under torch.use_deterministic_algorithms(True) the
+    additions run in the fixed order of read_gather_backward_det, so the result is the same bits on every call."""
     grad_out = grad_out.contiguous()
     _f32c(grad_out, "grad_out")
     B, D, h, w = grad_out.shape
     g = torch.zeros((N, D), dtype=torch.float32, device=grad_out.device)
-    L.check(L.load().read_gather_backward(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(),
-                                          L.stream_ptr()))
+    lib = L.load()
+    if torch.are_deterministic_algorithms_enabled():
+        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, N), grad_out.device, "gather backward")
+        L.check(lib.read_gather_backward_det(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(), ws.data_ptr(),
+                                             L.stream_ptr()))
+        return g
+    L.check(lib.read_gather_backward(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(), L.stream_ptr()))
     return g
+
+
+def det_workspace(nbytes, device, what):
+    """Workspace of a deterministic entry point (nbytes from its *_workspace_bytes query; -1: the shape is not supported)."""
+    if nbytes < 0:
+        raise RuntimeError(f"read_b200: {what}: shape not supported by the deterministic kernels")
+    return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=device)
 
 
 def nchw_to_nhwc(x, act_bf16):

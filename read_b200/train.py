@@ -15,6 +15,7 @@ per pyramid level, READ/models/texture.py:55-63) and a dense ``torch.optim.RMSpr
 The net's own backward still runs through torch's operators (library path, DESIGN.md §7).
 """
 import ctypes
+import warnings
 
 import torch
 
@@ -39,8 +40,14 @@ class _GatherSparse(torch.autograd.Function):
         if g.dtype != torch.float32:
             g = g.float()
         B, D, h, w = g.shape
-        L.check(L.load().read_gather_backward_sparse(g.data_ptr(), ids.data_ptr(), B, D, h, w, st.N, st.grad.data_ptr(),
-                                                     st.touched.data_ptr(), L.stream_ptr()))
+        lib = L.load()
+        if torch.are_deterministic_algorithms_enabled():
+            ws = ops.det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, st.N), g.device, "sparse gather backward")
+            L.check(lib.read_gather_backward_sparse_det(g.data_ptr(), ids.data_ptr(), B, D, h, w, st.N, st.grad.data_ptr(),
+                                                        st.touched.data_ptr(), ws.data_ptr(), L.stream_ptr()))
+            return None, None, None
+        L.check(lib.read_gather_backward_sparse(g.data_ptr(), ids.data_ptr(), B, D, h, w, st.N, st.grad.data_ptr(),
+                                                st.touched.data_ptr(), L.stream_ptr()))
         return None, None, None
 
 
@@ -153,7 +160,18 @@ class SparseRMSprop:
 def exchange_sparse_grads(texture, group=None, capacity=None):
     """Data-parallel join of the descriptor gradients: every rank contributes its touched (id, grad[D]) rows, every rank ends up
     with the SUM over ranks in its accumulator (and the union of the flags) - what all-reducing the dense [N,D] gradient would
-    give, for a few MB of traffic.  Returns the number of rows this rank sent."""
+    give, for a few MB of traffic.  Returns the number of rows this rank sent.
+
+    The compaction and the scatter of received rows use atomics, so the accumulator's last bits can vary from run to run.  Under
+    torch.use_deterministic_algorithms(True) this raises a RuntimeError before any communication, as torch does for its own
+    nondeterministic ops; with warn_only=True it warns instead and proceeds."""
+    if torch.are_deterministic_algorithms_enabled():
+        msg = ("read_b200.train.exchange_sparse_grads does not have a deterministic implementation, but you set "
+               "'torch.use_deterministic_algorithms(True)'. You can turn off determinism just for this operation, or you can use "
+               "the 'warn_only=True' option, if that's acceptable for your application.")
+        if not torch.is_deterministic_algorithms_warn_only_enabled():
+            raise RuntimeError(msg)
+        warnings.warn(msg)
     import torch.distributed as dist
     sp = enable_sparse_grad(texture)
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
