@@ -146,6 +146,32 @@ int read_pyramid_resolve_gather(const float *tex_nd, int D, int64_t N, uint64_t 
 int read_gather_backward(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                          float *grad_tex_nd, void *stream);
 
+/* Batches whose items sample different textures (a training batch that mixes scenes), D == 8.  The table travels BY VALUE in the
+ * kernel parameters (no device-side table, no host-to-device copy).  Item b of the call samples slot slot[b]; its ids are clamped
+ * to [0, N[slot] - 1] of its OWN texture, and its empty pixels (id 0) go to point 0 of that texture.
+ *   read_gather_from_index_items     : read_gather_from_index per item, one launch (ids [n_items, h, w] f32, out [n_items, 8, h, w]
+ *                                      or NHWC); bit-identical to one read_gather_from_index call per item
+ *   read_gather_backward_items       : read_gather_backward per item into its slot's grad_nd (dense [N, 8] accumulators)
+ *   read_gather_backward_sparse_items: read_gather_backward_sparse per item into its slot's grad_nd, setting its slot's touched
+ * A slot with grad_nd == NULL receives nothing (its texture needs no gradient); a slot no item uses is left unchanged.  Pixels of
+ * id 0 are pre-reduced per block and per slot in shared memory.  grad_out is NCHW f32 [n_items, 8, h, w]. */
+#define READ_MAX_TEX_SLOTS 16
+#define READ_MAX_TEX_ITEMS 64
+typedef struct read_tex_table {
+    const float *tex_nd[READ_MAX_TEX_SLOTS];    /* slot s: point-major [N[s], 8] f32 descriptors, 16B aligned (forward) */
+    int64_t N[READ_MAX_TEX_SLOTS];
+    float *grad_nd[READ_MAX_TEX_SLOTS];         /* slot s: [N[s], 8] f32 accumulator (backward), or NULL */
+    unsigned char *touched[READ_MAX_TEX_SLOTS]; /* slot s: [N[s]] u8 flags (sparse backward) */
+    int32_t n_slots;                            /* 1 .. READ_MAX_TEX_SLOTS */
+    int32_t n_items;                            /* 1 .. READ_MAX_TEX_ITEMS: the batch size of the call */
+    uint8_t slot[READ_MAX_TEX_ITEMS];           /* item -> slot, < n_slots */
+} read_tex_table;
+int read_gather_from_index_items(const read_tex_table *table, const float *ids, int h, int w, int layout, int activation, void *out,
+                                 void *stream);
+int read_gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream);
+int read_gather_backward_sparse_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                      void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Gated convolution (BasicConv, READ/models/unet.py:22-53) with everything around it fused:
  *   y = bn_scale * ( A(conv_f(x)+b_f) * sigmoid(conv_m(x)+b_m) ) + bn_shift  [+ residual]
@@ -464,6 +490,13 @@ int read_vgg_image_grad_masked(const void *dx, const void *mask, int n, int H, i
  *       whose pixels cross chunk boundaries gets its runs' sums added in chunk order (the first run's sum, + the next, ...).  That
  *       sum is added once to row id (grad_tex_nd, or grad_nd with touched[id] = 1), per channel independently.
  *       workspace: read_gather_backward_det_workspace_bytes(B, D, h, w, N); B*h*w < 2^31, N < 2^31
+ *   read_gather_backward_items_det / read_gather_backward_sparse_items_det : read_gather_backward_items / _sparse_items.  Order:
+ *       the same passes over ONE key space that stacks the slots' rows in slot order: with base[s] = N[0] + ... + N[s-1],
+ *       key[p] = base[slot[b]] + clamp(id[p], 0, N[slot[b]] - 1) for the flat pixel p = (b*h + y)*w + x of item b.  So the pixels
+ *       are sorted stably by (slot, clamped id), each (slot, id)'s pixels in ascending p (items in item order), and the same
+ *       128-position chunks, run sums and chunk-order combination give each row's sum, added once to row id of its slot.  Runs
+ *       never span two slots (their keys differ).  Slots with grad_nd == NULL take part in the sort but receive nothing.
+ *       workspace: read_gather_backward_det_workspace_bytes(n_items, 8, h, w, base[n_slots]); base[n_slots] < 2^31
  *   read_gate_backward_det, read_bn_backward_reduce_det, read_gate_backward_batch_stats_det, read_bn_backward_reduce_items_det,
  *   read_gate_backward_batch_stats_items_det : the per-channel sums leave each CTA through the workspace (the CTA's threads added
  *       in thread order) and the last CTA to finish adds the CTAs' rows in a fixed order.  workspace: read_gate_det_workspace_bytes
@@ -478,6 +511,10 @@ int read_gather_backward_det(const float *grad_out, const float *ids, int B, int
                              void *workspace, void *stream);
 int read_gather_backward_sparse_det(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
                                     unsigned char *touched, void *workspace, void *stream);
+int read_gather_backward_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                   void *workspace, void *stream);
+int read_gather_backward_sparse_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                          void *workspace, void *stream);
 int64_t read_gate_det_workspace_bytes(int items, int C);
 int read_gate_backward_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                            const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,

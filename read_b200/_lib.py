@@ -44,6 +44,15 @@ class ReadConvDesc(ctypes.Structure):
     ]
 
 
+MAX_TEX_SLOTS, MAX_TEX_ITEMS = 16, 64
+
+
+class ReadTexTable(ctypes.Structure):
+    _fields_ = [("tex_nd", c_vp * MAX_TEX_SLOTS), ("N", c_i64 * MAX_TEX_SLOTS), ("grad_nd", c_vp * MAX_TEX_SLOTS),
+                ("touched", c_vp * MAX_TEX_SLOTS), ("n_slots", ctypes.c_int32), ("n_items", ctypes.c_int32),
+                ("slot", ctypes.c_uint8 * MAX_TEX_ITEMS)]
+
+
 class ReadHaloDesc(ctypes.Structure):
     _fields_ = [("src_up", c_vp), ("src_dn", c_vp), ("peer_up_slot", c_vp), ("peer_dn_slot", c_vp),
                 ("peer_up_flag", c_vp), ("peer_dn_flag", c_vp), ("slot_from_up", c_vp), ("slot_from_dn", c_vp),
@@ -88,6 +97,11 @@ _SIGS = {
     "read_pyramid_resolve_gather": (c_int, [c_vp, c_int, c_i64, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                             ctypes.POINTER(c_vp), c_int, c_vp]),
     "read_gather_backward": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp]),
+    "read_gather_from_index_items": (c_int, [ctypes.POINTER(ReadTexTable), c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "read_gather_backward_items": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp]),
+    "read_gather_backward_sparse_items": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp]),
+    "read_gather_backward_items_det": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp, c_vp]),
+    "read_gather_backward_sparse_items_det": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp, c_vp]),
     "read_generic_npad": (c_int, [c_int]),
     "read_pack_weights_generic": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp]),
     "read_tc_weight_elems": (c_i64, [c_int, c_int, c_int]),

@@ -10,19 +10,23 @@ Contract kept (what train.py, viewer.py and READ/gl/nn.py:76-129 rely on):
   the keys that follow it are concatenated in front of the samples) + ``'id'``; returns ``[B,3,H,W]`` (and, with
   ``return_input=True``, the LAST item's multi-scale net input, as the reference's loop leaves it).
 
-Eval-mode batches that share one texture run as ONE batched net pass (equivalent under eval-mode BatchNorm, SURVEY.md §8a
-"Batching"); in training mode the reference's per-item loop is kept, because BatchNorm statistics are per call there, unless the
-net normalises each item on its own (``UNet.train_batchnorm = 'per_item'``): then one batched pass computes what the loop does.
+Eval-mode batches run as ONE batched net pass (equivalent under eval-mode BatchNorm, SURVEY.md §8a "Batching"); in training mode
+the reference's per-item loop is kept, because BatchNorm statistics are per call there, unless the net normalises each item on its
+own (``UNet.train_batchnorm = 'per_item'``): then one batched pass computes what the loop does.  A batch that mixes scenes takes
+the batched pass too, its items sampling their own textures in one gather (``_texture_table`` says when); otherwise it keeps the
+loop.
 
 Extra fast path (not in the reference): ``render(points, total_m, W, H)`` goes points -> packed z-buffer pyramid -> feature
 pyramid -> net without materialising index maps, including the viewer's ``supersampling`` and ``temporal_average`` options.
 """
+import functools
+
 import torch
 import torch.nn as nn
 
 from . import ops
 from . import _lib as L
-from .texture import PointTexture
+from .texture import PointTexture, sample_items
 
 
 def _as_id_list(texture_ids):
@@ -72,7 +76,7 @@ class NetAndTexture(nn.Module):
     # ------------------------------------------------------------------ index-map path
     def _multiscale_input(self, texture, item):
         """One net input per 'uv' key: [extra channels that follow the key ..., texture samples], reduced by 1/ss when
-        supersampling (compose.py:143-165)."""
+        supersampling (compose.py:143-165).  ``texture``: the module (or any callable) that samples a 'uv' map."""
         keys = list(item)
         assert 'uv' in keys[0], 'first input must be uv'
         groups = []                                   # [(uv key, [extra keys])]
@@ -90,31 +94,60 @@ class NetAndTexture(nn.Module):
             scales.append(x)
         return scales
 
+    def _texture_table(self, texture_ids):
+        """(textures, slots) for ONE net call over a batch whose items use two or more textures (item b samples
+        ``textures[slots[b]]``, texture.sample_items), or None when the batch keeps the per-item loop: the textures must be
+        PointTextures with 8 channels on one device, with one activation and one gradient mode (requires_grad, sparse or dense),
+        at most 16 of them for at most 64 items."""
+        distinct = list(dict.fromkeys(texture_ids))
+        if not 2 <= len(distinct) <= L.MAX_TEX_SLOTS or len(texture_ids) > L.MAX_TEX_ITEMS:
+            return None
+        textures = [self._texture(tid) for tid in distinct]
+        if not all(isinstance(t, PointTexture) and t.texture_.dim() == 3 and t.texture_.shape[1] == 8 for t in textures):
+            return None
+        if (len({t.activation for t in textures}) != 1 or len({t.texture_.device for t in textures}) != 1
+                or len({(t.texture_.requires_grad, bool(getattr(t, '_sparse_requested', False))) for t in textures}) != 1):
+            return None
+        slot = {tid: s for s, tid in enumerate(distinct)}
+        return textures, [slot[tid] for tid in texture_ids]
+
     def _direct_engine_forward(self, maps, texture_ids):
-        """Inference shortcut of the index-map surface (VERDICT r01 #12): one scene, four 'uv' maps and nothing else, no
-        supersampling / temporal average / autograd -> the descriptors are gathered from the index maps STRAIGHT into the engine's
-        NHWC inputs (same values as PointTexture.forward followed by the engine's NCHW f32 -> NHWC conversion: both round the same
-        f32 sample once) and the net runs; returns None when the call does not qualify."""
+        """Inference shortcut of the index-map surface (VERDICT r01 #12): four 'uv' maps and nothing else, no supersampling /
+        temporal average / autograd -> the descriptors are gathered from the index maps STRAIGHT into the engine's NHWC inputs
+        (same values as PointTexture.forward followed by the engine's NCHW f32 -> NHWC conversion: both round the same f32 sample
+        once) and the net runs; items of different scenes read their own textures in the same launch.  Returns None when the call
+        does not qualify."""
         net = self.net
-        if (self.ss != 1 or self.temporal_average or net.training or getattr(net, '_is_replica', False) or len(set(texture_ids)) != 1
+        if (self.ss != 1 or self.temporal_average or net.training or getattr(net, '_is_replica', False)
                 or len(maps) != 4 or not all('uv' in k for k in maps)):
             return None
-        tex = self._texture(texture_ids[0])
-        if not isinstance(tex, PointTexture) or not tex.texture_.is_cuda or tex.texture_.shape[1] != 8:
+        if len(set(texture_ids)) == 1:
+            textures, slots = [self._texture(texture_ids[0])], None
+        else:
+            table = self._texture_table(texture_ids)
+            if table is None:
+                return None
+            textures, slots = table
+        if not all(isinstance(t, PointTexture) and t.texture_.is_cuda and t.texture_.shape[1] == 8 for t in textures):
             return None
-        if torch.is_grad_enabled() and (tex.texture_.requires_grad or any(p.requires_grad for p in net.parameters())):
+        if torch.is_grad_enabled() and (any(t.texture_.requires_grad for t in textures)
+                                        or any(p.requires_grad for p in net.parameters())):
             return None
         vals = list(maps.values())
         B, _, H, W = vals[0].shape
         if len(texture_ids) != B or H % 16 or W % 16 or any(tuple(v.shape) != (B, 1, H >> l, W >> l) for l, v in enumerate(vals)):
             return None
+        tex = textures[0]
         dev = tex.texture_.device
         eng = net.engine(B, H, W, dev)
         layout = L.FEAT_NHWC_BF16 if eng.bf16 else L.FEAT_NHWC_F32
-        nd = tex.point_major()
+        nds = [t.point_major() for t in textures]
         for l, v in enumerate(vals):
             ids = v[:, 0].to(dev, torch.float32).contiguous()
-            ops.gather_from_index(nd, ids, layout, tex.activation, out=eng.inputs[l])
+            if slots is None:
+                ops.gather_from_index(nds[0], ids, layout, tex.activation, out=eng.inputs[l])
+            else:
+                ops.gather_from_index_items(nds, slots, ids, layout, tex.activation, out=eng.inputs[l])
         return eng.run().clone()
 
     def forward(self, inputs, **kwargs):
@@ -126,10 +159,13 @@ class NetAndTexture(nn.Module):
                 return out
         one_texture = len(set(texture_ids)) == 1
         items_apart = not self.net.training or getattr(self.net, 'train_batchnorm', 'batch') == 'per_item'
-        if one_texture and len(texture_ids) > 1 and not self.temporal_average and items_apart:
+        batchable = len(texture_ids) > 1 and not self.temporal_average and items_apart
+        table = None if one_texture or not batchable else self._texture_table(texture_ids)
+        if batchable and (one_texture or table is not None):
             # eval-mode BatchNorm is per-pixel affine, and per-item train-mode BatchNorm normalises each item with its own
-            # statistics: B batch-1 passes == one batch-B pass
-            net_input = self._multiscale_input(self._texture(texture_ids[0]), maps)
+            # statistics: B batch-1 passes == one batch-B pass; items of different scenes sample their own textures in one gather
+            sample = self._texture(texture_ids[0]) if one_texture else functools.partial(sample_items, *table)
+            net_input = self._multiscale_input(sample, maps)
             out = self.net(*net_input, **kwargs)
             net_input = [t[-1:] for t in net_input]              # the reference returns the last item's input
         else:

@@ -48,6 +48,27 @@ inline bool bn_channels_ok(int C) { return C == 16 || C == 32 || C == 64 || (C %
         rb::count_launch();                                                                    \
     } while (0)
 
+// shared argument checks of the multi-texture gather entry points (read_tex_table, include/read_b200.h)
+inline int check_tex_table(const read_tex_table *t, int h, int w, bool forward, bool sparse, const char *what)
+{
+    RB_CHECK_ARG(t != nullptr, "%s: null table", what);
+    RB_CHECK_ARG(t->n_slots >= 1 && t->n_slots <= READ_MAX_TEX_SLOTS, "%s: n_slots %d not in 1..%d", what, t->n_slots,
+                 READ_MAX_TEX_SLOTS);
+    RB_CHECK_ARG(t->n_items >= 1 && t->n_items <= READ_MAX_TEX_ITEMS, "%s: n_items %d not in 1..%d", what, t->n_items,
+                 READ_MAX_TEX_ITEMS);
+    RB_CHECK_ARG(h >= 0 && w >= 0, "%s: bad shape", what);
+    for (int b = 0; b < t->n_items; ++b) RB_CHECK_ARG(t->slot[b] < t->n_slots, "%s: item %d maps to slot %d", what, b, t->slot[b]);
+    for (int s = 0; s < t->n_slots; ++s) {
+        RB_CHECK_ARG(t->N[s] >= 1, "%s: slot %d has no points", what, s);
+        if (forward)
+            RB_CHECK_ARG(t->tex_nd[s] && (reinterpret_cast<uintptr_t>(t->tex_nd[s]) & 15) == 0,
+                         "%s: slot %d: descriptors must be non-null and 16B aligned", what, s);
+        else if (sparse)
+            RB_CHECK_ARG(!t->grad_nd[s] || t->touched[s], "%s: slot %d: an accumulator without touched flags", what, s);
+    }
+    return READ_OK;
+}
+
 // max positive int64: larger than any real key (depth bits <= 0x3F800000) under BOTH signed and unsigned
 // comparison, so a min-reduction may be typed int64 (torch.distributed / ncclInt64) or uint64.
 static constexpr unsigned long long ZBUF_EMPTY = 0x7FFFFFFFFFFFFFFFull;

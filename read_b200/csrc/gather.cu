@@ -2,6 +2,7 @@
 // Replaces PointTexture.forward and its autograd backward (READ/models/texture.py:42-70):
 //   feat[b,c,y,x] = texture_[0,c,(int64)idx[b,0,y,x]]      (empty pixel carries idx 0 -> point 0)
 // Descriptors are read from a point-major [N,D] shadow so a pixel touches one 32-byte sector.
+// gather_items_kernel: the same for a batch whose items sample different textures (a texture table in the kernel parameters).
 #include "common.cuh"
 
 namespace rb {
@@ -87,6 +88,46 @@ __global__ void gather_kernel(const float *__restrict__ tex, int D, long long N,
                 else if (LAYOUT == READ_FEAT_NHWC_F32) static_cast<float *>(out)[p * D + c] = v;
                 else static_cast<__nv_bfloat16 *>(out)[p * D + c] = __float2bfloat16_rn(v);
             }
+        }
+    }
+}
+
+// gather_kernel<0, LAYOUT> at D == 8 for a batch whose items sample different textures: item b reads slot t.slot[b] of the table
+// (kernel parameter space), with its ids clamped to that texture's N
+template <int LAYOUT>
+__global__ void gather_items_kernel(const __grid_constant__ read_tex_table t, const float *__restrict__ ids, int h, int w, int act,
+                                    void *__restrict__ out)
+{
+    const long long hw = (long long)h * w;
+    const long long total = (long long)t.n_items * hw;
+    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total;
+         p += (long long)gridDim.x * blockDim.x) {
+        const long long b = p / hw, q = p - b * hw;
+        const int s = t.slot[b];
+        const long long N = t.N[s];
+        long long id = (long long)ids[p];
+        if (id < 0) id = 0;
+        if (id >= N) id = N - 1;
+        const float4 *tp = reinterpret_cast<const float4 *>(t.tex_nd[s] + id * 8);
+        const float4 a = __ldg(tp), c = __ldg(tp + 1);
+        float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
+        if (act != READ_TEXACT_NONE) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = tex_act(v[i], act);
+        }
+        if (LAYOUT == READ_FEAT_NCHW_F32) {
+            float *o = static_cast<float *>(out) + b * 8 * hw + q;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) o[i * hw] = v[i];
+        } else if (LAYOUT == READ_FEAT_NHWC_F32) {
+            float4 *o = reinterpret_cast<float4 *>(static_cast<float *>(out) + p * 8);
+            o[0] = make_float4(v[0], v[1], v[2], v[3]);
+            o[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {
+            __nv_bfloat162 r[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) r[i] = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
+            *reinterpret_cast<uint4 *>(static_cast<__nv_bfloat16 *>(out) + p * 8) = *reinterpret_cast<uint4 *>(r);
         }
     }
 }
@@ -439,6 +480,28 @@ int read_gather_from_index(const float *tex_nd, int D, int64_t N, const float *i
     int rc = check_gather(tex_nd, D, N, ids, B, h, w, out);
     if (rc) return rc;
     return launch_gather<0>(tex_nd, D, N, ids, B, h, w, layout, activation, out, (cudaStream_t)stream);
+}
+
+int read_gather_from_index_items(const read_tex_table *table, const float *ids, int h, int w, int layout, int activation, void *out,
+                                 void *stream)
+{
+    int rc = check_tex_table(table, h, w, true, false, "gather (items)");
+    if (rc) return rc;
+    RB_CHECK_ARG(ids && out && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "gather (items): null or unaligned ids / output");
+    const long long total = (long long)table->n_items * h * w;
+    if (total == 0) return READ_OK;
+    const unsigned g = grid_for(total);
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (layout) {
+    case READ_FEAT_NCHW_F32: gather_items_kernel<READ_FEAT_NCHW_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    case READ_FEAT_NHWC_F32: gather_items_kernel<READ_FEAT_NHWC_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    case READ_FEAT_NHWC_BF16: gather_items_kernel<READ_FEAT_NHWC_BF16><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    default:
+        set_error("gather (items): unknown layout %d", layout);
+        return READ_ERR_INVALID;
+    }
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 int read_gather_from_zbuf(const float *tex_nd, int D, int64_t N, const uint64_t *zbuf_level, int B, int h, int w,

@@ -10,6 +10,8 @@
 //   combine  the thread of a segment's first chunk adds the segment's chunk sums in chunk order, starting from its own, and adds
 //            the result to the row once
 // So each row has exactly one writer per call, and the dense (grad_tex_nd) and sparse (grad_nd + touched) forms share the code.
+// A batch whose items sample different textures (read_tex_table) runs the same chunk and combine bodies over one key space that
+// stacks the slots' rows, key = base[slot] + clamped id; the row writer (SdRowsItems) maps a key back to its slot's row.
 #include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
@@ -37,12 +39,51 @@ __device__ __forceinline__ void sd_add_row(float *out, unsigned char *touched, u
     if (SPARSE && c == 0) touched[id] = 1;
 }
 
-// thread (chunk k, channel c): the runs of equal ids in sorted positions [k * SD_CHUNK, (k + 1) * SD_CHUNK)
+// where a row's sum goes: row `key` of one texture (the single-texture entry points) ...
 template <bool SPARSE>
-__global__ void __launch_bounds__(SD_THREADS)
-sd_chunk_kernel(const float *__restrict__ go, const unsigned *__restrict__ key, const int *__restrict__ pix, long long total,
-                int D, long long hw, long long nchunks, float *__restrict__ out, unsigned char *__restrict__ touched,
-                float *__restrict__ first, float *__restrict__ last)
+struct SdRowsOne {
+    float *out;
+    unsigned char *touched;
+    __device__ __forceinline__ void add(unsigned key, int D, int c, float s) const { sd_add_row<SPARSE>(out, touched, key, D, c, s); }
+};
+
+// ... or, for a batch whose items sample different textures, row key - base[s] of the slot s whose key range holds the key: the
+// slots' rows are stacked in slot order into one key space, base[s] = N[0] + ... + N[s-1]
+struct SdItems {
+    read_tex_table t;
+    unsigned base[READ_MAX_TEX_SLOTS + 1];
+};
+
+template <bool SPARSE>
+struct SdRowsItems {
+    const SdItems &a;
+    __device__ __forceinline__ void add(unsigned key, int D, int c, float s) const
+    {
+        int sl = 0;
+        while (sl + 1 < a.t.n_slots && key >= a.base[sl + 1]) ++sl;
+        if (a.t.grad_nd[sl] != nullptr) sd_add_row<SPARSE>(a.t.grad_nd[sl], a.t.touched[sl], key - a.base[sl], D, c, s);
+    }
+};
+
+__global__ void sd_keys_items_kernel(const float *__restrict__ ids, long long total, long long hw, const __grid_constant__ SdItems a,
+                                     unsigned *__restrict__ key, int *__restrict__ pix)
+{
+    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total; p += (long long)gridDim.x * blockDim.x) {
+        const int s = a.t.slot[p / hw];
+        const long long N = a.t.N[s];
+        long long id = (long long)ids[p];
+        if (id < 0) id = 0;
+        if (id >= N) id = N - 1;
+        key[p] = a.base[s] + (unsigned)id;
+        pix[p] = (int)p;
+    }
+}
+
+// thread (chunk k, channel c): the runs of equal ids in sorted positions [k * SD_CHUNK, (k + 1) * SD_CHUNK)
+template <class Rows>
+__device__ __forceinline__ void sd_chunk_body(const float *__restrict__ go, const unsigned *__restrict__ key, const int *__restrict__ pix,
+                                              long long total, int D, long long hw, long long nchunks, const Rows &rows,
+                                              float *__restrict__ first, float *__restrict__ last)
 {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nchunks * D; t += (long long)gridDim.x * blockDim.x) {
         const long long k = t / D, i0 = k * SD_CHUNK, i1 = i0 + SD_CHUNK < total ? i0 + SD_CHUNK : total;
@@ -58,7 +99,7 @@ sd_chunk_kernel(const float *__restrict__ go, const unsigned *__restrict__ key, 
             // the run [head, i] ends here: a whole segment, or a piece of one that crosses a chunk boundary
             const bool starts = head > 0 ? key[head - 1] != id : true, ends = nx != id;
             if (starts && ends) {
-                sd_add_row<SPARSE>(out, touched, id, D, c, s);
+                rows.add(id, D, c, s);
             } else {
                 if (head == i0) first[t] = s;
                 if (i + 1 == i1) last[t] = s;
@@ -70,12 +111,29 @@ sd_chunk_kernel(const float *__restrict__ go, const unsigned *__restrict__ key, 
     }
 }
 
-// thread (chunk k, channel c): if chunk k holds the first piece of a segment that continues into chunk k + 1, it adds the segment's
-// pieces in chunk order and writes the row
 template <bool SPARSE>
 __global__ void __launch_bounds__(SD_THREADS)
-sd_combine_kernel(const unsigned *__restrict__ key, long long total, int D, long long nchunks, const float *__restrict__ first,
-                  const float *__restrict__ last, float *__restrict__ out, unsigned char *__restrict__ touched)
+sd_chunk_kernel(const float *__restrict__ go, const unsigned *__restrict__ key, const int *__restrict__ pix, long long total,
+                int D, long long hw, long long nchunks, float *__restrict__ out, unsigned char *__restrict__ touched,
+                float *__restrict__ first, float *__restrict__ last)
+{
+    sd_chunk_body(go, key, pix, total, D, hw, nchunks, SdRowsOne<SPARSE>{out, touched}, first, last);
+}
+
+template <bool SPARSE>
+__global__ void __launch_bounds__(SD_THREADS)
+sd_chunk_items_kernel(const float *__restrict__ go, const unsigned *__restrict__ key, const int *__restrict__ pix, long long total,
+                      long long hw, long long nchunks, const __grid_constant__ SdItems a, float *__restrict__ first,
+                      float *__restrict__ last)
+{
+    sd_chunk_body(go, key, pix, total, 8, hw, nchunks, SdRowsItems<SPARSE>{a}, first, last);
+}
+
+// thread (chunk k, channel c): if chunk k holds the first piece of a segment that continues into chunk k + 1, it adds the segment's
+// pieces in chunk order and writes the row
+template <class Rows>
+__device__ __forceinline__ void sd_combine_body(const unsigned *__restrict__ key, long long total, int D, long long nchunks,
+                                                const float *__restrict__ first, const float *__restrict__ last, const Rows &rows)
 {
     for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nchunks * D; t += (long long)gridDim.x * blockDim.x) {
         const long long k = t / D, i0 = k * SD_CHUNK, i1 = i0 + SD_CHUNK;
@@ -93,8 +151,24 @@ sd_combine_kernel(const unsigned *__restrict__ key, long long total, int D, long
         const long long kend = (lo - 1) / SD_CHUNK;                    // the segment's last chunk
         float s = last[t];
         for (long long k2 = k + 1; k2 <= kend; ++k2) s += first[k2 * D + c];
-        sd_add_row<SPARSE>(out, touched, id, D, c, s);
+        rows.add(id, D, c, s);
     }
+}
+
+template <bool SPARSE>
+__global__ void __launch_bounds__(SD_THREADS)
+sd_combine_kernel(const unsigned *__restrict__ key, long long total, int D, long long nchunks, const float *__restrict__ first,
+                  const float *__restrict__ last, float *__restrict__ out, unsigned char *__restrict__ touched)
+{
+    sd_combine_body(key, total, D, nchunks, first, last, SdRowsOne<SPARSE>{out, touched});
+}
+
+template <bool SPARSE>
+__global__ void __launch_bounds__(SD_THREADS)
+sd_combine_items_kernel(const unsigned *__restrict__ key, long long total, long long nchunks, const float *__restrict__ first,
+                        const float *__restrict__ last, const __grid_constant__ SdItems a)
+{
+    sd_combine_body(key, total, 8, nchunks, first, last, SdRowsItems<SPARSE>{a});
 }
 
 struct SdLayout {
@@ -162,6 +236,43 @@ static int sd_run(const float *go, const float *ids, int B, int D, int h, int w,
     return READ_OK;
 }
 
+template <bool SPARSE>
+static int sd_run_items(const float *go, const float *ids, const read_tex_table *table, int h, int w, void *workspace, cudaStream_t st,
+                        const char *what)
+{
+    int rc = check_tex_table(table, h, w, false, SPARSE, what);
+    if (rc) return rc;
+    RB_CHECK_ARG(go && ids && workspace, "%s: null pointer", what);
+    SdItems a{};
+    a.t = *table;
+    long long base = 0;
+    for (int s = 0; s < table->n_slots; ++s) {
+        a.base[s] = (unsigned)base;
+        base += table->N[s];
+        RB_CHECK_ARG(base <= 0x7FFFFFFFll, "%s: the slots hold 2^31 points or more", what);
+    }
+    a.base[table->n_slots] = (unsigned)base;
+    SdLayout L;
+    RB_CHECK_ARG(sd_layout(table->n_items, 8, h, w, base, L), "%s: bad shape", what);
+    if (L.total == 0) return READ_OK;
+    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "%s: workspace must be 16B aligned", what);
+    char *ws = (char *)workspace;
+    unsigned *key_in = (unsigned *)(ws + L.key_in), *key = (unsigned *)(ws + L.key_out);
+    int *pix_in = (int *)(ws + L.pix_in), *pix = (int *)(ws + L.pix_out);
+    float *first = (float *)(ws + L.first), *last = (float *)(ws + L.last);
+    const long long hw = (long long)h * w;
+    sd_keys_items_kernel<<<sd_grid(L.total), SD_THREADS, 0, st>>>(ids, L.total, hw, a, key_in, pix_in);
+    RB_LAUNCH_CHECK();
+    size_t temp_bytes = L.temp_bytes;
+    RB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.temp, temp_bytes, key_in, key, pix_in, pix, (int)L.total, 0, L.end_bit, st));
+    count_launch();
+    sd_chunk_items_kernel<SPARSE><<<sd_grid(L.nchunks * 8), SD_THREADS, 0, st>>>(go, key, pix, L.total, hw, L.nchunks, a, first, last);
+    RB_LAUNCH_CHECK();
+    sd_combine_items_kernel<SPARSE><<<sd_grid(L.nchunks * 8), SD_THREADS, 0, st>>>(key, L.total, L.nchunks, first, last, a);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -187,6 +298,19 @@ int read_gather_backward_sparse_det(const float *grad_out, const float *ids, int
 {
     RB_CHECK_ARG(grad_out && ids && grad_nd && touched && workspace, "gather backward (sparse, deterministic): null pointer");
     return sd_run<true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, workspace, (cudaStream_t)stream);
+}
+
+int read_gather_backward_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                   void *workspace, void *stream)
+{
+    return sd_run_items<false>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream, "gather backward (items, deterministic)");
+}
+
+int read_gather_backward_sparse_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                          void *workspace, void *stream)
+{
+    return sd_run_items<true>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
+                              "gather backward (sparse, items, deterministic)");
 }
 
 }  // extern "C"

@@ -3,6 +3,8 @@
 // torch.optim.RMSprop over all N points (READ/pipelines/ogl.py:16,97-102) - 160-320 MB of gradient and 3 x 320 MB of optimizer
 // traffic per step for a few 10^4 visible points.  Here everything past the net's input gradient touches only visible points:
 //   gather_backward_sparse   grad[id,:] += dL/dfeat[:, pixel]  (point-major accumulator) and touched[id] = 1
+//   gather_backward_items    the same (sparse or dense) for a batch whose items sample different textures: each item's pixels go
+//                            to its own texture's accumulator (a batch that mixes scenes in one net call)
 //   sparse_rmsprop           for touched points only: lazily decayed square_avg, parameter update written to BOTH the
 //                            checkpoint-layout parameter [1,D,N] and its point-major shadow [N,D], gradient row and flag cleared
 //   compact / scatter pairs  (id, grad[D]) lists for the data-parallel exchange: ranks all-gather their touched rows instead of
@@ -41,6 +43,49 @@ __global__ void gather_backward_sparse_kernel(const float *__restrict__ go, cons
     if (zero_any) {
         for (int c = threadIdx.x; c < D; c += blockDim.x) atomicAdd(gt + c, zero_acc[c]);
         if (threadIdx.x == 0) touched[0] = 1;
+    }
+}
+
+// gather_backward_kernel (SPARSE = false) / gather_backward_sparse_kernel (true) at D == 8 for a batch whose items sample different
+// textures: item b's pixels go to slot t.slot[b]'s accumulator.  Point 0 is pre-reduced per block AND per slot (a shared [slot][8]
+// accumulator): with one shared row, every empty pixel of one slot's sparse crop would serialise on another's point 0.
+template <bool SPARSE>
+__global__ void gather_backward_items_kernel(const float *__restrict__ go, const float *__restrict__ ids,
+                                             const __grid_constant__ read_tex_table t, int h, int w)
+{
+    __shared__ float zero_acc[READ_MAX_TEX_SLOTS][8];
+    __shared__ int zero_any[READ_MAX_TEX_SLOTS];
+    for (int i = threadIdx.x; i < READ_MAX_TEX_SLOTS * 8; i += blockDim.x) zero_acc[i >> 3][i & 7] = 0.f;
+    for (int i = threadIdx.x; i < READ_MAX_TEX_SLOTS; i += blockDim.x) zero_any[i] = 0;
+    __syncthreads();
+    const long long hw = (long long)h * w;
+    const long long total = (long long)t.n_items * hw;
+    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total; p += (long long)gridDim.x * blockDim.x) {
+        const long long b = p / hw, q = p - b * hw;
+        const int s = t.slot[b];
+        float *gt = t.grad_nd[s];
+        if (gt == nullptr) continue;
+        const long long N = t.N[s];
+        long long id = (long long)ids[p];
+        if (id < 0) id = 0;
+        if (id >= N) id = N - 1;
+        const float *g = go + b * 8 * hw + q;
+        if (id == 0) {
+            zero_any[s] = 1;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) atomicAdd(&zero_acc[s][c], g[c * hw]);
+        } else {
+#pragma unroll
+            for (int c = 0; c < 8; ++c) atomicAdd(gt + id * 8 + c, g[c * hw]);
+            if (SPARSE) t.touched[s][id] = 1;
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < t.n_slots * 8; i += blockDim.x) {
+        const int s = i >> 3, c = i & 7;
+        if (!zero_any[s]) continue;
+        atomicAdd(t.grad_nd[s] + c, zero_acc[s][c]);
+        if (SPARSE && c == 0) t.touched[s][0] = 1;
     }
 }
 
@@ -154,6 +199,20 @@ static unsigned tgrid(long long total)
     return (unsigned)blocks;
 }
 
+template <bool SPARSE>
+static int gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream,
+                                 const char *what)
+{
+    int rc = check_tex_table(table, h, w, false, SPARSE, what);
+    if (rc) return rc;
+    RB_CHECK_ARG(grad_out && ids, "%s: null pointer", what);
+    const long long total = (long long)table->n_items * h * w;
+    if (total == 0) return READ_OK;
+    gather_backward_items_kernel<SPARSE><<<tgrid(total), 256, 0, (cudaStream_t)stream>>>(grad_out, ids, *table, h, w);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -171,6 +230,17 @@ int read_gather_backward_sparse(const float *grad_out, const float *ids, int B, 
                                                                                                 touched);
     RB_LAUNCH_CHECK();
     return READ_OK;
+}
+
+int read_gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream)
+{
+    return gather_backward_items<false>(grad_out, ids, table, h, w, stream, "gather backward (items)");
+}
+
+int read_gather_backward_sparse_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
+                                      void *stream)
+{
+    return gather_backward_items<true>(grad_out, ids, table, h, w, stream, "gather backward (sparse, items)");
 }
 
 int read_sparse_rmsprop_step(float *param_cn, float *shadow_nd, float *grad_nd, unsigned char *touched, float *square_avg,

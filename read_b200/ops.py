@@ -245,6 +245,64 @@ def gather_backward(grad_out, ids, N):
     return g
 
 
+def tex_table(slots, N, tex=None, grad=None, touched=None):
+    """The multi-texture kernels' table (read_tex_table): item b samples slot ``slots[b]``; per slot its point count ``N[s]`` and,
+    as the call needs them, its [N, 8] descriptors ``tex[s]``, its [N, 8] accumulator ``grad[s]`` (None: the slot receives nothing)
+    and its [N] ``touched`` flags."""
+    if not 1 <= len(N) <= L.MAX_TEX_SLOTS or not 1 <= len(slots) <= L.MAX_TEX_ITEMS:
+        raise RuntimeError(f"read_b200: a texture table holds 1..{L.MAX_TEX_SLOTS} textures and 1..{L.MAX_TEX_ITEMS} items")
+    t = L.ReadTexTable()
+    t.n_slots, t.n_items = len(N), len(slots)
+    for s, n in enumerate(N):
+        t.N[s] = int(n)
+        for field, seq in (("tex_nd", tex), ("grad_nd", grad), ("touched", touched)):
+            if seq is not None and seq[s] is not None:
+                getattr(t, field)[s] = seq[s].data_ptr()
+    for b, s in enumerate(slots):
+        t.slot[b] = int(s)
+    return t
+
+
+def gather_from_index_items(tex_nds, slots, ids, layout=L.FEAT_NCHW_F32, activation="none", out=None):
+    """gather_from_index for a batch whose item b samples ``tex_nds[slots[b]]`` ([N_s, 8] f32 point-major): one launch.
+    ids [B,h,w] f32 cuda (contiguous), B = len(slots)."""
+    _f32c(ids, "ids")
+    B, h, w = ids.shape
+    if B != len(slots):
+        raise RuntimeError("read_b200: one slot per item")
+    for nd in tex_nds:
+        _f32c(nd, "texture")
+        if nd.dim() != 2 or nd.shape[1] != 8:
+            raise RuntimeError("read_b200: the multi-texture gather takes [N, 8] descriptors")
+    out = _feat_out(B, 8, h, w, layout, ids.device, out)
+    t = tex_table(slots, [nd.shape[0] for nd in tex_nds], tex=tex_nds)
+    L.check(L.load().read_gather_from_index_items(ctypes.byref(t), ids.data_ptr(), h, w, layout, L.TEXACT[activation],
+                                                  out.data_ptr(), L.stream_ptr()))
+    return out
+
+
+def gather_backward_items(grad_out, ids, slots, N, grads, touched=None):
+    """Backward of gather_from_index_items: item b's pixels scatter-add into ``grads[slots[b]]`` ([N_s, 8] f32 accumulators; None: the
+    slot receives nothing) and, when ``touched`` is given (the sparse form), set ``touched[slots[b]]``.  grad_out [B,8,h,w] f32.  Under
+    torch.use_deterministic_algorithms(True) the additions run in the fixed order of read_gather_backward_items_det."""
+    grad_out = grad_out.contiguous()
+    _f32c(grad_out, "grad_out")
+    _f32c(ids, "ids")
+    B, D, h, w = grad_out.shape
+    if D != 8 or tuple(ids.shape) != (B, h, w) or B != len(slots):
+        raise RuntimeError("read_b200: multi-texture gather backward: shape mismatch")
+    t = tex_table(slots, N, grad=grads, touched=touched)
+    lib, sparse = L.load(), touched is not None
+    if torch.are_deterministic_algorithms_enabled():
+        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, 8, h, w, sum(int(n) for n in N)), grad_out.device,
+                           "multi-texture gather backward")
+        fn = lib.read_gather_backward_sparse_items_det if sparse else lib.read_gather_backward_items_det
+        L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, ws.data_ptr(), L.stream_ptr()))
+        return
+    fn = lib.read_gather_backward_sparse_items if sparse else lib.read_gather_backward_items
+    L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, L.stream_ptr()))
+
+
 def det_workspace(nbytes, device, what):
     """Workspace of a deterministic entry point (nbytes from its *_workspace_bytes query; -1: the shape is not supported)."""
     if nbytes < 0:

@@ -37,6 +37,58 @@ class _Gather(torch.autograd.Function):
         return ops.texture_to_channel_major(g_nd), None         # [1,C,N]
 
 
+class _GatherItems(torch.autograd.Function):
+    """_Gather / train._GatherSparse for a batch whose item b samples ``textures[slots[b]]``: one gather and one scatter per call.
+    Sparse: every slot's accumulator receives its items' gradient and the Function returns None; dense: one [1, 8, N] gradient per
+    texture.  A texture whose parameter does not require grad gets None and its accumulator is left alone."""
+
+    @staticmethod
+    def forward(ctx, ids, slots, textures, sparse, *params):
+        ctx.save_for_backward(ids)
+        ctx.slots, ctx.textures, ctx.sparse = slots, textures, sparse
+        return ops.gather_from_index_items([t.point_major() for t in textures], slots, ids, L.FEAT_NCHW_F32)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (ids,) = ctx.saved_tensors
+        need = ctx.needs_input_grad[4:]
+        g = grad_out if grad_out.dtype == torch.float32 else grad_out.float()
+        N = [t.texture_.shape[-1] for t in ctx.textures]
+        if ctx.sparse:
+            st = [t._sparse if n else None for t, n in zip(ctx.textures, need)]
+            ops.gather_backward_items(g, ids, ctx.slots, N, [None if s is None else s.grad for s in st],
+                                      [None if s is None else s.touched for s in st])
+            return (None,) * (4 + len(N))
+        grads = [torch.zeros((n, 8), dtype=torch.float32, device=g.device) if r else None for n, r in zip(N, need)]
+        ops.gather_backward_items(g, ids, ctx.slots, N, grads)
+        return (None,) * 4 + tuple(None if gd is None else ops.texture_to_channel_major(gd) for gd in grads)
+
+
+def sample_items(textures, slots, inputs):
+    """``PointTexture.forward`` for a batch whose item b samples ``textures[slots[b]]``, in one gather launch (and one scatter in the
+    backward).  The textures are PointTextures with 8 channels, one activation and one gradient mode (read_b200.compose checks)."""
+    ids = inputs[:, 0]
+    for t in textures:
+        if not t.texture_.is_cuda:
+            raise RuntimeError("read_b200.PointTexture: texture must be on a CUDA device (no CPU fallback)")
+    ids = ids.to(textures[0].texture_.device, torch.float32).contiguous()
+    act = textures[0].activation
+    params = [t.texture_ for t in textures]
+    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+        sparse = getattr(textures[0], '_sparse_requested', False)
+        if sparse:
+            from . import train
+            for t in textures:
+                train.enable_sparse_grad(t)
+        sample = _GatherItems.apply(ids, tuple(slots), tuple(textures), sparse, *params)
+        if act == 'sigmoid':
+            return torch.sigmoid(sample)
+        if act == 'tanh':
+            return torch.tanh(sample)
+        return sample
+    return ops.gather_from_index_items([t.point_major() for t in textures], slots, ids, L.FEAT_NCHW_F32, act)
+
+
 _INITIALISERS = {'zeros': torch.zeros, 'rand': torch.rand}
 
 
