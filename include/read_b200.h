@@ -105,6 +105,9 @@ unsigned read_raster_direct_mask(int W, int H, int L);
  */
 int read_zbuf_resolve(const uint64_t *zbuf_level, int64_t pixels, float *index_out, float *depth_out,
                       void *stream);
+/* read_zbuf_resolve with an int32 index: the key's low 32 bits (the point id), 0 = empty.  For clouds of more than 2^24 + 1
+ * points, whose ids a float32 map cannot all hold; the caller keeps N < 2^31. */
+int read_zbuf_resolve_i32(const uint64_t *zbuf_level, int64_t pixels, int32_t *index_out, float *depth_out, void *stream);
 
 /*
  * Replaces: pcpr.forward itself (pcpr_cuda.cpp:23-37): one level, B views.
@@ -145,6 +148,13 @@ int read_pyramid_resolve_gather(const float *tex_nd, int D, int64_t N, uint64_t 
  * id 0, so point 0 receives their gradient exactly like the reference. */
 int read_gather_backward(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                          float *grad_tex_nd, void *stream);
+/* Int32 index maps (clouds of more than 2^24 + 1 points): every entry point that reads an index map has an _i32 twin taking
+ * `const int32_t *ids`, with otherwise the same arguments, clamping (id < 0 -> 0, id >= N -> N - 1), semantics and, for the
+ * deterministic forms, the same workspace query and order of additions.  The float forms are unchanged. */
+int read_gather_from_index_i32(const float *tex_nd, int D, int64_t N, const int32_t *ids, int B, int h, int w, int layout,
+                               int activation, void *out, void *stream);
+int read_gather_backward_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                             void *stream);
 
 /* Batches whose items sample different textures (a training batch that mixes scenes), D == 8.  The table travels BY VALUE in the
  * kernel parameters (no device-side table, no host-to-device copy).  Item b of the call samples slot slot[b]; its ids are clamped
@@ -171,6 +181,11 @@ int read_gather_from_index_items(const read_tex_table *table, const float *ids, 
 int read_gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream);
 int read_gather_backward_sparse_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
                                       void *stream);
+int read_gather_from_index_items_i32(const read_tex_table *table, const int32_t *ids, int h, int w, int layout, int activation,
+                                     void *out, void *stream);
+int read_gather_backward_items_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w, void *stream);
+int read_gather_backward_sparse_items_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                          void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Gated convolution (BasicConv, READ/models/unet.py:22-53) with everything around it fused:
@@ -333,6 +348,8 @@ int read_halo_exchange(const read_halo_desc *d, void *stream);
  *   read_scatter_pairs          : grad_nd[id,:] += grads[k,:], touched[id] = 1 (pairs received from other ranks) */
 int read_gather_backward_sparse(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                                 float *grad_nd, unsigned char *touched, void *stream);
+int read_gather_backward_sparse_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
+                                    unsigned char *touched, void *stream);
 int read_sparse_rmsprop_step(float *param_cn, float *shadow_nd, float *grad_nd, unsigned char *touched, float *square_avg,
                              int32_t *last_step, int64_t N, int D, int step, float lr, float alpha, float eps, float weight_decay,
                              void *stream);
@@ -515,6 +532,15 @@ int read_gather_backward_items_det(const float *grad_out, const float *ids, cons
                                    void *workspace, void *stream);
 int read_gather_backward_sparse_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
                                           void *workspace, void *stream);
+/* int32 index maps: the same workspace query and order; only the key build reads the other type */
+int read_gather_backward_det_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                                 void *workspace, void *stream);
+int read_gather_backward_sparse_det_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N,
+                                        float *grad_nd, unsigned char *touched, void *workspace, void *stream);
+int read_gather_backward_items_det_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                       void *workspace, void *stream);
+int read_gather_backward_sparse_items_det_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                              void *workspace, void *stream);
 int64_t read_gate_det_workspace_bytes(int items, int C);
 int read_gate_backward_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                            const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,

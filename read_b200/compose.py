@@ -143,7 +143,7 @@ class NetAndTexture(nn.Module):
         layout = L.FEAT_NHWC_BF16 if eng.bf16 else L.FEAT_NHWC_F32
         nds = [t.point_major() for t in textures]
         for l, v in enumerate(vals):
-            ids = v[:, 0].to(dev, torch.float32).contiguous()
+            ids = ops.index_map(v[:, 0], dev)
             if slots is None:
                 ops.gather_from_index(nds[0], ids, layout, tex.activation, out=eng.inputs[l])
             else:
@@ -203,11 +203,13 @@ class NetAndTexture(nn.Module):
 
         ``self.ss`` > 1 renders the pyramid at ss x (W, H) and reduces every level's features bilinearly, ``temporal_average``
         blends each level with the previous frame's (already blended) input - both exactly as ``forward`` does on index maps.
-        ``want_maps``: also return the float (index, depth) maps per level; ``return_input``: also return the net input
+        ``want_maps``: also return the (index, depth) maps per level, index maps of ``ops.index_map_dtype(N)`` (float32 up to
+        2^24 + 1 points, int32 above); ``return_input``: also return the net input
         (list of [B,8,h,w] f32, the reference's ``net_input``); ``clone_output=False`` hands out the engine's own output buffer
         (valid until the next frame) for callers that consume it immediately."""
         store = xyz if isinstance(xyz, ops.SortedPoints) else None
         pts = store.pts4 if store is not None else xyz
+        map_dtype = ops.index_map_dtype(store.n if store is not None else pts.shape[0])      # ValueError at 2^31 points or more
         L.require_device()
         lib = L.load()
         texture = self._texture(texture_id)
@@ -255,7 +257,7 @@ class NetAndTexture(nn.Module):
             out = out.clone()
         extras = []
         if want_maps:
-            extras.append([ops.zbuf_resolve(pyr, l) for l in range(n_levels)])
+            extras.append([ops.zbuf_resolve(pyr, l, index_dtype=map_dtype) for l in range(n_levels)])
         if return_input:
             extras.append([ops.nhwc_to_nchw(t) for t in eng.inputs])
         return (out, *extras) if extras else out

@@ -39,7 +39,7 @@ __device__ __forceinline__ float tex_act(float v, int act)
     return v;
 }
 
-// SRC: 0 = float index map, 1 = packed zbuf
+// SRC: 0 = float index map, 1 = packed zbuf, 2 = int32 index map (clouds of more than 2^24 + 1 points)
 template <int SRC, int LAYOUT>
 __global__ void gather_kernel(const float *__restrict__ tex, int D, long long N, const void *__restrict__ src, int B,
                               int h, int w, int act, void *__restrict__ out)
@@ -51,6 +51,8 @@ __global__ void gather_kernel(const float *__restrict__ tex, int D, long long N,
         long long id;
         if (SRC == 0) {
             id = (long long)static_cast<const float *>(src)[p];           // texture.py:52 .long()
+        } else if (SRC == 2) {
+            id = static_cast<const int32_t *>(src)[p];
         } else {
             const unsigned long long k = static_cast<const unsigned long long *>(src)[p];
             id = (k == ZBUF_EMPTY) ? 0ll : (long long)(k & 0xFFFFFFFFull);
@@ -93,9 +95,9 @@ __global__ void gather_kernel(const float *__restrict__ tex, int D, long long N,
 }
 
 // gather_kernel<0, LAYOUT> at D == 8 for a batch whose items sample different textures: item b reads slot t.slot[b] of the table
-// (kernel parameter space), with its ids clamped to that texture's N
-template <int LAYOUT>
-__global__ void gather_items_kernel(const __grid_constant__ read_tex_table t, const float *__restrict__ ids, int h, int w, int act,
+// (kernel parameter space), with its ids clamped to that texture's N.  IdT: float or int32_t index map
+template <typename IdT, int LAYOUT>
+__global__ void gather_items_kernel(const __grid_constant__ read_tex_table t, const IdT *__restrict__ ids, int h, int w, int act,
                                     void *__restrict__ out)
 {
     const long long hw = (long long)h * w;
@@ -133,8 +135,9 @@ __global__ void gather_items_kernel(const __grid_constant__ read_tex_table t, co
 }
 
 // grad_tex[id,:] += grad_out[b,:,q].  Empty pixels (id 0) are pre-reduced per block in shared memory:
-// in a sparse view millions of pixels would otherwise serialise on point 0's 8 addresses.
-__global__ void gather_backward_kernel(const float *__restrict__ go, const float *__restrict__ ids, int B, int D, int h,
+// in a sparse view millions of pixels would otherwise serialise on point 0's 8 addresses.  IdT: float or int32_t index map.
+template <typename IdT>
+__global__ void gather_backward_kernel(const float *__restrict__ go, const IdT *__restrict__ ids, int B, int D, int h,
                                        int w, long long N, float *__restrict__ gt)
 {
     extern __shared__ float zero_acc[];   // [D]
@@ -442,6 +445,40 @@ __global__ void stage_inputs_kernel(const float *__restrict__ src, int B, int hs
     }
 }
 
+template <typename IdT>
+static int gather_items(const read_tex_table *table, const IdT *ids, int h, int w, int layout, int activation, void *out, cudaStream_t st)
+{
+    int rc = check_tex_table(table, h, w, true, false, "gather (items)");
+    if (rc) return rc;
+    RB_CHECK_ARG(ids && out && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "gather (items): null or unaligned ids / output");
+    const long long total = (long long)table->n_items * h * w;
+    if (total == 0) return READ_OK;
+    const unsigned g = grid_for(total);
+    switch (layout) {
+    case READ_FEAT_NCHW_F32: gather_items_kernel<IdT, READ_FEAT_NCHW_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    case READ_FEAT_NHWC_F32: gather_items_kernel<IdT, READ_FEAT_NHWC_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    case READ_FEAT_NHWC_BF16: gather_items_kernel<IdT, READ_FEAT_NHWC_BF16><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
+    default:
+        set_error("gather (items): unknown layout %d", layout);
+        return READ_ERR_INVALID;
+    }
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+template <typename IdT>
+static int gather_backward(const float *grad_out, const IdT *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                           cudaStream_t st)
+{
+    RB_CHECK_ARG(grad_out && ids && grad_tex_nd, "gather backward: null pointer");
+    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward: bad shape");
+    const long long total = (long long)B * h * w;
+    if (total == 0) return READ_OK;
+    gather_backward_kernel<IdT><<<grid_for(total), 256, D * sizeof(float), st>>>(grad_out, ids, B, D, h, w, N, grad_tex_nd);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -482,26 +519,24 @@ int read_gather_from_index(const float *tex_nd, int D, int64_t N, const float *i
     return launch_gather<0>(tex_nd, D, N, ids, B, h, w, layout, activation, out, (cudaStream_t)stream);
 }
 
+int read_gather_from_index_i32(const float *tex_nd, int D, int64_t N, const int32_t *ids, int B, int h, int w, int layout,
+                               int activation, void *out, void *stream)
+{
+    int rc = check_gather(tex_nd, D, N, ids, B, h, w, out);
+    if (rc) return rc;
+    return launch_gather<2>(tex_nd, D, N, ids, B, h, w, layout, activation, out, (cudaStream_t)stream);
+}
+
 int read_gather_from_index_items(const read_tex_table *table, const float *ids, int h, int w, int layout, int activation, void *out,
                                  void *stream)
 {
-    int rc = check_tex_table(table, h, w, true, false, "gather (items)");
-    if (rc) return rc;
-    RB_CHECK_ARG(ids && out && (reinterpret_cast<uintptr_t>(out) & 15) == 0, "gather (items): null or unaligned ids / output");
-    const long long total = (long long)table->n_items * h * w;
-    if (total == 0) return READ_OK;
-    const unsigned g = grid_for(total);
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (layout) {
-    case READ_FEAT_NCHW_F32: gather_items_kernel<READ_FEAT_NCHW_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
-    case READ_FEAT_NHWC_F32: gather_items_kernel<READ_FEAT_NHWC_F32><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
-    case READ_FEAT_NHWC_BF16: gather_items_kernel<READ_FEAT_NHWC_BF16><<<g, 256, 0, st>>>(*table, ids, h, w, activation, out); break;
-    default:
-        set_error("gather (items): unknown layout %d", layout);
-        return READ_ERR_INVALID;
-    }
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gather_items<float>(table, ids, h, w, layout, activation, out, (cudaStream_t)stream);
+}
+
+int read_gather_from_index_items_i32(const read_tex_table *table, const int32_t *ids, int h, int w, int layout, int activation,
+                                     void *out, void *stream)
+{
+    return gather_items<int32_t>(table, ids, h, w, layout, activation, out, (cudaStream_t)stream);
 }
 
 int read_gather_from_zbuf(const float *tex_nd, int D, int64_t N, const uint64_t *zbuf_level, int B, int h, int w,
@@ -549,14 +584,13 @@ int read_pyramid_resolve_gather(const float *tex_nd, int D, int64_t N, uint64_t 
 int read_gather_backward(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                          float *grad_tex_nd, void *stream)
 {
-    RB_CHECK_ARG(grad_out && ids && grad_tex_nd, "gather backward: null pointer");
-    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward: bad shape");
-    const long long total = (long long)B * h * w;
-    if (total == 0) return READ_OK;
-    gather_backward_kernel<<<grid_for(total), 256, D * sizeof(float), (cudaStream_t)stream>>>(grad_out, ids, B, D, h, w,
-                                                                                               N, grad_tex_nd);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gather_backward<float>(grad_out, ids, B, D, h, w, N, grad_tex_nd, (cudaStream_t)stream);
+}
+
+int read_gather_backward_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                             void *stream)
+{
+    return gather_backward<int32_t>(grad_out, ids, B, D, h, w, N, grad_tex_nd, (cudaStream_t)stream);
 }
 
 int read_stage_net_inputs(const float *src, int B, int hs, int ws, int C, int factor, float *last, int have_last, int act_dtype,

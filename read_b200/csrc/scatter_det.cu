@@ -20,7 +20,9 @@ namespace rb {
 
 constexpr int SD_CHUNK = 128, SD_THREADS = 256;
 
-__global__ void sd_keys_kernel(const float *__restrict__ ids, long long total, long long N, unsigned *__restrict__ key,
+// IdT: float or int32_t index map; only the key build reads the ids
+template <typename IdT>
+__global__ void sd_keys_kernel(const IdT *__restrict__ ids, long long total, long long N, unsigned *__restrict__ key,
                                int *__restrict__ pix)
 {
     for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total; p += (long long)gridDim.x * blockDim.x) {
@@ -65,7 +67,8 @@ struct SdRowsItems {
     }
 };
 
-__global__ void sd_keys_items_kernel(const float *__restrict__ ids, long long total, long long hw, const __grid_constant__ SdItems a,
+template <typename IdT>
+__global__ void sd_keys_items_kernel(const IdT *__restrict__ ids, long long total, long long hw, const __grid_constant__ SdItems a,
                                      unsigned *__restrict__ key, int *__restrict__ pix)
 {
     for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total; p += (long long)gridDim.x * blockDim.x) {
@@ -211,8 +214,8 @@ static unsigned sd_grid(long long n)
     return (unsigned)(blocks < 1 ? 1 : blocks > cap ? cap : blocks);
 }
 
-template <bool SPARSE>
-static int sd_run(const float *go, const float *ids, int B, int D, int h, int w, long long N, float *out, unsigned char *touched,
+template <typename IdT, bool SPARSE>
+static int sd_run(const float *go, const IdT *ids, int B, int D, int h, int w, long long N, float *out, unsigned char *touched,
                   void *workspace, cudaStream_t st)
 {
     SdLayout L;
@@ -223,7 +226,7 @@ static int sd_run(const float *go, const float *ids, int B, int D, int h, int w,
     unsigned *key_in = (unsigned *)(ws + L.key_in), *key = (unsigned *)(ws + L.key_out);
     int *pix_in = (int *)(ws + L.pix_in), *pix = (int *)(ws + L.pix_out);
     float *first = (float *)(ws + L.first), *last = (float *)(ws + L.last);
-    sd_keys_kernel<<<sd_grid(L.total), SD_THREADS, 0, st>>>(ids, L.total, N, key_in, pix_in);
+    sd_keys_kernel<IdT><<<sd_grid(L.total), SD_THREADS, 0, st>>>(ids, L.total, N, key_in, pix_in);
     RB_LAUNCH_CHECK();
     size_t temp_bytes = L.temp_bytes;
     RB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.temp, temp_bytes, key_in, key, pix_in, pix, (int)L.total, 0, L.end_bit, st));
@@ -236,8 +239,8 @@ static int sd_run(const float *go, const float *ids, int B, int D, int h, int w,
     return READ_OK;
 }
 
-template <bool SPARSE>
-static int sd_run_items(const float *go, const float *ids, const read_tex_table *table, int h, int w, void *workspace, cudaStream_t st,
+template <typename IdT, bool SPARSE>
+static int sd_run_items(const float *go, const IdT *ids, const read_tex_table *table, int h, int w, void *workspace, cudaStream_t st,
                         const char *what)
 {
     int rc = check_tex_table(table, h, w, false, SPARSE, what);
@@ -261,7 +264,7 @@ static int sd_run_items(const float *go, const float *ids, const read_tex_table 
     int *pix_in = (int *)(ws + L.pix_in), *pix = (int *)(ws + L.pix_out);
     float *first = (float *)(ws + L.first), *last = (float *)(ws + L.last);
     const long long hw = (long long)h * w;
-    sd_keys_items_kernel<<<sd_grid(L.total), SD_THREADS, 0, st>>>(ids, L.total, hw, a, key_in, pix_in);
+    sd_keys_items_kernel<IdT><<<sd_grid(L.total), SD_THREADS, 0, st>>>(ids, L.total, hw, a, key_in, pix_in);
     RB_LAUNCH_CHECK();
     size_t temp_bytes = L.temp_bytes;
     RB_CUDA(cub::DeviceRadixSort::SortPairs(ws + L.temp, temp_bytes, key_in, key, pix_in, pix, (int)L.total, 0, L.end_bit, st));
@@ -290,27 +293,56 @@ int read_gather_backward_det(const float *grad_out, const float *ids, int B, int
                              void *workspace, void *stream)
 {
     RB_CHECK_ARG(grad_out && ids && grad_tex_nd && workspace, "gather backward (deterministic): null pointer");
-    return sd_run<false>(grad_out, ids, B, D, h, w, N, grad_tex_nd, nullptr, workspace, (cudaStream_t)stream);
+    return sd_run<float, false>(grad_out, ids, B, D, h, w, N, grad_tex_nd, nullptr, workspace, (cudaStream_t)stream);
+}
+
+int read_gather_backward_det_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                                 void *workspace, void *stream)
+{
+    RB_CHECK_ARG(grad_out && ids && grad_tex_nd && workspace, "gather backward (deterministic): null pointer");
+    return sd_run<int32_t, false>(grad_out, ids, B, D, h, w, N, grad_tex_nd, nullptr, workspace, (cudaStream_t)stream);
 }
 
 int read_gather_backward_sparse_det(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
                                     unsigned char *touched, void *workspace, void *stream)
 {
     RB_CHECK_ARG(grad_out && ids && grad_nd && touched && workspace, "gather backward (sparse, deterministic): null pointer");
-    return sd_run<true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, workspace, (cudaStream_t)stream);
+    return sd_run<float, true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, workspace, (cudaStream_t)stream);
+}
+
+int read_gather_backward_sparse_det_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N,
+                                        float *grad_nd, unsigned char *touched, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(grad_out && ids && grad_nd && touched && workspace, "gather backward (sparse, deterministic): null pointer");
+    return sd_run<int32_t, true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, workspace, (cudaStream_t)stream);
 }
 
 int read_gather_backward_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
                                    void *workspace, void *stream)
 {
-    return sd_run_items<false>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream, "gather backward (items, deterministic)");
+    return sd_run_items<float, false>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
+                                      "gather backward (items, deterministic)");
+}
+
+int read_gather_backward_items_det_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                       void *workspace, void *stream)
+{
+    return sd_run_items<int32_t, false>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
+                                        "gather backward (items, deterministic)");
 }
 
 int read_gather_backward_sparse_items_det(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
                                           void *workspace, void *stream)
 {
-    return sd_run_items<true>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
-                              "gather backward (sparse, items, deterministic)");
+    return sd_run_items<float, true>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
+                                     "gather backward (sparse, items, deterministic)");
+}
+
+int read_gather_backward_sparse_items_det_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                              void *workspace, void *stream)
+{
+    return sd_run_items<int32_t, true>(grad_out, ids, table, h, w, workspace, (cudaStream_t)stream,
+                                       "gather backward (sparse, items, deterministic)");
 }
 
 }  // extern "C"

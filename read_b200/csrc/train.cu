@@ -16,7 +16,9 @@
 
 namespace rb {
 
-__global__ void gather_backward_sparse_kernel(const float *__restrict__ go, const float *__restrict__ ids, int B, int D, int h,
+// IdT: float or int32_t index map (every kernel of this file that reads ids)
+template <typename IdT>
+__global__ void gather_backward_sparse_kernel(const float *__restrict__ go, const IdT *__restrict__ ids, int B, int D, int h,
                                               int w, long long N, float *__restrict__ gt, unsigned char *__restrict__ touched)
 {
     extern __shared__ float zero_acc[];   // [D]: pixels that show point 0 (and every empty pixel) are pre-reduced per block
@@ -49,8 +51,8 @@ __global__ void gather_backward_sparse_kernel(const float *__restrict__ go, cons
 // gather_backward_kernel (SPARSE = false) / gather_backward_sparse_kernel (true) at D == 8 for a batch whose items sample different
 // textures: item b's pixels go to slot t.slot[b]'s accumulator.  Point 0 is pre-reduced per block AND per slot (a shared [slot][8]
 // accumulator): with one shared row, every empty pixel of one slot's sparse crop would serialise on another's point 0.
-template <bool SPARSE>
-__global__ void gather_backward_items_kernel(const float *__restrict__ go, const float *__restrict__ ids,
+template <typename IdT, bool SPARSE>
+__global__ void gather_backward_items_kernel(const float *__restrict__ go, const IdT *__restrict__ ids,
                                              const __grid_constant__ read_tex_table t, int h, int w)
 {
     __shared__ float zero_acc[READ_MAX_TEX_SLOTS][8];
@@ -199,8 +201,8 @@ static unsigned tgrid(long long total)
     return (unsigned)blocks;
 }
 
-template <bool SPARSE>
-static int gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream,
+template <typename IdT, bool SPARSE>
+static int gather_backward_items(const float *grad_out, const IdT *ids, const read_tex_table *table, int h, int w, void *stream,
                                  const char *what)
 {
     int rc = check_tex_table(table, h, w, false, SPARSE, what);
@@ -208,7 +210,20 @@ static int gather_backward_items(const float *grad_out, const float *ids, const 
     RB_CHECK_ARG(grad_out && ids, "%s: null pointer", what);
     const long long total = (long long)table->n_items * h * w;
     if (total == 0) return READ_OK;
-    gather_backward_items_kernel<SPARSE><<<tgrid(total), 256, 0, (cudaStream_t)stream>>>(grad_out, ids, *table, h, w);
+    gather_backward_items_kernel<IdT, SPARSE><<<tgrid(total), 256, 0, (cudaStream_t)stream>>>(grad_out, ids, *table, h, w);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+template <typename IdT>
+static int gather_backward_sparse(const float *grad_out, const IdT *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
+                                  unsigned char *touched, cudaStream_t st)
+{
+    RB_CHECK_ARG(grad_out && ids && grad_nd && touched, "gather backward (sparse): null pointer");
+    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward (sparse): bad shape");
+    const long long total = (long long)B * h * w;
+    if (total == 0) return READ_OK;
+    gather_backward_sparse_kernel<IdT><<<tgrid(total), 256, D * sizeof(float), st>>>(grad_out, ids, B, D, h, w, N, grad_nd, touched);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -222,25 +237,35 @@ extern "C" {
 int read_gather_backward_sparse(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                                 float *grad_nd, unsigned char *touched, void *stream)
 {
-    RB_CHECK_ARG(grad_out && ids && grad_nd && touched, "gather backward (sparse): null pointer");
-    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward (sparse): bad shape");
-    const long long total = (long long)B * h * w;
-    if (total == 0) return READ_OK;
-    gather_backward_sparse_kernel<<<tgrid(total), 256, D * sizeof(float), (cudaStream_t)stream>>>(grad_out, ids, B, D, h, w, N, grad_nd,
-                                                                                                touched);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gather_backward_sparse<float>(grad_out, ids, B, D, h, w, N, grad_nd, touched, (cudaStream_t)stream);
+}
+
+int read_gather_backward_sparse_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
+                                    unsigned char *touched, void *stream)
+{
+    return gather_backward_sparse<int32_t>(grad_out, ids, B, D, h, w, N, grad_nd, touched, (cudaStream_t)stream);
 }
 
 int read_gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream)
 {
-    return gather_backward_items<false>(grad_out, ids, table, h, w, stream, "gather backward (items)");
+    return gather_backward_items<float, false>(grad_out, ids, table, h, w, stream, "gather backward (items)");
+}
+
+int read_gather_backward_items_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w, void *stream)
+{
+    return gather_backward_items<int32_t, false>(grad_out, ids, table, h, w, stream, "gather backward (items)");
 }
 
 int read_gather_backward_sparse_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w,
                                       void *stream)
 {
-    return gather_backward_items<true>(grad_out, ids, table, h, w, stream, "gather backward (sparse, items)");
+    return gather_backward_items<float, true>(grad_out, ids, table, h, w, stream, "gather backward (sparse, items)");
+}
+
+int read_gather_backward_sparse_items_i32(const float *grad_out, const int32_t *ids, const read_tex_table *table, int h, int w,
+                                          void *stream)
+{
+    return gather_backward_items<int32_t, true>(grad_out, ids, table, h, w, stream, "gather backward (sparse, items)");
 }
 
 int read_sparse_rmsprop_step(float *param_cn, float *shadow_nd, float *grad_nd, unsigned char *touched, float *square_avg,

@@ -22,14 +22,16 @@ class MyRender:
             self.update_ds(ds_list)
 
     def update_ds(self, ds_list):
+        clouds = {ds.id: np.asarray(ds.scene_data['pointcloud']['xyz']) for ds in ds_list}
+        # one index-map dtype for every render() of this renderer, from the largest cloud: float32 (the reference's pcpr format)
+        # while float32 holds every id, int32 above 2^24 + 1 points; ValueError at 2^31 points or more
+        self.index_dtype = ops.index_map_dtype(max(c.shape[0] for c in clouds.values()))
         L.require_device()
         self.ds_list = ds_list
         self.ds_ids = [d.id for d in ds_list]
         self.tgt_sh = self.ds_list[0].tgt_sh
         dev = torch.device("cuda", torch.cuda.current_device())
-        self.points = {
-            ds.id: torch.from_numpy(np.ascontiguousarray(np.asarray(ds.scene_data['pointcloud']['xyz']), dtype=np.float32)).to(dev)
-            for ds in ds_list}
+        self.points = {i: torch.from_numpy(np.ascontiguousarray(c, dtype=np.float32)).to(dev) for i, c in clouds.items()}
 
     def _pyramid(self, B, W, H, n_levels, dev):
         key = (B, W, H, n_levels, dev)
@@ -52,7 +54,7 @@ class MyRender:
         W, H = int(self.tgt_sh[0]), int(self.tgt_sh[1])
         sizes = ops.level_sizes(W, H, n_levels)
         dev = next(iter(self.points.values())).device
-        idx_levels = [torch.zeros((nb, h, w), dtype=torch.float32, device=dev) for (w, h) in sizes]
+        idx_levels = [torch.zeros((nb, h, w), dtype=self.index_dtype, device=dev) for (w, h) in sizes]
         dep_levels = [torch.zeros((nb, h, w), dtype=torch.float32, device=dev) for (w, h) in sizes]
         for ds_id in self.ds_ids:
             sel = torch.where(ids_t == ds_id)[0]
@@ -64,7 +66,7 @@ class MyRender:
             ops.raster_project(pyr, self.points[ds_id], m)
             sel_d = sel.to(dev)
             for l in range(n_levels):
-                i, d = ops.zbuf_resolve(pyr, l)
+                i, d = ops.zbuf_resolve(pyr, l, index_dtype=self.index_dtype)
                 idx_levels[l][sel_d] = i
                 dep_levels[l][sel_d] = d
         for l, k in enumerate(input_format):

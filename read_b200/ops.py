@@ -46,6 +46,37 @@ def _f32c(t, name):
     return t
 
 
+FLOAT_EXACT_POINTS = (1 << 24) + 1      # float32 holds every integer 0 .. 2^24: the ids of a cloud of up to 2^24 + 1 points
+
+
+def index_map_dtype(n_points):
+    """dtype of the index maps of a cloud of ``n_points`` points: float32, the reference's ``pcpr`` format, while float32 holds every
+    id 0 .. n_points - 1 exactly (n_points <= 2^24 + 1); int32 above, with the same values (the point id, 0 for an empty pixel).
+    Clouds of 2^31 points or more raise ValueError: their ids do not fit an int32 map."""
+    n = int(n_points)
+    if n >= 1 << 31:
+        raise ValueError(f"read_b200: a cloud of {n} points is too large; point ids must stay below 2^31")
+    return torch.int32 if n > FLOAT_EXACT_POINTS else torch.float32
+
+
+def _ids(t, name="ids"):
+    """Check an index map for the gather kernels: float32 or int32, contiguous, on the device.  Returns the suffix of the matching
+    entry points ('' for float32, '_i32' for int32)."""
+    if t.dtype not in (torch.float32, torch.int32):
+        raise RuntimeError(f"{name} must be a float32 or int32 index map, got {t.dtype}")
+    if not t.is_contiguous():
+        raise RuntimeError(f"{name} must be contiguous")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor")
+    return "_i32" if t.dtype == torch.int32 else ""
+
+
+def index_map(ids, device):
+    """An index map as the gather kernels take it: int32 maps stay int32, any other dtype becomes float32 (the reference's format),
+    contiguous on ``device``."""
+    return ids.to(device, torch.int32 if ids.dtype == torch.int32 else torch.float32).contiguous()
+
+
 def raster_project(pyr, xyz, total_m, id_base=0, derive=True):
     """Project xyz [n,3] (cuda f32) through total_m [B,4,4] (cuda f32) into an already-cleared pyramid."""
     L.require_device()
@@ -136,12 +167,16 @@ def raster_derive(pyr):
     L.check(L.load().read_raster_derive_levels(pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(), L.stream_ptr()))
 
 
-def zbuf_resolve(pyr, l, want_index=True, want_depth=True):
+def zbuf_resolve(pyr, l, want_index=True, want_depth=True, index_dtype=torch.float32):
+    """Level ``l`` as (index [B,h,w], depth [B,h,w] f32) maps; ``index_dtype`` float32 or int32 (``index_map_dtype``)."""
+    if index_dtype not in (torch.float32, torch.int32):
+        raise RuntimeError(f"read_b200: index maps are float32 or int32, not {index_dtype}")
     w, h = pyr.sizes[l]
     z = pyr.level(l)
-    idx = torch.empty((pyr.B, h, w), dtype=torch.float32, device=z.device) if want_index else None
+    idx = torch.empty((pyr.B, h, w), dtype=index_dtype, device=z.device) if want_index else None
     dep = torch.empty((pyr.B, h, w), dtype=torch.float32, device=z.device) if want_depth else None
-    L.check(L.load().read_zbuf_resolve(z.data_ptr(), pyr.B * w * h, L.ptr(idx), L.ptr(dep), L.stream_ptr()))
+    fn = L.load().read_zbuf_resolve_i32 if index_dtype == torch.int32 else L.load().read_zbuf_resolve
+    L.check(fn(z.data_ptr(), pyr.B * w * h, L.ptr(idx), L.ptr(dep), L.stream_ptr()))
     return idx, dep
 
 
@@ -191,13 +226,13 @@ def _feat_out(B, D, h, w, layout, device, out):
 
 
 def gather_from_index(tex_nd, ids, layout=L.FEAT_NCHW_F32, activation="none", out=None):
-    """ids [B,h,w] f32 cuda (contiguous) -> features."""
-    _f32c(ids, "ids")
+    """ids [B,h,w] f32 or int32 cuda (contiguous) -> features."""
+    sfx = _ids(ids)
     B, h, w = ids.shape
     N, D = tex_nd.shape
     out = _feat_out(B, D, h, w, layout, ids.device, out)
-    L.check(L.load().read_gather_from_index(tex_nd.data_ptr(), D, N, ids.data_ptr(), B, h, w, layout,
-                                            L.TEXACT[activation], out.data_ptr(), L.stream_ptr()))
+    L.check(getattr(L.load(), "read_gather_from_index" + sfx)(tex_nd.data_ptr(), D, N, ids.data_ptr(), B, h, w, layout,
+                                                            L.TEXACT[activation], out.data_ptr(), L.stream_ptr()))
     return out
 
 
@@ -229,8 +264,10 @@ def fused_resolve_supported(pyr, D=8):
 
 
 def gather_backward(grad_out, ids, N):
-    """grad_out [B,D,h,w] f32, ids [B,h,w] f32 -> grad [N,D] f32 (scatter-add).  Under torch.use_deterministic_algorithms(True) the
-    additions run in the fixed order of read_gather_backward_det, so the result is the same bits on every call."""
+    """grad_out [B,D,h,w] f32, ids [B,h,w] f32 or int32 -> grad [N,D] f32 (scatter-add).  Under
+    torch.use_deterministic_algorithms(True) the additions run in the fixed order of read_gather_backward_det, so the result is the
+    same bits on every call."""
+    sfx = _ids(ids)
     grad_out = grad_out.contiguous()
     _f32c(grad_out, "grad_out")
     B, D, h, w = grad_out.shape
@@ -238,11 +275,30 @@ def gather_backward(grad_out, ids, N):
     lib = L.load()
     if torch.are_deterministic_algorithms_enabled():
         ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, N), grad_out.device, "gather backward")
-        L.check(lib.read_gather_backward_det(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(), ws.data_ptr(),
-                                             L.stream_ptr()))
+        L.check(getattr(lib, "read_gather_backward_det" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(),
+                                                               ws.data_ptr(), L.stream_ptr()))
         return g
-    L.check(lib.read_gather_backward(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(), L.stream_ptr()))
+    L.check(getattr(lib, "read_gather_backward" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(),
+                                                       L.stream_ptr()))
     return g
+
+
+def gather_backward_sparse(grad_out, ids, N, grad_nd, touched):
+    """Sparse form of gather_backward: scatter-add into the persistent [N,D] accumulator ``grad_nd`` and set ``touched`` [N] u8
+    (read_gather_backward_sparse; under torch.use_deterministic_algorithms(True), read_gather_backward_sparse_det).
+    grad_out [B,D,h,w] f32 contiguous, ids [B,h,w] f32 or int32."""
+    _f32c(grad_out, "grad_out")
+    sfx = _ids(ids)
+    B, D, h, w = grad_out.shape
+    lib = L.load()
+    if torch.are_deterministic_algorithms_enabled():
+        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, N), grad_out.device, "sparse gather backward")
+        L.check(getattr(lib, "read_gather_backward_sparse_det" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N,
+                                                                      grad_nd.data_ptr(), touched.data_ptr(), ws.data_ptr(),
+                                                                      L.stream_ptr()))
+        return
+    L.check(getattr(lib, "read_gather_backward_sparse" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, grad_nd.data_ptr(),
+                                                              touched.data_ptr(), L.stream_ptr()))
 
 
 def tex_table(slots, N, tex=None, grad=None, touched=None):
@@ -265,8 +321,8 @@ def tex_table(slots, N, tex=None, grad=None, touched=None):
 
 def gather_from_index_items(tex_nds, slots, ids, layout=L.FEAT_NCHW_F32, activation="none", out=None):
     """gather_from_index for a batch whose item b samples ``tex_nds[slots[b]]`` ([N_s, 8] f32 point-major): one launch.
-    ids [B,h,w] f32 cuda (contiguous), B = len(slots)."""
-    _f32c(ids, "ids")
+    ids [B,h,w] f32 or int32 cuda (contiguous), B = len(slots)."""
+    sfx = _ids(ids)
     B, h, w = ids.shape
     if B != len(slots):
         raise RuntimeError("read_b200: one slot per item")
@@ -276,8 +332,8 @@ def gather_from_index_items(tex_nds, slots, ids, layout=L.FEAT_NCHW_F32, activat
             raise RuntimeError("read_b200: the multi-texture gather takes [N, 8] descriptors")
     out = _feat_out(B, 8, h, w, layout, ids.device, out)
     t = tex_table(slots, [nd.shape[0] for nd in tex_nds], tex=tex_nds)
-    L.check(L.load().read_gather_from_index_items(ctypes.byref(t), ids.data_ptr(), h, w, layout, L.TEXACT[activation],
-                                                  out.data_ptr(), L.stream_ptr()))
+    L.check(getattr(L.load(), "read_gather_from_index_items" + sfx)(ctypes.byref(t), ids.data_ptr(), h, w, layout,
+                                                                  L.TEXACT[activation], out.data_ptr(), L.stream_ptr()))
     return out
 
 
@@ -287,7 +343,7 @@ def gather_backward_items(grad_out, ids, slots, N, grads, touched=None):
     torch.use_deterministic_algorithms(True) the additions run in the fixed order of read_gather_backward_items_det."""
     grad_out = grad_out.contiguous()
     _f32c(grad_out, "grad_out")
-    _f32c(ids, "ids")
+    sfx = _ids(ids)
     B, D, h, w = grad_out.shape
     if D != 8 or tuple(ids.shape) != (B, h, w) or B != len(slots):
         raise RuntimeError("read_b200: multi-texture gather backward: shape mismatch")
@@ -296,10 +352,10 @@ def gather_backward_items(grad_out, ids, slots, N, grads, touched=None):
     if torch.are_deterministic_algorithms_enabled():
         ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, 8, h, w, sum(int(n) for n in N)), grad_out.device,
                            "multi-texture gather backward")
-        fn = lib.read_gather_backward_sparse_items_det if sparse else lib.read_gather_backward_items_det
+        fn = getattr(lib, ("read_gather_backward_sparse_items_det" if sparse else "read_gather_backward_items_det") + sfx)
         L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, ws.data_ptr(), L.stream_ptr()))
         return
-    fn = lib.read_gather_backward_sparse_items if sparse else lib.read_gather_backward_items
+    fn = getattr(lib, ("read_gather_backward_sparse_items" if sparse else "read_gather_backward_items") + sfx)
     L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, L.stream_ptr()))
 
 

@@ -9,6 +9,10 @@ contiguous (RuntimeError otherwise, pcpr_cuda.cpp:17-21,32-34), results are CPU 
 kernel picks its own persistent launch shape).  Output is deterministic: min depth, ties -> lowest id,
 empty -> 0 — the sequential semantics of DepthProject, which the reference kernel only approximates under
 contention (SURVEY.md §8 a3'').
+
+The index map is float32, the reference's native format, so it is exact only for clouds of up to 2^24 + 1 points: above that,
+ids beyond 2^24 are rounded to a neighbouring even id.  Larger clouds go through ``read_b200.myrender.MyRender``, whose maps are
+int32 for them (``ops.index_map_dtype``).
 """
 import torch
 

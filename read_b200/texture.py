@@ -1,7 +1,7 @@
 """Drop-in for ``READ.models.texture.PointTexture`` (READ/models/texture.py:14-70).
 
 Same constructor, same parameter (``texture_`` [1,C,N] f32, so checkpoints load unchanged), same forward
-contract (ids [B,1|3,h,w] float -> [B,C,h,w] f32).  The gather and its backward (scatter-add into
+contract (ids [B,1|3,h,w] float -> [B,C,h,w] f32; int32 maps, which clouds of more than 2^24 + 1 points get, pass unconverted).  The gather and its backward (scatter-add into
 ``texture_.grad``) are hand-written CUDA kernels reading a point-major [N,C] shadow of the parameter.
 """
 import torch
@@ -71,7 +71,7 @@ def sample_items(textures, slots, inputs):
     for t in textures:
         if not t.texture_.is_cuda:
             raise RuntimeError("read_b200.PointTexture: texture must be on a CUDA device (no CPU fallback)")
-    ids = ids.to(textures[0].texture_.device, torch.float32).contiguous()
+    ids = ops.index_map(ids, textures[0].texture_.device)
     act = textures[0].activation
     params = [t.texture_ for t in textures]
     if torch.is_grad_enabled() and any(p.requires_grad for p in params):
@@ -139,7 +139,7 @@ class PointTexture(Texture):
             ids = inputs[:, 0]                                   # BxHxW
         if not self.texture_.is_cuda:
             raise RuntimeError("read_b200.PointTexture: texture must be on a CUDA device (no CPU fallback)")
-        ids = ids.to(self.texture_.device, torch.float32).contiguous()
+        ids = ops.index_map(ids, self.texture_.device)
         if torch.is_grad_enabled() and self.texture_.requires_grad:
             if getattr(self, '_sparse_requested', False):
                 # training with read_b200.train.SparseRMSprop: the backward scatter-adds into a persistent point-major accumulator

@@ -39,15 +39,7 @@ class _GatherSparse(torch.autograd.Function):
         g = grad_out.contiguous()
         if g.dtype != torch.float32:
             g = g.float()
-        B, D, h, w = g.shape
-        lib = L.load()
-        if torch.are_deterministic_algorithms_enabled():
-            ws = ops.det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, st.N), g.device, "sparse gather backward")
-            L.check(lib.read_gather_backward_sparse_det(g.data_ptr(), ids.data_ptr(), B, D, h, w, st.N, st.grad.data_ptr(),
-                                                        st.touched.data_ptr(), ws.data_ptr(), L.stream_ptr()))
-            return None, None, None
-        L.check(lib.read_gather_backward_sparse(g.data_ptr(), ids.data_ptr(), B, D, h, w, st.N, st.grad.data_ptr(),
-                                                st.touched.data_ptr(), L.stream_ptr()))
+        ops.gather_backward_sparse(g, ids, st.N, st.grad, st.touched)
         return None, None, None
 
 
