@@ -345,7 +345,19 @@ int read_halo_exchange(const read_halo_desc *d, void *stream);
  *                                 cleared.  step counts optimizer steps from 1.
  *   read_square_avg_dense       : the dense optimizer's square_avg [1,D,N] after `step` steps (state_dict export)
  *   read_compact_touched        : touched rows -> (id, grad[D]) pairs; *count (zeroed by the caller) receives their number
- *   read_scatter_pairs          : grad_nd[id,:] += grads[k,:], touched[id] = 1 (pairs received from other ranks) */
+ *   read_scatter_pairs          : grad_nd[id,:] += grads[k,:], touched[id] = 1 (pairs received from other ranks)
+ * The L2 regulariser of PointTexture (reg_weight * mean(param^2), READ/models/texture.py:40-41) without a dense gradient: its
+ * gradient is k * param with one scalar k per texture, so the step takes k instead of a [1,D,N] gradient.  D in 1..16, N >= 1.
+ *   read_reg_loss_workspace_bytes : size of the workspace of read_reg_loss (-1 for a bad shape)
+ *   read_reg_loss               : *out (device f32 scalar) = reg_weight * sum(param_cn^2) / (D * N) over param_cn [1,D,N] f32.
+ *                                 fp32 partials of 4 words accumulated in fp64 per thread, then a fixed-order fp64 combine (the
+ *                                 grid depends only on the device): repeated calls give the same bits.  param_cn and workspace
+ *                                 16-byte aligned; the workspace (caller-owned) must not be shared by concurrent calls.
+ *   read_sparse_rmsprop_step_reg: read_sparse_rmsprop_step with the regulariser's gradient added for EVERY point: g = (touched[i] ?
+ *                                 grad_nd[i,c] : 0) + fl(k * param[c,i]) (two roundings), k = *reg_coef (device f32, e.g. 2 *
+ *                                 the upstream gradient * reg_weight / numel), then weight decay, the lazy decay by alpha^(step -
+ *                                 last_step[i]) and the update, written to param_cn and shadow_nd; touched rows and flags are
+ *                                 cleared and last_step[i] = step for all points. */
 int read_gather_backward_sparse(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                                 float *grad_nd, unsigned char *touched, void *stream);
 int read_gather_backward_sparse_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
@@ -359,6 +371,11 @@ int read_compact_touched(const float *grad_nd, const unsigned char *touched, int
                          int32_t *out_ids, float *out_grads, void *stream);
 int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int64_t N, float *grad_nd, unsigned char *touched,
                        void *stream);
+int64_t read_reg_loss_workspace_bytes(int D, int64_t N);
+int read_reg_loss(const float *param_cn, int D, int64_t N, double reg_weight, float *out, void *workspace, void *stream);
+int read_sparse_rmsprop_step_reg(float *param_cn, float *shadow_nd, float *grad_nd, unsigned char *touched, float *square_avg,
+                                 int32_t *last_step, int64_t N, int D, int step, float lr, float alpha, float eps, float weight_decay,
+                                 const float *reg_coef, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Backward of the gated convs, bf16 training with eval-mode BatchNorm (read_b200/blocks.py): the 3x3 stride-1 convs (the residual

@@ -80,6 +80,11 @@ _SIGS = {
     "read_square_avg_dense": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, ctypes.c_float, c_vp, c_vp]),
     "read_compact_touched": (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_vp]),
     "read_scatter_pairs": (c_int, [c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
+    # the L2 regulariser of PointTexture without a dense gradient (read_b200.train._RegLoss)
+    "read_reg_loss_workspace_bytes": (c_i64, [c_int, c_i64]),
+    "read_reg_loss": (c_int, [c_vp, c_int, c_i64, ctypes.c_double, c_vp, c_vp, c_vp]),
+    "read_sparse_rmsprop_step_reg": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, ctypes.c_float, ctypes.c_float,
+                                             ctypes.c_float, ctypes.c_float, c_vp, c_vp]),
     "read_ipc_alloc": (c_int, [c_i64, ctypes.POINTER(c_vp), ctypes.c_char_p]),
     "read_ipc_open": (c_int, [ctypes.c_char_p, ctypes.POINTER(c_vp)]),
     "read_ipc_close": (c_int, [c_vp]),

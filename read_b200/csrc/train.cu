@@ -91,31 +91,102 @@ __global__ void gather_backward_items_kernel(const float *__restrict__ go, const
     }
 }
 
+// L2 regulariser of PointTexture (reg_weight * mean(texture^2)): *out = w * sum(param^2) / numel over the whole [1,D,N] parameter.
+// Each thread squares and adds 4 consecutive words in fp32 (one float4) and accumulates those partials in fp64; the CTA's threads
+// are combined by a fixed tree in shared memory, the CTAs' sums by the last CTA to finish (counter + fence, as bn_stats_kernel), in
+// CTA order.  The grid depends on the device alone, so two calls on the same parameter give the same bits.
+constexpr int RL_THREADS = 256;
+constexpr int RL_MAX_CTAS = 4096;
+
+__device__ __forceinline__ double rl_block_sum(double v, double *red)
+{
+    red[threadIdx.x] = v;
+    __syncthreads();
+#pragma unroll
+    for (int s = RL_THREADS / 2; s > 0; s >>= 1) {
+        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        __syncthreads();
+    }
+    return red[0];
+}
+
+__global__ void __launch_bounds__(RL_THREADS)
+reg_loss_kernel(const float *__restrict__ param, long long numel, double w, float *__restrict__ out, double *__restrict__ part,
+                unsigned int *__restrict__ counter)
+{
+    __shared__ double red[RL_THREADS];
+    __shared__ bool last;
+    const long long n4 = numel >> 2, stride = (long long)gridDim.x * RL_THREADS;
+    const long long tid = blockIdx.x * (long long)RL_THREADS + threadIdx.x;
+    const float4 *p4 = reinterpret_cast<const float4 *>(param);
+    double acc = 0.0;
+#pragma unroll 4
+    for (long long v = tid; v < n4; v += stride) {
+        const float4 a = __ldcs(p4 + v);
+        acc += (double)fmaf(a.w, a.w, fmaf(a.z, a.z, fmaf(a.y, a.y, a.x * a.x)));
+    }
+    if (tid < (numel & 3)) {                                     // the last numel % 4 words: threads 0.. of CTA 0
+        const float x = param[n4 * 4 + tid];
+        acc += (double)(x * x);
+    }
+    const double cta = rl_block_sum(acc, red);
+    if (threadIdx.x == 0) part[blockIdx.x] = cta;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(counter, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    double s = 0.0;
+    for (unsigned b = threadIdx.x; b < gridDim.x; b += RL_THREADS) s += __ldcg(part + b);
+    const double total = rl_block_sum(s, red);
+    if (threadIdx.x == 0) {
+        *out = (float)(w * total / (double)numel);
+        *counter = 0u;
+    }
+}
+
 // one thread per point; D <= 16.  D == 8 (the reference's descriptor size) takes a fully unrolled path: the point's 2 + 2 + 8 loads
 // (gradient row, square_avg row, 8 channel-major parameter words) are all in flight before the first use - the generic loop below
 // made 16 dependent DRAM round trips per touched point and ran slower than the DENSE torch optimizer.
+// REG: the step of a texture whose L2 regulariser was back-propagated (read_sparse_rmsprop_step_reg).  Its gradient k * param
+// reaches every point, so every point is updated with g = (touched ? acc : 0) + fl(k * param), k read from *reg_coef; the decay
+// of the points that were not updated since last_step still applies lazily.
+template <bool REG>
 __global__ void sparse_rmsprop_kernel(float *__restrict__ param_cn, float *__restrict__ shadow_nd, float *__restrict__ grad_nd,
                                       unsigned char *__restrict__ touched, float *__restrict__ square_avg, int *__restrict__ last_step,
-                                      long long N, int D, int step, float lr, float alpha, float eps, float weight_decay)
+                                      long long N, int D, int step, float lr, float alpha, float eps, float weight_decay,
+                                      const float *__restrict__ reg_coef)
 {
+    const float k = REG ? *reg_coef : 0.f;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < N; i += (long long)gridDim.x * blockDim.x) {
-        if (!touched[i]) continue;
-        touched[i] = 0;
+        bool t = true;
+        if constexpr (REG) {
+            t = touched[i] != 0;
+            if (t) touched[i] = 0;
+        } else {
+            if (!touched[i]) continue;
+            touched[i] = 0;
+        }
         const int dt = step - last_step[i];
         last_step[i] = step;
         const float decay = dt == 1 ? alpha : powf(alpha, (float)dt);
         if (D == 8) {
             float4 *gp = reinterpret_cast<float4 *>(grad_nd + i * 8), *qp = reinterpret_cast<float4 *>(square_avg + i * 8);
-            const float4 g0 = gp[0], g1 = gp[1], q0 = qp[0], q1 = qp[1];
+            const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4 g0 = t ? gp[0] : zero, g1 = t ? gp[1] : zero, q0 = qp[0], q1 = qp[1];
             float p[8];
 #pragma unroll
             for (int c = 0; c < 8; ++c) p[c] = param_cn[(long long)c * N + i];
-            gp[0] = make_float4(0.f, 0.f, 0.f, 0.f);
-            gp[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (t) {
+                gp[0] = make_float4(0.f, 0.f, 0.f, 0.f);
+                gp[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
             float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
             float q[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
+                if (REG) g[c] = __fadd_rn(g[c], __fmul_rn(k, p[c]));          // two roundings, as autograd's sum of the two terms
                 if (weight_decay != 0.f) g[c] = fmaf(weight_decay, p[c], g[c]);
                 q[c] = fmaf(decay, q[c], (1.f - alpha) * g[c] * g[c]);
                 p[c] -= lr * g[c] / (sqrtf(q[c]) + eps);
@@ -131,9 +202,10 @@ __global__ void sparse_rmsprop_kernel(float *__restrict__ param_cn, float *__res
             continue;
         }
         for (int c = 0; c < D; ++c) {
-            float g = grad_nd[i * D + c];
-            grad_nd[i * D + c] = 0.f;
+            float g = t ? grad_nd[i * D + c] : 0.f;
+            if (t) grad_nd[i * D + c] = 0.f;
             float p = param_cn[(long long)c * N + i];
+            if (REG) g = __fadd_rn(g, __fmul_rn(k, p));
             if (weight_decay != 0.f) g = fmaf(weight_decay, p, g);
             // torch.optim.RMSprop (momentum 0, not centered): sq = alpha sq + (1 - alpha) g^2; p -= lr g / (sqrt(sq) + eps)
             const float sq = fmaf(decay, square_avg[i * D + c], (1.f - alpha) * g * g);
@@ -274,8 +346,46 @@ int read_sparse_rmsprop_step(float *param_cn, float *shadow_nd, float *grad_nd, 
 {
     RB_CHECK_ARG(param_cn && grad_nd && touched && square_avg && last_step, "sparse rmsprop: null pointer");
     RB_CHECK_ARG(N >= 1 && D >= 1 && D <= 16 && step >= 1, "sparse rmsprop: bad shape / step");
-    sparse_rmsprop_kernel<<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg, last_step, N, D,
-                                                                      step, lr, alpha, eps, weight_decay);
+    sparse_rmsprop_kernel<false><<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg, last_step,
+                                                                             N, D, step, lr, alpha, eps, weight_decay, nullptr);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int read_sparse_rmsprop_step_reg(float *param_cn, float *shadow_nd, float *grad_nd, unsigned char *touched, float *square_avg,
+                                 int32_t *last_step, int64_t N, int D, int step, float lr, float alpha, float eps, float weight_decay,
+                                 const float *reg_coef, void *stream)
+{
+    RB_CHECK_ARG(param_cn && grad_nd && touched && square_avg && last_step && reg_coef, "sparse rmsprop (reg): null pointer");
+    RB_CHECK_ARG(N >= 1 && D >= 1 && D <= 16 && step >= 1, "sparse rmsprop (reg): bad shape / step");
+    sparse_rmsprop_kernel<true><<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg, last_step,
+                                                                            N, D, step, lr, alpha, eps, weight_decay, reg_coef);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+int64_t read_reg_loss_workspace_bytes(int D, int64_t N)
+{
+    if (D < 1 || D > 16 || N < 1) return -1;
+    return 256 + (int64_t)RL_MAX_CTAS * (int64_t)sizeof(double);
+}
+
+int read_reg_loss(const float *param_cn, int D, int64_t N, double reg_weight, float *out, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(param_cn && out && workspace, "reg_loss: null pointer");
+    RB_CHECK_ARG(N >= 1 && D >= 1 && D <= 16, "reg_loss: bad shape (D %d, N %lld)", D, (long long)N);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(param_cn) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
+                 "reg_loss: param and workspace must be 16B aligned");
+    const long long numel = (long long)D * N;
+    long long blocks = ((numel >> 2) + RL_THREADS - 1) / RL_THREADS;
+    const long long cap = 8ll * num_sms() < RL_MAX_CTAS ? 8ll * num_sms() : RL_MAX_CTAS;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned int *counter = (unsigned int *)workspace;
+    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), st));
+    reg_loss_kernel<<<(unsigned)blocks, RL_THREADS, 0, st>>>(param_cn, numel, reg_weight, out, (double *)((char *)workspace + 256),
+                                                            counter);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

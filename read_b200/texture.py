@@ -114,10 +114,20 @@ class PointTexture(Texture):
 
     def null_grad(self):
         self.texture_.grad = None
+        sp = getattr(self, '_sparse', None)
+        if sp is not None:                             # the pending regulariser's gradient goes with it, as texture_.grad does
+            sp.reg_coef = None
 
     def reg_loss(self):
-        """L2 regulariser of texture.py:40-41: reg_weight * mean(texture^2)."""
-        return self.reg_weight * self.texture_.square().mean()
+        """L2 regulariser of texture.py:40-41: reg_weight * mean(texture^2).  A CUDA texture in sparse mode (SparseRMSprop) that
+        needs a gradient takes train._RegLoss: the value from our reduction kernel, and a backward that leaves the gradient as one
+        scalar for the optimizer step instead of a dense texture_.grad.  Otherwise (reg_weight 0 included) the torch expression."""
+        t = self.texture_
+        if (self.reg_weight != 0 and getattr(self, '_sparse_requested', False) and t.is_cuda and torch.is_grad_enabled()
+                and t.requires_grad):
+            from . import train
+            return train._RegLoss.apply(t, self)
+        return self.reg_weight * t.square().mean()
 
     def point_major(self):
         """[N,C] shadow of ``texture_`` on its device, refreshed whenever the parameter changes."""

@@ -8,7 +8,8 @@ per pyramid level, READ/models/texture.py:55-63) and a dense ``torch.optim.RMSpr
   accumulator and flags the touched points (``texture_.grad`` stays ``None``: nothing dense is ever materialised);
 * ``SparseRMSprop`` is a drop-in for the reference's descriptor optimizer (same hyper-parameters, ``param_groups`` whose ``lr`` the
   pipeline rescales, ``step() / zero_grad() / state_dict()``): it updates only touched points, with the skipped ``square_avg``
-  decays applied lazily - the result equals the dense optimizer's;
+  decays applied lazily - the result equals the dense optimizer's.  ``PointTexture.reg_loss`` (``--reg_weight``) in sparse mode
+  back-propagates one scalar per texture (``_RegLoss``), and the step after it updates every point with that term added;
 * ``exchange_sparse_grads`` is the data-parallel join: ranks all-gather their touched ``(id, grad[D])`` rows (a few MB) instead
   of all-reducing ``[N, D]`` gradients or re-broadcasting the texture as ``nn.DataParallel`` does (train.py:138-139).
 
@@ -18,6 +19,7 @@ import ctypes
 import warnings
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib as L
 from . import ops
@@ -43,6 +45,33 @@ class _GatherSparse(torch.autograd.Function):
         return None, None, None
 
 
+class _RegLoss(torch.autograd.Function):
+    """``PointTexture.reg_loss`` (reg_weight * mean(texture_^2), READ/models/texture.py:40-41) in sparse mode.  Its gradient is
+    k * texture_ with k = 2 * u * reg_weight / numel for the upstream gradient u, so the backward records the scalar k in the
+    texture's sparse state (summed over calls) instead of a dense [1, D, N] gradient; SparseRMSprop.step applies it to every point.
+    k is computed with the device ops autograd runs for the torch expression (u * w, / numel, * 2), so k * texture_ has the bits of
+    the gradient autograd would give."""
+
+    @staticmethod
+    def forward(ctx, texture_, tex_module):
+        p = texture_.detach()
+        D, N = p.shape[1], p.shape[2]
+        ctx.tex, ctx.w, ctx.numel = tex_module, float(tex_module.reg_weight), D * N
+        lib = L.load()
+        ws = torch.empty(int(lib.read_reg_loss_workspace_bytes(D, N)), dtype=torch.uint8, device=p.device)
+        out = torch.empty((), dtype=torch.float32, device=p.device)
+        L.check(lib.read_reg_loss(p.data_ptr(), D, N, ctx.w, out.data_ptr(), ws.data_ptr(), L.stream_ptr()))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, u):
+        sp = enable_sparse_grad(ctx.tex)
+        k = u * ctx.w / ctx.numel * 2
+        sp.reg_coef = k if sp.reg_coef is None else sp.reg_coef + k
+        return None, None
+
+
 class SparseGradState:
     def __init__(self, texture):
         p = texture.texture_
@@ -51,6 +80,7 @@ class SparseGradState:
         self.D, self.N = p.shape[1], p.shape[2]
         self.grad = torch.zeros((self.N, self.D), dtype=torch.float32, device=p.device)       # point-major accumulator
         self.touched = torch.zeros((self.N,), dtype=torch.uint8, device=p.device)
+        self.reg_coef = None        # 0-d device f32: the pending regulariser's gradient coefficient k (_RegLoss), or None
 
 
 def enable_sparse_grad(texture):
@@ -80,7 +110,8 @@ def touched_count(texture):
 class SparseRMSprop:
     """RMSprop (torch defaults: alpha 0.99, eps 1e-8, no momentum, not centered) over PointTexture descriptors, touching only the
     points that received a gradient since the last step.  ``textures``: one PointTexture or a list (one param group each, like the
-    reference's multi-scene ``extra_optimizer``, ogl.py:136-144)."""
+    reference's multi-scene ``extra_optimizer``, ogl.py:136-144).  A texture whose regulariser was back-propagated since its last
+    step (a pending ``reg_coef``) gets the dense-term step instead: every point, with g = accumulated row + reg_coef * param."""
 
     def __init__(self, textures, lr=1e-2, alpha=0.99, eps=1e-8, weight_decay=0.0):
         if not isinstance(textures, (list, tuple)):
@@ -114,9 +145,14 @@ class SparseRMSprop:
         for t, g in zip(self.textures, self.param_groups):
             sp, st = enable_sparse_grad(t), self._state(t)
             shadow = t.point_major()                 # kept in sync by the kernel: no dense re-transposition after the step
-            L.check(lib.read_sparse_rmsprop_step(t.texture_.data_ptr(), shadow.data_ptr(), sp.grad.data_ptr(), sp.touched.data_ptr(),
-                                                 st["square_avg"].data_ptr(), st["last_step"].data_ptr(), sp.N, sp.D, self._steps,
-                                                 float(g["lr"]), float(g["alpha"]), float(g["eps"]), float(g["weight_decay"]), sp_))
+            args = (t.texture_.data_ptr(), shadow.data_ptr(), sp.grad.data_ptr(), sp.touched.data_ptr(), st["square_avg"].data_ptr(),
+                    st["last_step"].data_ptr(), sp.N, sp.D, self._steps, float(g["lr"]), float(g["alpha"]), float(g["eps"]),
+                    float(g["weight_decay"]))
+            if sp.reg_coef is None:
+                L.check(lib.read_sparse_rmsprop_step(*args, sp_))
+            else:                                    # the regulariser's gradient reaches every point: the dense-term step
+                coef, sp.reg_coef = sp.reg_coef, None
+                L.check(lib.read_sparse_rmsprop_step_reg(*args, coef.data_ptr(), sp_))
         return loss
 
     def dense_square_avg(self, t):
