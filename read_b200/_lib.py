@@ -176,19 +176,13 @@ _SIGS = {
     "read_nchw_f32_to_nhwc": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_nhwc_to_nchw_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_launch_count": (c_i64, []),
-    # int32 index maps (clouds of more than 2^24 + 1 points): the float entry points' twins
-    "read_zbuf_resolve_i32": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
-    "read_gather_from_index_i32": (c_int, [c_vp, c_int, c_i64, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
-    "read_gather_from_index_items_i32": (c_int, [ctypes.POINTER(ReadTexTable), c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
-    "read_gather_backward_i32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp]),
-    "read_gather_backward_sparse_i32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
-    "read_gather_backward_items_i32": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp]),
-    "read_gather_backward_sparse_items_i32": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp]),
-    "read_gather_backward_det_i32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
-    "read_gather_backward_sparse_det_i32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
-    "read_gather_backward_items_det_i32": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp, c_vp]),
-    "read_gather_backward_sparse_items_det_i32": (c_int, [c_vp, c_vp, ctypes.POINTER(ReadTexTable), c_int, c_int, c_vp, c_vp]),
 }
+# int32 index maps (clouds of more than 2^24 + 1 points): each float entry point's twin is bound like it (the map is a pointer)
+for _name in ("read_zbuf_resolve", "read_gather_from_index", "read_gather_from_index_items", "read_gather_backward",
+              "read_gather_backward_sparse", "read_gather_backward_items", "read_gather_backward_sparse_items",
+              "read_gather_backward_det", "read_gather_backward_sparse_det", "read_gather_backward_items_det",
+              "read_gather_backward_sparse_items_det"):
+    _SIGS[_name + "_i32"] = _SIGS[_name]
 
 EXPORTS = tuple(sorted(_SIGS))
 _lib = None

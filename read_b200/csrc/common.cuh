@@ -15,6 +15,12 @@ void set_error(const char *fmt, ...);
 extern std::atomic<long long> g_launches;
 inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int num_sms();
+// grid of a grid-stride kernel over n items in blocks of 256 threads: one item per thread, at most 16 blocks per SM
+inline unsigned grid_for(long long n)
+{
+    const long long blocks = (n + 255) / 256, cap = 16ll * num_sms();
+    return (unsigned)(blocks < 1 ? 1 : blocks > cap ? cap : blocks);
+}
 // channel counts of the train-mode BatchNorm entry points (bn_train.cu, conv_bwd.cu): the gate backward's, without 48
 inline bool bn_channels_ok(int C) { return C == 16 || C == 32 || C == 64 || (C % 64 == 0 && C > 0 && C <= 256); }
 

@@ -1,5 +1,5 @@
-// Descriptor gather / scatter-add for sm_90a.
-// Replaces PointTexture.forward and its autograd backward (READ/models/texture.py:42-70):
+// Descriptor gather for sm_90a.
+// Replaces PointTexture.forward (READ/models/texture.py:42-70; its autograd backward, the scatter-add, is in train.cu):
 //   feat[b,c,y,x] = texture_[0,c,(int64)idx[b,0,y,x]]      (empty pixel carries idx 0 -> point 0)
 // Descriptors are read from a point-major [N,D] shadow so a pixel touches one 32-byte sector.
 // gather_items_kernel: the same for a batch whose items sample different textures (a texture table in the kernel parameters).
@@ -132,35 +132,6 @@ __global__ void gather_items_kernel(const __grid_constant__ read_tex_table t, co
             *reinterpret_cast<uint4 *>(static_cast<__nv_bfloat16 *>(out) + p * 8) = *reinterpret_cast<uint4 *>(r);
         }
     }
-}
-
-// grad_tex[id,:] += grad_out[b,:,q].  Empty pixels (id 0) are pre-reduced per block in shared memory:
-// in a sparse view millions of pixels would otherwise serialise on point 0's 8 addresses.  IdT: float or int32_t index map.
-template <typename IdT>
-__global__ void gather_backward_kernel(const float *__restrict__ go, const IdT *__restrict__ ids, int B, int D, int h,
-                                       int w, long long N, float *__restrict__ gt)
-{
-    extern __shared__ float zero_acc[];   // [D]
-    for (int c = threadIdx.x; c < D; c += blockDim.x) zero_acc[c] = 0.f;
-    __syncthreads();
-    const long long hw = (long long)h * w;
-    const long long total = (long long)B * hw;
-    for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total;
-         p += (long long)gridDim.x * blockDim.x) {
-        long long id = (long long)ids[p];
-        if (id < 0) id = 0;
-        if (id >= N) id = N - 1;
-        const long long b = p / hw, q = p - b * hw;
-        const float *g = go + b * D * hw + q;
-        if (id == 0) {
-            for (int c = 0; c < D; ++c) atomicAdd(&zero_acc[c], g[c * hw]);
-        } else {
-            for (int c = 0; c < D; ++c) atomicAdd(gt + id * D + c, g[c * hw]);
-        }
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < D; c += blockDim.x)
-        if (zero_acc[c] != 0.f) atomicAdd(gt + c, zero_acc[c]);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -369,15 +340,6 @@ __global__ void __launch_bounds__(256) pyramid_resolve_gather_r1_kernel(const __
     }
 }
 
-static unsigned grid_for(long long total, int threads = 256)
-{
-    long long blocks = (total + threads - 1) / threads;
-    const long long cap = (long long)num_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    return (unsigned)blocks;
-}
-
 template <int SRC>
 static int launch_gather(const float *tex, int D, long long N, const void *src, int B, int h, int w, int layout,
                          int act, void *out, cudaStream_t st)
@@ -462,19 +424,6 @@ static int gather_items(const read_tex_table *table, const IdT *ids, int h, int 
         set_error("gather (items): unknown layout %d", layout);
         return READ_ERR_INVALID;
     }
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-template <typename IdT>
-static int gather_backward(const float *grad_out, const IdT *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
-                           cudaStream_t st)
-{
-    RB_CHECK_ARG(grad_out && ids && grad_tex_nd, "gather backward: null pointer");
-    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward: bad shape");
-    const long long total = (long long)B * h * w;
-    if (total == 0) return READ_OK;
-    gather_backward_kernel<IdT><<<grid_for(total), 256, D * sizeof(float), st>>>(grad_out, ids, B, D, h, w, N, grad_tex_nd);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -579,18 +528,6 @@ int read_pyramid_resolve_gather(const float *tex_nd, int D, int64_t N, uint64_t 
 #undef RB_PRG
     RB_LAUNCH_CHECK();
     return READ_OK;
-}
-
-int read_gather_backward(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
-                         float *grad_tex_nd, void *stream)
-{
-    return gather_backward<float>(grad_out, ids, B, D, h, w, N, grad_tex_nd, (cudaStream_t)stream);
-}
-
-int read_gather_backward_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
-                             void *stream)
-{
-    return gather_backward<int32_t>(grad_out, ids, B, D, h, w, N, grad_tex_nd, (cudaStream_t)stream);
 }
 
 int read_stage_net_inputs(const float *src, int B, int hs, int ws, int C, int factor, float *last, int have_last, int act_dtype,

@@ -2,7 +2,8 @@
 // through a dense [D, B*N] index_add_ per pyramid level (READ/models/texture.py:55-63 under autograd) and steps a dense
 // torch.optim.RMSprop over all N points (READ/pipelines/ogl.py:16,97-102) - 160-320 MB of gradient and 3 x 320 MB of optimizer
 // traffic per step for a few 10^4 visible points.  Here everything past the net's input gradient touches only visible points:
-//   gather_backward_sparse   grad[id,:] += dL/dfeat[:, pixel]  (point-major accumulator) and touched[id] = 1
+//   gather_backward          grad[id,:] += dL/dfeat[:, pixel]  (point-major accumulator) and, in the sparse form, touched[id] = 1;
+//                            the dense form is the backward of the gather (PointTexture's autograd)
 //   gather_backward_items    the same (sparse or dense) for a batch whose items sample different textures: each item's pixels go
 //                            to its own texture's accumulator (a batch that mixes scenes in one net call)
 //   sparse_rmsprop           for touched points only: lazily decayed square_avg, parameter update written to BOTH the
@@ -17,11 +18,15 @@
 namespace rb {
 
 // IdT: float or int32_t index map (every kernel of this file that reads ids)
-template <typename IdT>
-__global__ void gather_backward_sparse_kernel(const float *__restrict__ go, const IdT *__restrict__ ids, int B, int D, int h,
-                                              int w, long long N, float *__restrict__ gt, unsigned char *__restrict__ touched)
+// gt[id,:] += grad_out[b,:,q] for every pixel; SPARSE (read_gather_backward_sparse) also sets touched[id].  Pixels that show point 0
+// (and every empty pixel) are pre-reduced per block in shared memory: in a sparse view millions of pixels would otherwise serialise
+// on point 0's D addresses.  The block's point-0 sum is flushed by the rule of its form: sparse when any pixel of the block hit id 0
+// (setting touched[0]), dense per channel when the sum is non-zero (so a row that holds -0.0 keeps it when no pixel adds to it).
+template <typename IdT, bool SPARSE>
+__global__ void gather_backward_kernel(const float *__restrict__ go, const IdT *__restrict__ ids, int B, int D, int h, int w,
+                                       long long N, float *__restrict__ gt, unsigned char *__restrict__ touched)
 {
-    extern __shared__ float zero_acc[];   // [D]: pixels that show point 0 (and every empty pixel) are pre-reduced per block
+    extern __shared__ float zero_acc[];   // [D]
     for (int c = threadIdx.x; c < D; c += blockDim.x) zero_acc[c] = 0.f;
     __syncthreads();
     const long long hw = (long long)h * w;
@@ -38,19 +43,21 @@ __global__ void gather_backward_sparse_kernel(const float *__restrict__ go, cons
             for (int c = 0; c < D; ++c) atomicAdd(&zero_acc[c], g[c * hw]);
         } else {
             for (int c = 0; c < D; ++c) atomicAdd(gt + id * D + c, g[c * hw]);
-            touched[id] = 1;
+            if (SPARSE) touched[id] = 1;
         }
     }
-    const int zero_any = __syncthreads_or(any_zero ? 1 : 0);
-    if (zero_any) {
-        for (int c = threadIdx.x; c < D; c += blockDim.x) atomicAdd(gt + c, zero_acc[c]);
-        if (threadIdx.x == 0) touched[0] = 1;
-    }
+    bool flush = true;
+    if (SPARSE) flush = __syncthreads_or(any_zero ? 1 : 0);
+    else __syncthreads();
+    if (!flush) return;
+    for (int c = threadIdx.x; c < D; c += blockDim.x)
+        if (SPARSE || zero_acc[c] != 0.f) atomicAdd(gt + c, zero_acc[c]);
+    if (SPARSE && threadIdx.x == 0) touched[0] = 1;
 }
 
-// gather_backward_kernel (SPARSE = false) / gather_backward_sparse_kernel (true) at D == 8 for a batch whose items sample different
-// textures: item b's pixels go to slot t.slot[b]'s accumulator.  Point 0 is pre-reduced per block AND per slot (a shared [slot][8]
-// accumulator): with one shared row, every empty pixel of one slot's sparse crop would serialise on another's point 0.
+// gather_backward_kernel at D == 8 for a batch whose items sample different textures: item b's pixels go to slot t.slot[b]'s
+// accumulator.  Point 0 is pre-reduced per block AND per slot (a shared [slot][8] accumulator): with one shared row, every empty
+// pixel of one slot's sparse crop would serialise on another's point 0.
 template <typename IdT, bool SPARSE>
 __global__ void gather_backward_items_kernel(const float *__restrict__ go, const IdT *__restrict__ ids,
                                              const __grid_constant__ read_tex_table t, int h, int w)
@@ -264,13 +271,19 @@ __global__ void scatter_pairs_kernel(const int *__restrict__ ids, const float *_
     }
 }
 
-static unsigned tgrid(long long total)
+template <typename IdT, bool SPARSE>
+static int gather_backward(const float *grad_out, const IdT *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
+                           unsigned char *touched, void *stream)
 {
-    long long blocks = (total + 255) / 256;
-    const long long cap = (long long)num_sms() * 16;
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    return (unsigned)blocks;
+    const char *what = SPARSE ? "gather backward (sparse)" : "gather backward";
+    RB_CHECK_ARG(grad_out && ids && grad_nd && (touched || !SPARSE), "%s: null pointer", what);
+    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "%s: bad shape", what);
+    const long long total = (long long)B * h * w;
+    if (total == 0) return READ_OK;
+    gather_backward_kernel<IdT, SPARSE><<<grid_for(total), 256, D * sizeof(float), (cudaStream_t)stream>>>(grad_out, ids, B, D, h, w,
+                                                                                                          N, grad_nd, touched);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 template <typename IdT, bool SPARSE>
@@ -282,20 +295,7 @@ static int gather_backward_items(const float *grad_out, const IdT *ids, const re
     RB_CHECK_ARG(grad_out && ids, "%s: null pointer", what);
     const long long total = (long long)table->n_items * h * w;
     if (total == 0) return READ_OK;
-    gather_backward_items_kernel<IdT, SPARSE><<<tgrid(total), 256, 0, (cudaStream_t)stream>>>(grad_out, ids, *table, h, w);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-template <typename IdT>
-static int gather_backward_sparse(const float *grad_out, const IdT *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
-                                  unsigned char *touched, cudaStream_t st)
-{
-    RB_CHECK_ARG(grad_out && ids && grad_nd && touched, "gather backward (sparse): null pointer");
-    RB_CHECK_ARG(D >= 1 && D <= 1024 && N >= 1 && B >= 0 && h >= 0 && w >= 0, "gather backward (sparse): bad shape");
-    const long long total = (long long)B * h * w;
-    if (total == 0) return READ_OK;
-    gather_backward_sparse_kernel<IdT><<<tgrid(total), 256, D * sizeof(float), st>>>(grad_out, ids, B, D, h, w, N, grad_nd, touched);
+    gather_backward_items_kernel<IdT, SPARSE><<<grid_for(total), 256, 0, (cudaStream_t)stream>>>(grad_out, ids, *table, h, w);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -306,16 +306,28 @@ using namespace rb;
 
 extern "C" {
 
+int read_gather_backward(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                         void *stream)
+{
+    return gather_backward<float, false>(grad_out, ids, B, D, h, w, N, grad_tex_nd, nullptr, stream);
+}
+
+int read_gather_backward_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_tex_nd,
+                             void *stream)
+{
+    return gather_backward<int32_t, false>(grad_out, ids, B, D, h, w, N, grad_tex_nd, nullptr, stream);
+}
+
 int read_gather_backward_sparse(const float *grad_out, const float *ids, int B, int D, int h, int w, int64_t N,
                                 float *grad_nd, unsigned char *touched, void *stream)
 {
-    return gather_backward_sparse<float>(grad_out, ids, B, D, h, w, N, grad_nd, touched, (cudaStream_t)stream);
+    return gather_backward<float, true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, stream);
 }
 
 int read_gather_backward_sparse_i32(const float *grad_out, const int32_t *ids, int B, int D, int h, int w, int64_t N, float *grad_nd,
                                     unsigned char *touched, void *stream)
 {
-    return gather_backward_sparse<int32_t>(grad_out, ids, B, D, h, w, N, grad_nd, touched, (cudaStream_t)stream);
+    return gather_backward<int32_t, true>(grad_out, ids, B, D, h, w, N, grad_nd, touched, stream);
 }
 
 int read_gather_backward_items(const float *grad_out, const float *ids, const read_tex_table *table, int h, int w, void *stream)
@@ -346,8 +358,8 @@ int read_sparse_rmsprop_step(float *param_cn, float *shadow_nd, float *grad_nd, 
 {
     RB_CHECK_ARG(param_cn && grad_nd && touched && square_avg && last_step, "sparse rmsprop: null pointer");
     RB_CHECK_ARG(N >= 1 && D >= 1 && D <= 16 && step >= 1, "sparse rmsprop: bad shape / step");
-    sparse_rmsprop_kernel<false><<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg, last_step,
-                                                                             N, D, step, lr, alpha, eps, weight_decay, nullptr);
+    sparse_rmsprop_kernel<false><<<grid_for(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg,
+                                                                                last_step, N, D, step, lr, alpha, eps, weight_decay, nullptr);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -358,8 +370,8 @@ int read_sparse_rmsprop_step_reg(float *param_cn, float *shadow_nd, float *grad_
 {
     RB_CHECK_ARG(param_cn && grad_nd && touched && square_avg && last_step && reg_coef, "sparse rmsprop (reg): null pointer");
     RB_CHECK_ARG(N >= 1 && D >= 1 && D <= 16 && step >= 1, "sparse rmsprop (reg): bad shape / step");
-    sparse_rmsprop_kernel<true><<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg, last_step,
-                                                                            N, D, step, lr, alpha, eps, weight_decay, reg_coef);
+    sparse_rmsprop_kernel<true><<<grid_for(N), 256, 0, (cudaStream_t)stream>>>(param_cn, shadow_nd, grad_nd, touched, square_avg,
+                                                                               last_step, N, D, step, lr, alpha, eps, weight_decay, reg_coef);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -394,7 +406,7 @@ int read_square_avg_dense(const float *square_avg, const int32_t *last_step, int
                           void *stream)
 {
     RB_CHECK_ARG(square_avg && last_step && out_cn && N >= 1 && D >= 1, "square_avg_dense: bad arguments");
-    square_avg_materialize_kernel<<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(square_avg, last_step, N, D, step, alpha, out_cn);
+    square_avg_materialize_kernel<<<grid_for(N), 256, 0, (cudaStream_t)stream>>>(square_avg, last_step, N, D, step, alpha, out_cn);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -403,7 +415,7 @@ int read_compact_touched(const float *grad_nd, const unsigned char *touched, int
                          int32_t *out_ids, float *out_grads, void *stream)
 {
     RB_CHECK_ARG(grad_nd && touched && count && out_ids && out_grads && N >= 1 && D >= 1 && capacity >= 0, "compact_touched: bad arguments");
-    compact_touched_kernel<<<tgrid(N), 256, 0, (cudaStream_t)stream>>>(grad_nd, touched, N, D, count, capacity, out_ids, out_grads);
+    compact_touched_kernel<<<grid_for(N), 256, 0, (cudaStream_t)stream>>>(grad_nd, touched, N, D, count, capacity, out_ids, out_grads);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -414,7 +426,7 @@ int read_scatter_pairs(const int32_t *ids, const float *grads, int n, int D, int
     RB_CHECK_ARG(n >= 0 && D >= 1 && N >= 1, "scatter_pairs: bad arguments");
     if (n == 0) return READ_OK;
     RB_CHECK_ARG(ids && grads && grad_nd && touched, "scatter_pairs: null pointer");
-    scatter_pairs_kernel<<<tgrid((long long)n * D), 256, 0, (cudaStream_t)stream>>>(ids, grads, n, D, N, grad_nd, touched);
+    scatter_pairs_kernel<<<grid_for((long long)n * D), 256, 0, (cudaStream_t)stream>>>(ids, grads, n, D, N, grad_nd, touched);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

@@ -263,42 +263,45 @@ def fused_resolve_supported(pyr, D=8):
     return pyr.L == 4 and D == 8 and pyr.direct_mask == 1 and pyr.W % 8 == 0 and pyr.H % 8 == 0
 
 
+def _gather_backward(grad_out, ids, N, grad=None, touched=None, slots=None):
+    """The descriptor-gradient scatter behind gather_backward, gather_backward_sparse and gather_backward_items: grad_out [B,D,h,w]
+    f32 is added into ``grad`` ([N,D] f32; None: a fresh zeroed one, returned) and, when ``touched`` is given (the sparse form),
+    touched[id] is set.  With ``slots``, item b's pixels go to slot slots[b] and N, grad and touched are per-slot lists (D = 8).
+    Under torch.use_deterministic_algorithms(True) the additions run in the fixed order of the *_det entry points."""
+    sfx = _ids(ids)
+    _f32c(grad_out, "grad_out")
+    B, D, h, w = grad_out.shape
+    if slots is None:
+        n_keys = N
+        if grad is None:
+            grad = torch.zeros((N, D), dtype=torch.float32, device=grad_out.device)
+        args = [B, D, h, w, N, grad.data_ptr()] + ([] if touched is None else [touched.data_ptr()])
+    else:
+        if D != 8 or tuple(ids.shape) != (B, h, w) or B != len(slots):
+            raise RuntimeError("read_b200: multi-texture gather backward: shape mismatch")
+        n_keys, table = sum(int(n) for n in N), tex_table(slots, N, grad=grad, touched=touched)
+        args = [ctypes.byref(table), h, w]
+    name = "read_gather_backward" + ("" if touched is None else "_sparse") + ("" if slots is None else "_items")
+    lib, ws = L.load(), None
+    if torch.are_deterministic_algorithms_enabled():
+        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, n_keys), grad_out.device, name)
+        name, args = name + "_det", args + [ws.data_ptr()]
+    L.check(getattr(lib, name + sfx)(grad_out.data_ptr(), ids.data_ptr(), *args, L.stream_ptr()))
+    return grad
+
+
 def gather_backward(grad_out, ids, N):
     """grad_out [B,D,h,w] f32, ids [B,h,w] f32 or int32 -> grad [N,D] f32 (scatter-add).  Under
     torch.use_deterministic_algorithms(True) the additions run in the fixed order of read_gather_backward_det, so the result is the
     same bits on every call."""
-    sfx = _ids(ids)
-    grad_out = grad_out.contiguous()
-    _f32c(grad_out, "grad_out")
-    B, D, h, w = grad_out.shape
-    g = torch.zeros((N, D), dtype=torch.float32, device=grad_out.device)
-    lib = L.load()
-    if torch.are_deterministic_algorithms_enabled():
-        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, N), grad_out.device, "gather backward")
-        L.check(getattr(lib, "read_gather_backward_det" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(),
-                                                               ws.data_ptr(), L.stream_ptr()))
-        return g
-    L.check(getattr(lib, "read_gather_backward" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, g.data_ptr(),
-                                                       L.stream_ptr()))
-    return g
+    return _gather_backward(grad_out.contiguous(), ids, N)
 
 
 def gather_backward_sparse(grad_out, ids, N, grad_nd, touched):
     """Sparse form of gather_backward: scatter-add into the persistent [N,D] accumulator ``grad_nd`` and set ``touched`` [N] u8
     (read_gather_backward_sparse; under torch.use_deterministic_algorithms(True), read_gather_backward_sparse_det).
     grad_out [B,D,h,w] f32 contiguous, ids [B,h,w] f32 or int32."""
-    _f32c(grad_out, "grad_out")
-    sfx = _ids(ids)
-    B, D, h, w = grad_out.shape
-    lib = L.load()
-    if torch.are_deterministic_algorithms_enabled():
-        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, D, h, w, N), grad_out.device, "sparse gather backward")
-        L.check(getattr(lib, "read_gather_backward_sparse_det" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N,
-                                                                      grad_nd.data_ptr(), touched.data_ptr(), ws.data_ptr(),
-                                                                      L.stream_ptr()))
-        return
-    L.check(getattr(lib, "read_gather_backward_sparse" + sfx)(grad_out.data_ptr(), ids.data_ptr(), B, D, h, w, N, grad_nd.data_ptr(),
-                                                              touched.data_ptr(), L.stream_ptr()))
+    _gather_backward(grad_out, ids, N, grad_nd, touched)
 
 
 def tex_table(slots, N, tex=None, grad=None, touched=None):
@@ -341,22 +344,7 @@ def gather_backward_items(grad_out, ids, slots, N, grads, touched=None):
     """Backward of gather_from_index_items: item b's pixels scatter-add into ``grads[slots[b]]`` ([N_s, 8] f32 accumulators; None: the
     slot receives nothing) and, when ``touched`` is given (the sparse form), set ``touched[slots[b]]``.  grad_out [B,8,h,w] f32.  Under
     torch.use_deterministic_algorithms(True) the additions run in the fixed order of read_gather_backward_items_det."""
-    grad_out = grad_out.contiguous()
-    _f32c(grad_out, "grad_out")
-    sfx = _ids(ids)
-    B, D, h, w = grad_out.shape
-    if D != 8 or tuple(ids.shape) != (B, h, w) or B != len(slots):
-        raise RuntimeError("read_b200: multi-texture gather backward: shape mismatch")
-    t = tex_table(slots, N, grad=grads, touched=touched)
-    lib, sparse = L.load(), touched is not None
-    if torch.are_deterministic_algorithms_enabled():
-        ws = det_workspace(lib.read_gather_backward_det_workspace_bytes(B, 8, h, w, sum(int(n) for n in N)), grad_out.device,
-                           "multi-texture gather backward")
-        fn = getattr(lib, ("read_gather_backward_sparse_items_det" if sparse else "read_gather_backward_items_det") + sfx)
-        L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, ws.data_ptr(), L.stream_ptr()))
-        return
-    fn = getattr(lib, ("read_gather_backward_sparse_items" if sparse else "read_gather_backward_items") + sfx)
-    L.check(fn(grad_out.data_ptr(), ids.data_ptr(), ctypes.byref(t), h, w, L.stream_ptr()))
+    _gather_backward(grad_out.contiguous(), ids, N, grads, touched, slots)
 
 
 def det_workspace(nbytes, device, what):
