@@ -95,6 +95,16 @@ int read_raster_project_sorted(const float *pts4, int64_t n, const float *total_
  * i.e. zbuf + b*W*H): the multi-GPU frame path, where every rank rasterises its spatial tile for all views of the step. */
 int read_raster_project_sorted_views(const float *pts4, int64_t n, const float *total_m, int B, int W, int H, int L,
                                      uint64_t *zbuf, void *stream);
+/* Segmented store (scene editing and stitching, read_b200.ops.SegmentedPoints): pts4 is [n,4] f32 = (x, y, z, bit pattern of
+ * the GLOBAL point id), n a multiple of 1024.  Segment i covers chunks [seg_first_chunk[i], + seg_chunks[i]) of 1024 rows
+ * (segments may share rows: instances), is drawn with its matrices seg_m[i] ([nseg, B, 16] f32 on the device) and is skipped
+ * entirely when seg_visible[i] is 0.  The table (host arrays) travels as kernel parameters.  Padding rows carry NaN
+ * coordinates and an id word other than 0xFFFFFFFF.  Like read_raster_project_sorted_views: B <= 8 views in ONE pass,
+ * level 0 of nested levels only. */
+#define READ_MAX_SEGMENTS 128
+int read_raster_project_segments(const float *pts4, int64_t n, const int64_t *seg_first_chunk, const int64_t *seg_chunks,
+                                 const uint8_t *seg_visible, int nseg, const float *seg_m, int B, int W, int H, int L,
+                                 uint64_t *zbuf, void *stream);
 /* Bitmask of levels rasterised with direct atomics (bit l set) for this geometry. */
 unsigned read_raster_direct_mask(int W, int H, int L);
 

@@ -45,6 +45,7 @@ class ReadConvDesc(ctypes.Structure):
 
 
 MAX_TEX_SLOTS, MAX_TEX_ITEMS = 16, 64
+MAX_SEGMENTS = 128           # READ_MAX_SEGMENTS: segments per read_raster_project_segments launch
 
 
 class ReadTexTable(ctypes.Structure):
@@ -74,6 +75,8 @@ _SIGS = {
     "read_raster_derive_levels": (c_int, [c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_raster_project_sorted": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_vp, c_vp]),
     "read_raster_project_sorted_views": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "read_raster_project_segments": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_vp,
+                                             c_vp]),
     "read_gather_backward_sparse": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
     "read_sparse_rmsprop_step": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, ctypes.c_float, ctypes.c_float,
                                          ctypes.c_float, ctypes.c_float, c_vp]),

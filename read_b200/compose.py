@@ -206,14 +206,19 @@ class NetAndTexture(nn.Module):
         ``want_maps``: also return the (index, depth) maps per level, index maps of ``ops.index_map_dtype(N)`` (float32 up to
         2^24 + 1 points, int32 above); ``return_input``: also return the net input
         (list of [B,8,h,w] f32, the reference's ``net_input``); ``clone_output=False`` hands out the engine's own output buffer
-        (valid until the next frame) for callers that consume it immediately."""
-        store = xyz if isinstance(xyz, ops.SortedPoints) else None
+        (valid until the next frame) for callers that consume it immediately.
+
+        An ``ops.SegmentedPoints`` store (read_b200.scene_edit) takes ``total_m`` as the per-segment matrices ``seg_m``
+        [nseg, B, 4, 4]; its index maps hold global ids, which index the composed texture."""
+        segmented = isinstance(xyz, ops.SegmentedPoints)
+        store = xyz if segmented or isinstance(xyz, ops.SortedPoints) else None
         pts = store.pts4 if store is not None else xyz
-        map_dtype = ops.index_map_dtype(store.n if store is not None else pts.shape[0])      # ValueError at 2^31 points or more
+        n_ids = store.n_ids if segmented else (store.n if store is not None else pts.shape[0])
+        map_dtype = ops.index_map_dtype(n_ids)                  # ValueError at 2^31 points or more
         L.require_device()
         lib = L.load()
         texture = self._texture(texture_id)
-        B = total_m.shape[0]
+        B = total_m.shape[1] if segmented else total_m.shape[0]
         ss = int(self.ss)
         Wr, Hr = W * ss, H * ss
         eng = self.net.engine(B, H, W, pts.device)
@@ -233,7 +238,10 @@ class NetAndTexture(nn.Module):
         if store is not None:
             if pyr.direct_mask != 1:
                 raise RuntimeError("a SortedPoints store renders frames with nested levels; pass the [N,3] cloud otherwise")
-            ops.raster_project_sorted(pyr, store, total_m)
+            if segmented:
+                ops.raster_project_segments(pyr, store, total_m)
+            else:
+                ops.raster_project_sorted(pyr, store, total_m)
             if not fused_ok:
                 ops.raster_derive(pyr)
         else:

@@ -163,6 +163,82 @@ def raster_project_sorted(pyr, store, total_m):
                                                      pyr.H, pyr.L, pyr.buf.data_ptr() + v0 * plane, sp))
 
 
+SEGMENT_CHUNK = 1024                     # rows per chunk of the segmented rasterizer; every segment is padded to whole chunks
+MAX_SEGMENTS = L.MAX_SEGMENTS
+
+
+class SegmentedPoints:
+    """Composed, device-resident point store for scene editing and stitching (read_b200.scene_edit).
+
+    Built from ``parts``: a list of ``(xyz [n,3] f32, ids [n] int64)``, each a group of points with their GLOBAL ids (the row of
+    their descriptors in the composed descriptor table).  Each part becomes one block of ``pts4`` rows: its points sorted on
+    their own as a ``SortedPoints`` store, with the global id in the id word, then padded to whole ``SEGMENT_CHUNK`` chunks with
+    rows (NaN, NaN, NaN, id 0) that the rasterizer culls, so that a chunk never spans two segments.  ``segments`` lists, per
+    segment, the part whose rows it draws (default: one segment per part); several segments over one part are instances.
+
+    Per segment: ``first_chunk`` / ``chunks`` (its row range in chunks), ``visible`` (host flag, set with ``set_visible``) and
+    ``ids`` (its part's global ids).  ``n`` is the row count including padding, ``n_ids`` the number of global ids (the index
+    maps' dtype follows ``index_map_dtype(n_ids)``)."""
+
+    def __init__(self, parts, segments=None, n_ids=None, cell=0.25):
+        segments = list(range(len(parts))) if segments is None else [int(s) for s in segments]
+        if len(segments) > MAX_SEGMENTS:
+            raise ValueError(f"read_b200: {len(segments)} segments; at most {MAX_SEGMENTS} per store")
+        if any(not 0 <= s < len(parts) for s in segments):
+            raise ValueError("read_b200: a segment refers to a part that does not exist")
+        blocks, part_rows, row = [], [], 0
+        self.part_ids = []
+        for xyz, ids in parts:
+            ids = torch.as_tensor(ids, dtype=torch.int64, device=xyz.device).reshape(-1)
+            if ids.shape[0] != xyz.shape[0]:
+                raise ValueError("read_b200: one global id per point")
+            if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= 1 << 31):
+                raise ValueError("read_b200: global point ids must lie in [0, 2^31)")
+            sp = SortedPoints(xyz.contiguous(), cell)
+            rows = -(-sp.n // SEGMENT_CHUNK) * SEGMENT_CHUNK
+            blk = torch.empty((rows, 4), dtype=torch.float32, device=xyz.device)
+            blk[sp.n:, :3] = float("nan")
+            blk[sp.n:, 3] = 0.0                                            # id word 0 (0xFFFFFFFF would stall the ring)
+            if sp.n:
+                blk[:sp.n, :3] = sp.pts4[:, :3]
+                blk[:sp.n, 3] = ids[sp.perm].to(torch.int32).view(torch.float32)
+            blocks.append(blk)
+            part_rows.append((row, rows))
+            self.part_ids.append(ids)
+            row += rows
+        dev = parts[0][0].device if parts else torch.device("cpu")
+        self.pts4 = torch.cat(blocks) if blocks else torch.empty((0, 4), dtype=torch.float32, device=dev)
+        self.n = self.pts4.shape[0]
+        self.n_ids = int(n_ids) if n_ids is not None else sum(int(i.numel()) for i in self.part_ids)
+        self.segment_part = segments
+        self.nseg = len(segments)
+        self.first_chunk = (ctypes.c_int64 * max(self.nseg, 1))(*[part_rows[p][0] // SEGMENT_CHUNK for p in segments])
+        self.chunks = (ctypes.c_int64 * max(self.nseg, 1))(*[part_rows[p][1] // SEGMENT_CHUNK for p in segments])
+        self.visible = (ctypes.c_uint8 * max(self.nseg, 1))(*([1] * self.nseg))
+
+    def ids(self, seg):
+        """Global ids of the points segment ``seg`` draws (in their part's order)."""
+        return self.part_ids[self.segment_part[seg]]
+
+    def set_visible(self, seg, visible):
+        self.visible[seg] = 1 if visible else 0
+
+
+def raster_project_segments(pyr, store, seg_m):
+    """Level 0 of a cleared pyramid from a SegmentedPoints store in one pass over its visible segments (finish with raster_derive
+    / pyramid_resolve_gather).  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, segment s drawn with seg_m[s], B <= 8."""
+    L.require_device()
+    _f32c(seg_m, "seg_m")
+    _f32c(store.pts4, "segmented store")
+    if seg_m.dim() != 4 or tuple(seg_m.shape[:2]) != (store.nseg, pyr.B) or tuple(seg_m.shape[2:]) != (4, 4):
+        raise RuntimeError(f"read_b200: seg_m must be [{store.nseg}, {pyr.B}, 4, 4], got {tuple(seg_m.shape)}")
+    if pyr.direct_mask != 1:
+        raise RuntimeError("the segmented rasterizer needs nested pyramid levels")
+    L.check(L.load().read_raster_project_segments(store.pts4.data_ptr(), store.n, store.first_chunk, store.chunks, store.visible,
+                                                  store.nseg, seg_m.data_ptr(), pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(),
+                                                  L.stream_ptr()))
+
+
 def raster_derive(pyr):
     L.check(L.load().read_raster_derive_levels(pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(), L.stream_ptr()))
 

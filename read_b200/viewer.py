@@ -98,3 +98,68 @@ class FrameRenderer:
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
                                              rgba.data_ptr(), L.stream_ptr()))
         return {'output': rgba, 'net_input': net_input}
+
+
+class SceneRenderer:
+    """``FrameRenderer`` for a composed scene (read_b200.scene_edit.SceneComposer): several scenes, moved / hidden / instanced
+    objects, all rendered in one rasterizer pass over the composer's segmented store.  ``infer`` keeps ``FrameRenderer.infer``'s
+    contract exactly.  Edits made on the composer between two ``infer`` calls show in the second frame; a layout change (a scene,
+    object or instance added) re-sorts the points once, a transform or visibility change moves no point data."""
+
+    def __init__(self, composer, net_state_dict, viewport_size, supersampling=1, temporal_average=False, flip_vertical=False,
+                 return_net_input=True, n_levels=4):
+        W, H = int(viewport_size[0]), int(viewport_size[1])
+        assert W % 16 == 0, f'set width {16 * (W // 16)}'
+        assert H % 16 == 0, f'set height {16 * (H // 16)}'
+        assert int(supersampling) >= 1, 'supersampling must be a positive integer'
+        self.device = composer.device
+        L.require_device(self.device.index)
+        ss = int(supersampling)
+        if L.load().read_raster_direct_mask(W * ss, H * ss, n_levels) != 1:
+            raise ValueError("read_b200: a composed scene renders frames whose pyramid levels nest (each exactly half of the last)")
+        self.composer = composer
+        self.W, self.H, self.n_levels = W, H, n_levels
+        self.flip_vertical = bool(flip_vertical)
+        self.return_net_input = bool(return_net_input)
+        net = UNet()
+        net.load_state_dict(net_state_dict, strict=True)
+        self._tex = composer.texture
+        self.model = NetAndTexture(net, {0: self._tex}, ss, temporal_average=bool(temporal_average))
+        self.model.load_textures(0)
+        self.model.to(self.device).eval()
+        # per-frame [nseg, 1, 4, 4] matrices through a ring of pinned staging buffers (see FrameRenderer._upload_camera)
+        self._m_host = [torch.empty((ops.MAX_SEGMENTS, 1, 4, 4), dtype=torch.float32).pin_memory() for _ in range(4)]
+        self._m_used = [None] * 4
+        self._m_i = 0
+
+    def _upload(self, seg_m):
+        i = self._m_i
+        self._m_i = (i + 1) % len(self._m_host)
+        if self._m_used[i] is not None:
+            self._m_used[i].synchronize()                # the copy that last read this staging buffer (4 frames ago) has run
+        host = self._m_host[i][:seg_m.shape[0]]
+        host.copy_(torch.from_numpy(seg_m))
+        m = host.to(self.device, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._m_used[i] = ev
+        return m
+
+    def infer(self, proj_matrix, view_matrix):
+        """-> {'output': [H,W,4] f32 cuda tensor, 'net_input': list of the four [1,8,h,w] f32 net inputs (None with
+        ``return_net_input=False``)}, as ``FrameRenderer.infer``; both fresh tensors."""
+        comp = self.composer
+        if comp.texture is not self._tex:                # a scene was added: the composed descriptor table grew
+            self._tex = comp.texture
+            self.model._textures[0] = self._tex
+            self.model.add_module('0', self._tex.to(self.device))
+        store = comp.store
+        seg_m = self._upload(comp.segment_matrices(FrameRenderer.total_matrix(proj_matrix, view_matrix)))
+        with torch.no_grad():
+            res = self.model.render(store, seg_m, self.W, self.H, n_levels=self.n_levels, return_input=self.return_net_input,
+                                    clone_output=False)
+        out, net_input = res if self.return_net_input else (res, None)
+        rgba = torch.empty((self.H, self.W, 4), dtype=torch.float32, device=self.device)
+        L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
+                                             rgba.data_ptr(), L.stream_ptr()))
+        return {'output': rgba, 'net_input': net_input}
