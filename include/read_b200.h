@@ -105,6 +105,26 @@ int read_raster_project_sorted_views(const float *pts4, int64_t n, const float *
 int read_raster_project_segments(const float *pts4, int64_t n, const int64_t *seg_first_chunk, const int64_t *seg_chunks,
                                  const uint8_t *seg_visible, int nseg, const float *seg_m, int B, int W, int H, int L,
                                  uint64_t *zbuf, void *stream);
+/* Segmented store with view-frustum culling of its chunks, up to READ_MAX_SEGMENTS_CULLED segments; the table lives on the
+ * device, so a frame needs no host-side table walk and no synchronisation.
+ *   seg_table   [nseg, 3] int32 on the device: (first chunk, chunk count, matrix slot) of segment s; matrices at
+ *               seg_m[slot] ([nseg, B, 16] f32).  A segment whose range lies outside the store's n / 1024 chunks, or whose
+ *               slot is not below nseg, draws nothing.
+ *   nunits      the number of (segment, chunk) units = the sum of the table's chunk counts (units past it are not drawn).
+ *   chunk_boxes [n / 1024, 6] f32: (min x, y, z, max x, y, z) of the non-NaN rows of each chunk; an all-padding chunk has
+ *               min > max (an empty box).
+ *   seg_visible [nseg] uint8 on the device (0 = hidden).
+ * One launch culls every unit whose segment is hidden or whose box lies outside the clip volume in all B views (DESIGN.md
+ * §4.1: the float64 test is conservative with respect to the per-point float32 test, so the frame is bit-identical to
+ * read_raster_project_segments), compacts the survivors in segment-then-chunk order into the workspace, and a persistent
+ * rasterizer draws them.  workspace: read_raster_cull_workspace_bytes(nunits) bytes of device memory, 16-byte aligned; its
+ * first 4 bytes hold the surviving-unit count (uint32) once the launch has run.  B <= 8, level 0 of nested levels only. */
+#define READ_MAX_SEGMENTS_CULLED 4096
+int64_t read_raster_cull_workspace_bytes(int64_t nunits);
+int read_raster_project_segments_culled(const float *pts4, int64_t n, const int32_t *seg_table, int nseg, int64_t nunits,
+                                        const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
+                                        void *workspace, int64_t workspace_bytes, int B, int W, int H, int L, uint64_t *zbuf,
+                                        void *stream);
 /* Bitmask of levels rasterised with direct atomics (bit l set) for this geometry. */
 unsigned read_raster_direct_mask(int W, int H, int L);
 

@@ -46,6 +46,7 @@ class ReadConvDesc(ctypes.Structure):
 
 MAX_TEX_SLOTS, MAX_TEX_ITEMS = 16, 64
 MAX_SEGMENTS = 128           # READ_MAX_SEGMENTS: segments per read_raster_project_segments launch
+MAX_SEGMENTS_CULLED = 4096   # READ_MAX_SEGMENTS_CULLED: segments per read_raster_project_segments_culled launch
 
 
 class ReadTexTable(ctypes.Structure):
@@ -77,6 +78,9 @@ _SIGS = {
     "read_raster_project_sorted_views": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_raster_project_segments": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_vp,
                                              c_vp]),
+    "read_raster_cull_workspace_bytes": (c_i64, [c_i64]),
+    "read_raster_project_segments_culled": (c_int, [c_vp, c_i64, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int,
+                                                    c_int, c_int, c_vp, c_vp]),
     "read_gather_backward_sparse": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_i64, c_vp, c_vp, c_vp]),
     "read_sparse_rmsprop_step": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, ctypes.c_float, ctypes.c_float,
                                          ctypes.c_float, ctypes.c_float, c_vp]),

@@ -196,7 +196,8 @@ class NetAndTexture(nn.Module):
         return st
 
     @torch.no_grad()
-    def render(self, xyz, total_m, W, H, texture_id=0, n_levels=4, want_maps=False, return_input=False, clone_output=True):
+    def render(self, xyz, total_m, W, H, texture_id=0, n_levels=4, want_maps=False, return_input=False, clone_output=True,
+               seg_visible=None):
         """points [N,3] (cuda f32) or an ``ops.SortedPoints`` store + total_m [B,4,4] (cuda f32) -> RGB [B,3,H,W] f32 (a fresh
         tensor), all on device, one pass over the cloud.  A sorted store serves frames whose levels nest; the result is
         bit-identical to rendering the unsorted cloud (the z-buffer is a min over (depth | original id) keys).
@@ -209,7 +210,9 @@ class NetAndTexture(nn.Module):
         (valid until the next frame) for callers that consume it immediately.
 
         An ``ops.SegmentedPoints`` store (read_b200.scene_edit) takes ``total_m`` as the per-segment matrices ``seg_m``
-        [nseg, B, 4, 4]; its index maps hold global ids, which index the composed texture."""
+        [nseg, B, 4, 4]; its index maps hold global ids, which index the composed texture.  It is drawn by the culled rasterizer
+        (``ops.raster_project_segments_culled``): only the chunks that are visible and may meet some view's frustum are read.
+        ``seg_visible``: its [nseg] uint8 visibility flags already on the device (default: the store's host flags)."""
         segmented = isinstance(xyz, ops.SegmentedPoints)
         store = xyz if segmented or isinstance(xyz, ops.SortedPoints) else None
         pts = store.pts4 if store is not None else xyz
@@ -239,7 +242,7 @@ class NetAndTexture(nn.Module):
             if pyr.direct_mask != 1:
                 raise RuntimeError("a SortedPoints store renders frames with nested levels; pass the [N,3] cloud otherwise")
             if segmented:
-                ops.raster_project_segments(pyr, store, total_m)
+                ops.raster_project_segments_culled(pyr, store, total_m, seg_visible)
             else:
                 ops.raster_project_sorted(pyr, store, total_m)
             if not fused_ok:

@@ -164,7 +164,7 @@ def raster_project_sorted(pyr, store, total_m):
 
 
 SEGMENT_CHUNK = 1024                     # rows per chunk of the segmented rasterizer; every segment is padded to whole chunks
-MAX_SEGMENTS = L.MAX_SEGMENTS
+MAX_SEGMENTS = L.MAX_SEGMENTS_CULLED     # per store; the table-in-parameters entry (raster_project_segments) takes 128
 
 
 class SegmentedPoints:
@@ -178,7 +178,13 @@ class SegmentedPoints:
 
     Per segment: ``first_chunk`` / ``chunks`` (its row range in chunks), ``visible`` (host flag, set with ``set_visible``) and
     ``ids`` (its part's global ids).  ``n`` is the row count including padding, ``n_ids`` the number of global ids (the index
-    maps' dtype follows ``index_map_dtype(n_ids)``)."""
+    maps' dtype follows ``index_map_dtype(n_ids)``).
+
+    For the culled rasterizer (``raster_project_segments_culled``), built once per layout on the store's device:
+    ``boxes`` [n / SEGMENT_CHUNK, 6] f32, the axis-aligned box (min x, y, z, max x, y, z) of the rows of each chunk that hold a
+    point (padding rows left out; a chunk of padding only gets the empty box +inf / -inf, which always culls); ``seg_table``
+    [nseg, 3] int32, (first chunk, chunk count, matrix slot = the segment's index) per segment; ``nunits`` the number of
+    (segment, chunk) units, the sum of the chunk counts."""
 
     def __init__(self, parts, segments=None, n_ids=None, cell=0.25):
         segments = list(range(len(parts))) if segments is None else [int(s) for s in segments]
@@ -186,7 +192,7 @@ class SegmentedPoints:
             raise ValueError(f"read_b200: {len(segments)} segments; at most {MAX_SEGMENTS} per store")
         if any(not 0 <= s < len(parts) for s in segments):
             raise ValueError("read_b200: a segment refers to a part that does not exist")
-        blocks, part_rows, row = [], [], 0
+        blocks, boxes, part_rows, row = [], [], [], 0
         self.part_ids = []
         for xyz, ids in parts:
             ids = torch.as_tensor(ids, dtype=torch.int64, device=xyz.device).reshape(-1)
@@ -203,6 +209,7 @@ class SegmentedPoints:
                 blk[:sp.n, :3] = sp.pts4[:, :3]
                 blk[:sp.n, 3] = ids[sp.perm].to(torch.int32).view(torch.float32)
             blocks.append(blk)
+            boxes.append(_chunk_boxes(blk))
             part_rows.append((row, rows))
             self.part_ids.append(ids)
             row += rows
@@ -215,6 +222,11 @@ class SegmentedPoints:
         self.first_chunk = (ctypes.c_int64 * max(self.nseg, 1))(*[part_rows[p][0] // SEGMENT_CHUNK for p in segments])
         self.chunks = (ctypes.c_int64 * max(self.nseg, 1))(*[part_rows[p][1] // SEGMENT_CHUNK for p in segments])
         self.visible = (ctypes.c_uint8 * max(self.nseg, 1))(*([1] * self.nseg))
+        self.boxes = torch.cat(boxes) if boxes else torch.empty((0, 6), dtype=torch.float32, device=dev)
+        self.seg_table = torch.tensor([[self.first_chunk[s], self.chunks[s], s] for s in range(self.nseg)],
+                                      dtype=torch.int32).reshape(-1, 3).to(dev)
+        self.nunits = sum(self.chunks[s] for s in range(self.nseg))
+        self._cull_ws = None                     # workspace of the culled rasterizer; its first word: the last surviving count
 
     def ids(self, seg):
         """Global ids of the points segment ``seg`` draws (in their part's order)."""
@@ -222,6 +234,17 @@ class SegmentedPoints:
 
     def set_visible(self, seg, visible):
         self.visible[seg] = 1 if visible else 0
+
+    def visible_flags(self):
+        """The host visibility flags as a [nseg] uint8 tensor sharing their memory (writes show in ``visible``)."""
+        return torch.frombuffer(self.visible, dtype=torch.uint8)[:self.nseg]
+
+
+def _chunk_boxes(blk):
+    """[rows / SEGMENT_CHUNK, 6] (min xyz, max xyz) over the rows of each chunk without NaN (padding); +inf / -inf if none."""
+    v = blk.view(-1, SEGMENT_CHUNK, 4)[:, :, :3]
+    pad = torch.isnan(v).any(2, keepdim=True)
+    return torch.cat([torch.where(pad, float("inf"), v).amin(1), torch.where(pad, float("-inf"), v).amax(1)], 1)
 
 
 def raster_project_segments(pyr, store, seg_m):
@@ -237,6 +260,43 @@ def raster_project_segments(pyr, store, seg_m):
     L.check(L.load().read_raster_project_segments(store.pts4.data_ptr(), store.n, store.first_chunk, store.chunks, store.visible,
                                                   store.nseg, seg_m.data_ptr(), pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(),
                                                   L.stream_ptr()))
+
+
+def raster_project_segments_culled(pyr, store, seg_m, visible=None):
+    """Level 0 of a cleared pyramid from a SegmentedPoints store of up to MAX_SEGMENTS segments, drawing only the (segment,
+    chunk) units that are visible and whose chunk box may intersect the clip volume of some view (culled and compacted on the
+    device, no host synchronisation; finish with raster_derive / pyramid_resolve_gather).  The pyramid is bit-identical to
+    raster_project_segments'.  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, B <= 8; visible: [nseg] uint8 on the device,
+    or None to upload the store's host flags here."""
+    L.require_device()
+    _f32c(seg_m, "seg_m")
+    _f32c(store.pts4, "segmented store")
+    if seg_m.dim() != 4 or tuple(seg_m.shape[:2]) != (store.nseg, pyr.B) or tuple(seg_m.shape[2:]) != (4, 4):
+        raise RuntimeError(f"read_b200: seg_m must be [{store.nseg}, {pyr.B}, 4, 4], got {tuple(seg_m.shape)}")
+    if pyr.direct_mask != 1:
+        raise RuntimeError("the segmented rasterizer needs nested pyramid levels")
+    if visible is None:
+        visible = store.visible_flags().to(seg_m.device)
+    if visible.dtype != torch.uint8 or tuple(visible.shape) != (store.nseg,) or not visible.is_contiguous() or not visible.is_cuda:
+        raise RuntimeError(f"read_b200: visible must be a contiguous [{store.nseg}] uint8 CUDA tensor")
+    lib = L.load()
+    need = lib.read_raster_cull_workspace_bytes(store.nunits)
+    if store._cull_ws is None or store._cull_ws.numel() < need or store._cull_ws.device != seg_m.device:
+        store._cull_ws = torch.empty(need, dtype=torch.uint8, device=seg_m.device)
+    ws = store._cull_ws
+    L.check(lib.read_raster_project_segments_culled(store.pts4.data_ptr(), store.n, store.seg_table.data_ptr(), store.nseg,
+                                                    store.nunits, store.boxes.data_ptr(), visible.data_ptr(), seg_m.data_ptr(),
+                                                    ws.data_ptr(), ws.numel(), pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(),
+                                                    L.stream_ptr()))
+
+
+def last_surviving_units(store):
+    """Synchronise the device and return how many (segment, chunk) units the last raster_project_segments_culled call on
+    ``store`` drew (None before the first).  For tests and benchmarks: it stalls the pipeline."""
+    if store._cull_ws is None:
+        return None
+    torch.cuda.synchronize(store._cull_ws.device)
+    return int(store._cull_ws[:4].cpu().view(torch.int32)[0])
 
 
 def raster_derive(pyr):

@@ -6,7 +6,7 @@ global ids ``base + original id``, bases in the order scenes are added, and the 
 concatenated in that order, so the descriptor gather runs unchanged over global ids.  An *object* is a set of a scene's points
 carved out of the scene's static segment into a segment of its own with a transform ``M``; an *instance* is one more segment
 over an object's rows with its own transform (the same points and descriptors drawn twice).  Every scene, object and instance
-is one segment, at most ``ops.MAX_SEGMENTS`` in all.
+is one segment, at most ``ops.MAX_SEGMENTS`` (4096) in all.
 
 Matrix rule (the parity contract the tests restate): the matrix of a segment for view ``total_m`` (``FrameRenderer.total_matrix``,
 float32) is ``T = total_m @ P_scene @ M``, with ``M`` the identity for the static segment, the object's transform for an object
@@ -14,8 +14,9 @@ and the instance's for an instance; the product is formed in float64 and rounded
 identity placement and transform give ``total_m`` bit for bit.  Rows act on column vectors, as in the kernel:
 ``c_i = row_i . (x, y, z, 1)``.
 
-Edits.  ``set_transform`` and ``set_visible`` are O(1): they change a host-side 4x4 or one visibility flag and never touch point
-data.  Adding a scene, object or instance changes the layout; the store is rebuilt (points re-sorted per segment) the next time it
+Edits.  ``set_transform`` and ``set_visible`` change a host-side 4x4 or one visibility flag and never touch point data; the
+per-segment matrices and flags are kept in arrays, so a frame's host work (``segment_matrices``, the visibility bytes) is a few
+vectorised numpy operations whatever the segment count.  Adding a scene, object or instance changes the layout; the store is rebuilt (points re-sorted per segment) the next time it
 is asked for.  A scene hidden with ``set_visible`` hides its objects and instances too; hiding an object leaves its instances.
 """
 import numpy as np
@@ -51,6 +52,14 @@ class SceneComposer:
         self._tex = None         # composed PointTexture [1, 8, total]
         self._store = None       # ops.SegmentedPoints, rebuilt after a layout change
         self._segments = []      # per segment: (handle, scene index)
+        self._scene_P = np.empty((0, 4, 4))            # [scenes, 4, 4] placements (mirror of the dicts' "P")
+        self._scene_vis = np.empty((0,), dtype=bool)   # [scenes] flags (mirror of the dicts' "visible")
+        # per segment of the built layout: scene index, M (identity for a scene's static part), is-a-scene, own flag
+        self._seg_scene = np.empty((0,), dtype=np.int64)
+        self._seg_M = np.empty((0, 4, 4))
+        self._seg_is_scene = np.empty((0,), dtype=bool)
+        self._seg_own_vis = np.empty((0,), dtype=bool)
+        self._seg_of = {}        # (kind, index) of an object or instance -> its segment
         self.total = 0
 
     # ------------------------------------------------------------------ layout
@@ -84,6 +93,8 @@ class SceneComposer:
         h = _Handle("scene", len(self._scenes))
         h.base = self.total
         self._scenes.append(dict(xyz=xyz.to(self.device).contiguous(), base=self.total, n=n, P=P, visible=True, objects=[]))
+        self._scene_P = np.concatenate([self._scene_P, P[None]])
+        self._scene_vis = np.append(self._scene_vis, True)
         self.total += n
         t = tex.detach().to(self.device, torch.float32)
         cat = t if self._tex is None else torch.cat([self._tex.texture_.detach(), t], 2)
@@ -115,14 +126,25 @@ class SceneComposer:
     def add_instance(self, obj, transform):
         """One more copy of object ``obj`` drawn with its own 4x4 ``transform``: a segment over the SAME rows (no point or
         descriptor is copied; the instance's pixels carry the object's global ids)."""
+        return self.add_instances(obj, _mat4(transform, "transform")[None])[0]
+
+    def add_instances(self, obj, transforms):
+        """K more copies of object ``obj`` at once, one per 4x4 of ``transforms`` [K,4,4]: the same as K ``add_instance`` calls
+        (handles in order), with one layout change."""
         ob = self._object(obj)
-        M = _mat4(transform, "transform")
-        self._check_segments(1)
-        h = _Handle("instance", len(self._instances))
-        self._instances.append(dict(object=obj.index, M=M, visible=True))
-        ob["instances"].append(h.index)
-        self._store = None
-        return h
+        T = np.asarray(transforms, dtype=np.float64)
+        if T.ndim != 3 or T.shape[1:] != (4, 4) or not np.all(np.isfinite(T)):
+            raise ValueError("read_b200: transforms must be finite [K, 4, 4] matrices")
+        self._check_segments(T.shape[0])
+        handles = []
+        for M in T:
+            h = _Handle("instance", len(self._instances))
+            self._instances.append(dict(object=obj.index, M=M.copy(), visible=True))
+            ob["instances"].append(h.index)
+            handles.append(h)
+        if handles:
+            self._store = None
+        return handles
 
     # ------------------------------------------------------------------ O(1) edits
     def _scene(self, h):
@@ -143,12 +165,24 @@ class SceneComposer:
     def set_transform(self, handle, M):
         """A scene's placement, an object's or an instance's transform (4x4).  Host-side only: takes effect on the next frame."""
         e = self._entry(handle)
-        e["P" if handle.kind == "scene" else "M"] = _mat4(M, "transform")
+        M = _mat4(M, "transform")
+        if handle.kind == "scene":
+            e["P"] = M
+            self._scene_P[handle.index] = M
+        else:
+            e["M"] = M
+            seg = self._seg_of.get((handle.kind, handle.index)) if self._store is not None else None
+            if seg is not None:
+                self._seg_M[seg] = M
 
     def set_visible(self, handle, visible):
         """Show or hide a scene (with its objects and instances), an object or an instance: one flag, no point data moves."""
         self._entry(handle)["visible"] = bool(visible)
+        if handle.kind == "scene":
+            self._scene_vis[handle.index] = bool(visible)
         if self._store is not None:
+            if handle.kind != "scene":
+                self._seg_own_vis[self._seg_of[(handle.kind, handle.index)]] = bool(visible)
             self._apply_visibility()
 
     # ------------------------------------------------------------------ what the renderer reads
@@ -190,20 +224,24 @@ class SceneComposer:
                 segments.append(obj_part[o])
                 self._segments.append((_Handle("instance", i), ob["scene"]))
         self._store = ops.SegmentedPoints(parts, segments, n_ids=self.total, cell=self.cell)
+        self._seg_scene = np.array([si for _, si in self._segments], dtype=np.int64)
+        self._seg_is_scene = np.array([h.kind == "scene" for h, _ in self._segments], dtype=bool)
+        self._seg_M = np.stack([np.eye(4) if h.kind == "scene" else self._entry(h)["M"] for h, _ in self._segments])
+        self._seg_own_vis = np.array([h.kind == "scene" or self._entry(h)["visible"] for h, _ in self._segments], dtype=bool)
+        self._seg_of = {(h.kind, h.index): s for s, (h, _) in enumerate(self._segments) if h.kind != "scene"}
         self._apply_visibility()
 
     def _apply_visibility(self):
-        for s, (h, si) in enumerate(self._segments):
-            self._store.set_visible(s, self._scenes[si]["visible"] and (h.kind == "scene" or self._entry(h)["visible"]))
+        # a segment is drawn when its scene is shown and (for an object or instance) its own flag is set
+        self._store.visible_flags().copy_(torch.from_numpy(self._scene_vis[self._seg_scene] & self._seg_own_vis))
 
     def segment_transforms(self):
-        """[nseg, 4, 4] float64: P_scene @ M of every segment, in the store's segment order."""
+        """[nseg, 4, 4] float64: P_scene @ M of every segment, in the store's segment order (a scene's static part: P itself)."""
         if self._store is None:
             self._build()
-        out = np.empty((len(self._segments), 4, 4))
-        for s, (h, si) in enumerate(self._segments):
-            P = self._scenes[si]["P"]
-            out[s] = P if h.kind == "scene" else P @ self._entry(h)["M"]
+        P = self._scene_P[self._seg_scene]
+        out = np.matmul(P, self._seg_M)
+        out[self._seg_is_scene] = P[self._seg_is_scene]
         return out
 
     def segment_matrices(self, total_m):

@@ -127,23 +127,27 @@ class SceneRenderer:
         self.model = NetAndTexture(net, {0: self._tex}, ss, temporal_average=bool(temporal_average))
         self.model.load_textures(0)
         self.model.to(self.device).eval()
-        # per-frame [nseg, 1, 4, 4] matrices through a ring of pinned staging buffers (see FrameRenderer._upload_camera)
-        self._m_host = [torch.empty((ops.MAX_SEGMENTS, 1, 4, 4), dtype=torch.float32).pin_memory() for _ in range(4)]
+        # per frame, the [nseg, 1, 4, 4] matrices and the [nseg] visibility bytes in ONE copy, through a ring of pinned staging
+        # buffers (see FrameRenderer._upload_camera)
+        self._m_host = [torch.empty(ops.MAX_SEGMENTS * 65, dtype=torch.uint8).pin_memory() for _ in range(4)]
         self._m_used = [None] * 4
         self._m_i = 0
 
-    def _upload(self, seg_m):
+    def _upload(self, seg_m, visible):
+        """-> (seg_m, visible) on the device: [nseg, 1, 4, 4] f32 and [nseg] uint8."""
         i = self._m_i
         self._m_i = (i + 1) % len(self._m_host)
         if self._m_used[i] is not None:
             self._m_used[i].synchronize()                # the copy that last read this staging buffer (4 frames ago) has run
-        host = self._m_host[i][:seg_m.shape[0]]
-        host.copy_(torch.from_numpy(seg_m))
-        m = host.to(self.device, non_blocking=True)
+        nseg = seg_m.shape[0]
+        host = self._m_host[i][:nseg * 65]
+        host[:nseg * 64].view(torch.float32).copy_(torch.from_numpy(seg_m).reshape(-1))
+        host[nseg * 64:].copy_(visible)
+        dev = host.to(self.device, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
         self._m_used[i] = ev
-        return m
+        return dev[:nseg * 64].view(torch.float32).view(nseg, 1, 4, 4), dev[nseg * 64:]
 
     def infer(self, proj_matrix, view_matrix):
         """-> {'output': [H,W,4] f32 cuda tensor, 'net_input': list of the four [1,8,h,w] f32 net inputs (None with
@@ -154,10 +158,11 @@ class SceneRenderer:
             self.model._textures[0] = self._tex
             self.model.add_module('0', self._tex.to(self.device))
         store = comp.store
-        seg_m = self._upload(comp.segment_matrices(FrameRenderer.total_matrix(proj_matrix, view_matrix)))
+        seg_m, visible = self._upload(comp.segment_matrices(FrameRenderer.total_matrix(proj_matrix, view_matrix)),
+                                      store.visible_flags())
         with torch.no_grad():
             res = self.model.render(store, seg_m, self.W, self.H, n_levels=self.n_levels, return_input=self.return_net_input,
-                                    clone_output=False)
+                                    clone_output=False, seg_visible=visible)
         out, net_input = res if self.return_net_input else (res, None)
         rgba = torch.empty((self.H, self.W, 4), dtype=torch.float32, device=self.device)
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
