@@ -180,37 +180,6 @@ int read_conv_plan_set_max_ctas(read_conv_plan *p, int max_ctas)
     return READ_OK;
 }
 
-int64_t read_raster_cull_workspace_bytes(int64_t nunits) { return nunits < 0 ? -1 : cull_workspace_bytes(nunits); }
-
-int read_raster_project_segments_culled(const float *pts4, int64_t n, const int32_t *seg_table, int nseg, int64_t nunits,
-                                        const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
-                                        void *workspace, int64_t workspace_bytes, int B, int W, int H, int L, uint64_t *zbuf,
-                                        void *stream)
-{
-    RB_CHECK_ARG(n >= 0 && n % 1024 == 0, "raster_segments_culled: the store holds whole 1024-row chunks (n = %lld)", (long long)n);
-    RB_CHECK_ARG(n < (1ll << 32) - 1, "raster_segments_culled: at most 2^32 - 2 rows");
-    RB_CHECK_ARG(n == 0 || (pts4 != nullptr && chunk_boxes != nullptr), "raster_segments_culled: null store or chunk boxes");
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(pts4) & 15) == 0, "raster_segments_culled: the store must be 16-byte aligned");
-    RB_CHECK_ARG(nseg >= 0 && nseg <= READ_MAX_SEGMENTS_CULLED, "raster_segments_culled: %d segments, at most %d per launch", nseg,
-                 READ_MAX_SEGMENTS_CULLED);
-    RB_CHECK_ARG(nseg == 0 || (seg_table && seg_visible && seg_m), "raster_segments_culled: null segment table, visibility or seg_m");
-    RB_CHECK_ARG(nunits >= 0 && nunits < (1ll << 31), "raster_segments_culled: %lld units, at most 2^31 - 1", (long long)nunits);
-    RB_CHECK_ARG(nunits == 0 || nseg > 0, "raster_segments_culled: units without segments");
-    RB_CHECK_ARG(B >= 1 && B <= 8, "raster_segments_culled: 1 <= B <= 8 views per launch");
-    RB_CHECK_ARG(W >= 1 && H >= 1, "raster_segments_culled: target size must be positive");
-    RB_CHECK_ARG(L >= 1 && L <= READ_MAX_LEVELS, "raster_segments_culled: 1 <= L <= %d", READ_MAX_LEVELS);
-    RB_CHECK_ARG(zbuf != nullptr, "raster_segments_culled: null zbuf");
-    RB_CHECK_ARG(read_raster_direct_mask(W, H, L) == 1u,
-                 "raster_segments_culled: needs nested levels (every level exactly half of the previous one)");
-    RB_CHECK_ARG((long long)W * H < (1ll << 31), "raster_segments_culled: level 0 too large");
-    RB_CHECK_ARG(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0,
-                 "raster_segments_culled: the workspace must be non-null and 16-byte aligned");
-    RB_CHECK_ARG(workspace_bytes >= cull_workspace_bytes(nunits), "raster_segments_culled: workspace of %lld bytes, %lld needed",
-                 (long long)workspace_bytes, cull_workspace_bytes(nunits));
-    return launch_segments_culled(pts4, n, seg_table, nseg, nunits, chunk_boxes, seg_visible, seg_m, workspace, B, W, H,
-                                  reinterpret_cast<unsigned long long *>(zbuf), (cudaStream_t)stream);
-}
-
 void read_conv_plan_destroy(read_conv_plan *p)
 {
     if (!p) return;

@@ -21,11 +21,6 @@ inline unsigned grid_for(long long n)
     const long long blocks = (n + 255) / 256, cap = 16ll * num_sms();
     return (unsigned)(blocks < 1 ? 1 : blocks > cap ? cap : blocks);
 }
-// culled segmented rasterizer (raster.cu), behind read_raster_project_segments_culled (api.cu)
-long long cull_workspace_bytes(long long nunits);
-int launch_segments_culled(const float *pts4, long long n, const int *seg_table, int nseg, long long nunits,
-                           const float *boxes, const uint8_t *vis, const float *seg_m, void *ws, int B, int W, int H,
-                           unsigned long long *zbuf, cudaStream_t st);
 // channel counts of the train-mode BatchNorm entry points (bn_train.cu, conv_bwd.cu): the gate backward's, without 48
 inline bool bn_channels_ok(int C) { return C == 16 || C == 32 || C == 64 || (C % 64 == 0 && C > 0 && C <= 256); }
 

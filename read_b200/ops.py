@@ -247,9 +247,9 @@ def _chunk_boxes(blk):
     return torch.cat([torch.where(pad, float("inf"), v).amin(1), torch.where(pad, float("-inf"), v).amax(1)], 1)
 
 
-def raster_project_segments(pyr, store, seg_m):
-    """Level 0 of a cleared pyramid from a SegmentedPoints store in one pass over its visible segments (finish with raster_derive
-    / pyramid_resolve_gather).  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, segment s drawn with seg_m[s], B <= 8."""
+def _check_segmented(pyr, store, seg_m):
+    """The checks both segmented rasterizer wrappers make: seg_m [nseg, B, 4, 4] f32 contiguous on the device, the store's rows
+    f32 contiguous on the device, nested pyramid levels."""
     L.require_device()
     _f32c(seg_m, "seg_m")
     _f32c(store.pts4, "segmented store")
@@ -257,6 +257,12 @@ def raster_project_segments(pyr, store, seg_m):
         raise RuntimeError(f"read_b200: seg_m must be [{store.nseg}, {pyr.B}, 4, 4], got {tuple(seg_m.shape)}")
     if pyr.direct_mask != 1:
         raise RuntimeError("the segmented rasterizer needs nested pyramid levels")
+
+
+def raster_project_segments(pyr, store, seg_m):
+    """Level 0 of a cleared pyramid from a SegmentedPoints store in one pass over its visible segments (finish with raster_derive
+    / pyramid_resolve_gather).  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, segment s drawn with seg_m[s], B <= 8."""
+    _check_segmented(pyr, store, seg_m)
     L.check(L.load().read_raster_project_segments(store.pts4.data_ptr(), store.n, store.first_chunk, store.chunks, store.visible,
                                                   store.nseg, seg_m.data_ptr(), pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(),
                                                   L.stream_ptr()))
@@ -268,13 +274,7 @@ def raster_project_segments_culled(pyr, store, seg_m, visible=None):
     device, no host synchronisation; finish with raster_derive / pyramid_resolve_gather).  The pyramid is bit-identical to
     raster_project_segments'.  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, B <= 8; visible: [nseg] uint8 on the device,
     or None to upload the store's host flags here."""
-    L.require_device()
-    _f32c(seg_m, "seg_m")
-    _f32c(store.pts4, "segmented store")
-    if seg_m.dim() != 4 or tuple(seg_m.shape[:2]) != (store.nseg, pyr.B) or tuple(seg_m.shape[2:]) != (4, 4):
-        raise RuntimeError(f"read_b200: seg_m must be [{store.nseg}, {pyr.B}, 4, 4], got {tuple(seg_m.shape)}")
-    if pyr.direct_mask != 1:
-        raise RuntimeError("the segmented rasterizer needs nested pyramid levels")
+    _check_segmented(pyr, store, seg_m)
     if visible is None:
         visible = store.visible_flags().to(seg_m.device)
     if visible.dtype != torch.uint8 or tuple(visible.shape) != (store.nseg,) or not visible.is_contiguous() or not visible.is_cuda:
