@@ -405,6 +405,182 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
     if (issuer) bulk_wait_group<0>();     // the stores have read shared memory and written the outputs before the CTA retires
 }
 
+// ------------------------------------------------------------------ weight-stationary body: 3x3 stride-1, 32 -> 32 channels
+// At 32 channels the kernel above spends more shared-memory time moving the 128 x 288 activation operand through ldmatrix than
+// its MMAs take.  Here the roles swap: the weights (64 rows = 32 conv_f + 32 conv_m channels, K = 9 taps x 32 channels) are
+// wgmma's register A operand, loaded ONCE per CTA (72 registers per thread), and the 128 pixels of a tile are N, read by the
+// tensor core straight out of the halo tile: 18 m64n128k16 per tile and no A loads.
+//   halo tile   no swizzle, [8-channel chunk][18 rows][10 px][16 B], one 4-D TMA per chunk (box {8, 10, 18, 1}, chunk stride
+//               padded to 128 B).  Every core matrix (8 px x 16 B) is 128 contiguous bytes, and tap (ky, kx) is the start
+//               address + ky * row + kx * 16 B: LBO = the chunk stride, SBO = the row stride.
+//   A rows      the ldmatrix row addresses pick the packed weight rows so that warp w's rows 0..7 are conv_f and rows 8..15
+//               conv_m of the SAME channels 8w .. 8w+7: each thread then holds both gates of one channel for 32 pixels (tile
+//               row j = accumulator group j, pixels 2 (l & 3), + 1), and the weight packing is the other body's.
+//   epilogue    epilogue_smem's arithmetic per element; the residual comes in with ldmatrix.trans and the output goes back with
+//               stmatrix.trans (8 channels x 8 pixels per block) into the 64-byte-swizzled NHWC stage, stored by one TMA.
+// Warp roles: the producer warp as above; each consumer warpgroup takes whole tiles (the CTA's even / odd ones), so one
+// warpgroup's epilogue runs under the other's MMAs.  One CTA per SM (72 + 64 registers per thread are live across the MMAs).
+constexpr int WS_E_STAGES = 4;                 // two per consumer warpgroup: tile k uses stage k % 4
+constexpr int WS_BAR_EFULL = BAR_BRES + 2, WS_BAR_EEMPTY = WS_BAR_EFULL + WS_E_STAGES, WS_BAR_PARAMS = WS_BAR_EEMPTY + WS_E_STAGES;
+constexpr uint32_t WS_ROW_BYTES = (TC_TW + 2) * 16u;                  // one halo row of one 8-channel chunk
+constexpr uint32_t WS_CHUNK_BYTES = ((TC_TH + 2) * WS_ROW_BYTES + 127u) & ~127u;   // TMA destinations are 128 B aligned
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
+{
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (s_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t *smem_al = smem_raw + (smem_base - s_u32(smem_raw));
+
+    const uint32_t b_region = smem_base + a.b_region_off;
+    const uint32_t e_region = smem_base + a.e_region_off;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + WS_E_STAGES * a.e_bytes);
+    const uint32_t bar0 = s_u32(bars);
+    const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
+    const uint32_t efull0 = bar0 + 8 * WS_BAR_EFULL, eempty0 = bar0 + 8 * WS_BAR_EEMPTY;
+    float4 *s_par = reinterpret_cast<float4 *>(bars + WS_BAR_PARAMS);
+
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    if (a.pdl) pdl_launch_dependents();
+    for (int i = threadIdx.x; i < a.Cout; i += TC_THREADS) s_par[i] = make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]);
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
+        tma_prefetch_desc(&tm.a[0]);
+        tma_prefetch_desc(&tmB);
+        if (a.epi.residual) tma_prefetch_desc(&tm.res);
+        for (int s = 0; s < TC_MAX_STAGES; ++s) {
+            mbar_init(afull0 + 8 * s, 1);
+            mbar_init(aempty0 + 8 * s, 4);          // the four warps of the warpgroup that took the tile
+        }
+        for (int s = 0; s < WS_E_STAGES; ++s) {
+            mbar_init(efull0 + 8 * s, 1);
+            mbar_init(eempty0 + 8 * s, 1);
+        }
+        mbar_init(bres, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    const int total_tiles = a.tiles_x * a.tiles_y * a.B;   // one n-tile
+
+    if (warp == TC_PRODUCER_WARP) {
+        if (elect_one()) {
+            mbar_arrive_expect_tx(bres, 9u * a.b_bytes);
+            for (int i = 0; i < 9; ++i) tma_load_2d(&tmB, bres, b_region + (uint32_t)i * a.b_bytes, 0, i * a.n_tile);
+        }
+        __syncwarp();
+        if (a.pdl) pdl_wait();
+        uint32_t as = 0, aph = 0;
+        int k = 0;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++k) {
+            const TileCoord tc_ = decode_tile(t, a);
+            const int x0 = tc_.tx * TC_TW, y0 = tc_.ty * TC_TH;
+            mbar_wait(aempty0 + 8 * as, aph ^ 1u);
+            if (elect_one()) {
+                const uint32_t full = afull0 + 8 * as, dst = smem_base + as * a.a_bytes;
+                mbar_arrive_expect_tx(full, a.a_tx_bytes);
+#pragma unroll
+                for (int c = 0; c < 4; ++c) tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, x0 - 1, y0 - 1, tc_.b);
+            }
+            __syncwarp();
+            if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
+            const int es = k % WS_E_STAGES;
+            mbar_wait(eempty0 + 8 * es, ((uint32_t)(k / WS_E_STAGES) & 1u) ^ 1u);
+            if (elect_one()) {
+                const uint32_t full = efull0 + 8 * es;
+                mbar_arrive_expect_tx(full, a.e_tx_bytes);          // a plain arrival without a residual
+                if (a.epi.residual) tma_load_4d(&tm.res, full, e_region + es * a.e_bytes, 0, x0, y0, tc_.b);
+            }
+            __syncwarp();
+        }
+        return;
+    }
+
+    const int wg = warp >> 2, wiw = warp & 3;
+    if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
+    mbar_wait(bres, 0);
+    uint32_t wa[9][2][4];
+    {
+        // packed row n: conv_f channel n (n < 32), conv_m channel n - 32; 64-byte swizzled rows of 32 channels
+        const uint32_t n = 8u * wiw + (lane & 7) + 32u * ((lane >> 3) & 1);
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap)
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk)
+                ldmatrix_x4(b_region + (uint32_t)tap * a.b_bytes + swz(n * 64u + 32u * kk + 16u * (lane >> 4), 64u), wa[tap][kk]);
+    }
+    const float4 par = s_par[8 * wiw + (lane >> 2)];
+    // this lane's ldmatrix / stmatrix row in the stage: pixel lane & 7 of tile row lane >> 3 (+ 4 per block), channels 8 wiw..
+    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
+    const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
+    int e_pend = -1;
+    uint32_t as = (uint32_t)wg, aph = 0;            // a_stages >= 2
+    for (int k = wg, t = blockIdx.x + wg * gridDim.x; t < total_tiles; k += 2, t += 2 * gridDim.x) {
+        const TileCoord tc_ = decode_tile(t, a);
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        mbar_wait(afull0 + 8 * as, aph);
+        const uint32_t stage = smem_base + as * a.a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap)
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk)
+                Wgmma<128>::mma(acc, wa[tap][kk],
+                                wgmma_desc_noswz(stage + (uint32_t)(tap / 3) * WS_ROW_BYTES + (uint32_t)(tap % 3) * 16u + 2u * kk * WS_CHUNK_BYTES,
+                                                 WS_CHUNK_BYTES, WS_ROW_BYTES),
+                                1u);
+        wgmma_commit();
+        if (issuer && e_pend >= 0) {     // the previous tile's store has read its stage: the producer may refill it
+            bulk_wait_group_read<0>();
+            mbar_arrive(eempty0 + 8 * e_pend);
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(aempty0 + 8 * as);
+        as += 2;
+        if (as >= (uint32_t)a.a_stages) { as -= (uint32_t)a.a_stages; aph ^= 1u; }
+
+        const int es = k % WS_E_STAGES;
+        mbar_wait(efull0 + 8 * es, (uint32_t)(k / WS_E_STAGES) & 1u);
+        const uint32_t st = e_region + es * a.e_bytes;
+#pragma unroll
+        for (int j0 = 0; j0 < TC_TH; j0 += 4) {
+            const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
+            uint32_t rv[4] = {0u, 0u, 0u, 0u};
+            if (a.epi.residual) ldmatrix_x4_trans(addr, rv);
+            uint32_t ov[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int j = j0 + i;
+                const float f0 = acc[4 * j] + par.x, f1 = acc[4 * j + 1] + par.x;
+                const float m0 = acc[4 * j + 2] + par.y, m1 = acc[4 * j + 3] + par.y;
+                float y0, y1;
+                if (a.epi.elu) {
+                    y0 = gate_fast<true>(f0, m0, par.z, par.w);
+                    y1 = gate_fast<true>(f1, m1, par.z, par.w);
+                } else {
+                    y0 = gate_fast<false>(f0, m0, par.z, par.w);
+                    y1 = gate_fast<false>(f1, m1, par.z, par.w);
+                }
+                const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
+                ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
+            }
+            stmatrix_x4_trans(addr, ov);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + wg, 128);
+        if (issuer) {
+            tma_store_4d(&tm.out, st, 0, tc_.tx * TC_TW, tc_.ty * TC_TH, tc_.b);    // clipped at the image edge
+            bulk_commit_group();
+        }
+        e_pend = es;
+    }
+    if (issuer) bulk_wait_group<0>();
+}
+
 // ------------------------------------------------------------------ weight packing
 // out[((tap*kchunks + kc) * n_total + n) * cin_blk + kk],  n -> (tile nt, f|m half, channel)
 __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int cout_pad, int Cin,
@@ -578,7 +754,15 @@ struct TcPlan {
     TcArgs args;
     size_t smem_bytes;
     int reverse;
+    int ws;                                // runs gated_conv_tc_ws_kernel (tc_ws_layer)
 };
+
+// The layers of the weight-stationary body: 3x3 stride-1 32 -> 32 gated convs with an NHWC output and at most a residual
+static bool tc_ws_layer(const read_conv_desc &d)
+{
+    return d.k == 3 && d.stride == 1 && d.Cin == 32 && d.Cout == 32 && d.n_src == 1 && d.out_mode == READ_OUT_NHWC &&
+           d.out2 == nullptr && d.addin == nullptr;
+}
 
 int tc_plan_create(const read_conv_desc &d, TcPlan **out)
 {
@@ -604,6 +788,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     RB_CHECK_ARG(p != nullptr, "wgmma conv: out of host memory");
 
     const bool s2 = d.stride == 2;
+    p->ws = tc_ws_layer(d) ? 1 : 0;
     const int halo_rows = s2 ? TC_TH + 1 : TC_TH + d.k - 1;
     const int halo_w = s2 ? TC_TW + 1 : TC_TW + d.k - 1;
     const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -615,10 +800,11 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         cuuint64_t strides[3] = {(cuuint64_t)sv.C * 2, (cuuint64_t)sv.W * sv.C * 2, (cuuint64_t)sv.H * sv.W * sv.C * 2};
         // traversal stride f in x and y (conv stride 2, or a nearest-down source): the box spans (n-1)*f+1 input
         // elements and delivers n of them
-        cuuint32_t box[4] = {(cuuint32_t)g.cin_blk, (cuuint32_t)((halo_w - 1) * f + 1), (cuuint32_t)((halo_rows - 1) * f + 1), 1};
+        // (the weight-stationary body loads the halo one 8-channel chunk at a time, unswizzled)
+        cuuint32_t box[4] = {(cuuint32_t)(p->ws ? 8 : g.cin_blk), (cuuint32_t)((halo_w - 1) * f + 1), (cuuint32_t)((halo_rows - 1) * f + 1), 1};
         cuuint32_t estr[4] = {1, f, f, 1};
         CUresult r = enc(&p->tmA.a[si], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(sv.ptr), dims, strides, box,
-                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, p->ws ? CU_TENSOR_MAP_SWIZZLE_NONE : sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             set_error("wgmma conv: cuTensorMapEncodeTiled(activations, source %d) failed with %d", si, (int)r);
@@ -659,7 +845,8 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     if (!nchw) {
         const int oc = raw ? g.n_tile : half;             // channels of one output pixel in the tile
         const int ocb = oc < 64 ? oc : 64, acb = g.n_tile < 64 ? g.n_tile : 64;
-        bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH / 2, "out");
+        // stored per warpgroup (8 rows), or per tile by the weight-stationary body
+        bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, p->ws ? TC_TH : TC_TH / 2, "out");
         if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
         if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
         if (ok && d.residual)
@@ -696,7 +883,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         }
     }
     a.a_tx_bytes = (uint32_t)halo_rows * halo_w * g.cin_blk * 2u;
-    a.tile_bytes = (a.a_tx_bytes + 1023u) & ~1023u;    // tiles stay 1 KB aligned (swizzle patterns are address based)
+    a.tile_bytes = ((p->ws ? 4u * WS_CHUNK_BYTES : a.a_tx_bytes) + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
@@ -710,13 +897,13 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         a.e_bytes = out_b + out2_b + add_b;
         a.e_tx_bytes = (d.residual ? out_b : 0u) + out2_b + add_b;
     }
-    const uint32_t e_ring = TC_E_STAGES * a.e_bytes;
+    const uint32_t e_ring = (p->ws ? WS_E_STAGES : TC_E_STAGES) * a.e_bytes;
     // the rings get what a CTA may have minus the alignment pad, barriers and per-channel parameters (smem_bytes below)
-    const uint32_t fixed = 1024 + 8 * BAR_PARAMS + 16 * (uint32_t)g.cout_pad + 64;
+    const uint32_t fixed = 1024 + 8 * (p->ws ? WS_BAR_PARAMS : BAR_PARAMS) + 16 * (uint32_t)g.cout_pad + 64;
     const uint32_t budget_2 = TC_SMEM_PER_SM / 2 - 1024 - fixed, budget_1 = TC_SMEM_PER_CTA - fixed;
     // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights, the epilogue ring and >= 3 A
     // stages in half of the SM
-    a.ctas_per_sm = (tc_ctas_per_sm(g.n_tile) > 1 && g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX &&
+    a.ctas_per_sm = (!p->ws && tc_ctas_per_sm(g.n_tile) > 1 && g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX &&
                      total_b + e_ring + 3 * a.a_bytes <= budget_2) ? 2 : 1;
     const uint32_t budget = a.ctas_per_sm > 1 ? budget_2 : budget_1;
     a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && total_b + e_ring + 2 * a.a_bytes <= budget) ? 1 : 0;
@@ -737,6 +924,11 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         int st = (int)((budget - 3 * a.a_bytes - e_ring) / a.b_bytes);
         a.b_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
+    }
+    if (p->ws && (!a.b_resident || a.a_stages < 2)) {      // cannot happen at 32 channels; the kernel relies on both
+        set_error("wgmma conv: weight-stationary layer without resident weights or two A stages");
+        delete p;
+        return READ_ERR_UNSUPPORTED;
     }
     a.b_region_off = (uint32_t)a.a_stages * a.a_bytes;
     a.e_region_off = a.b_region_off + b_region_bytes;
@@ -788,6 +980,13 @@ static int launch_tc_kn(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lc
     return READ_ERR_UNSUPPORTED;
 }
 
+static int launch_tc_ws(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
+    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_ws_kernel, p->tmA, p->tmB, a));
+    return READ_OK;
+}
+
 int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
 {
     TcArgs a = p->args;
@@ -811,7 +1010,8 @@ int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
     lcfg.attrs = lattr;
     lcfg.numAttrs = a.pdl ? 1 : 0;
     int rc;
-    if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
+    if (p->ws) rc = launch_tc_ws(p, a, lcfg);
+    else if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 3) rc = launch_tc_kn<3, 1>(p, a, lcfg);
     else if (a.stride == 2 && a.ksize == 3) rc = launch_tc_kn<3, 2>(p, a, lcfg);
     else if (a.stride == 2 && a.ksize == 4) rc = launch_tc_kn<4, 2>(p, a, lcfg);

@@ -150,6 +150,23 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4])
                  : "memory");
 }
 
+// The same four 8x8 blocks transposed: lane l receives elements (2 * (l & 3), l >> 2) and (2 * (l & 3) + 1, l >> 2) of each block,
+// i.e. with memory rows = pixels of 8 channels it holds channel l >> 2 of pixels 2 * (l & 3), + 1
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4])
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+// its inverse: four 8x8 blocks from the fragment layout, stored transposed (lane l supplies the address of memory row l & 7 of block l >> 3)
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4])
+{
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+                 "r"(r[3])
+                 : "memory");
+}
+
 // Byte offset inside a tile written by TMA (or by hand) with the 32/64/128-byte swizzle of a row of row_bytes (32, 64, 128) bytes:
 // the 16-byte chunk index is XORed with the row index modulo row_bytes / 16.  The tile base is 1 KB aligned.
 __device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t row_bytes)
@@ -170,6 +187,13 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t row_byte
     d |= (uint64_t)((8u * row_bytes) >> 4) << 32;
     d |= layout << 62;
     return d;
+}
+
+// K-major descriptor without swizzle: 8 x 16-byte core matrices of 128 contiguous bytes, lbo = byte stride between the two
+// 8-element K halves of a K step, sbo = byte stride between consecutive 8-row groups; the start needs only 16-byte alignment.
+__device__ __forceinline__ uint64_t wgmma_desc_noswz(uint32_t saddr, uint32_t lbo, uint32_t sbo)
+{
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (uint64_t)(lbo >> 4) << 16 | (uint64_t)(sbo >> 4) << 32;
 }
 
 // D[64 x N] (+)= A[64 x 16] (registers, mma.m16n8k16 fragment layout per warp) * B[N x 16] (K-major shared-memory descriptor),
