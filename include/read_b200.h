@@ -125,6 +125,38 @@ int read_raster_project_segments_culled(const float *pts4, int64_t n, const int3
                                         const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
                                         void *workspace, int64_t workspace_bytes, int B, int W, int H, int L, uint64_t *zbuf,
                                         void *stream);
+/* Point sprites (the reference's _pN / _psN input formats and per-point sizes; DESIGN.md §4.2).  A point is clipped, keyed and
+ * given its centre pixel (xx, yy) exactly as at 1 pixel; it then covers a wd x wd square of pixels of each level:
+ *   size  = N of the level's key (_pN), or max(1, N / c2) with c2 the point's clip-space z and an IEEE fp32 division (_psN);
+ *           a per-point size s > 0 replaces N in either form, s == 0 keeps N;
+ *   wd    = min(READ_MAX_POINT_SIZE, max(1, floor(size + 0.5)));
+ *   odd wd = 2k+1: columns xx-k .. xx+k; even wd = 2k: columns xr-k .. xr+k-1 with xr = xx + (u - xx >= 0.5), rows likewise;
+ *   pixels outside the level are dropped, and every covered pixel takes the (depth | id) key through the 64-bit min.
+ * A level with N = 1 in the _pN form and no per-point sizes is a 1-pixel level: it is derived by the 2x2 min from the level
+ * before it when that is a 1-pixel level of exactly twice its size, as today.  Every other level, sprite or not, is drawn
+ * directly in the same pass over the store, so the levels need not nest.  The three entry points take the stores of
+ * read_raster_project_sorted_views, read_raster_project_segments and read_raster_project_segments_culled with the same
+ * arguments, write EVERY level of the (cleared) B-view pyramid (no derive step follows), and take B > 8 views for the sorted
+ * store (one pass per 8 views).
+ *   size[l], relative[l]  level l's N (finite, > 0) and form (0: _pN, 1: _psN), for l < L;
+ *   point_sizes           NULL, or one float per store row (>= 0, finite), 16-byte aligned and padded with zeros to whole
+ *                         1024-row chunks (the segmented stores already are); sorted and segmented stores permute it with
+ *                         their rows. */
+#define READ_MAX_POINT_SIZE 64
+typedef struct {
+    float size[READ_MAX_LEVELS];
+    int32_t relative[READ_MAX_LEVELS];
+    const float *point_sizes;
+} read_sprite_desc;
+int read_raster_sprites_sorted(const float *pts4, int64_t n, const float *total_m, int B, int W, int H, int L,
+                               const read_sprite_desc *desc, uint64_t *zbuf, void *stream);
+int read_raster_sprites_segments(const float *pts4, int64_t n, const int64_t *seg_first_chunk, const int64_t *seg_chunks,
+                                 const uint8_t *seg_visible, int nseg, const float *seg_m, int B, int W, int H, int L,
+                                 const read_sprite_desc *desc, uint64_t *zbuf, void *stream);
+int read_raster_sprites_segments_culled(const float *pts4, int64_t n, const int32_t *seg_table, int nseg, int64_t nunits,
+                                        const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
+                                        void *workspace, int64_t workspace_bytes, int B, int W, int H, int L,
+                                        const read_sprite_desc *desc, uint64_t *zbuf, void *stream);
 /* Bitmask of levels rasterised with direct atomics (bit l set) for this geometry. */
 unsigned read_raster_direct_mask(int W, int H, int L);
 

@@ -55,6 +55,14 @@ class ReadTexTable(ctypes.Structure):
                 ("slot", ctypes.c_uint8 * MAX_TEX_ITEMS)]
 
 
+MAX_LEVELS = 8              # READ_MAX_LEVELS
+MAX_POINT_SIZE = 64         # READ_MAX_POINT_SIZE: widest point sprite, in pixels
+
+
+class ReadSpriteDesc(ctypes.Structure):
+    _fields_ = [("size", ctypes.c_float * MAX_LEVELS), ("relative", ctypes.c_int32 * MAX_LEVELS), ("point_sizes", c_vp)]
+
+
 class ReadHaloDesc(ctypes.Structure):
     _fields_ = [("src_up", c_vp), ("src_dn", c_vp), ("peer_up_slot", c_vp), ("peer_dn_slot", c_vp),
                 ("peer_up_flag", c_vp), ("peer_dn_flag", c_vp), ("slot_from_up", c_vp), ("slot_from_dn", c_vp),
@@ -100,6 +108,11 @@ _SIGS = {
     "read_halo_exchange": (c_int, [ctypes.POINTER(ReadHaloDesc), c_vp]),
     "read_stage_net_inputs": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp, c_vp]),
     "read_raster_direct_mask": (c_u32, [c_int, c_int, c_int]),
+    "read_raster_sprites_sorted": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, ctypes.POINTER(ReadSpriteDesc), c_vp, c_vp]),
+    "read_raster_sprites_segments": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                             ctypes.POINTER(ReadSpriteDesc), c_vp, c_vp]),
+    "read_raster_sprites_segments_culled": (c_int, [c_vp, c_i64, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int,
+                                                    c_int, c_int, ctypes.POINTER(ReadSpriteDesc), c_vp, c_vp]),
     "read_zbuf_resolve": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
     "read_pcpr_forward": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "read_texture_to_point_major": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp]),

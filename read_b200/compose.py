@@ -25,6 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from . import sprites
 from . import _lib as L
 from .texture import PointTexture, sample_items
 
@@ -197,7 +198,7 @@ class NetAndTexture(nn.Module):
 
     @torch.no_grad()
     def render(self, xyz, total_m, W, H, texture_id=0, n_levels=4, want_maps=False, return_input=False, clone_output=True,
-               seg_visible=None):
+               seg_visible=None, input_format=None):
         """points [N,3] (cuda f32) or an ``ops.SortedPoints`` store + total_m [B,4,4] (cuda f32) -> RGB [B,3,H,W] f32 (a fresh
         tensor), all on device, one pass over the cloud.  A sorted store serves frames whose levels nest; the result is
         bit-identical to rendering the unsorted cloud (the z-buffer is a min over (depth | original id) keys).
@@ -212,7 +213,12 @@ class NetAndTexture(nn.Module):
         An ``ops.SegmentedPoints`` store (read_b200.scene_edit) takes ``total_m`` as the per-segment matrices ``seg_m``
         [nseg, B, 4, 4]; its index maps hold global ids, which index the composed texture.  It is drawn by the culled rasterizer
         (``ops.raster_project_segments_culled``): only the chunks that are visible and may meet some view's frustum are read.
-        ``seg_visible``: its [nseg] uint8 visibility flags already on the device (default: the store's host flags)."""
+        ``seg_visible``: its [nseg] uint8 visibility flags already on the device (default: the store's host flags).
+
+        ``input_format``: the checkpoint's format string; its first ``n_levels`` keys give each level's point size (``_pN`` /
+        ``_psN``, read_b200.sprites), and a store's per-point sizes (``psize``) apply.  Frames with larger points are drawn as point
+        sprites from the store (SortedPoints or SegmentedPoints, whose levels need not nest) and gathered level by level;
+        ``None`` (the default), or only 1-pixel levels and no per-point sizes, renders as without it."""
         segmented = isinstance(xyz, ops.SegmentedPoints)
         store = xyz if segmented or isinstance(xyz, ops.SortedPoints) else None
         pts = store.pts4 if store is not None else xyz
@@ -234,11 +240,18 @@ class NetAndTexture(nn.Module):
         act_layout = L.FEAT_NHWC_BF16 if eng.bf16 else L.FEAT_NHWC_F32
         gather_layout = L.FEAT_NHWC_F32 if staged else act_layout
         gather_out = st['feat'] if staged else eng.inputs
-        fused_ok = (not want_maps) and texture.activation == 'none' and ops.fused_resolve_supported(pyr, tex.shape[1])
+        levels = None if input_format is None else sprites.sprite_levels(input_format, n_levels)
+        sprite = levels is not None and not sprites.one_pixel(levels, store.psize if store is not None else None)
+        if sprite and store is None:
+            raise ValueError("read_b200: point sprites are drawn from an ops.SortedPoints or ops.SegmentedPoints store")
+        fused_ok = (not sprite and not want_maps and texture.activation == 'none'
+                    and ops.fused_resolve_supported(pyr, tex.shape[1]))
 
         if not (fused_ok and st['clean']):
             pyr.clear()
-        if store is not None:
+        if sprite:
+            ops.raster_project_sprites(pyr, store, total_m, levels, visible=seg_visible)
+        elif store is not None:
             if pyr.direct_mask != 1:
                 raise RuntimeError("a SortedPoints store renders frames with nested levels; pass the [N,3] cloud otherwise")
             if segmented:

@@ -4,19 +4,25 @@ Differences in HOW (not WHAT): the point clouds are uploaded once in ``update_ds
 (the reference re-uploads N*12 bytes per level per call, pcpr_cuda.cpp:29); all L levels and all views of a
 dataset id are produced by ONE pass over the points (the reference projects every point L times); outputs are
 bit-identical to a sequential execution of the reference kernel.
+
+``point_sprites=True`` honours the point sizes the reference's GL renderer draws (``READ/datasets/dynamic.py:66-99``): each key's
+``_pN`` / ``_psN`` and ``scene_data['point_sizes']`` when present (read_b200.sprites).  The default, like ``src``'s ``MyRender``,
+ignores them and draws 1-pixel points.
 """
 import numpy as np
 import torch
 
 from . import ops
+from . import sprites
 from . import _lib as L
 
 inv = np.linalg.inv
 
 
 class MyRender:
-    def __init__(self, ds_list=None, device_outputs=False):
+    def __init__(self, ds_list=None, device_outputs=False, point_sprites=False):
         self.device_outputs = device_outputs
+        self.point_sprites = bool(point_sprites)
         self._pyr = {}
         if ds_list:
             self.update_ds(ds_list)
@@ -32,6 +38,12 @@ class MyRender:
         self.tgt_sh = self.ds_list[0].tgt_sh
         dev = torch.device("cuda", torch.cuda.current_device())
         self.points = {i: torch.from_numpy(np.ascontiguousarray(c, dtype=np.float32)).to(dev) for i, c in clouds.items()}
+        self.stores = {}
+        if self.point_sprites:
+            # sprite frames are drawn from sorted stores, which carry each dataset's per-point sizes
+            for ds in ds_list:
+                sizes = ds.scene_data.get('point_sizes') if hasattr(ds.scene_data, 'get') else None
+                self.stores[ds.id] = ops.SortedPoints(self.points[ds.id], point_sizes=sizes)
 
     def _pyramid(self, B, W, H, n_levels, dev):
         key = (B, W, H, n_levels, dev)
@@ -52,6 +64,7 @@ class MyRender:
         total_m = torch.from_numpy(proj_matrix @ inv(view_matrix))          # myrender.py:28-30, same numpy call
 
         W, H = int(self.tgt_sh[0]), int(self.tgt_sh[1])
+        levels = sprites.sprite_levels(input_format, n_levels) if self.point_sprites else None
         sizes = ops.level_sizes(W, H, n_levels)
         dev = next(iter(self.points.values())).device
         idx_levels = [torch.zeros((nb, h, w), dtype=self.index_dtype, device=dev) for (w, h) in sizes]
@@ -63,7 +76,11 @@ class MyRender:
             m = total_m[sel].contiguous().to(dev)
             pyr = self._pyramid(int(sel.numel()), W, H, n_levels, dev)
             pyr.clear()
-            ops.raster_project(pyr, self.points[ds_id], m)
+            store = self.stores.get(ds_id)
+            if levels is not None and not sprites.one_pixel(levels, store.psize):
+                ops.raster_project_sprites(pyr, store, m, levels)
+            else:
+                ops.raster_project(pyr, self.points[ds_id], m)
             sel_d = sel.to(dev)
             for l in range(n_levels):
                 i, d = ops.zbuf_resolve(pyr, l, index_dtype=self.index_dtype)

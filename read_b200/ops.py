@@ -4,6 +4,7 @@ import ctypes
 import torch
 
 from . import _lib as L
+from . import sprites
 
 
 def level_sizes(W, H, n_levels):
@@ -96,9 +97,12 @@ class SortedPoints:
     ``pts4`` is ``[N,4]`` f32 = (x, y, z, bit pattern of the ORIGINAL point id); rows are ordered by the Morton code of the
     point's 3-D grid cell (``cell`` metres, ties in original order), so consecutive rows are neighbours in space.  The
     original ids travel with the points: index maps, checkpoints and ``PointTexture`` keep the reference's numbering.
-    Built once per scene with torch ops on the device (scene load, not the per-frame path)."""
+    Built once per scene with torch ops on the device (scene load, not the per-frame path).
 
-    def __init__(self, xyz, cell=0.25):
+    ``point_sizes``: optional [N] per-point sprite sizes (``scene_data['point_sizes']``, see read_b200.sprites), permuted with the
+    points into ``psize`` (float32 on the store's device, padded with zeros to whole SEGMENT_CHUNK chunks); None otherwise."""
+
+    def __init__(self, xyz, cell=0.25, point_sizes=None):
         # the sort itself is plain torch (runs wherever xyz lives); only the rasterizer needs the device
         if xyz.dtype != torch.float32:
             raise RuntimeError("in_points must be a float tensor")
@@ -110,9 +114,13 @@ class SortedPoints:
         if n >= 1 << 32:
             raise RuntimeError("point ids must fit 32 bits")
         self.n, self.cell = n, float(cell)
+        sizes = None if point_sizes is None else sprites.check_point_sizes(point_sizes, n).to(xyz.device)
+        self.psize = None
         if n == 0:
             self.pts4 = torch.empty((0, 4), dtype=torch.float32, device=xyz.device)
             self.perm = torch.empty((0,), dtype=torch.int64, device=xyz.device)
+            if sizes is not None:
+                self.psize = _padded_sizes(sizes)
             return
         lo = xyz.min(0).values
         q = torch.floor((xyz - lo) / self.cell).to(torch.int64).clamp_(0, (1 << 21) - 1)
@@ -133,16 +141,28 @@ class SortedPoints:
         pts4[:, :3] = xyz[self.perm]
         pts4[:, 3] = ids.view(torch.float32)
         self.pts4 = pts4
+        if sizes is not None:
+            self.psize = _padded_sizes(sizes[self.perm])
 
 
     def shard(self, start, count):
         """Rows [start, start+count) of the sorted store as a store of their own: a contiguous range of the Morton order
         is a compact spatial tile of the scene (the multi-GPU partition, SURVEY.md §8e)."""
+        if self.psize is not None:
+            raise ValueError("read_b200: a store with point sizes is not sharded (point sprites are single-GPU)")
         sub = object.__new__(SortedPoints)
-        sub.n, sub.cell = int(count), self.cell
+        sub.n, sub.cell, sub.psize = int(count), self.cell, None
         sub.pts4 = self.pts4[start:start + count]
         sub.perm = self.perm[start:start + count]
         return sub
+
+
+def _padded_sizes(sizes):
+    """[n] f32 -> [ceil(n / SEGMENT_CHUNK) * SEGMENT_CHUNK] f32, zero-padded: the rasterizer streams whole chunks of sizes."""
+    n = sizes.shape[0]
+    out = torch.zeros(max(-(-n // SEGMENT_CHUNK), 1) * SEGMENT_CHUNK, dtype=torch.float32, device=sizes.device)
+    out[:n] = sizes
+    return out
 
 
 def raster_project_sorted(pyr, store, total_m):
@@ -170,7 +190,7 @@ MAX_SEGMENTS = L.MAX_SEGMENTS_CULLED     # per store; the table-in-parameters en
 class SegmentedPoints:
     """Composed, device-resident point store for scene editing and stitching (read_b200.scene_edit).
 
-    Built from ``parts``: a list of ``(xyz [n,3] f32, ids [n] int64)``, each a group of points with their GLOBAL ids (the row of
+    Built from ``parts``: a list of ``(xyz [n,3] f32, ids [n] int64)`` or ``(xyz, ids, point_sizes [n])``, each a group of points with their GLOBAL ids (the row of
     their descriptors in the composed descriptor table).  Each part becomes one block of ``pts4`` rows: its points sorted on
     their own as a ``SortedPoints`` store, with the global id in the id word, then padded to whole ``SEGMENT_CHUNK`` chunks with
     rows (NaN, NaN, NaN, id 0) that the rasterizer culls, so that a chunk never spans two segments.  ``segments`` lists, per
@@ -184,7 +204,10 @@ class SegmentedPoints:
     ``boxes`` [n / SEGMENT_CHUNK, 6] f32, the axis-aligned box (min x, y, z, max x, y, z) of the rows of each chunk that hold a
     point (padding rows left out; a chunk of padding only gets the empty box +inf / -inf, which always culls); ``seg_table``
     [nseg, 3] int32, (first chunk, chunk count, matrix slot = the segment's index) per segment; ``nunits`` the number of
-    (segment, chunk) units, the sum of the chunk counts."""
+    (segment, chunk) units, the sum of the chunk counts.
+
+    ``psize``: when some part has point sizes, [n] f32 per row (permuted with the rows; 0 for padding rows and for the points of
+    parts without sizes, which keep the keys' sizes); None otherwise."""
 
     def __init__(self, parts, segments=None, n_ids=None, cell=0.25):
         segments = list(range(len(parts))) if segments is None else [int(s) for s in segments]
@@ -194,7 +217,10 @@ class SegmentedPoints:
             raise ValueError("read_b200: a segment refers to a part that does not exist")
         blocks, boxes, part_rows, row = [], [], [], 0
         self.part_ids = []
-        for xyz, ids in parts:
+        sized = any(len(p) > 2 and p[2] is not None for p in parts)
+        size_blocks = []
+        for part in parts:
+            xyz, ids = part[0], part[1]
             ids = torch.as_tensor(ids, dtype=torch.int64, device=xyz.device).reshape(-1)
             if ids.shape[0] != xyz.shape[0]:
                 raise ValueError("read_b200: one global id per point")
@@ -208,6 +234,13 @@ class SegmentedPoints:
             if sp.n:
                 blk[:sp.n, :3] = sp.pts4[:, :3]
                 blk[:sp.n, 3] = ids[sp.perm].to(torch.int32).view(torch.float32)
+            if sized:
+                sz = torch.zeros(rows, dtype=torch.float32, device=xyz.device)
+                if len(part) > 2 and part[2] is not None and sp.n:
+                    sz[:sp.n] = sprites.check_point_sizes(part[2], sp.n).to(xyz.device)[sp.perm]
+                elif len(part) > 2 and part[2] is not None:
+                    sprites.check_point_sizes(part[2], 0)
+                size_blocks.append(sz)
             blocks.append(blk)
             boxes.append(_chunk_boxes(blk))
             part_rows.append((row, rows))
@@ -216,6 +249,7 @@ class SegmentedPoints:
         dev = parts[0][0].device if parts else torch.device("cpu")
         self.pts4 = torch.cat(blocks) if blocks else torch.empty((0, 4), dtype=torch.float32, device=dev)
         self.n = self.pts4.shape[0]
+        self.psize = torch.cat(size_blocks) if sized else None
         self.n_ids = int(n_ids) if n_ids is not None else sum(int(i.numel()) for i in self.part_ids)
         self.segment_part = segments
         self.nseg = len(segments)
@@ -247,15 +281,15 @@ def _chunk_boxes(blk):
     return torch.cat([torch.where(pad, float("inf"), v).amin(1), torch.where(pad, float("-inf"), v).amax(1)], 1)
 
 
-def _check_segmented(pyr, store, seg_m):
-    """The checks both segmented rasterizer wrappers make: seg_m [nseg, B, 4, 4] f32 contiguous on the device, the store's rows
-    f32 contiguous on the device, nested pyramid levels."""
+def _check_segmented(pyr, store, seg_m, nested=True):
+    """The checks the segmented rasterizer wrappers make: seg_m [nseg, B, 4, 4] f32 contiguous on the device, the store's rows
+    f32 contiguous on the device, nested pyramid levels (not for point sprites)."""
     L.require_device()
     _f32c(seg_m, "seg_m")
     _f32c(store.pts4, "segmented store")
     if seg_m.dim() != 4 or tuple(seg_m.shape[:2]) != (store.nseg, pyr.B) or tuple(seg_m.shape[2:]) != (4, 4):
         raise RuntimeError(f"read_b200: seg_m must be [{store.nseg}, {pyr.B}, 4, 4], got {tuple(seg_m.shape)}")
-    if pyr.direct_mask != 1:
+    if nested and pyr.direct_mask != 1:
         raise RuntimeError("the segmented rasterizer needs nested pyramid levels")
 
 
@@ -268,6 +302,18 @@ def raster_project_segments(pyr, store, seg_m):
                                                   L.stream_ptr()))
 
 
+def _culled_inputs(store, seg_m, visible):
+    """(visible flags on the device, the store's workspace) for the culled rasterizers."""
+    if visible is None:
+        visible = store.visible_flags().to(seg_m.device)
+    if visible.dtype != torch.uint8 or tuple(visible.shape) != (store.nseg,) or not visible.is_contiguous() or not visible.is_cuda:
+        raise RuntimeError(f"read_b200: visible must be a contiguous [{store.nseg}] uint8 CUDA tensor")
+    need = L.load().read_raster_cull_workspace_bytes(store.nunits)
+    if store._cull_ws is None or store._cull_ws.numel() < need or store._cull_ws.device != seg_m.device:
+        store._cull_ws = torch.empty(need, dtype=torch.uint8, device=seg_m.device)
+    return visible, store._cull_ws
+
+
 def raster_project_segments_culled(pyr, store, seg_m, visible=None):
     """Level 0 of a cleared pyramid from a SegmentedPoints store of up to MAX_SEGMENTS segments, drawing only the (segment,
     chunk) units that are visible and whose chunk box may intersect the clip volume of some view (culled and compacted on the
@@ -275,19 +321,47 @@ def raster_project_segments_culled(pyr, store, seg_m, visible=None):
     raster_project_segments'.  seg_m: [nseg, B, 4, 4] f32 contiguous on the device, B <= 8; visible: [nseg] uint8 on the device,
     or None to upload the store's host flags here."""
     _check_segmented(pyr, store, seg_m)
-    if visible is None:
-        visible = store.visible_flags().to(seg_m.device)
-    if visible.dtype != torch.uint8 or tuple(visible.shape) != (store.nseg,) or not visible.is_contiguous() or not visible.is_cuda:
-        raise RuntimeError(f"read_b200: visible must be a contiguous [{store.nseg}] uint8 CUDA tensor")
+    visible, ws = _culled_inputs(store, seg_m, visible)
     lib = L.load()
-    need = lib.read_raster_cull_workspace_bytes(store.nunits)
-    if store._cull_ws is None or store._cull_ws.numel() < need or store._cull_ws.device != seg_m.device:
-        store._cull_ws = torch.empty(need, dtype=torch.uint8, device=seg_m.device)
-    ws = store._cull_ws
     L.check(lib.read_raster_project_segments_culled(store.pts4.data_ptr(), store.n, store.seg_table.data_ptr(), store.nseg,
                                                     store.nunits, store.boxes.data_ptr(), visible.data_ptr(), seg_m.data_ptr(),
                                                     ws.data_ptr(), ws.numel(), pyr.B, pyr.W, pyr.H, pyr.L, pyr.buf.data_ptr(),
                                                     L.stream_ptr()))
+
+
+def raster_project_sprites(pyr, store, total_m, levels, kernel="culled", visible=None):
+    """Every level of a cleared pyramid from a SortedPoints or SegmentedPoints store, drawn as point sprites (read_b200.sprites):
+    ``levels`` [(N, relative)] per level; the store's ``psize`` (if any) gives the per-point sizes.  One pass over the store per
+    8 views (sorted store) or for all B <= 8 views (segmented store); the levels need not nest, and no derive step follows.
+    total_m: [B,4,4] (sorted store) or seg_m [nseg, B, 4, 4] (segmented store) f32 contiguous on the device.  A segmented store
+    is drawn by the culled rasterizer (``kernel="culled"``, with ``visible`` as in raster_project_segments_culled) or the
+    parameter-table one (``kernel="segments"``)."""
+    if len(levels) != pyr.L:
+        raise ValueError(f"read_b200: {len(levels)} sprite levels for a {pyr.L}-level pyramid")
+    d = sprites.desc(levels, store.psize)
+    lib, sp = L.load(), L.stream_ptr()
+    if isinstance(store, SortedPoints):
+        L.require_device()
+        _f32c(total_m, "total_m")
+        _f32c(store.pts4, "sorted store")
+        if total_m.dim() != 3 or total_m.shape[0] != pyr.B:
+            raise RuntimeError("batch_size check")
+        L.check(lib.read_raster_sprites_sorted(store.pts4.data_ptr(), store.n, total_m.data_ptr(), pyr.B, pyr.W, pyr.H, pyr.L,
+                                               ctypes.byref(d), pyr.buf.data_ptr(), sp))
+        return
+    _check_segmented(pyr, store, total_m, nested=False)
+    if kernel == "segments":
+        L.check(lib.read_raster_sprites_segments(store.pts4.data_ptr(), store.n, store.first_chunk, store.chunks, store.visible,
+                                                 store.nseg, total_m.data_ptr(), pyr.B, pyr.W, pyr.H, pyr.L, ctypes.byref(d),
+                                                 pyr.buf.data_ptr(), sp))
+        return
+    if kernel != "culled":
+        raise ValueError(f"read_b200: unknown segmented rasterizer {kernel!r}")
+    visible, ws = _culled_inputs(store, total_m, visible)
+    L.check(lib.read_raster_sprites_segments_culled(store.pts4.data_ptr(), store.n, store.seg_table.data_ptr(), store.nseg,
+                                                    store.nunits, store.boxes.data_ptr(), visible.data_ptr(), total_m.data_ptr(),
+                                                    ws.data_ptr(), ws.numel(), pyr.B, pyr.W, pyr.H, pyr.L, ctypes.byref(d),
+                                                    pyr.buf.data_ptr(), sp))
 
 
 def last_surviving_units(store):

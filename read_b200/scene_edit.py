@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import ops
+from . import sprites
 from .texture import PointTexture
 
 
@@ -68,10 +69,12 @@ class SceneComposer:
         if n > ops.MAX_SEGMENTS:
             raise ValueError(f"read_b200: a composed scene holds at most {ops.MAX_SEGMENTS} segments (scenes + objects + instances)")
 
-    def add_scene(self, xyz, texture, placement=None):
+    def add_scene(self, xyz, texture, placement=None, point_sizes=None):
         """Add a cloud ``xyz`` [N,3] with its descriptors (``[1,8,N]`` tensor or ``PointTexture``) and an optional 4x4
-        ``placement`` into the composed world.  Returns the scene's handle; its points' global ids are ``handle.base + id``."""
+        ``placement`` into the composed world.  Returns the scene's handle; its points' global ids are ``handle.base + id``.
+        ``point_sizes``: optional [N] per-point sprite sizes (read_b200.sprites), shared by the scene's objects and instances."""
         n = int(xyz.shape[0])
+        sizes = None if point_sizes is None else sprites.check_point_sizes(point_sizes, n)
         if self.total + n >= 1 << 31:
             raise ValueError(f"read_b200: a composed scene of {self.total + n} points is too large; point ids must stay below 2^31")
         activation = texture.activation if isinstance(texture, PointTexture) else 'none'
@@ -92,7 +95,8 @@ class SceneComposer:
         self._activation = activation
         h = _Handle("scene", len(self._scenes))
         h.base = self.total
-        self._scenes.append(dict(xyz=xyz.to(self.device).contiguous(), base=self.total, n=n, P=P, visible=True, objects=[]))
+        self._scenes.append(dict(xyz=xyz.to(self.device).contiguous(), base=self.total, n=n, P=P, visible=True, objects=[],
+                                 sizes=None if sizes is None else sizes.to(self.device)))
         self._scene_P = np.concatenate([self._scene_P, P[None]])
         self._scene_vis = np.append(self._scene_vis, True)
         self.total += n
@@ -212,7 +216,7 @@ class SceneComposer:
             static = torch.nonzero(keep).reshape(-1)
             for ids in [static] + [self._objects[o]["ids"] for o in sc["objects"]]:
                 dev_ids = ids.to(self.device)
-                parts.append((sc["xyz"][dev_ids], dev_ids + sc["base"]))
+                parts.append((sc["xyz"][dev_ids], dev_ids + sc["base"], None if sc["sizes"] is None else sc["sizes"][dev_ids]))
             segments.append(len(parts) - 1 - len(sc["objects"]))
             self._segments.append((_Handle("scene", si), si))
             for j, o in enumerate(sc["objects"]):

@@ -11,6 +11,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from . import sprites
 from .compose import NetAndTexture
 from .texture import PointTexture
 from .unet import UNet
@@ -18,12 +19,15 @@ from .unet import UNet
 
 class FrameRenderer:
     def __init__(self, xyz, net_state_dict, texture, viewport_size, supersampling=1, temporal_average=False,
-                 device=None, flip_vertical=False, n_levels=4, return_net_input=True):
+                 device=None, flip_vertical=False, n_levels=4, return_net_input=True, input_format=None, point_sizes=None):
         """xyz: [N,3] float32 (numpy / tensor); net_state_dict: UNet checkpoint ``state_dict``; texture: the
         ``[1,8,N]`` descriptor tensor (``PointTexture.texture_``) or a ``PointTexture``; viewport_size: (W, H) of the output
         frame.  ``supersampling`` / ``temporal_average``: the options of READ/gl/nn.py:76,100-103 (the pyramid is rendered at
         ss x the viewport and reduced bilinearly; every level is averaged with the previous frame's input), served on the fused
-        path.  ``return_net_input=False`` skips materialising the reference's ``net_input`` list (4 small transposes)."""
+        path.  ``return_net_input=False`` skips materialising the reference's ``net_input`` list (4 small transposes).
+        ``input_format``: the checkpoint's format string (``args.input_format``); its first ``n_levels`` keys' ``_pN`` / ``_psN``
+        point sizes are drawn as point sprites (read_b200.sprites).  ``point_sizes``: optional [N] per-point sizes (the scene's
+        ``point_sizes``), which replace the keys' sizes where > 0; without ``input_format`` every level is a ``_p1`` key."""
         W, H = int(viewport_size[0]), int(viewport_size[1])
         factor = 16
         assert W % 16 == 0, f'set width {factor * (W // factor)}'          # READ/gl/nn.py:107-109
@@ -38,7 +42,13 @@ class FrameRenderer:
         # scene load: spatially sorted device store (original ids travel with the points), see ops.SortedPoints
         ss = int(supersampling)
         nested = L.load().read_raster_direct_mask(W * ss, H * ss, n_levels) == 1   # every level exactly half of the previous one
-        self.store = ops.SortedPoints(self.xyz) if nested else None
+        if point_sizes is not None and input_format is None:
+            input_format = ','.join(['uv_1d'] * n_levels)
+        self.input_format = input_format
+        levels = None if input_format is None else sprites.sprite_levels(input_format, n_levels)
+        sprite = levels is not None and not sprites.one_pixel(levels, point_sizes)
+        # point sprites are drawn from the sorted store whatever the level sizes
+        self.store = ops.SortedPoints(self.xyz, point_sizes=point_sizes) if nested or sprite else None
         net = UNet()
         net.load_state_dict(net_state_dict, strict=True)
         if not isinstance(texture, PointTexture):
@@ -92,7 +102,8 @@ class FrameRenderer:
         m = self._upload_camera(self.total_matrix(proj_matrix, view_matrix))
         with torch.no_grad():
             res = self.model.render(self.store if self.store is not None else self.xyz, m, self.W, self.H,
-                                    n_levels=self.n_levels, return_input=self.return_net_input, clone_output=False)
+                                    n_levels=self.n_levels, return_input=self.return_net_input, clone_output=False,
+                                    input_format=self.input_format)
         out, net_input = res if self.return_net_input else (res, None)                       # out: [1,3,H,W] f32
         rgba = torch.empty((self.H, self.W, 4), dtype=torch.float32, device=self.device)
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
@@ -107,7 +118,9 @@ class SceneRenderer:
     object or instance added) re-sorts the points once, a transform or visibility change moves no point data."""
 
     def __init__(self, composer, net_state_dict, viewport_size, supersampling=1, temporal_average=False, flip_vertical=False,
-                 return_net_input=True, n_levels=4):
+                 return_net_input=True, n_levels=4, input_format=None):
+        """``input_format``: the checkpoint's format string, as for FrameRenderer; the scenes' ``point_sizes`` (SceneComposer.add_scene)
+        apply with it.  Point-sprite frames need not have nested levels."""
         W, H = int(viewport_size[0]), int(viewport_size[1])
         assert W % 16 == 0, f'set width {16 * (W // 16)}'
         assert H % 16 == 0, f'set height {16 * (H // 16)}'
@@ -115,7 +128,9 @@ class SceneRenderer:
         self.device = composer.device
         L.require_device(self.device.index)
         ss = int(supersampling)
-        if L.load().read_raster_direct_mask(W * ss, H * ss, n_levels) != 1:
+        self.input_format = input_format
+        levels = None if input_format is None else sprites.sprite_levels(input_format, n_levels)
+        if (levels is None or sprites.one_pixel(levels)) and L.load().read_raster_direct_mask(W * ss, H * ss, n_levels) != 1:
             raise ValueError("read_b200: a composed scene renders frames whose pyramid levels nest (each exactly half of the last)")
         self.composer = composer
         self.W, self.H, self.n_levels = W, H, n_levels
@@ -162,7 +177,7 @@ class SceneRenderer:
                                       store.visible_flags())
         with torch.no_grad():
             res = self.model.render(store, seg_m, self.W, self.H, n_levels=self.n_levels, return_input=self.return_net_input,
-                                    clone_output=False, seg_visible=visible)
+                                    clone_output=False, seg_visible=visible, input_format=self.input_format)
         out, net_input = res if self.return_net_input else (res, None)
         rgba = torch.empty((self.H, self.W, 4), dtype=torch.float32, device=self.device)
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
