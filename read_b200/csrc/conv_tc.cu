@@ -581,6 +581,215 @@ gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant
     if (issuer) bulk_wait_group<0>();
 }
 
+// ------------------------------------------------------------------ weight-stationary body: 3x3 stride-1, 64 -> 64 channels
+// The same role swap at 64 channels: D[128 weight rows = 64 conv_f + 64 conv_m][128 pixels] += W[128, K = 9 taps x 64] X[128, K].
+// The weights (144 KB) no longer fit in registers, so they are wgmma's SHARED-MEMORY A operand, resident for the CTA's life.
+//   A rows      the producer loads each tap's packed [128 rows: f0..63, m0..63][64 K] tile as sixteen 8-row boxes (one 1 KB
+//               128-byte-swizzle atom each) and lays them out f-group g, m-group g, f-group g + 1, ...: warpgroup h's 64 rows of a
+//               tap are the 8 KB at h * 8 KB, and warp w's 16 rows are conv_f then conv_m of channels 32h + 8w .. + 7, so each
+//               thread holds both gates of one channel for 32 pixels as in the 32-channel body.  The packing is unchanged.
+//   B (pixels)  the 32-channel body's unswizzled halo tile with eight 8-channel chunks (23 KB per stage); K step kk starts at
+//               chunk 2 kk, tap (ky, kx) adds ky * row + kx * 16 B.
+//   overlap     both warpgroups work on the same tile (warpgroup h: output channels 32h .. 32h + 31, 36 m64n128k16 per tile)
+//               and each keeps TWO accumulator sets: tile t's epilogue runs under tile t + 1's MMAs.  Those are issued in four
+//               groups between the epilogue's four 4-row blocks: issued as one batch of 36, they held the warps back until
+//               most of them had run (0.143 ms per layer against 0.113 ms interleaved, H100 80GB HBM3 at 700 W).  The tile
+//               loop is unrolled by two so the set of each tile is known at compile time.
+//   epilogue    as in the 32-channel body; warpgroup h owns the [128 px][32 ch] 64-byte-swizzled block h of the epilogue stage
+//               and stores it with its own TMA store.
+// Shared memory: 144 KB weights + 2 halo stages + 2 epilogue stages of 16 KB + barriers and parameters, one CTA per SM.
+constexpr uint32_t WS64_TAP_BYTES = 128u * 64u * 2u;     // one tap's packed weight tile
+constexpr uint32_t WS64_BLOCK_BYTES = 128u * 32u * 2u;   // one warpgroup's 32-channel block of an epilogue stage
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
+{
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t smem_base = (s_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t *smem_al = smem_raw + (smem_base - s_u32(smem_raw));
+
+    const uint32_t b_region = smem_base + a.b_region_off;
+    const uint32_t e_region = smem_base + a.e_region_off;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + TC_E_STAGES * a.e_bytes);
+    const uint32_t bar0 = s_u32(bars);
+    const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
+    const uint32_t efull0 = bar0 + 8 * BAR_EFULL, eempty0 = bar0 + 8 * BAR_EEMPTY;
+    float4 *s_par = reinterpret_cast<float4 *>(bars + BAR_PARAMS);
+
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    if (a.pdl) pdl_launch_dependents();
+    for (int i = threadIdx.x; i < a.Cout; i += TC_THREADS) s_par[i] = make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]);
+    if (warp == TC_PRODUCER_WARP && lane == 0) {
+        tma_prefetch_desc(&tm.a[0]);
+        tma_prefetch_desc(&tmB);
+        if (a.epi.residual) tma_prefetch_desc(&tm.res);
+        for (int s = 0; s < a.a_stages; ++s) {
+            mbar_init(afull0 + 8 * s, 1);
+            mbar_init(aempty0 + 8 * s, TC_CONSUMER_WARPS);
+        }
+        for (int s = 0; s < TC_E_STAGES; ++s) {
+            mbar_init(efull0 + 8 * s, 1);
+            mbar_init(eempty0 + 8 * s, 2);          // one arrival per consumer warpgroup
+        }
+        mbar_init(bres, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    const int total_tiles = a.tiles_x * a.tiles_y * a.B;   // one n-tile
+
+    if (warp == TC_PRODUCER_WARP) {
+        if (elect_one()) {
+            mbar_arrive_expect_tx(bres, 9u * WS64_TAP_BYTES);
+            for (int tap = 0; tap < 9; ++tap)
+                for (int g = 0; g < 8; ++g) {
+                    const uint32_t dst = b_region + (uint32_t)tap * WS64_TAP_BYTES + (uint32_t)g * 2048u;
+                    tma_load_2d(&tmB, bres, dst, 0, tap * 128 + 8 * g);                // conv_f channels 8g .. 8g + 7
+                    tma_load_2d(&tmB, bres, dst + 1024u, 0, tap * 128 + 64 + 8 * g);   // conv_m, the same channels
+                }
+        }
+        __syncwarp();
+        if (a.pdl) pdl_wait();
+        uint32_t as = 0, aph = 0, es = 0, eph = 0;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+            const TileCoord tc_ = decode_tile(t, a);
+            const int x0 = tc_.tx * TC_TW, y0 = tc_.ty * TC_TH;
+            mbar_wait(aempty0 + 8 * as, aph ^ 1u);
+            if (elect_one()) {
+                const uint32_t full = afull0 + 8 * as, dst = smem_base + as * a.a_bytes;
+                mbar_arrive_expect_tx(full, a.a_tx_bytes);
+#pragma unroll
+                for (int c = 0; c < 8; ++c) tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, x0 - 1, y0 - 1, tc_.b);
+            }
+            __syncwarp();
+            if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
+            mbar_wait(eempty0 + 8 * es, eph ^ 1u);
+            if (elect_one()) {
+                const uint32_t full = efull0 + 8 * es, dst = e_region + es * a.e_bytes;
+                mbar_arrive_expect_tx(full, a.e_tx_bytes);          // a plain arrival without a residual
+                if (a.epi.residual) {
+                    tma_load_4d(&tm.res, full, dst, 0, x0, y0, tc_.b);
+                    tma_load_4d(&tm.res, full, dst + WS64_BLOCK_BYTES, 32, x0, y0, tc_.b);
+                }
+            }
+            __syncwarp();
+            if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
+        }
+        return;
+    }
+
+    const int wg = warp >> 2, wiw = warp & 3;
+    if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
+    mbar_wait(bres, 0);
+    const float4 par = s_par[32 * wg + 8 * wiw + (lane >> 2)];
+    // this lane's ldmatrix / stmatrix row in the warpgroup's block: pixel lane & 7 of tile row lane >> 3 (+ 4 per block),
+    // channels 8 wiw ..
+    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
+    const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
+    int e_pend = -1;
+    uint32_t as = 0, aph = 0, es = 0, eph = 0;       // halo and epilogue stages of tile t
+
+    // The MMAs of taps [tap0, tap1) of one tile, committed as one group.  The weight rows' base (this warpgroup's 64 rows of tap
+    // 0) comes through a shuffle of wg: warp-uniform to the compiler, so the descriptors live in uniform registers (otherwise
+    // ptxas serialises every wgmma), and computed per call, so the compiler does not hoist 36 loop-invariant descriptors out of
+    // the tile loop and spill them.
+    auto mma_taps = [&](float (&acc)[64], uint32_t stage, int tap0, int tap1) {
+        const uint32_t w_base = b_region + (uint32_t)__shfl_sync(0xffffffffu, wg, 0) * 8192u;
+        wgmma_fence();
+#pragma unroll
+        for (int tap = tap0; tap < tap1; ++tap)
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+                wgmma_ss_m64n128k16(acc, wgmma_desc(w_base + (uint32_t)tap * WS64_TAP_BYTES + 32u * kk, 128u),
+                                    wgmma_desc_noswz(stage + (uint32_t)(tap / 3) * WS_ROW_BYTES + (uint32_t)(tap % 3) * 16u +
+                                                         2u * kk * WS_CHUNK_BYTES,
+                                                     WS_CHUNK_BYTES, WS_ROW_BYTES),
+                                    1u);
+        wgmma_commit();
+    };
+    auto zero = [](float (&acc)[64]) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    };
+    // tile t's MMAs (into cur) are in flight: issue tile t + gridDim.x's into nxt and run tile t's epilogue under them.  The
+    // next tile's MMAs go out in four groups (taps 0-2, 3-4, 5-6, 7-8) between the epilogue's four 4-row blocks, so the epilogue
+    // does not wait behind the issue of all 36.
+    int t = blockIdx.x;
+    auto step = [&](float (&cur)[64], float (&nxt)[64]) {
+        const int tn = t + (int)gridDim.x;
+        uint32_t as_n = as + 1u, aph_n = aph;
+        if (as_n == (uint32_t)a.a_stages) { as_n = 0; aph_n ^= 1u; }
+        const uint32_t stage_n = smem_base + as_n * a.a_bytes;
+        if (tn < total_tiles) {
+            mbar_wait(afull0 + 8 * as_n, aph_n);
+            zero(nxt);
+            mma_taps(nxt, stage_n, 0, 3);
+        }
+        if (issuer && e_pend >= 0) {     // the previous tile's store has read its stage: the producer may refill it
+            bulk_wait_group_read<0>();
+            mbar_arrive(eempty0 + 8 * e_pend);
+        }
+        if (tn < total_tiles) wgmma_wait<1>();      // tile t's MMAs have retired
+        else wgmma_wait<0>();
+        wgmma_fence_acc(cur);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(aempty0 + 8 * as);
+        as = as_n;
+        aph = aph_n;
+
+        mbar_wait(efull0 + 8 * es, eph);
+        const uint32_t st = e_region + es * a.e_bytes + (uint32_t)wg * WS64_BLOCK_BYTES;
+#pragma unroll
+        for (int j0 = 0; j0 < TC_TH; j0 += 4) {
+            const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
+            uint32_t rv[4] = {0u, 0u, 0u, 0u};
+            if (a.epi.residual) ldmatrix_x4_trans(addr, rv);
+            uint32_t ov[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int j = j0 + i;
+                const float f0 = cur[4 * j] + par.x, f1 = cur[4 * j + 1] + par.x;
+                const float m0 = cur[4 * j + 2] + par.y, m1 = cur[4 * j + 3] + par.y;
+                float y0, y1;
+                if (a.epi.elu) {
+                    y0 = gate_fast<true>(f0, m0, par.z, par.w);
+                    y1 = gate_fast<true>(f1, m1, par.z, par.w);
+                } else {
+                    y0 = gate_fast<false>(f0, m0, par.z, par.w);
+                    y1 = gate_fast<false>(f1, m1, par.z, par.w);
+                }
+                const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
+                ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
+            }
+            stmatrix_x4_trans(addr, ov);
+            if (j0 < TC_TH - 4 && tn < total_tiles) mma_taps(nxt, stage_n, 3 + j0 / 2, 5 + j0 / 2);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(1 + wg, 128);
+        if (issuer) {
+            const TileCoord tc_ = decode_tile(t, a);
+            tma_store_4d(&tm.out, st, 32 * wg, tc_.tx * TC_TW, tc_.ty * TC_TH, tc_.b);    // clipped at the image edge
+            bulk_commit_group();
+        }
+        e_pend = (int)es;
+        if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
+        t = tn;
+        return t < total_tiles;
+    };
+
+    float acc0[64], acc1[64];
+    if (t < total_tiles) {
+        mbar_wait(afull0, 0);
+        zero(acc0);
+        mma_taps(acc0, smem_base, 0, 9);
+        while (step(acc0, acc1) && step(acc1, acc0)) {
+        }
+        wgmma_wait<0>();
+    }
+    if (issuer) bulk_wait_group<0>();
+}
+
 // ------------------------------------------------------------------ weight packing
 // out[((tap*kchunks + kc) * n_total + n) * cin_blk + kk],  n -> (tile nt, f|m half, channel)
 __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int cout_pad, int Cin,
@@ -754,14 +963,16 @@ struct TcPlan {
     TcArgs args;
     size_t smem_bytes;
     int reverse;
-    int ws;                                // runs gated_conv_tc_ws_kernel (tc_ws_layer)
+    int ws;                                // 0, or the channel count of a weight-stationary layer (tc_ws_layer): 32 runs
+                                           // gated_conv_tc_ws_kernel, 64 gated_conv_tc_ws64_kernel
 };
 
-// The layers of the weight-stationary body: 3x3 stride-1 32 -> 32 gated convs with an NHWC output and at most a residual
+// The layers of the weight-stationary bodies: 3x3 stride-1 C -> C gated convs, C = 32 or 64, with an NHWC output and at most
+// a residual
 static bool tc_ws_layer(const read_conv_desc &d)
 {
-    return d.k == 3 && d.stride == 1 && d.Cin == 32 && d.Cout == 32 && d.n_src == 1 && d.out_mode == READ_OUT_NHWC &&
-           d.out2 == nullptr && d.addin == nullptr;
+    return d.k == 3 && d.stride == 1 && (d.Cin == 32 || d.Cin == 64) && d.Cout == d.Cin && d.n_src == 1 &&
+           d.out_mode == READ_OUT_NHWC && d.out2 == nullptr && d.addin == nullptr;
 }
 
 int tc_plan_create(const read_conv_desc &d, TcPlan **out)
@@ -788,7 +999,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     RB_CHECK_ARG(p != nullptr, "wgmma conv: out of host memory");
 
     const bool s2 = d.stride == 2;
-    p->ws = tc_ws_layer(d) ? 1 : 0;
+    p->ws = tc_ws_layer(d) ? d.Cin : 0;
     const int halo_rows = s2 ? TC_TH + 1 : TC_TH + d.k - 1;
     const int halo_w = s2 ? TC_TW + 1 : TC_TW + d.k - 1;
     const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
@@ -817,7 +1028,8 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         const cuuint64_t rows = (cuuint64_t)d.k * d.k * g.kchunks * 2 * g.cout_pad;
         cuuint64_t dims[2] = {(cuuint64_t)g.cin_blk, rows};
         cuuint64_t strides[1] = {(cuuint64_t)g.cin_blk * 2};
-        cuuint32_t box[2] = {(cuuint32_t)g.cin_blk, (cuuint32_t)g.n_tile};
+        // (the 64-channel weight-stationary body loads 8-row boxes, one swizzle atom each, to interleave conv_f and conv_m)
+        cuuint32_t box[2] = {(cuuint32_t)g.cin_blk, (cuuint32_t)(p->ws == 64 ? 8 : g.n_tile)};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&p->tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(d.w_tc), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -844,14 +1056,15 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     const int half = g.n_tile / 2;
     if (!nchw) {
         const int oc = raw ? g.n_tile : half;             // channels of one output pixel in the tile
-        const int ocb = oc < 64 ? oc : 64, acb = g.n_tile < 64 ? g.n_tile : 64;
-        // stored per warpgroup (8 rows), or per tile by the weight-stationary body
+        // the 64-channel weight-stationary body loads and stores one 32-channel block per warpgroup
+        const int ocb = p->ws == 64 ? 32 : (oc < 64 ? oc : 64), acb = g.n_tile < 64 ? g.n_tile : 64;
+        // stored per warpgroup (8 rows), or per tile by the weight-stationary bodies
         bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, p->ws ? TC_TH : TC_TH / 2, "out");
         if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
         if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
         if (ok && d.residual)
             ok = raw ? enc_epi(&p->tmA.res, d.residual, 2 * d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH, "residual")
-                     : enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "residual");
+                     : enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, p->ws == 64 ? 32 : half, TC_TW, TC_TH, "residual");
         if (ok && d.addin) ok = enc_epi(&p->tmA.add, d.addin, g.n_tile, d.addin_W, d.addin_H, acb, TC_TW / 2, TC_TH / 2, "addin");
         if (!ok) {
             delete p;
@@ -883,7 +1096,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         }
     }
     a.a_tx_bytes = (uint32_t)halo_rows * halo_w * g.cin_blk * 2u;
-    a.tile_bytes = ((p->ws ? 4u * WS_CHUNK_BYTES : a.a_tx_bytes) + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
+    a.tile_bytes = ((p->ws ? (uint32_t)(p->ws / 8) * WS_CHUNK_BYTES : a.a_tx_bytes) + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
@@ -897,9 +1110,9 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         a.e_bytes = out_b + out2_b + add_b;
         a.e_tx_bytes = (d.residual ? out_b : 0u) + out2_b + add_b;
     }
-    const uint32_t e_ring = (p->ws ? WS_E_STAGES : TC_E_STAGES) * a.e_bytes;
+    const uint32_t e_ring = (p->ws == 32 ? WS_E_STAGES : TC_E_STAGES) * a.e_bytes;
     // the rings get what a CTA may have minus the alignment pad, barriers and per-channel parameters (smem_bytes below)
-    const uint32_t fixed = 1024 + 8 * (p->ws ? WS_BAR_PARAMS : BAR_PARAMS) + 16 * (uint32_t)g.cout_pad + 64;
+    const uint32_t fixed = 1024 + 8 * (p->ws == 32 ? WS_BAR_PARAMS : BAR_PARAMS) + 16 * (uint32_t)g.cout_pad + 64;
     const uint32_t budget_2 = TC_SMEM_PER_SM / 2 - 1024 - fixed, budget_1 = TC_SMEM_PER_CTA - fixed;
     // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights, the epilogue ring and >= 3 A
     // stages in half of the SM
@@ -925,8 +1138,11 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         a.b_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
     }
-    if (p->ws && (!a.b_resident || a.a_stages < 2)) {      // cannot happen at 32 channels; the kernel relies on both
-        set_error("wgmma conv: weight-stationary layer without resident weights or two A stages");
+    // the weight-stationary bodies rely on both.  At 64 channels: 144 KB of weights, two 23 KB halo stages, two 16 KB epilogue
+    // stages and about 2.7 KB of alignment pad, barriers and parameters, 224.7 KB of the 227 KB a CTA may have
+    if (p->ws && (!a.b_resident || a.a_stages < 2)) {
+        set_error("wgmma conv: weight-stationary layer without resident weights or two A stages (%u B of shared memory needed)",
+                  total_b + e_ring + 2 * a.a_bytes + fixed);
         delete p;
         return READ_ERR_UNSUPPORTED;
     }
@@ -987,6 +1203,13 @@ static int launch_tc_ws(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lc
     return READ_OK;
 }
 
+static int launch_tc_ws64(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
+{
+    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_ws64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
+    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_ws64_kernel, p->tmA, p->tmB, a));
+    return READ_OK;
+}
+
 int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
 {
     TcArgs a = p->args;
@@ -1010,7 +1233,8 @@ int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
     lcfg.attrs = lattr;
     lcfg.numAttrs = a.pdl ? 1 : 0;
     int rc;
-    if (p->ws) rc = launch_tc_ws(p, a, lcfg);
+    if (p->ws == 32) rc = launch_tc_ws(p, a, lcfg);
+    else if (p->ws == 64) rc = launch_tc_ws64(p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 3) rc = launch_tc_kn<3, 1>(p, a, lcfg);
     else if (a.stride == 2 && a.ksize == 3) rc = launch_tc_kn<3, 2>(p, a, lcfg);
