@@ -45,10 +45,12 @@ constexpr int TC_MAX_STAGES = 16;
 constexpr uint32_t TC_SMEM_PER_CTA = 227 * 1024, TC_SMEM_PER_SM = 228 * 1024;
 __host__ __device__ constexpr int tc_ctas_per_sm(int n_tile) { return n_tile <= 64 ? 2 : 1; }
 constexpr uint32_t TC_RESIDENT_MAX = 144 * 1024;
-// barrier slots (uint64 each)
 constexpr int TC_E_STAGES = 2;                 // epilogue stages
-constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_BRES = 64, BAR_EFULL = 66,
-              BAR_EEMPTY = BAR_EFULL + TC_E_STAGES, BAR_PARAMS = BAR_EEMPTY + TC_E_STAGES;
+// barrier slots (uint64 each): the A and B rings and the resident weights, then the full and empty barriers of a body's
+// e_stages epilogue stages; the per-channel parameters follow the barriers
+constexpr int BAR_AFULL = 0, BAR_AEMPTY = 16, BAR_BFULL = 32, BAR_BEMPTY = 48, BAR_BRES = 64;
+struct TcBarSlots { int efull, eempty, params; };
+__host__ __device__ constexpr TcBarSlots tc_bar_slots(int e_stages) { return {BAR_BRES + 2, BAR_BRES + 2 + e_stages, BAR_BRES + 2 + 2 * e_stages}; }
 constexpr uint32_t TC_CONSUMER_WARPS = 8;
 
 // activation tensor maps: one per source of a virtual concat (1x1 convs: torch.cat along channels, unet.py:88,105,263;
@@ -99,6 +101,15 @@ __device__ __forceinline__ TileCoord decode_tile(int t, const TcArgs &a)
     c.ty = m % a.tiles_y;
     c.b = m / a.tiles_y;
     return c;
+}
+
+// The issuer releases the epilogue stage e_pend once its previous TMA store has read it: the producer may refill it
+__device__ __forceinline__ void release_epilogue_stage(bool issuer, int e_pend, uint32_t eempty0)
+{
+    if (issuer && e_pend >= 0) {
+        bulk_wait_group_read<0>();
+        mbar_arrive(eempty0 + 8 * e_pend);
+    }
 }
 
 // Byte offset of channel c of pixel p in an epilogue region of P pixels: blocks of CB channels, each P rows of 2*CB bytes with
@@ -186,14 +197,15 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
     uint8_t *smem_al = smem_raw + (smem_base - s_u32(smem_raw));
 
     constexpr int ntaps = KS * KS;
+    constexpr TcBarSlots e_bars = tc_bar_slots(TC_E_STAGES);
     const uint32_t b_region = smem_base + a.b_region_off;
     const uint32_t e_region = smem_base + a.e_region_off;
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + TC_E_STAGES * a.e_bytes);
     const uint32_t bar0 = s_u32(bars);
     const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY;
     const uint32_t bfull0 = bar0 + 8 * BAR_BFULL, bempty0 = bar0 + 8 * BAR_BEMPTY, bres = bar0 + 8 * BAR_BRES;
-    const uint32_t efull0 = bar0 + 8 * BAR_EFULL, eempty0 = bar0 + 8 * BAR_EEMPTY;
-    float4 *s_par = reinterpret_cast<float4 *>(bars + BAR_PARAMS);
+    const uint32_t efull0 = bar0 + 8 * e_bars.efull, eempty0 = bar0 + 8 * e_bars.eempty;
+    float4 *s_par = reinterpret_cast<float4 *>(bars + e_bars.params);
 
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -375,10 +387,7 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
             const bool in[2] = {x0 < a.W && y0 < a.H, x0 < a.W && y0 + 1 < a.H};
             epilogue_tile<N>(acc, lane, tc_.b, ys, xs, in, tc_.nt, e);
         } else {
-            if (issuer && e_pend >= 0) {
-                bulk_wait_group_read<0>();
-                mbar_arrive(eempty0 + 8 * e_pend);
-            }
+            release_epilogue_stage(issuer, e_pend, eempty0);
             mbar_wait(efull0 + 8 * es, eph);
             epilogue_smem<N>(acc, smem_al + a.e_region_off + es * a.e_bytes, lane, 8 * wg + 2 * wiw, tc_.nt, s_par, a);
             fence_proxy_async_smem();
@@ -416,89 +425,174 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
 //   A rows      the ldmatrix row addresses pick the packed weight rows so that warp w's rows 0..7 are conv_f and rows 8..15
 //               conv_m of the SAME channels 8w .. 8w+7: each thread then holds both gates of one channel for 32 pixels (tile
 //               row j = accumulator group j, pixels 2 (l & 3), + 1), and the weight packing is the other body's.
-//   epilogue    epilogue_smem's arithmetic per element; the residual comes in with ldmatrix.trans and the output goes back with
-//               stmatrix.trans (8 channels x 8 pixels per block) into the 64-byte-swizzled NHWC stage, stored by one TMA.
+//   epilogue    ws_epilogue_rows: epilogue_smem's arithmetic per element; the residual comes in with ldmatrix.trans and the
+//               output goes back with stmatrix.trans (8 channels x 8 pixels per block) into the 64-byte-swizzled NHWC stage,
+//               stored by one TMA (ws_store_block).
 // Warp roles: the producer warp as above; each consumer warpgroup takes whole tiles (the CTA's even / odd ones), so one
 // warpgroup's epilogue runs under the other's MMAs.  One CTA per SM (72 + 64 registers per thread are live across the MMAs).
 constexpr int WS_E_STAGES = 4;                 // two per consumer warpgroup: tile k uses stage k % 4
-constexpr int WS_BAR_EFULL = BAR_BRES + 2, WS_BAR_EEMPTY = WS_BAR_EFULL + WS_E_STAGES, WS_BAR_PARAMS = WS_BAR_EEMPTY + WS_E_STAGES;
 constexpr uint32_t WS_ROW_BYTES = (TC_TW + 2) * 16u;                  // one halo row of one 8-channel chunk
 constexpr uint32_t WS_CHUNK_BYTES = ((TC_TH + 2) * WS_ROW_BYTES + 127u) & ~127u;   // TMA destinations are 128 B aligned
+constexpr uint32_t WS_BLOCK_BYTES = 128u * 32u * 2u;   // one 32-channel block of an epilogue stage
+
+// The shared memory of a weight-stationary body with E epilogue stages, from its 1 KB aligned base (offsets and sizes:
+// tc_plan_create): halo ring | resident weights | epilogue ring | barriers | per-channel parameters
+template <int E>
+struct WsSmem {
+    uint32_t base, b_region, e_region;
+    uint32_t afull0, aempty0, bres, efull0, eempty0;
+    float4 *par;
+    __device__ __forceinline__ explicit WsSmem(const TcArgs &a)
+    {
+        extern __shared__ uint8_t smem_raw[];
+        base = (s_u32(smem_raw) + 1023u) & ~1023u;
+        b_region = base + a.b_region_off;
+        e_region = base + a.e_region_off;
+        uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (base - s_u32(smem_raw)) + a.e_region_off + E * a.e_bytes);
+        const uint32_t bar0 = s_u32(bars);
+        afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
+        efull0 = bar0 + 8 * tc_bar_slots(E).efull, eempty0 = bar0 + 8 * tc_bar_slots(E).eempty;
+        par = reinterpret_cast<float4 *>(bars + tc_bar_slots(E).params);
+    }
+};
+
+// Prologue of the weight-stationary bodies (C = 32 and 64 channels): per-channel parameters, descriptor prefetch, and
+// the barriers, with a_arrivals per halo stage (the warps that read it) and e_arrivals per epilogue stage (the warpgroups that
+// store from it).
+template <int E>
+__device__ __forceinline__ void ws_prologue(const WsSmem<E> &sm, const TcMaps &tm, const CUtensorMap &tmB, const TcArgs &a,
+                                            uint32_t a_arrivals, uint32_t e_arrivals)
+{
+    if (a.pdl) pdl_launch_dependents();
+    for (int i = threadIdx.x; i < a.Cout; i += TC_THREADS) sm.par[i] = make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]);
+    if (threadIdx.x == 32 * TC_PRODUCER_WARP) {
+        tma_prefetch_desc(&tm.a[0]);
+        tma_prefetch_desc(&tmB);
+        if (a.epi.residual) tma_prefetch_desc(&tm.res);
+        for (int s = 0; s < a.a_stages; ++s) {
+            mbar_init(sm.afull0 + 8 * s, 1);
+            mbar_init(sm.aempty0 + 8 * s, a_arrivals);
+        }
+        for (int s = 0; s < E; ++s) {
+            mbar_init(sm.efull0 + 8 * s, 1);
+            mbar_init(sm.eempty0 + 8 * s, e_arrivals);
+        }
+        mbar_init(sm.bres, 1);
+        mbar_fence_init();
+    }
+    __syncthreads();
+}
+
+// Producer: tile tc's halo into the next stage (as, aph) of the halo ring, as C / 8 unswizzled 8-channel chunks from pixel
+// (x0 - 1, y0 - 1)
+template <int C, int E>
+__device__ __forceinline__ void ws_load_halo(const WsSmem<E> &sm, const TcMaps &tm, const TcArgs &a, const TileCoord &tc,
+                                             uint32_t &as, uint32_t &aph)
+{
+    mbar_wait(sm.aempty0 + 8 * as, aph ^ 1u);
+    if (elect_one()) {
+        const uint32_t full = sm.afull0 + 8 * as, dst = sm.base + as * a.a_bytes;
+        mbar_arrive_expect_tx(full, a.a_tx_bytes);
+#pragma unroll
+        for (int c = 0; c < C / 8; ++c)
+            tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, tc.tx * TC_TW - 1, tc.ty * TC_TH - 1, tc.b);
+    }
+    __syncwarp();
+    if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
+}
+
+// Producer: tile tc's residual into the next epilogue stage (es, eph), as C / 32 boxes of 32 channels, block h at h * 8 KB; a
+// plain arrival without a residual
+template <int C, int E>
+__device__ __forceinline__ void ws_load_residual(const WsSmem<E> &sm, const TcMaps &tm, const TcArgs &a, const TileCoord &tc,
+                                                 uint32_t &es, uint32_t &eph)
+{
+    mbar_wait(sm.eempty0 + 8 * es, eph ^ 1u);
+    if (elect_one()) {
+        const uint32_t full = sm.efull0 + 8 * es, dst = sm.e_region + es * a.e_bytes;
+        mbar_arrive_expect_tx(full, a.e_tx_bytes);
+        if (a.epi.residual)
+#pragma unroll
+            for (int h = 0; h < C / 32; ++h)
+                tma_load_4d(&tm.res, full, dst + (uint32_t)h * WS_BLOCK_BYTES, 32 * h, tc.tx * TC_TW, tc.ty * TC_TH, tc.b);
+    }
+    __syncwarp();
+    if (++es == (uint32_t)E) { es = 0; eph ^= 1u; }
+}
+
+// Consumer: tile rows j0 .. j0 + 3 of the epilogue, in place in the warpgroup's 64-byte-swizzled [128 px][32 ch] block st of an
+// epilogue stage.  acc holds both gates of this thread's channel (parameters par) for two pixels of every tile row.  The
+// residual comes in with ldmatrix.trans, the arithmetic is epilogue_smem's per element, and the bf16 output goes back with
+// stmatrix.trans.
+__device__ __forceinline__ void ws_epilogue_rows(const float (&acc)[64], int j0, uint32_t st, float4 par, const EpiArgs &e)
+{
+    const int lane = threadIdx.x & 31, wiw = (threadIdx.x >> 5) & 3;
+    // this lane's ldmatrix / stmatrix row: pixel lane & 7 of tile row j0 + (lane >> 3), channels 8 wiw ..
+    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
+    const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
+    uint32_t rv[4] = {0u, 0u, 0u, 0u};
+    if (e.residual) ldmatrix_x4_trans(addr, rv);
+    uint32_t ov[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int j = j0 + i;
+        const float f0 = acc[4 * j] + par.x, f1 = acc[4 * j + 1] + par.x;
+        const float m0 = acc[4 * j + 2] + par.y, m1 = acc[4 * j + 3] + par.y;
+        float y0, y1;
+        if (e.elu) {
+            y0 = gate_fast<true>(f0, m0, par.z, par.w);
+            y1 = gate_fast<true>(f1, m1, par.z, par.w);
+        } else {
+            y0 = gate_fast<false>(f0, m0, par.z, par.w);
+            y1 = gate_fast<false>(f1, m1, par.z, par.w);
+        }
+        const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
+        ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
+    }
+    stmatrix_x4_trans(addr, ov);
+}
+
+// Consumer: the warpgroup's finished block st, output channels c0 .. c0 + 31 of tile t, made visible to the TMA unit and stored
+// by the issuer (the TMA unit clips the box at the image edge)
+__device__ __forceinline__ void ws_store_block(const TcMaps &tm, const TcArgs &a, uint32_t st, int c0, int t, int wg, bool issuer)
+{
+    fence_proxy_async_smem();
+    named_bar_sync(1 + wg, 128);
+    if (issuer) {
+        const TileCoord tc = decode_tile(t, a);
+        tma_store_4d(&tm.out, st, c0, tc.tx * TC_TW, tc.ty * TC_TH, tc.b);
+        bulk_commit_group();
+    }
+}
 
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
 {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (s_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t *smem_al = smem_raw + (smem_base - s_u32(smem_raw));
-
-    const uint32_t b_region = smem_base + a.b_region_off;
-    const uint32_t e_region = smem_base + a.e_region_off;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + WS_E_STAGES * a.e_bytes);
-    const uint32_t bar0 = s_u32(bars);
-    const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
-    const uint32_t efull0 = bar0 + 8 * WS_BAR_EFULL, eempty0 = bar0 + 8 * WS_BAR_EEMPTY;
-    float4 *s_par = reinterpret_cast<float4 *>(bars + WS_BAR_PARAMS);
-
+    const WsSmem<WS_E_STAGES> sm(a);
+    ws_prologue(sm, tm, tmB, a, 4, 1);      // a tile's halo and epilogue stages belong to the one warpgroup that takes it
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
-    if (a.pdl) pdl_launch_dependents();
-    for (int i = threadIdx.x; i < a.Cout; i += TC_THREADS) s_par[i] = make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]);
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        tma_prefetch_desc(&tm.a[0]);
-        tma_prefetch_desc(&tmB);
-        if (a.epi.residual) tma_prefetch_desc(&tm.res);
-        for (int s = 0; s < TC_MAX_STAGES; ++s) {
-            mbar_init(afull0 + 8 * s, 1);
-            mbar_init(aempty0 + 8 * s, 4);          // the four warps of the warpgroup that took the tile
-        }
-        for (int s = 0; s < WS_E_STAGES; ++s) {
-            mbar_init(efull0 + 8 * s, 1);
-            mbar_init(eempty0 + 8 * s, 1);
-        }
-        mbar_init(bres, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
-
     const int total_tiles = a.tiles_x * a.tiles_y * a.B;   // one n-tile
 
     if (warp == TC_PRODUCER_WARP) {
         if (elect_one()) {
-            mbar_arrive_expect_tx(bres, 9u * a.b_bytes);
-            for (int i = 0; i < 9; ++i) tma_load_2d(&tmB, bres, b_region + (uint32_t)i * a.b_bytes, 0, i * a.n_tile);
+            mbar_arrive_expect_tx(sm.bres, 9u * a.b_bytes);
+            for (int i = 0; i < 9; ++i) tma_load_2d(&tmB, sm.bres, sm.b_region + (uint32_t)i * a.b_bytes, 0, i * a.n_tile);
         }
         __syncwarp();
         if (a.pdl) pdl_wait();
-        uint32_t as = 0, aph = 0;
-        int k = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++k) {
+        uint32_t as = 0, aph = 0, es = 0, eph = 0;
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const TileCoord tc_ = decode_tile(t, a);
-            const int x0 = tc_.tx * TC_TW, y0 = tc_.ty * TC_TH;
-            mbar_wait(aempty0 + 8 * as, aph ^ 1u);
-            if (elect_one()) {
-                const uint32_t full = afull0 + 8 * as, dst = smem_base + as * a.a_bytes;
-                mbar_arrive_expect_tx(full, a.a_tx_bytes);
-#pragma unroll
-                for (int c = 0; c < 4; ++c) tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, x0 - 1, y0 - 1, tc_.b);
-            }
-            __syncwarp();
-            if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
-            const int es = k % WS_E_STAGES;
-            mbar_wait(eempty0 + 8 * es, ((uint32_t)(k / WS_E_STAGES) & 1u) ^ 1u);
-            if (elect_one()) {
-                const uint32_t full = efull0 + 8 * es;
-                mbar_arrive_expect_tx(full, a.e_tx_bytes);          // a plain arrival without a residual
-                if (a.epi.residual) tma_load_4d(&tm.res, full, e_region + es * a.e_bytes, 0, x0, y0, tc_.b);
-            }
-            __syncwarp();
+            ws_load_halo<32>(sm, tm, a, tc_, as, aph);
+            ws_load_residual<32>(sm, tm, a, tc_, es, eph);
         }
         return;
     }
 
     const int wg = warp >> 2, wiw = warp & 3;
     if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
-    mbar_wait(bres, 0);
+    mbar_wait(sm.bres, 0);
     uint32_t wa[9][2][4];
     {
         // packed row n: conv_f channel n (n < 32), conv_m channel n - 32; 64-byte swizzled rows of 32 channels
@@ -507,21 +601,18 @@ gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant
         for (int tap = 0; tap < 9; ++tap)
 #pragma unroll
             for (int kk = 0; kk < 2; ++kk)
-                ldmatrix_x4(b_region + (uint32_t)tap * a.b_bytes + swz(n * 64u + 32u * kk + 16u * (lane >> 4), 64u), wa[tap][kk]);
+                ldmatrix_x4(sm.b_region + (uint32_t)tap * a.b_bytes + swz(n * 64u + 32u * kk + 16u * (lane >> 4), 64u), wa[tap][kk]);
     }
-    const float4 par = s_par[8 * wiw + (lane >> 2)];
-    // this lane's ldmatrix / stmatrix row in the stage: pixel lane & 7 of tile row lane >> 3 (+ 4 per block), channels 8 wiw..
-    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
+    const float4 par = sm.par[8 * wiw + (lane >> 2)];
     const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
     int e_pend = -1;
     uint32_t as = (uint32_t)wg, aph = 0;            // a_stages >= 2
     for (int k = wg, t = blockIdx.x + wg * gridDim.x; t < total_tiles; k += 2, t += 2 * gridDim.x) {
-        const TileCoord tc_ = decode_tile(t, a);
         float acc[64];
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-        mbar_wait(afull0 + 8 * as, aph);
-        const uint32_t stage = smem_base + as * a.a_bytes;
+        mbar_wait(sm.afull0 + 8 * as, aph);
+        const uint32_t stage = sm.base + as * a.a_bytes;
         wgmma_fence();
 #pragma unroll
         for (int tap = 0; tap < 9; ++tap)
@@ -532,50 +623,20 @@ gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant
                                                  WS_CHUNK_BYTES, WS_ROW_BYTES),
                                 1u);
         wgmma_commit();
-        if (issuer && e_pend >= 0) {     // the previous tile's store has read its stage: the producer may refill it
-            bulk_wait_group_read<0>();
-            mbar_arrive(eempty0 + 8 * e_pend);
-        }
+        release_epilogue_stage(issuer, e_pend, sm.eempty0);
         wgmma_wait<0>();
         wgmma_fence_acc(acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(aempty0 + 8 * as);
+        if (lane == 0) mbar_arrive(sm.aempty0 + 8 * as);
         as += 2;
         if (as >= (uint32_t)a.a_stages) { as -= (uint32_t)a.a_stages; aph ^= 1u; }
 
         const int es = k % WS_E_STAGES;
-        mbar_wait(efull0 + 8 * es, (uint32_t)(k / WS_E_STAGES) & 1u);
-        const uint32_t st = e_region + es * a.e_bytes;
+        mbar_wait(sm.efull0 + 8 * es, (uint32_t)(k / WS_E_STAGES) & 1u);
+        const uint32_t st = sm.e_region + es * a.e_bytes;
 #pragma unroll
-        for (int j0 = 0; j0 < TC_TH; j0 += 4) {
-            const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
-            uint32_t rv[4] = {0u, 0u, 0u, 0u};
-            if (a.epi.residual) ldmatrix_x4_trans(addr, rv);
-            uint32_t ov[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int j = j0 + i;
-                const float f0 = acc[4 * j] + par.x, f1 = acc[4 * j + 1] + par.x;
-                const float m0 = acc[4 * j + 2] + par.y, m1 = acc[4 * j + 3] + par.y;
-                float y0, y1;
-                if (a.epi.elu) {
-                    y0 = gate_fast<true>(f0, m0, par.z, par.w);
-                    y1 = gate_fast<true>(f1, m1, par.z, par.w);
-                } else {
-                    y0 = gate_fast<false>(f0, m0, par.z, par.w);
-                    y1 = gate_fast<false>(f1, m1, par.z, par.w);
-                }
-                const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
-                ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
-            }
-            stmatrix_x4_trans(addr, ov);
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(1 + wg, 128);
-        if (issuer) {
-            tma_store_4d(&tm.out, st, 0, tc_.tx * TC_TW, tc_.ty * TC_TH, tc_.b);    // clipped at the image edge
-            bulk_commit_group();
-        }
+        for (int j0 = 0; j0 < TC_TH; j0 += 4) ws_epilogue_rows(acc, j0, st, par, a.epi);
+        ws_store_block(tm, a, st, 0, t, wg, issuer);
         e_pend = es;
     }
     if (issuer) bulk_wait_group<0>();
@@ -599,54 +660,24 @@ gated_conv_tc_ws_kernel(const __grid_constant__ TcMaps tm, const __grid_constant
 //               and stores it with its own TMA store.
 // Shared memory: 144 KB weights + 2 halo stages + 2 epilogue stages of 16 KB + barriers and parameters, one CTA per SM.
 constexpr uint32_t WS64_TAP_BYTES = 128u * 64u * 2u;     // one tap's packed weight tile
-constexpr uint32_t WS64_BLOCK_BYTES = 128u * 32u * 2u;   // one warpgroup's 32-channel block of an epilogue stage
 
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
 {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (s_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t *smem_al = smem_raw + (smem_base - s_u32(smem_raw));
-
-    const uint32_t b_region = smem_base + a.b_region_off;
-    const uint32_t e_region = smem_base + a.e_region_off;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_al + a.e_region_off + TC_E_STAGES * a.e_bytes);
-    const uint32_t bar0 = s_u32(bars);
-    const uint32_t afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
-    const uint32_t efull0 = bar0 + 8 * BAR_EFULL, eempty0 = bar0 + 8 * BAR_EEMPTY;
-    float4 *s_par = reinterpret_cast<float4 *>(bars + BAR_PARAMS);
-
+    const WsSmem<TC_E_STAGES> sm(a);
+    ws_prologue(sm, tm, tmB, a, TC_CONSUMER_WARPS, 2);      // both warpgroups read every halo stage and store from every epilogue stage
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
-    if (a.pdl) pdl_launch_dependents();
-    for (int i = threadIdx.x; i < a.Cout; i += TC_THREADS) s_par[i] = make_float4(a.bias_f[i], a.bias_m[i], a.scale[i], a.shift[i]);
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        tma_prefetch_desc(&tm.a[0]);
-        tma_prefetch_desc(&tmB);
-        if (a.epi.residual) tma_prefetch_desc(&tm.res);
-        for (int s = 0; s < a.a_stages; ++s) {
-            mbar_init(afull0 + 8 * s, 1);
-            mbar_init(aempty0 + 8 * s, TC_CONSUMER_WARPS);
-        }
-        for (int s = 0; s < TC_E_STAGES; ++s) {
-            mbar_init(efull0 + 8 * s, 1);
-            mbar_init(eempty0 + 8 * s, 2);          // one arrival per consumer warpgroup
-        }
-        mbar_init(bres, 1);
-        mbar_fence_init();
-    }
-    __syncthreads();
-
     const int total_tiles = a.tiles_x * a.tiles_y * a.B;   // one n-tile
 
     if (warp == TC_PRODUCER_WARP) {
         if (elect_one()) {
-            mbar_arrive_expect_tx(bres, 9u * WS64_TAP_BYTES);
+            mbar_arrive_expect_tx(sm.bres, 9u * WS64_TAP_BYTES);
             for (int tap = 0; tap < 9; ++tap)
                 for (int g = 0; g < 8; ++g) {
-                    const uint32_t dst = b_region + (uint32_t)tap * WS64_TAP_BYTES + (uint32_t)g * 2048u;
-                    tma_load_2d(&tmB, bres, dst, 0, tap * 128 + 8 * g);                // conv_f channels 8g .. 8g + 7
-                    tma_load_2d(&tmB, bres, dst + 1024u, 0, tap * 128 + 64 + 8 * g);   // conv_m, the same channels
+                    const uint32_t dst = sm.b_region + (uint32_t)tap * WS64_TAP_BYTES + (uint32_t)g * 2048u;
+                    tma_load_2d(&tmB, sm.bres, dst, 0, tap * 128 + 8 * g);                // conv_f channels 8g .. 8g + 7
+                    tma_load_2d(&tmB, sm.bres, dst + 1024u, 0, tap * 128 + 64 + 8 * g);   // conv_m, the same channels
                 }
         }
         __syncwarp();
@@ -654,38 +685,16 @@ gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_consta
         uint32_t as = 0, aph = 0, es = 0, eph = 0;
         for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
             const TileCoord tc_ = decode_tile(t, a);
-            const int x0 = tc_.tx * TC_TW, y0 = tc_.ty * TC_TH;
-            mbar_wait(aempty0 + 8 * as, aph ^ 1u);
-            if (elect_one()) {
-                const uint32_t full = afull0 + 8 * as, dst = smem_base + as * a.a_bytes;
-                mbar_arrive_expect_tx(full, a.a_tx_bytes);
-#pragma unroll
-                for (int c = 0; c < 8; ++c) tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, x0 - 1, y0 - 1, tc_.b);
-            }
-            __syncwarp();
-            if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
-            mbar_wait(eempty0 + 8 * es, eph ^ 1u);
-            if (elect_one()) {
-                const uint32_t full = efull0 + 8 * es, dst = e_region + es * a.e_bytes;
-                mbar_arrive_expect_tx(full, a.e_tx_bytes);          // a plain arrival without a residual
-                if (a.epi.residual) {
-                    tma_load_4d(&tm.res, full, dst, 0, x0, y0, tc_.b);
-                    tma_load_4d(&tm.res, full, dst + WS64_BLOCK_BYTES, 32, x0, y0, tc_.b);
-                }
-            }
-            __syncwarp();
-            if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
+            ws_load_halo<64>(sm, tm, a, tc_, as, aph);
+            ws_load_residual<64>(sm, tm, a, tc_, es, eph);
         }
         return;
     }
 
     const int wg = warp >> 2, wiw = warp & 3;
     if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
-    mbar_wait(bres, 0);
-    const float4 par = s_par[32 * wg + 8 * wiw + (lane >> 2)];
-    // this lane's ldmatrix / stmatrix row in the warpgroup's block: pixel lane & 7 of tile row lane >> 3 (+ 4 per block),
-    // channels 8 wiw ..
-    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
+    mbar_wait(sm.bres, 0);
+    const float4 par = sm.par[32 * wg + 8 * wiw + (lane >> 2)];
     const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
     int e_pend = -1;
     uint32_t as = 0, aph = 0, es = 0, eph = 0;       // halo and epilogue stages of tile t
@@ -695,7 +704,7 @@ gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_consta
     // ptxas serialises every wgmma), and computed per call, so the compiler does not hoist 36 loop-invariant descriptors out of
     // the tile loop and spill them.
     auto mma_taps = [&](float (&acc)[64], uint32_t stage, int tap0, int tap1) {
-        const uint32_t w_base = b_region + (uint32_t)__shfl_sync(0xffffffffu, wg, 0) * 8192u;
+        const uint32_t w_base = sm.b_region + (uint32_t)__shfl_sync(0xffffffffu, wg, 0) * 8192u;
         wgmma_fence();
 #pragma unroll
         for (int tap = tap0; tap < tap1; ++tap)
@@ -720,58 +729,29 @@ gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_consta
         const int tn = t + (int)gridDim.x;
         uint32_t as_n = as + 1u, aph_n = aph;
         if (as_n == (uint32_t)a.a_stages) { as_n = 0; aph_n ^= 1u; }
-        const uint32_t stage_n = smem_base + as_n * a.a_bytes;
+        const uint32_t stage_n = sm.base + as_n * a.a_bytes;
         if (tn < total_tiles) {
-            mbar_wait(afull0 + 8 * as_n, aph_n);
+            mbar_wait(sm.afull0 + 8 * as_n, aph_n);
             zero(nxt);
             mma_taps(nxt, stage_n, 0, 3);
         }
-        if (issuer && e_pend >= 0) {     // the previous tile's store has read its stage: the producer may refill it
-            bulk_wait_group_read<0>();
-            mbar_arrive(eempty0 + 8 * e_pend);
-        }
+        release_epilogue_stage(issuer, e_pend, sm.eempty0);
         if (tn < total_tiles) wgmma_wait<1>();      // tile t's MMAs have retired
         else wgmma_wait<0>();
         wgmma_fence_acc(cur);
         __syncwarp();
-        if (lane == 0) mbar_arrive(aempty0 + 8 * as);
+        if (lane == 0) mbar_arrive(sm.aempty0 + 8 * as);
         as = as_n;
         aph = aph_n;
 
-        mbar_wait(efull0 + 8 * es, eph);
-        const uint32_t st = e_region + es * a.e_bytes + (uint32_t)wg * WS64_BLOCK_BYTES;
+        mbar_wait(sm.efull0 + 8 * es, eph);
+        const uint32_t st = sm.e_region + es * a.e_bytes + (uint32_t)wg * WS_BLOCK_BYTES;
 #pragma unroll
         for (int j0 = 0; j0 < TC_TH; j0 += 4) {
-            const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
-            uint32_t rv[4] = {0u, 0u, 0u, 0u};
-            if (a.epi.residual) ldmatrix_x4_trans(addr, rv);
-            uint32_t ov[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int j = j0 + i;
-                const float f0 = cur[4 * j] + par.x, f1 = cur[4 * j + 1] + par.x;
-                const float m0 = cur[4 * j + 2] + par.y, m1 = cur[4 * j + 3] + par.y;
-                float y0, y1;
-                if (a.epi.elu) {
-                    y0 = gate_fast<true>(f0, m0, par.z, par.w);
-                    y1 = gate_fast<true>(f1, m1, par.z, par.w);
-                } else {
-                    y0 = gate_fast<false>(f0, m0, par.z, par.w);
-                    y1 = gate_fast<false>(f1, m1, par.z, par.w);
-                }
-                const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
-                ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
-            }
-            stmatrix_x4_trans(addr, ov);
+            ws_epilogue_rows(cur, j0, st, par, a.epi);
             if (j0 < TC_TH - 4 && tn < total_tiles) mma_taps(nxt, stage_n, 3 + j0 / 2, 5 + j0 / 2);
         }
-        fence_proxy_async_smem();
-        named_bar_sync(1 + wg, 128);
-        if (issuer) {
-            const TileCoord tc_ = decode_tile(t, a);
-            tma_store_4d(&tm.out, st, 32 * wg, tc_.tx * TC_TW, tc_.ty * TC_TH, tc_.b);    // clipped at the image edge
-            bulk_commit_group();
-        }
+        ws_store_block(tm, a, st, 32 * wg, t, wg, issuer);
         e_pend = (int)es;
         if (++es == (uint32_t)TC_E_STAGES) { es = 0; eph ^= 1u; }
         t = tn;
@@ -780,9 +760,9 @@ gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_consta
 
     float acc0[64], acc1[64];
     if (t < total_tiles) {
-        mbar_wait(afull0, 0);
+        mbar_wait(sm.afull0, 0);
         zero(acc0);
-        mma_taps(acc0, smem_base, 0, 9);
+        mma_taps(acc0, sm.base, 0, 9);
         while (step(acc0, acc1) && step(acc1, acc0)) {
         }
         wgmma_wait<0>();
@@ -975,6 +955,37 @@ static bool tc_ws_layer(const read_conv_desc &d)
            d.out_mode == READ_OUT_NHWC && d.out2 == nullptr && d.addin == nullptr;
 }
 
+// The plan values that depend on the kernel body, for a layer whose halo tile is a_tx_bytes and whose weights, like its
+// activations, have the swizzle sw of their K chunk.  The weight-stationary bodies read the halo as unswizzled 8-channel chunks
+// and load the residual and store the output as 32-channel blocks of whole tiles; the 64-channel body loads its weights as
+// 8-row boxes, one swizzle atom each, to interleave conv_f and conv_m.
+struct TcBodyLayout {
+    int ws;                                // TcPlan::ws
+    int halo_c;                            // channels of one halo box
+    CUtensorMapSwizzle halo_sw;
+    int w_rows;                            // rows of one weight box
+    int epi_c, out_rows;                   // channels of the output and residual boxes, rows of the output box
+    uint32_t tile_bytes;                   // TcArgs::tile_bytes
+    int e_stages;                          // epilogue stages
+};
+static TcBodyLayout tc_body_layout(const read_conv_desc &d, const TcGeom &g, uint32_t a_tx_bytes, CUtensorMapSwizzle sw)
+{
+    const int oc = d.out_mode == READ_OUT_RAW_NHWC ? g.n_tile : g.n_tile / 2;     // channels of one output pixel in the tile
+    TcBodyLayout L{0, g.cin_blk, sw, g.n_tile, oc < 64 ? oc : 64, TC_TH / 2, a_tx_bytes, TC_E_STAGES};
+    if (tc_ws_layer(d)) {
+        L.ws = d.Cin;
+        L.halo_c = 8;
+        L.halo_sw = CU_TENSOR_MAP_SWIZZLE_NONE;
+        if (d.Cin == 64) L.w_rows = 8;
+        L.epi_c = 32;
+        L.out_rows = TC_TH;
+        L.tile_bytes = (uint32_t)(d.Cin / 8) * WS_CHUNK_BYTES;
+        if (d.Cin == 32) L.e_stages = WS_E_STAGES;
+    }
+    L.tile_bytes = (L.tile_bytes + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
+    return L;
+}
+
 int tc_plan_create(const read_conv_desc &d, TcPlan **out)
 {
     TcGeom g;
@@ -999,11 +1010,13 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     RB_CHECK_ARG(p != nullptr, "wgmma conv: out of host memory");
 
     const bool s2 = d.stride == 2;
-    p->ws = tc_ws_layer(d) ? d.Cin : 0;
     const int halo_rows = s2 ? TC_TH + 1 : TC_TH + d.k - 1;
     const int halo_w = s2 ? TC_TW + 1 : TC_TW + d.k - 1;
+    const uint32_t a_tx_bytes = (uint32_t)halo_rows * halo_w * g.cin_blk * 2u;
     const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
                                   : (g.cin_blk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+    const TcBodyLayout L = tc_body_layout(d, g, a_tx_bytes, sw);
+    p->ws = L.ws;
     for (int si = 0; si < d.n_src; ++si) {   // activations: dims {C, W, H, B}; box = one halo tile (all filter taps)
         const read_src &sv = d.src[si];
         const unsigned f = (d.n_src > 1 && sv.mode == READ_SRC_NEAREST_DOWN) ? (unsigned)sv.factor : (s2 ? 2u : 1u);
@@ -1011,11 +1024,10 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         cuuint64_t strides[3] = {(cuuint64_t)sv.C * 2, (cuuint64_t)sv.W * sv.C * 2, (cuuint64_t)sv.H * sv.W * sv.C * 2};
         // traversal stride f in x and y (conv stride 2, or a nearest-down source): the box spans (n-1)*f+1 input
         // elements and delivers n of them
-        // (the weight-stationary body loads the halo one 8-channel chunk at a time, unswizzled)
-        cuuint32_t box[4] = {(cuuint32_t)(p->ws ? 8 : g.cin_blk), (cuuint32_t)((halo_w - 1) * f + 1), (cuuint32_t)((halo_rows - 1) * f + 1), 1};
+        cuuint32_t box[4] = {(cuuint32_t)L.halo_c, (cuuint32_t)((halo_w - 1) * f + 1), (cuuint32_t)((halo_rows - 1) * f + 1), 1};
         cuuint32_t estr[4] = {1, f, f, 1};
         CUresult r = enc(&p->tmA.a[si], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(sv.ptr), dims, strides, box,
-                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, p->ws ? CU_TENSOR_MAP_SWIZZLE_NONE : sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                         estr, CU_TENSOR_MAP_INTERLEAVE_NONE, L.halo_sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
             set_error("wgmma conv: cuTensorMapEncodeTiled(activations, source %d) failed with %d", si, (int)r);
@@ -1028,8 +1040,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         const cuuint64_t rows = (cuuint64_t)d.k * d.k * g.kchunks * 2 * g.cout_pad;
         cuuint64_t dims[2] = {(cuuint64_t)g.cin_blk, rows};
         cuuint64_t strides[1] = {(cuuint64_t)g.cin_blk * 2};
-        // (the 64-channel weight-stationary body loads 8-row boxes, one swizzle atom each, to interleave conv_f and conv_m)
-        cuuint32_t box[2] = {(cuuint32_t)g.cin_blk, (cuuint32_t)(p->ws == 64 ? 8 : g.n_tile)};
+        cuuint32_t box[2] = {(cuuint32_t)g.cin_blk, (cuuint32_t)L.w_rows};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&p->tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(d.w_tc), dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1055,16 +1066,11 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     };
     const int half = g.n_tile / 2;
     if (!nchw) {
-        const int oc = raw ? g.n_tile : half;             // channels of one output pixel in the tile
-        // the 64-channel weight-stationary body loads and stores one 32-channel block per warpgroup
-        const int ocb = p->ws == 64 ? 32 : (oc < 64 ? oc : 64), acb = g.n_tile < 64 ? g.n_tile : 64;
-        // stored per warpgroup (8 rows), or per tile by the weight-stationary bodies
-        bool ok = enc_epi(&p->tmA.out, d.out, raw ? 2 * d.Cout : d.Cout, d.Wout, d.Hout, ocb, TC_TW, p->ws ? TC_TH : TC_TH / 2, "out");
+        const int out_c = raw ? 2 * d.Cout : d.Cout, acb = g.n_tile < 64 ? g.n_tile : 64;     // out_c: also the residual's
+        bool ok = enc_epi(&p->tmA.out, d.out, out_c, d.Wout, d.Hout, L.epi_c, TC_TW, L.out_rows, "out");
         if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
         if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
-        if (ok && d.residual)
-            ok = raw ? enc_epi(&p->tmA.res, d.residual, 2 * d.Cout, d.Wout, d.Hout, ocb, TC_TW, TC_TH, "residual")
-                     : enc_epi(&p->tmA.res, d.residual, d.Cout, d.Wout, d.Hout, p->ws == 64 ? 32 : half, TC_TW, TC_TH, "residual");
+        if (ok && d.residual) ok = enc_epi(&p->tmA.res, d.residual, out_c, d.Wout, d.Hout, L.epi_c, TC_TW, TC_TH, "residual");
         if (ok && d.addin) ok = enc_epi(&p->tmA.add, d.addin, g.n_tile, d.addin_W, d.addin_H, acb, TC_TW / 2, TC_TH / 2, "addin");
         if (!ok) {
             delete p;
@@ -1095,8 +1101,8 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
             a.src_shift[si] = sh;
         }
     }
-    a.a_tx_bytes = (uint32_t)halo_rows * halo_w * g.cin_blk * 2u;
-    a.tile_bytes = ((p->ws ? (uint32_t)(p->ws / 8) * WS_CHUNK_BYTES : a.a_tx_bytes) + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
+    a.a_tx_bytes = a_tx_bytes;
+    a.tile_bytes = L.tile_bytes;
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
@@ -1110,9 +1116,9 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         a.e_bytes = out_b + out2_b + add_b;
         a.e_tx_bytes = (d.residual ? out_b : 0u) + out2_b + add_b;
     }
-    const uint32_t e_ring = (p->ws == 32 ? WS_E_STAGES : TC_E_STAGES) * a.e_bytes;
+    const uint32_t e_ring = (uint32_t)L.e_stages * a.e_bytes;
     // the rings get what a CTA may have minus the alignment pad, barriers and per-channel parameters (smem_bytes below)
-    const uint32_t fixed = 1024 + 8 * (p->ws == 32 ? WS_BAR_PARAMS : BAR_PARAMS) + 16 * (uint32_t)g.cout_pad + 64;
+    const uint32_t fixed = 1024 + 8 * tc_bar_slots(L.e_stages).params + 16 * (uint32_t)g.cout_pad + 64;
     const uint32_t budget_2 = TC_SMEM_PER_SM / 2 - 1024 - fixed, budget_1 = TC_SMEM_PER_CTA - fixed;
     // two CTAs per SM when the kernel instance allows it and the layer keeps resident weights, the epilogue ring and >= 3 A
     // stages in half of the SM
@@ -1168,11 +1174,12 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
 
 int g_tc_pdl = 1;         // programmatic dependent launch between consecutive conv kernels (read_set_option "tc_pdl")
 
-template <int KS, int STR, int KKN, int N>
-static int launch_tc(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
+typedef void (*TcKernel)(TcMaps, CUtensorMap, TcArgs);
+
+static int launch_tc(TcKernel kernel, const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
 {
-    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_kernel<KS, STR, KKN, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
-    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_kernel<KS, STR, KKN, N>, p->tmA, p->tmB, a));
+    RB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
+    RB_CUDA(cudaLaunchKernelEx(&lcfg, kernel, p->tmA, p->tmB, a));
     return READ_OK;
 }
 
@@ -1182,10 +1189,10 @@ static int launch_tc_kn(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lc
     const int kkn = a.cin_blk / 16;
 #define RB_TC_N(KKN_)                                                                       \
     switch (a.n_tile) {                                                                     \
-    case 16: return launch_tc<KS, STR, KKN_, 16>(p, a, lcfg);                               \
-    case 32: return launch_tc<KS, STR, KKN_, 32>(p, a, lcfg);                               \
-    case 64: return launch_tc<KS, STR, KKN_, 64>(p, a, lcfg);                               \
-    case 128: return launch_tc<KS, STR, KKN_, 128>(p, a, lcfg);                             \
+    case 16: return launch_tc(gated_conv_tc_kernel<KS, STR, KKN_, 16>, p, a, lcfg);         \
+    case 32: return launch_tc(gated_conv_tc_kernel<KS, STR, KKN_, 32>, p, a, lcfg);         \
+    case 64: return launch_tc(gated_conv_tc_kernel<KS, STR, KKN_, 64>, p, a, lcfg);         \
+    case 128: return launch_tc(gated_conv_tc_kernel<KS, STR, KKN_, 128>, p, a, lcfg);       \
     default: break;                                                                         \
     }
     if (kkn == 1) { RB_TC_N(1) }
@@ -1194,20 +1201,6 @@ static int launch_tc_kn(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lc
 #undef RB_TC_N
     set_error("wgmma conv: no kernel instance for cin_blk=%d n_tile=%d", a.cin_blk, a.n_tile);
     return READ_ERR_UNSUPPORTED;
-}
-
-static int launch_tc_ws(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
-{
-    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
-    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_ws_kernel, p->tmA, p->tmB, a));
-    return READ_OK;
-}
-
-static int launch_tc_ws64(const TcPlan *p, const TcArgs &a, cudaLaunchConfig_t &lcfg)
-{
-    RB_CUDA(cudaFuncSetAttribute(gated_conv_tc_ws64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_bytes));
-    RB_CUDA(cudaLaunchKernelEx(&lcfg, gated_conv_tc_ws64_kernel, p->tmA, p->tmB, a));
-    return READ_OK;
 }
 
 int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
@@ -1233,8 +1226,8 @@ int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
     lcfg.attrs = lattr;
     lcfg.numAttrs = a.pdl ? 1 : 0;
     int rc;
-    if (p->ws == 32) rc = launch_tc_ws(p, a, lcfg);
-    else if (p->ws == 64) rc = launch_tc_ws64(p, a, lcfg);
+    if (p->ws == 32) rc = launch_tc(gated_conv_tc_ws_kernel, p, a, lcfg);
+    else if (p->ws == 64) rc = launch_tc(gated_conv_tc_ws64_kernel, p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 3) rc = launch_tc_kn<3, 1>(p, a, lcfg);
     else if (a.stride == 2 && a.ksize == 3) rc = launch_tc_kn<3, 2>(p, a, lcfg);

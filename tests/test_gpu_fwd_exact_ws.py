@@ -5,11 +5,14 @@
   finds no tile (one, two and three persistent CTAs and the full grid, in both tile orders);
 * enough tiles per CTA that the halo ring (13 stages) and the four epilogue stages wrap several times;
 * ELU with a residual and neither, at ragged W and H and B = 1 and 2.
+
+A CONV_TCGEN05 plan does not say which kernel body it runs, so one more test reads the launched kernel's name from the profiler.
 """
 import pytest
 
 import fwd_exact_util as X
 from test_gpu_fwd_exact import _run_case, gate_pinned  # noqa: F401  (gate_pinned is a module fixture)
+from test_gpu_fwd_exact_ws64 import _kernels_launched
 
 pytestmark = pytest.mark.gpu
 
@@ -26,3 +29,13 @@ WS_CASES = [
 @pytest.mark.parametrize("case", WS_CASES, ids=lambda c: c.id)
 def test_ws_forward_is_exact(case, gate_pinned):  # noqa: F811
     _run_case(case, gate_pinned)
+
+
+@pytest.mark.parametrize("case, body", [
+    (WS_CASES[0], "gated_conv_tc_ws_kernel"),
+    # the training path's recomputed [f | m] of the same shape keeps the general body
+    (X.Case("RAW 3x3 32->32", "tma", ((32, "id", 1),), 32, 3, 1, 1, 17, 9, out="raw"), "gated_conv_tc_kernel"),
+], ids=lambda v: v.id if isinstance(v, X.Case) else v)
+def test_32_channel_layer_runs_its_body(case, body):
+    names = _kernels_launched(case)
+    assert len(names) == 1 and body in next(iter(names)), f"{case.id}: launched {names}, expected {body}"
