@@ -90,6 +90,13 @@ def _launch(lib, src, cout, w_tc, par, elu, out_mode, out, residual=None, k=3, s
         lib.read_conv_plan_destroy(plan)
 
 
+def _launch_raw(lib, src, cout, w_tc, out, residual=None, k=3, stride=1):
+    """A _launch with RAW output (the [f | m] accumulators, no epilogue): the kernel still stages ``cout`` epilogue parameters,
+    which RAW output never uses, so they are zeros."""
+    zeros = torch.zeros(cout, dtype=torch.float32, device=out.device)
+    _launch(lib, src, cout, w_tc, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, residual, k=k, stride=stride)
+
+
 # packed filters per GatedConv: module -> (key, dict of filters); see _packed
 _FILTERS = weakref.WeakKeyDictionary()
 cache_filters = True        # False: pack on every call (measurement of the cache, scripts/bench_train_bf16.py)
@@ -236,68 +243,33 @@ def conv_forward(lib, src, c, out, residual=None):
 
 def gate_backward(lib, g, fm, c, dfm):
     """[df | dm] (into ``dfm``, RAW column order) and [dbias_f, dbias_m, dgamma, dbeta] (fp32 [4, C]) of the FoldedConv ``c`` from
-    its output gradient ``g`` and the recomputed [f | m]; a train-mode norm adds the terms through the batch statistics."""
-    st = L.stream_ptr()
-    P = g.numel() // c.C
-    red = torch.zeros((4, c.C), dtype=torch.float32, device=g.device)  # dbias_f, dbias_m, dgamma, dbeta
-    if torch.are_deterministic_algorithms_enabled():
-        return _gate_backward_det(lib, g, fm, c, dfm, P, red, st)
-    if c.items is not None:
-        items, P = g.shape[0], g.shape[1] * g.shape[2]
-        sums = torch.zeros((2, items, c.C), dtype=torch.float32, device=g.device)     # sum dy, sum dy * xhat per item
-        L.check(lib.read_bn_backward_reduce_items(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
-                                                  c.bm.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), sums[0].data_ptr(),
-                                                  sums[1].data_ptr(), st))
-        L.check(lib.read_gate_backward_batch_stats_items(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
-                                                         c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
-                                                         sums[0].data_ptr(), sums[1].data_ptr(), dfm.data_ptr(),
-                                                         red[0].data_ptr(), red[1].data_ptr(), st))
+    its output gradient ``g`` and the recomputed [f | m]; a train-mode norm adds the terms through the batch statistics (per item
+    with per-item statistics).  Under torch.use_deterministic_algorithms(True) the *_det entry points combine the sums in a fixed
+    order."""
+    st, C = L.stream_ptr(), c.C
+    red = torch.zeros((4, C), dtype=torch.float32, device=g.device)    # dbias_f, dbias_m, dgamma, dbeta
+    mode = "eval" if not c.batch else "batch" if c.items is None else "items"
+    items = g.shape[0] if mode == "items" else 1
+    P = g.numel() // (items * C)
+    det = "_det" if torch.are_deterministic_algorithms_enabled() else ""
+    ws = ops.det_workspace(lib.read_gate_det_workspace_bytes(items, C), g.device, "gate backward") if det else None
+    tail = ([ws.data_ptr()] if det else []) + [st]
+    head = [g.data_ptr(), fm.data_ptr(), *([items] if mode == "items" else []), P, C, int(c.elu), c.bf.data_ptr(),
+            c.bm.data_ptr()]
+    if mode == "eval":
+        L.check(getattr(lib, "read_gate_backward" + det)(*head, c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
+                                                         dfm.data_ptr(), *(r.data_ptr() for r in red), *tail))
+        return red
+    # sum dy, sum dy * xhat: dbeta and dgamma, per item ([items, C]) with per-item statistics
+    sums = (red[3], red[2]) if mode == "batch" else torch.zeros((2, items, C), dtype=torch.float32, device=g.device)
+    form = ("_items" if mode == "items" else "") + det
+    L.check(getattr(lib, "read_bn_backward_reduce" + form)(*head, c.mean.data_ptr(), c.inv.data_ptr(), sums[0].data_ptr(),
+                                                           sums[1].data_ptr(), *tail))
+    L.check(getattr(lib, "read_gate_backward_batch_stats" + form)(*head, c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
+                                                                  sums[0].data_ptr(), sums[1].data_ptr(), dfm.data_ptr(),
+                                                                  red[0].data_ptr(), red[1].data_ptr(), *tail))
+    if mode == "items":
         red[3], red[2] = sums[0].sum(0), sums[1].sum(0)
-        return red
-    if c.batch:
-        L.check(lib.read_bn_backward_reduce(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                            c.mean.data_ptr(), c.inv.data_ptr(), red[3].data_ptr(), red[2].data_ptr(), st))
-        L.check(lib.read_gate_backward_batch_stats(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(),
-                                                   c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
-                                                   red[3].data_ptr(), red[2].data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
-                                                   red[1].data_ptr(), st))
-        return red
-    L.check(lib.read_gate_backward(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                   c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(),
-                                   red[0].data_ptr(), red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), st))
-    return red
-
-
-def _gate_backward_det(lib, g, fm, c, dfm, P, red, st):
-    """gate_backward under torch.use_deterministic_algorithms(True): the same passes through the *_det entry points, whose sums
-    are combined in a fixed order."""
-    items = g.shape[0] if c.items is not None else 1
-    ws = ops.det_workspace(lib.read_gate_det_workspace_bytes(items, c.C), g.device, "gate backward")
-    if c.items is not None:
-        P = g.shape[1] * g.shape[2]
-        sums = torch.zeros((2, items, c.C), dtype=torch.float32, device=g.device)
-        L.check(lib.read_bn_backward_reduce_items_det(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu), c.bf.data_ptr(),
-                                                      c.bm.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), sums[0].data_ptr(),
-                                                      sums[1].data_ptr(), ws.data_ptr(), st))
-        L.check(lib.read_gate_backward_batch_stats_items_det(g.data_ptr(), fm.data_ptr(), items, P, c.C, int(c.elu),
-                                                             c.bf.data_ptr(), c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(),
-                                                             c.inv.data_ptr(), sums[0].data_ptr(), sums[1].data_ptr(),
-                                                             dfm.data_ptr(), red[0].data_ptr(), red[1].data_ptr(), ws.data_ptr(),
-                                                             st))
-        red[3], red[2] = sums[0].sum(0), sums[1].sum(0)
-        return red
-    if c.batch:
-        L.check(lib.read_bn_backward_reduce_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                                c.mean.data_ptr(), c.inv.data_ptr(), red[3].data_ptr(), red[2].data_ptr(),
-                                                ws.data_ptr(), st))
-        L.check(lib.read_gate_backward_batch_stats_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(),
-                                                       c.bm.data_ptr(), c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(),
-                                                       red[3].data_ptr(), red[2].data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
-                                                       red[1].data_ptr(), ws.data_ptr(), st))
-        return red
-    L.check(lib.read_gate_backward_det(g.data_ptr(), fm.data_ptr(), P, c.C, int(c.elu), c.bf.data_ptr(), c.bm.data_ptr(),
-                                       c.scale.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), dfm.data_ptr(), red[0].data_ptr(),
-                                       red[1].data_ptr(), red[2].data_ptr(), red[3].data_ptr(), ws.data_ptr(), st))
     return red
 
 
@@ -317,6 +289,32 @@ def conv_wgrad(lib, dfm, x, B, Hout, Wout, C, k, stride, dwf, dwm, st):
                                     dwm.data_ptr(), st))
 
 
+def _out_grad(gout, C):
+    """The output gradient ``gout`` (NCHW) as NHWC bf16 with the C channels the conv runs at: a conv run padded to C gets 0 as
+    the gradient of its padded channels."""
+    gp = gout.float()
+    if gp.shape[1] < C:
+        gp = torch.cat([gp, gp.new_zeros((gp.shape[0], C - gp.shape[1]) + tuple(gp.shape[2:]))], 1)
+    return ops.nchw_to_nhwc(gp.contiguous(), True)
+
+
+def _param_grads(lib, g, fm, c, dfm, srcs, need, cout):
+    """[dwf, dbias_f, dwm, dbias_m, dgamma, dbeta] of the FoldedConv ``c`` from its output gradient ``g`` and recomputed [f | m]:
+    the gate backward into ``dfm``, then the weight gradient over each NHWC source in ``srcs`` (skipped when no weight needs one,
+    as for a frozen net).  ``need`` are the 6 parameters' needs_input_grad flags: a gradient nobody asks for is None, the others
+    are sliced to the conv's ``cout`` real channels."""
+    red = gate_backward(lib, g, fm, c, dfm)
+    dwf = dwm = None
+    if need[0] or need[2]:
+        B, Hout, Wout, _ = dfm.shape
+        dws = [[torch.zeros((c.C, s.shape[3], c.k, c.k), dtype=torch.float32, device=dfm.device) for _ in range(2)] for s in srcs]
+        for s, (wf_s, wm_s) in zip(srcs, dws):
+            conv_wgrad(lib, dfm, s, B, Hout, Wout, c.C, c.k, c.stride, wf_s, wm_s, L.stream_ptr())
+        dwf, dwm = dws[0] if len(srcs) == 1 else (torch.cat(w, 1) for w in zip(*dws))
+    grads = [dwf, red[0], dwm, red[1], red[2], red[3]]
+    return [gr[:cout] if n else None for gr, n in zip(grads, need)]
+
+
 def dgrad(dfm, conv, residual=None):
     """Input gradient [B,H,W,Cin] (bf16) of ``conv`` (a FoldedConv) from [df | dm] in RAW column order, plus ``residual``."""
     lib = L.load()
@@ -329,8 +327,7 @@ def dgrad(dfm, conv, residual=None):
         L.check(lib.read_conv3x3_dgrad_cin8(dfm.data_ptr(), conv.wf.data_ptr(), conv.wm.data_ptr(), B, H, W, conv.C,
                                             out.data_ptr(), L.stream_ptr()))
         return out
-    zeros = torch.zeros(cin, dtype=torch.float32, device=dfm.device)      # a RAW launch reads no epilogue parameters
-    _launch(lib, dfm, cin // 2, conv.w_dgrad, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, residual)
+    _launch_raw(lib, dfm, cin // 2, conv.w_dgrad, out, residual)
     return out
 
 
@@ -371,12 +368,11 @@ class ResStackFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gout):
-        lib, st = L.load(), L.stream_ptr()
+        lib = L.load()
         inputs, convs = ctx.saved_tensors[:ctx.n_inputs], ctx.convs
         B, H, W, C = inputs[0].shape
-        dev = inputs[0].device
-        g = ops.nchw_to_nhwc(gout.float().contiguous(), True)             # gradient of the stack's output, NHWC bf16
-        fm = torch.empty((B, H, W, 2 * C), dtype=torch.bfloat16, device=dev)
+        g = _out_grad(gout, C)                                            # gradient of the stack's output, NHWC bf16
+        fm = torch.empty((B, H, W, 2 * C), dtype=torch.bfloat16, device=inputs[0].device)
         dfm = torch.empty_like(fm)
         grads = [None] * (6 * len(convs))
         g_block = g
@@ -385,17 +381,11 @@ class ResStackFn(torch.autograd.Function):
             if i % 2 == 1:
                 g_block = g                                               # gradient of this ResBlock's output
             _launch(lib, x_in, C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-            red = gate_backward(lib, g, fm, c, dfm)                       # dbias_f, dbias_m, dgamma, dbeta
-            dwf = dwm = None
-            if ctx.needs_input_grad[2 + 6 * i] or ctx.needs_input_grad[4 + 6 * i]:    # not for a frozen net
-                dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
-                conv_wgrad(lib, dfm, x_in, B, H, W, C, 3, 1, dwf, dwm, st)
-            grads[6 * i: 6 * i + 6] = [dwf, red[0], dwm, red[1], red[2], red[3]]
+            grads[6 * i: 6 * i + 6] = _param_grads(lib, g, fm, c, dfm, [x_in], ctx.needs_input_grad[2 + 6 * i: 8 + 6 * i], C)
             if i > 0 or ctx.needs_input_grad[0]:
                 # the first conv of a ResBlock adds the gradient that reaches its input through the skip
                 g = dgrad(dfm, c, residual=g_block if i % 2 == 0 else None)
         dx = ops.nhwc_to_nchw(g) if ctx.needs_input_grad[0] else None
-        grads = [gr if ctx.needs_input_grad[2 + k] else None for k, gr in enumerate(grads)]
         return (dx, None, *grads)
 
 
@@ -407,17 +397,19 @@ class ResStackItemsFn(ResStackFn):
         return ResStackFn._forward(ctx, x, mods, params, x.shape[0])
 
 
+def _stack_names(net, prefix):
+    return [f"{prefix}.layers.{i}.main.{j}" for i in range(net.num_res) for j in (0, 1)]
+
+
 def stack_convs(net, prefix):
     """The 8 GatedConvs of the stack ``prefix`` (e.g. 'Encoder.0') in forward order."""
-    return [net.get_submodule(f"{prefix}.layers.{i}.main.{j}") for i in range(net.num_res) for j in (0, 1)]
+    return [net.get_submodule(n) for n in _stack_names(net, prefix)]
 
 
 def res_stack(net, prefix, x, batch_stats=False, per_item=False):
     """bf16 forward of one EBlock / DBlock of ``net`` on the wgmma kernels, differentiable through ResStackFn."""
-    names = [f"{prefix}.layers.{i}.main.{j}" for i in range(net.num_res) for j in (0, 1)]
-    if per_item:
-        return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=names, per_item=True)
-    return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=names)
+    return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=_stack_names(net, prefix),
+                         per_item=per_item)
 
 
 def stack_params(mods):
@@ -499,26 +491,16 @@ class GatedConvFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gout):
-        lib, st = L.load(), L.stream_ptr()
+        lib = L.load()
         x_in, c, cout = ctx.saved_tensors[0], ctx.conv, ctx.cout
         need = ctx.needs_input_grad
         B, H, W, _ = x_in.shape
-        C, dev = c.C, x_in.device
-        gp = gout.float()
-        if cout < C:
-            gp = torch.cat([gp, gp.new_zeros((B, C - cout, H, W))], 1)   # the padded channels' output gradient is 0
-        g = ops.nchw_to_nhwc(gp.contiguous(), True)
-        fm = torch.empty((B, H, W, 2 * C), dtype=torch.bfloat16, device=dev)
+        g = _out_grad(gout, c.C)
+        fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=x_in.device)
         dfm = torch.empty_like(fm)
-        _launch(lib, x_in, C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-        red = gate_backward(lib, g, fm, c, dfm)                           # dbias_f, dbias_m, dgamma, dbeta
-        dwf = dwm = None
-        if need[3] or need[5]:                                            # not for a frozen net
-            dwf, dwm = torch.zeros_like(c.wf), torch.zeros_like(c.wm)
-            conv_wgrad(lib, dfm, x_in, B, H, W, C, 3, 1, dwf, dwm, st)
+        _launch(lib, x_in, c.C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
+        grads = _param_grads(lib, g, fm, c, dfm, [x_in], need[3:], cout)
         dx = ops.nhwc_to_nchw(dgrad(dfm, c)) if need[0] else None
-        grads = [dwf, red[0], dwm, red[1], red[2], red[3]]
-        grads = [gr[:cout] if gr is not None and need[3 + k] else None for k, gr in enumerate(grads)]
         return (dx, gout if need[1] else None, None, *grads)
 
 
@@ -556,15 +538,14 @@ def recompute_fm(lib, srcs, c):
     [f | m] of channels 64b .. 64b + 63."""
     d = _desc(srcs, c.C, c.k, c.stride)
     B, H, W = d.B, d.Hout, d.Wout
-    zeros = torch.zeros(c.C, dtype=torch.float32, device=srcs[0].device)  # a RAW launch reads no epilogue parameters
     if c.k != 1 or c.C <= 64:
         fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=srcs[0].device)
-        _launch(lib, srcs, c.C, c.w_tc, (zeros,) * 4, False, L.OUT_RAW_NHWC, fm, k=c.k, stride=c.stride)
+        _launch_raw(lib, srcs, c.C, c.w_tc, fm, k=c.k, stride=c.stride)
         return fm
     blocks_ = []
     for w in _fm64_filters(lib, srcs, c):
         out = torch.empty((B, H, W, 128), dtype=torch.bfloat16, device=srcs[0].device)
-        _launch(lib, srcs, 64, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
+        _launch_raw(lib, srcs, 64, w, out, k=1)
         blocks_.append(out)
     return torch.cat(blocks_, -1)
 
@@ -617,8 +598,7 @@ def dgrad_1x1(dfm, c, c0, cs):
         n_out = max(cn, 32)
         w = _dgrad1x1_filters(lib, c, a, cn, dfm.device)
         out = torch.empty((B, H, W, n_out), dtype=torch.bfloat16, device=dfm.device)
-        zeros = torch.zeros(n_out // 2, dtype=torch.float32, device=dfm.device)
-        _launch(lib, dfm, n_out // 2, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out, k=1)
+        _launch_raw(lib, dfm, n_out // 2, w, out, k=1)
         parts.append(out if cn == n_out else out[..., :cn])
     return parts[0] if len(parts) == 1 else torch.cat(parts, -1)
 
@@ -654,25 +634,12 @@ class MultiSourceConvFn(torch.autograd.Function):
         n_src, c, cout = ctx.n_src, ctx.conv, ctx.cout
         ts = ctx.saved_tensors[:n_src]
         need = ctx.needs_input_grad[2:]                                    # the sources, then the 6 parameters
-        C, dev = c.C, ts[0].device
-        B = ts[0].shape[0]
-        gp = gout.float()
-        if cout < C:
-            gp = torch.cat([gp, gp.new_zeros((B, C - cout) + tuple(gp.shape[2:]))], 1)  # the padded channels' gradient is 0
-        g = ops.nchw_to_nhwc(gp.contiguous(), True)
-        Hout, Wout = g.shape[1], g.shape[2]
+        g = _out_grad(gout, c.C)
+        B, Hout, Wout, C = g.shape
         fm = recompute_fm(lib, ts, c)
         dfm = torch.empty_like(fm)
-        red = gate_backward(lib, g, fm, c, dfm)                            # dbias_f, dbias_m, dgamma, dbeta
-        del fm
-        dwf = dwm = None
-        if need[n_src] or need[n_src + 2]:                                 # not for a frozen net
-            kk = (c.k, c.k)
-            dws = [(torch.zeros((C, t.shape[3]) + kk, device=dev), torch.zeros((C, t.shape[3]) + kk, device=dev)) for t in ts]
-            for t, (wf_s, wm_s) in zip(ts, dws):
-                conv_wgrad(lib, dfm, t, B, Hout, Wout, C, c.k, c.stride, wf_s, wm_s, st)
-            dwf = torch.cat([w[0] for w in dws], 1) if n_src > 1 else dws[0][0]
-            dwm = torch.cat([w[1] for w in dws], 1) if n_src > 1 else dws[0][1]
+        grads = _param_grads(lib, g, fm, c, dfm, ts, need[n_src:], cout)
+        del fm                                                             # the input gradient reads [df | dm] only
         dxs = [None] * n_src
         c0 = 0
         for i, t in enumerate(ts):
@@ -686,8 +653,6 @@ class MultiSourceConvFn(torch.autograd.Function):
                     dx = dgrad_1x1(dfm, c, c0, cs)
                 dxs[i] = ops.nhwc_to_nchw(dx.contiguous())
             c0 += cs
-        grads = [dwf, red[0], dwm, red[1], red[2], red[3]]
-        grads = [gr[:cout] if gr is not None and need[n_src + j] else None for j, gr in enumerate(grads)]
         return (None, None, *dxs, *grads)
 
 
@@ -704,7 +669,7 @@ def gated_conv_srcs(mod, xs, name=None, batch_stats=False, per_item=False):
     differentiable through MultiSourceConvFn.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels);
     a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors.  ``batch_stats``: a
     train-mode norm normalises with batch statistics (else it raises), each batch item with its own with ``per_item``."""
-    label = name or f"GatedConv(k={mod.k}, stride={mod.stride})"
+    label = _label(mod, name)
     xs = list(xs)
     if (mod.k, mod.stride) not in GEOMETRIES:
         raise ValueError(f"read_b200: {label}: gated_conv_srcs runs 1x1 and stride-2 3x3 / 4x4 convs (got k={mod.k}, "

@@ -28,14 +28,14 @@ __device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2
 // BATCH: train-mode BatchNorm (mean / inv_std are this batch's statistics over the P pixels).  Its backward adds the terms through
 // the statistics: dg = scale * (dy - sum_dy / P - xhat * sum_dy_xhat / P) = scale * dy + k1 * (g - mean) + k0 with
 // k1 = -scale * inv_std * sum_dy_xhat / P, k0 = -scale * sum_dy / P; the two sums (= dgamma, dbeta) come from bn_bwd_reduce_kernel,
-// so this instance accumulates no dgamma / dbeta.  BATCH = false compiles to the eval-mode kernel unchanged (the appended
-// parameters are never read).
+// so this instance accumulates no dgamma / dbeta.  BATCH = DET = PER_ITEM = false compiles to the eval-mode kernel unchanged (the
+// parameters of the other forms are never read).
 constexpr int GB_THREADS = 256, GB_MAX_C = 256;
 
 // ---- deterministic reduction (DET instances, torch.use_deterministic_algorithms): no atomics on the sums.
 // A CTA adds the per-thread sums of channel c in thread order (threads c / 8, c / 8 + G, ...) and stores them as its row of the
 // caller's workspace part[cta][NS][C] (cta = blockIdx.y * gridDim.x + blockIdx.x); the last CTA to finish (counter + fence, the
-// counter zeroed by the entry point and again by that CTA) combines the rows in a fixed order, see gate_det_combine.
+// counter zeroed by the launcher and again by that CTA) combines the rows in a fixed order, see gate_det_combine.
 __device__ __forceinline__ void gate_det_cta_sum(const float (&v)[8], int C, int G, int ppb, float *__restrict__ row)
 {
     __shared__ float buf[GB_THREADS * 8];
@@ -90,14 +90,14 @@ __device__ __forceinline__ void gate_det_combine(const float *part, int C, float
     if (threadIdx.x == 0) *counter = 0u;
 }
 
-template <bool ELU, bool BATCH, bool DET = false>
+template <bool ELU, bool BATCH, bool DET>
 __device__ __forceinline__ void
 gate_bwd_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
               const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
               const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
               float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
-              const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part = nullptr,
-              unsigned *__restrict__ counter = nullptr)
+              const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part,
+              unsigned *__restrict__ counter)
 {
     __shared__ float red[4][GB_MAX_C];
     if constexpr (!DET) {
@@ -192,45 +192,37 @@ gate_bwd_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restr
     }
 }
 
-template <bool ELU, bool BATCH>
+// PER_ITEM (train-mode BatchNorm per item, UNet.train_batchnorm = 'per_item'): item i = blockIdx.y is the P rows [i * P, (i + 1) * P)
+// with its own statistics (row i of the [items, C] scale / mean / inv_std / sums), so k1 / k0 come from item i's sums and P;
+// dbias_f / dbias_m accumulate over every item (DET: the last CTA combines every item into them).
+template <bool ELU, bool BATCH, bool DET, bool PER_ITEM>
 __global__ void __launch_bounds__(GB_THREADS)
 gate_bwd_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
                 const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
                 const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
                 float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
-                const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat)
+                const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part,
+                unsigned *__restrict__ counter)
 {
-    gate_bwd_body<ELU, BATCH>(dy, fm, P, C, half, bias_f, bias_m, scale, mean, inv_std, dfm, dbf, dbm, dgamma, dbeta, sum_dy,
-                              sum_dy_xhat);
-}
-
-// Per-item train-mode BatchNorm (UNet.train_batchnorm = 'per_item'): item i = blockIdx.y is the P rows [i * P, (i + 1) * P) with
-// its own statistics (row i of the [items, C] scale / mean / inv_std / sums), so k1 / k0 come from item i's sums and P; dbias_f /
-// dbias_m accumulate over every item.
-template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-gate_bwd_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                      const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
-                      const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
-                      float *__restrict__ dbf, float *__restrict__ dbm, const float *__restrict__ sum_dy,
-                      const float *__restrict__ sum_dy_xhat)
-{
-    const long long it = blockIdx.y, o = it * C;
-    gate_bwd_body<ELU, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, scale + o, mean + o, inv_std + o,
-                             dfm + it * P * 2 * C, dbf, dbm, nullptr, nullptr, sum_dy + o, sum_dy_xhat + o);
+    static_assert(BATCH || !PER_ITEM, "per-item statistics are train-mode BatchNorm's");
+    // dgamma / dbeta are unused under BATCH; the per-item forms pass them as constant nulls, which the DET combine folds
+    const long long it = PER_ITEM ? blockIdx.y : 0, o = it * C;
+    gate_bwd_body<ELU, BATCH, DET>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, scale + o, mean + o, inv_std + o,
+                                   dfm + it * P * 2 * C, dbf, dbm, PER_ITEM ? nullptr : dgamma, PER_ITEM ? nullptr : dbeta,
+                                   sum_dy + o, sum_dy_xhat + o, part, counter);
 }
 
 // ------------------------------------------------------------------ train-mode BatchNorm: backward reduction
 // sum_dy += sum dy, sum_dy_xhat += sum dy * (g - mean) * inv_std over the P pixels, with g = A(f + b_f) * sigmoid(m + b_m)
 // recomputed from the RAW [f | m] (mean / inv_std: the batch statistics of the forward).  These are dbeta and dgamma, and the
-// two terms the corrected gate backward (gate_bwd_kernel<ELU, true>) needs.  Same thread layout and reduction as the gate backward.
+// two terms the corrected gate backward (gate_bwd_kernel with BATCH) needs.  Same thread layout and reduction as the gate backward.
 // DET: the deterministic reduction above; PER_ITEM: the last CTA writes item r's sums to row r (sum_dy / sum_dy_xhat [items, C]).
-template <bool ELU, bool DET = false, bool PER_ITEM = false>
+template <bool ELU, bool DET, bool PER_ITEM>
 __device__ __forceinline__ void
 bn_bwd_reduce_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
                    const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
                    const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat,
-                   float *__restrict__ part = nullptr, unsigned *__restrict__ counter = nullptr)
+                   float *__restrict__ part, unsigned *__restrict__ counter)
 {
     __shared__ float red[2][GB_MAX_C];
     if constexpr (!DET) {
@@ -288,78 +280,18 @@ bn_bwd_reduce_body(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__
     }
 }
 
-template <bool ELU>
+// PER_ITEM: the sums of item blockIdx.y (its P rows, its mean / inv_std) into row blockIdx.y of [items, C]; under DET the body's
+// last CTA writes every row itself, so sum_dy / sum_dy_xhat are passed unshifted
+template <bool ELU, bool DET, bool PER_ITEM>
 __global__ void __launch_bounds__(GB_THREADS)
 bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
                      const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
-                     const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat)
+                     const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat,
+                     float *__restrict__ part, unsigned *__restrict__ counter)
 {
-    bn_bwd_reduce_body<ELU>(dy, fm, P, C, half, bias_f, bias_m, mean, inv_std, sum_dy, sum_dy_xhat);
-}
-
-// per item: the sums of item blockIdx.y (its P rows, its mean / inv_std) into row blockIdx.y of [items, C]
-template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-bn_bwd_reduce_items_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C,
-                           int half, const float *__restrict__ bias_f, const float *__restrict__ bias_m,
-                           const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy,
-                           float *__restrict__ sum_dy_xhat)
-{
-    const long long it = blockIdx.y, o = it * C;
-    bn_bwd_reduce_body<ELU>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o, sum_dy + o,
-                            sum_dy_xhat + o);
-}
-
-// Deterministic instances (torch.use_deterministic_algorithms): the bodies above with DET, the CTA partials in part / counter.
-// The per-item forms take the unshifted pointers: the body's last CTA combines every item (gate: into one dbias_f / dbias_m; BN
-// reduce: item r into row r).
-template <bool ELU, bool BATCH>
-__global__ void __launch_bounds__(GB_THREADS)
-gate_bwd_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                    const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
-                    const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
-                    float *__restrict__ dbf, float *__restrict__ dbm, float *__restrict__ dgamma, float *__restrict__ dbeta,
-                    const float *__restrict__ sum_dy, const float *__restrict__ sum_dy_xhat, float *__restrict__ part,
-                    unsigned *__restrict__ counter)
-{
-    gate_bwd_body<ELU, BATCH, true>(dy, fm, P, C, half, bias_f, bias_m, scale, mean, inv_std, dfm, dbf, dbm, dgamma, dbeta, sum_dy,
-                                    sum_dy_xhat, part, counter);
-}
-
-template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-gate_bwd_items_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                          const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ scale,
-                          const float *__restrict__ mean, const float *__restrict__ inv_std, __nv_bfloat16 *__restrict__ dfm,
-                          float *__restrict__ dbf, float *__restrict__ dbm, const float *__restrict__ sum_dy,
-                          const float *__restrict__ sum_dy_xhat, float *__restrict__ part, unsigned *__restrict__ counter)
-{
-    const long long it = blockIdx.y, o = it * C;
-    gate_bwd_body<ELU, true, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, scale + o, mean + o,
-                                   inv_std + o, dfm + it * P * 2 * C, dbf, dbm, nullptr, nullptr, sum_dy + o, sum_dy_xhat + o, part,
-                                   counter);
-}
-
-template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-bn_bwd_reduce_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C, int half,
-                         const float *__restrict__ bias_f, const float *__restrict__ bias_m, const float *__restrict__ mean,
-                         const float *__restrict__ inv_std, float *__restrict__ sum_dy, float *__restrict__ sum_dy_xhat,
-                         float *__restrict__ part, unsigned *__restrict__ counter)
-{
-    bn_bwd_reduce_body<ELU, true>(dy, fm, P, C, half, bias_f, bias_m, mean, inv_std, sum_dy, sum_dy_xhat, part, counter);
-}
-
-template <bool ELU>
-__global__ void __launch_bounds__(GB_THREADS)
-bn_bwd_reduce_items_det_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *__restrict__ fm, long long P, int C,
-                               int half, const float *__restrict__ bias_f, const float *__restrict__ bias_m,
-                               const float *__restrict__ mean, const float *__restrict__ inv_std, float *__restrict__ sum_dy,
-                               float *__restrict__ sum_dy_xhat, float *__restrict__ part, unsigned *__restrict__ counter)
-{
-    const long long it = blockIdx.y, o = it * C;
-    bn_bwd_reduce_body<ELU, true, true>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o,
-                                        sum_dy, sum_dy_xhat, part, counter);
+    const long long it = PER_ITEM ? blockIdx.y : 0, o = it * C, so = DET ? 0 : o;
+    bn_bwd_reduce_body<ELU, DET, PER_ITEM>(dy + it * P * C, fm + it * P * 2 * C, P, C, half, bias_f, bias_m, mean + o, inv_std + o,
+                                           sum_dy + so, sum_dy_xhat + so, part, counter);
 }
 
 // ------------------------------------------------------------------ weight gradient
@@ -823,6 +755,91 @@ static int launch_dgrad_s2(const void *dfm, const void *wt, int B, int Ho, int W
     return READ_OK;
 }
 
+// ------------------------------------------------------------------ launchers of the gate backward and the BN reduction
+// The ten entry points are forms of these two passes: eval-mode or batch statistics (BATCH, gate pass only), call-wide or per item
+// (PER_ITEM; the call-wide forms pass items = 1), atomic or deterministic sums (DET: the workspace holds the counter in its first
+// 256 bytes, then the CTA rows).
+
+// the [f | m] column order (blocks of 2*min(C, 64)) exists only for C <= 64 or C % 64 == 0, as in the forward RAW plan
+static bool gate_channels_ok(int C) { return C >= 16 && C <= GB_MAX_C && C % 16 == 0 && (C <= 64 || C % 64 == 0); }
+
+// CTAs per item of a gate pass: the call's CTAs are capped as for a single call of all the items' pixels, at 8 per SM, or for DET
+// at 2 per SM (the last CTA reads every CTA's row)
+static long long gate_grid(int items, bool det, int64_t pixels, int C)
+{
+    const int ppb = GB_THREADS / (C / 8);
+    long long blocks = (pixels + ppb - 1) / ppb, cap = (det ? 2ll : 8ll) * num_sms() / items;
+    if (cap < 1) cap = 1;
+    return blocks > cap ? cap : blocks;
+}
+
+// The argument checks after the null-pointer check, in the order each entry point has always made them: the atomic forms check C
+// before the alignment, the DET forms after the alignment of dy, fm and the workspace.  The batch-statistics forms need
+// bn_channels_ok(C) and 2 pixels; the eval-mode forms accept C = 48 and pixels == 0, and report a negative count with C.
+static int gate_pass_checks(const char *name, bool batch, bool det, bool per_item, int items, int64_t pixels, int C, const void *dy,
+                            const void *fm, const void *dfm, const void *workspace)
+{
+    const uintptr_t in = reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm);
+    if (per_item) RB_CHECK_ARG(items >= 1 && items <= 65535, "%s: items must lie in 1..65535 (got %d)", name, items);
+    if (det) {
+        const int minpx = batch ? 2 : 0;
+        RB_CHECK_ARG(pixels >= minpx, "%s: needs at least %d pixels (got %lld)", name, minpx, (long long)pixels);
+        RB_CHECK_ARG(((in | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0, "%s: tensors and workspace must be 16B aligned", name);
+    }
+    if (batch)
+        RB_CHECK_ARG(bn_channels_ok(C), "%s: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", name, GB_MAX_C, C);
+    else
+        RB_CHECK_ARG(gate_channels_ok(C) && pixels >= 0, "%s: C must be 16, 32, 48, 64 or a multiple of 64 up to %d (got %d)", name,
+                     GB_MAX_C, C);
+    if (batch && !det)
+        RB_CHECK_ARG(pixels >= 2, "%s: batch statistics need at least 2 pixels%s (got %lld)", name, per_item ? " per item" : "",
+                     (long long)pixels);
+    RB_CHECK_ARG(((in | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0, "%s: tensors must be 16B aligned", name);
+    return READ_OK;
+}
+
+template <bool BATCH, bool DET, bool PER_ITEM>
+static int gate_backward_launch(const char *name, int items, const void *dy, const void *fm, int64_t pixels, int C, int elu,
+                                const float *bias_f, const float *bias_m, const float *bn_scale, const float *bn_mean,
+                                const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f,
+                                float *dbias_m, float *dgamma, float *dbeta, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && dbias_f && dbias_m &&
+                     (BATCH ? sum_dy && sum_dy_xhat : dgamma && dbeta) && (!DET || workspace),
+                 "%s: null pointer", name);
+    if (const int rc = gate_pass_checks(name, BATCH, DET, PER_ITEM, items, pixels, C, dy, fm, dfm, workspace)) return rc;
+    if (pixels == 0) return READ_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    if (DET) RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? gate_bwd_kernel<true, BATCH, DET, PER_ITEM> : gate_bwd_kernel<false, BATCH, DET, PER_ITEM>;
+    k<<<dim3((unsigned)gate_grid(items, DET, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale, bn_mean,
+        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, sum_dy, sum_dy_xhat,
+        DET ? (float *)((char *)workspace + 256) : nullptr, counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+template <bool DET, bool PER_ITEM>
+static int bn_reduce_launch(const char *name, int items, const void *dy, const void *fm, int64_t pixels, int C, int elu,
+                            const float *bias_f, const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy,
+                            float *sum_dy_xhat, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat && (!DET || workspace),
+                 "%s: null pointer", name);
+    if (const int rc = gate_pass_checks(name, true, DET, PER_ITEM, items, pixels, C, dy, fm, nullptr, workspace)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    unsigned *counter = (unsigned *)workspace;
+    if (DET) RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
+    auto k = elu ? bn_bwd_reduce_kernel<true, DET, PER_ITEM> : bn_bwd_reduce_kernel<false, DET, PER_ITEM>;
+    k<<<dim3((unsigned)gate_grid(items, DET, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        bn_inv_std, sum_dy, sum_dy_xhat, DET ? (float *)((char *)workspace + 256) : nullptr, counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
 }  // namespace rb
 
 using namespace rb;
@@ -833,46 +850,16 @@ int read_gate_backward(const void *dy, const void *fm, int64_t pixels, int C, in
                        const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
                        float *dbias_m, float *dgamma, float *dbeta, void *stream)
 {
-    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && dbias_f && dbias_m && dgamma && dbeta,
-                 "gate_backward: null pointer");
-    // the [f | m] column order (blocks of 2*min(C, 64)) exists only for C <= 64 or C % 64 == 0, as in the forward RAW plan
-    RB_CHECK_ARG(C >= 16 && C <= GB_MAX_C && C % 16 == 0 && (C <= 64 || C % 64 == 0) && pixels >= 0,
-                 "gate_backward: C must be 16, 32, 48, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
-                 "gate_backward: tensors must be 16B aligned");
-    if (pixels == 0) return READ_OK;
-    const int half = C < 64 ? C : 64, ppb = GB_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb;
-    if (blocks > 8ll * num_sms()) blocks = 8ll * num_sms();
-    auto k = elu ? gate_bwd_kernel<true, false> : gate_bwd_kernel<false, false>;
-    k<<<(unsigned)blocks, GB_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, half, bias_f, bias_m, bn_scale, bn_mean,
-        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, nullptr, nullptr);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-static long long gate_grid(int64_t pixels, int C)
-{
-    const int ppb = GB_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb;
-    return blocks > 8ll * num_sms() ? 8ll * num_sms() : blocks;
+    return gate_backward_launch<false, false, false>("gate_backward", 1, dy, fm, pixels, C, elu, bias_f, bias_m, bn_scale, bn_mean,
+                                                     bn_inv_std, nullptr, nullptr, dfm, dbias_f, dbias_m, dgamma, dbeta, nullptr,
+                                                     stream);
 }
 
 int read_bn_backward_reduce(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                             const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat, void *stream)
 {
-    RB_CHECK_ARG(dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat, "bn_backward_reduce: null pointer");
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "bn_backward_reduce: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm)) & 15) == 0,
-                 "bn_backward_reduce: tensors must be 16B aligned");
-    auto k = elu ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>;
-    k<<<(unsigned)gate_grid(pixels, C), GB_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
-        bn_inv_std, sum_dy, sum_dy_xhat);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_reduce_launch<false, false>("bn_backward_reduce", 1, dy, fm, pixels, C, elu, bias_f, bias_m, bn_mean, bn_inv_std,
+                                          sum_dy, sum_dy_xhat, nullptr, stream);
 }
 
 int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
@@ -880,50 +867,17 @@ int read_gate_backward_batch_stats(const void *dy, const void *fm, int64_t pixel
                                    const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
                                    void *stream)
 {
-    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat && dbias_f &&
-                     dbias_m,
-                 "gate_backward_batch_stats: null pointer");
-    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "gate_backward_batch_stats: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
-                 "gate_backward_batch_stats: tensors must be 16B aligned");
-    auto k = elu ? gate_bwd_kernel<true, true> : gate_bwd_kernel<false, true>;
-    k<<<(unsigned)gate_grid(pixels, C), GB_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
-        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, nullptr, nullptr, sum_dy, sum_dy_xhat);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-// CTAs per item of the per-item gate passes: the call's CTAs are capped as for a single call of all the items' pixels
-static long long gate_grid_items(int items, int64_t pixels, int C)
-{
-    const int ppb = GB_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb, cap = 8ll * num_sms() / items;
-    if (cap < 1) cap = 1;
-    return blocks > cap ? cap : blocks;
+    return gate_backward_launch<true, false, false>("gate_backward_batch_stats", 1, dy, fm, pixels, C, elu, bias_f, bias_m, bn_scale,
+                                                    bn_mean, bn_inv_std, sum_dy, sum_dy_xhat, dfm, dbias_f, dbias_m, nullptr,
+                                                    nullptr, nullptr, stream);
 }
 
 int read_bn_backward_reduce_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu, const float *bias_f,
                                   const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy,
                                   float *sum_dy_xhat, void *stream)
 {
-    RB_CHECK_ARG(dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat,
-                 "bn_backward_reduce_items: null pointer");
-    RB_CHECK_ARG(items >= 1 && items <= 65535, "bn_backward_reduce_items: items must lie in 1..65535 (got %d)", items);
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "bn_backward_reduce_items: batch statistics need at least 2 pixels per item (got %lld)",
-                 (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm)) & 15) == 0,
-                 "bn_backward_reduce_items: tensors must be 16B aligned");
-    auto k = elu ? bn_bwd_reduce_items_kernel<true> : bn_bwd_reduce_items_kernel<false>;
-    k<<<dim3((unsigned)gate_grid_items(items, pixels, C), (unsigned)items), GB_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
-        bn_inv_std, sum_dy, sum_dy_xhat);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_reduce_launch<false, true>("bn_backward_reduce_items", items, dy, fm, pixels, C, elu, bias_f, bias_m, bn_mean,
+                                         bn_inv_std, sum_dy, sum_dy_xhat, nullptr, stream);
 }
 
 int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
@@ -931,22 +885,9 @@ int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int ite
                                          const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
                                          float *dbias_f, float *dbias_m, void *stream)
 {
-    RB_CHECK_ARG(dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std && sum_dy && sum_dy_xhat && dbias_f &&
-                     dbias_m,
-                 "gate_backward_batch_stats_items: null pointer");
-    RB_CHECK_ARG(items >= 1 && items <= 65535, "gate_backward_batch_stats_items: items must lie in 1..65535 (got %d)", items);
-    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "gate_backward_batch_stats_items: batch statistics need at least 2 pixels per item (got %lld)",
-                 (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(dfm)) & 15) == 0,
-                 "gate_backward_batch_stats_items: tensors must be 16B aligned");
-    auto k = elu ? gate_bwd_items_kernel<true> : gate_bwd_items_kernel<false>;
-    k<<<dim3((unsigned)gate_grid_items(items, pixels, C), (unsigned)items), GB_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
-        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, sum_dy, sum_dy_xhat);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gate_backward_launch<true, false, true>("gate_backward_batch_stats_items", items, dy, fm, pixels, C, elu, bias_f, bias_m,
+                                                   bn_scale, bn_mean, bn_inv_std, sum_dy, sum_dy_xhat, dfm, dbias_f, dbias_m,
+                                                   nullptr, nullptr, nullptr, stream);
 }
 
 int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream)
@@ -1039,69 +980,28 @@ int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wou
 }
 
 // ------------------------------------------------------------------ deterministic entry points
-// CTAs of the deterministic gate passes: at most 2 per SM (the last CTA reads every CTA's row), per item for the per-item forms
-static long long gate_det_grid(int items, int64_t pixels, int C)
-{
-    const int ppb = GB_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb, cap = 2ll * num_sms() / items;
-    if (cap < 1) cap = 1;
-    return blocks > cap ? cap : blocks;
-}
-
-static bool gate_det_ok(int C) { return C >= 16 && C <= GB_MAX_C && C % 16 == 0 && (C <= 64 || C % 64 == 0); }
-
 int64_t read_gate_det_workspace_bytes(int items, int C)
 {
-    if (!gate_det_ok(C) || items < 1 || items > 65535) return -1;
+    if (!gate_channels_ok(C) || items < 1 || items > 65535) return -1;
     const long long ctas = items > 2ll * num_sms() ? items : 2ll * num_sms();
     return 256 + ctas * 4 * C * (int64_t)sizeof(float);
 }
-
-#define GATE_DET_CHECKS(name, items, pixels, minpx, ...)                                                                        \
-    RB_CHECK_ARG(__VA_ARGS__, name ": null pointer");                                                                          \
-    RB_CHECK_ARG(items >= 1 && items <= 65535, name ": items must lie in 1..65535 (got %d)", items);                            \
-    RB_CHECK_ARG(pixels >= minpx, name ": needs at least %d pixels (got %lld)", minpx, (long long)pixels);                      \
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(fm) | reinterpret_cast<uintptr_t>(workspace)) & \
-                  15) == 0,                                                                                                    \
-                 name ": tensors and workspace must be 16B aligned")
 
 int read_gate_backward_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f, const float *bias_m,
                            const float *bn_scale, const float *bn_mean, const float *bn_inv_std, void *dfm, float *dbias_f,
                            float *dbias_m, float *dgamma, float *dbeta, void *workspace, void *stream)
 {
-    GATE_DET_CHECKS("gate_backward_det", 1, pixels, 0, dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean && bn_inv_std &&
-                                                           dbias_f && dbias_m && dgamma && dbeta && workspace);
-    RB_CHECK_ARG(gate_det_ok(C), "gate_backward_det: C must be 16, 32, 48, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_det: tensors must be 16B aligned");
-    if (pixels == 0) return READ_OK;
-    const cudaStream_t st = (cudaStream_t)stream;
-    unsigned *counter = (unsigned *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
-    auto k = elu ? gate_bwd_det_kernel<true, false> : gate_bwd_det_kernel<false, false>;
-    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale, bn_mean,
-        bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, nullptr, nullptr, (float *)((char *)workspace + 256),
-        counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gate_backward_launch<false, true, false>("gate_backward_det", 1, dy, fm, pixels, C, elu, bias_f, bias_m, bn_scale, bn_mean,
+                                                    bn_inv_std, nullptr, nullptr, dfm, dbias_f, dbias_m, dgamma, dbeta, workspace,
+                                                    stream);
 }
 
 int read_bn_backward_reduce_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
                                 const float *bias_m, const float *bn_mean, const float *bn_inv_std, float *sum_dy, float *sum_dy_xhat,
                                 void *workspace, void *stream)
 {
-    GATE_DET_CHECKS("bn_backward_reduce_det", 1, pixels, 2, dy && fm && bias_f && bias_m && bn_mean && bn_inv_std && sum_dy &&
-                                                                sum_dy_xhat && workspace);
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", GB_MAX_C, C);
-    const cudaStream_t st = (cudaStream_t)stream;
-    unsigned *counter = (unsigned *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
-    auto k = elu ? bn_bwd_reduce_det_kernel<true> : bn_bwd_reduce_det_kernel<false>;
-    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
-        bn_inv_std, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256), counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_reduce_launch<true, false>("bn_backward_reduce_det", 1, dy, fm, pixels, C, elu, bias_f, bias_m, bn_mean, bn_inv_std,
+                                         sum_dy, sum_dy_xhat, workspace, stream);
 }
 
 int read_gate_backward_batch_stats_det(const void *dy, const void *fm, int64_t pixels, int C, int elu, const float *bias_f,
@@ -1109,41 +1009,17 @@ int read_gate_backward_batch_stats_det(const void *dy, const void *fm, int64_t p
                                        const float *sum_dy, const float *sum_dy_xhat, void *dfm, float *dbias_f, float *dbias_m,
                                        void *workspace, void *stream)
 {
-    GATE_DET_CHECKS("gate_backward_batch_stats_det", 1, pixels, 2, dy && fm && dfm && bias_f && bias_m && bn_scale && bn_mean &&
-                                                                       bn_inv_std && sum_dy && sum_dy_xhat && dbias_f && dbias_m &&
-                                                                       workspace);
-    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_batch_stats_det: tensors must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    unsigned *counter = (unsigned *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
-    auto k = elu ? gate_bwd_det_kernel<true, true> : gate_bwd_det_kernel<false, true>;
-    k<<<(unsigned)gate_det_grid(1, pixels, C), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
-        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, nullptr, nullptr, sum_dy, sum_dy_xhat,
-        (float *)((char *)workspace + 256), counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gate_backward_launch<true, true, false>("gate_backward_batch_stats_det", 1, dy, fm, pixels, C, elu, bias_f, bias_m,
+                                                   bn_scale, bn_mean, bn_inv_std, sum_dy, sum_dy_xhat, dfm, dbias_f, dbias_m, nullptr,
+                                                   nullptr, workspace, stream);
 }
 
 int read_bn_backward_reduce_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
                                       const float *bias_f, const float *bias_m, const float *bn_mean, const float *bn_inv_std,
                                       float *sum_dy, float *sum_dy_xhat, void *workspace, void *stream)
 {
-    GATE_DET_CHECKS("bn_backward_reduce_items_det", items, pixels, 2, dy && fm && bias_f && bias_m && bn_mean && bn_inv_std &&
-                                                                          sum_dy && sum_dy_xhat && workspace);
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_backward_reduce_items_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    const cudaStream_t st = (cudaStream_t)stream;
-    unsigned *counter = (unsigned *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
-    auto k = elu ? bn_bwd_reduce_items_det_kernel<true> : bn_bwd_reduce_items_det_kernel<false>;
-    k<<<dim3((unsigned)gate_det_grid(items, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
-        bn_inv_std, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256), counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_reduce_launch<true, true>("bn_backward_reduce_items_det", items, dy, fm, pixels, C, elu, bias_f, bias_m, bn_mean,
+                                        bn_inv_std, sum_dy, sum_dy_xhat, workspace, stream);
 }
 
 int read_gate_backward_batch_stats_items_det(const void *dy, const void *fm, int items, int64_t pixels, int C, int elu,
@@ -1151,25 +1027,10 @@ int read_gate_backward_batch_stats_items_det(const void *dy, const void *fm, int
                                              const float *bn_inv_std, const float *sum_dy, const float *sum_dy_xhat, void *dfm,
                                              float *dbias_f, float *dbias_m, void *workspace, void *stream)
 {
-    GATE_DET_CHECKS("gate_backward_batch_stats_items_det", items, pixels, 2, dy && fm && dfm && bias_f && bias_m && bn_scale &&
-                                                                                 bn_mean && bn_inv_std && sum_dy && sum_dy_xhat &&
-                                                                                 dbias_f && dbias_m && workspace);
-    RB_CHECK_ARG(bn_channels_ok(C), "gate_backward_batch_stats_items_det: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)",
-                 GB_MAX_C, C);
-    RB_CHECK_ARG((reinterpret_cast<uintptr_t>(dfm) & 15) == 0, "gate_backward_batch_stats_items_det: tensors must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    unsigned *counter = (unsigned *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
-    auto k = elu ? gate_bwd_items_det_kernel<true> : gate_bwd_items_det_kernel<false>;
-    k<<<dim3((unsigned)gate_det_grid(items, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale,
-        bn_mean, bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, sum_dy, sum_dy_xhat, (float *)((char *)workspace + 256),
-        counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return gate_backward_launch<true, true, true>("gate_backward_batch_stats_items_det", items, dy, fm, pixels, C, elu, bias_f,
+                                                  bias_m, bn_scale, bn_mean, bn_inv_std, sum_dy, sum_dy_xhat, dfm, dbias_f, dbias_m,
+                                                  nullptr, nullptr, workspace, stream);
 }
-
-#undef GATE_DET_CHECKS
 
 static bool wgrad_geom_ok(int Hin, int Win, int Hout, int Wout, int k, int stride)
 {
