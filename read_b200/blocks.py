@@ -203,32 +203,22 @@ class FoldedConv:
 
 def bn_forward(lib, c, g, residual=None):
     """Train-mode BatchNorm of the FoldedConv ``c`` over its identity-epilogue output ``g`` (NHWC bf16, C channels), in place:
-    batch statistics, running-statistics update and y = g * scale + shift [+ residual]."""
-    st, n = L.stream_ptr(), c.norm
-    if c.items is not None:
-        _bn_forward_items(lib, c, g, residual)
-        return
-    P = g.numel() // c.C
-    ws = torch.empty(lib.read_bn_workspace_bytes(c.C), dtype=torch.uint8, device=g.device)
-    L.check(lib.read_bn_batch_stats(g.data_ptr(), P, c.C, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps, n.momentum,
-                                    n.running_mean.data_ptr(), n.running_var.data_ptr(), c.mean.data_ptr(), c.inv.data_ptr(), None,
-                                    c.scale.data_ptr(), c.shift.data_ptr(), ws.data_ptr(), st))
-    n.num_batches_tracked.add_(1)              # torch's own op: bumps the version UNet._weights_version sums
-    L.check(lib.read_bn_apply(g.data_ptr(), P, c.C, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual), g.data_ptr(), st))
-
-
-def _bn_forward_items(lib, c, g, residual):
-    """bn_forward with per-item statistics: item i of ``g`` ([items, H, W, C]) with its own; the running statistics are updated
-    once per item, in item order, and num_batches_tracked advances by the number of items, as that many single-item calls would."""
-    st, n = L.stream_ptr(), c.norm
-    items, P = g.shape[0], g.shape[1] * g.shape[2]
-    ws = torch.empty(lib.read_bn_workspace_bytes_items(items, c.C), dtype=torch.uint8, device=g.device)
-    L.check(lib.read_bn_batch_stats_items(g.data_ptr(), items, P, c.C, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps,
-                                          n.momentum, n.running_mean.data_ptr(), n.running_var.data_ptr(), c.mean.data_ptr(),
-                                          c.inv.data_ptr(), c.scale.data_ptr(), c.shift.data_ptr(), ws.data_ptr(), st))
-    n.num_batches_tracked.add_(items)
-    L.check(lib.read_bn_apply_items(g.data_ptr(), items, P, c.C, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual),
-                                    g.data_ptr(), st))
+    batch statistics, running-statistics update and y = g * scale + shift [+ residual].  With per-item statistics item i of ``g``
+    ([items, H, W, C]) is normalised with its own; the running statistics are updated once per item, in item order, and
+    num_batches_tracked advances by the number of items, as that many single-item calls would."""
+    st, n, C = L.stream_ptr(), c.norm, c.C
+    per_item = c.items is not None
+    items = g.shape[0] if per_item else 1
+    P, form = g.numel() // (items * C), "_items" if per_item else ""
+    ws = torch.empty(lib.read_bn_workspace_bytes_items(items, C) if per_item else lib.read_bn_workspace_bytes(C), dtype=torch.uint8,
+                     device=g.device)
+    head = [g.data_ptr(), *([items] if per_item else []), P, C]
+    L.check(getattr(lib, "read_bn_batch_stats" + form)(*head, c.n_real, c.gamma.data_ptr(), c.beta.data_ptr(), n.eps, n.momentum,
+                                                       n.running_mean.data_ptr(), n.running_var.data_ptr(), c.mean.data_ptr(),
+                                                       c.inv.data_ptr(), *([] if per_item else [None]), c.scale.data_ptr(),
+                                                       c.shift.data_ptr(), ws.data_ptr(), st))
+    n.num_batches_tracked.add_(items)          # torch's own op: bumps the version UNet._weights_version sums
+    L.check(getattr(lib, "read_bn_apply" + form)(*head, c.scale.data_ptr(), c.shift.data_ptr(), L.ptr(residual), g.data_ptr(), st))
 
 
 def conv_forward(lib, src, c, out, residual=None):

@@ -1,10 +1,11 @@
 // Train-mode BatchNorm of the gated convs (read_b200/blocks.py, batch_stats=True): the conv launch writes g = A(f + b_f) *
 // sigmoid(m + b_m) with an identity epilogue (scale 1, shift 0, no residual), then
-//   bn_stats   per-channel mean and biased variance of g over the P pixels of the call, inv_std, the folded scale / shift, and the
-//              in-place running-statistics update (torch.nn.BatchNorm2d's train-mode semantics), all on the device
-//   bn_apply   y = bf16(g * scale + shift [+ residual]), in place over g when the caller wants
-//   bn_stats_items / bn_apply_items: the same per batch item (UNet.train_batchnorm = 'per_item': item i of a call is normalised
-//              with its own statistics, and the running statistics end as B single-item calls would leave them)
+//   bn_stats_kernel<PER_ITEM>   per-channel mean and biased variance of g over the P pixels of the call, inv_std, the folded
+//                               scale / shift, and the in-place running-statistics update (torch.nn.BatchNorm2d's train-mode
+//                               semantics), all on the device
+//   bn_apply_kernel<PER_ITEM>   y = bf16(g * scale + shift [+ residual]), in place over g when the caller wants
+// PER_ITEM = true: the same per batch item (UNet.train_batchnorm = 'per_item': item i of a call is normalised with its own
+// statistics, and the running statistics end as B single-item calls would leave them).
 // The backward's reduction and corrected gate backward live next to the eval-mode gate backward (conv_bwd.cu).
 // The statistics are not fused into the TMA conv kernel's epilogue: its instances render every inference frame.
 #include "common.cuh"
@@ -22,10 +23,10 @@ namespace rb {
 // depend on scheduling and is the same run to run.
 constexpr int BN_THREADS = 256, BN_MAX_C = 256, BN_MAX_CTAS = 512, BN_PART = 3;   // workspace: (count, mean, M2) per CTA, channel
 
-// The body is shared by the call-wide kernel and the per-item one (ITEMS: the caller points g, the outputs, part and counter at
-// one item; var receives the unbiased variance var * P / (P - 1) for the running update and the running statistics are not
-// touched).  Returns whether this CTA was the last one, the one that wrote the outputs.
-template <bool ITEMS>
+// The body of both bn_stats_kernel instances (PER_ITEM: the caller points g, the outputs, part and counter at one item; var
+// receives the unbiased variance var * P / (P - 1) for the running update and the running statistics are not touched).  Returns
+// whether this CTA was the last one, the one that wrote the outputs.
+template <bool PER_ITEM>
 __device__ __forceinline__ bool
 bn_stats_body(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_real, const float *__restrict__ gamma,
               const float *__restrict__ beta, float eps, float momentum, float *__restrict__ running_mean,
@@ -132,12 +133,12 @@ bn_stats_body(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_rea
         const double sc = real ? (double)gamma[c] * is : 0.0;
         mean[c] = (float)mu;
         inv_std[c] = (float)is;
-        if constexpr (!ITEMS) {
+        if constexpr (!PER_ITEM) {
             if (var) var[c] = (float)v;
         }
         scale[c] = (float)sc;
         shift[c] = real ? (float)((double)beta[c] - mu * sc) : 0.f;
-        if constexpr (ITEMS) {
+        if constexpr (PER_ITEM) {
             var[c] = (float)(v * (double)P / (double)(P - 1));
         } else {
             if (real) {
@@ -150,34 +151,12 @@ bn_stats_body(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_rea
     return true;
 }
 
-__global__ void __launch_bounds__(BN_THREADS)
-bn_stats_kernel(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_real, const float *__restrict__ gamma,
-                const float *__restrict__ beta, float eps, float momentum, float *__restrict__ running_mean,
-                float *__restrict__ running_var, float *__restrict__ mean, float *__restrict__ inv_std, float *__restrict__ var,
-                float *__restrict__ scale, float *__restrict__ shift, double *__restrict__ part, unsigned int *__restrict__ counter)
+// The per-item pass's running-statistics update (bn_stats_kernel<true>).  Not a template: a template instance's flag would be laid
+// out after the statistics body's arrays and cost the kernel a byte more of shared memory.
+__device__ __forceinline__ void
+bn_items_running_update(int C, int n_real, float momentum, float *__restrict__ running_mean, float *__restrict__ running_var,
+                        const float *__restrict__ mean, const float *__restrict__ uvar, unsigned int *__restrict__ counter)
 {
-    bn_stats_body<false>(g, P, C, n_real, gamma, beta, eps, momentum, running_mean, running_var, mean, inv_std, var, scale, shift,
-                         part, counter);
-}
-
-// ------------------------------------------------------------------ per-item statistics
-// Item i = blockIdx.y of a call of gridDim.y items, its P pixels the rows [i * P, (i + 1) * P): the same CTA partition (gridDim.x
-// CTAs) and the same combine as bn_stats_kernel on those rows alone, so its mean / inv_std / scale / shift ([items, C]) are
-// bit-identical to a single-item call.  counter[0] counts the items that finished; the last CTA of the last one applies the
-// running-statistics update of every item in item order with bn_stats_kernel's expression, so the running statistics end
-// bit-identical to B single-item calls in a row.  A second counter rather than a follow-up launch: one launch per norm is what a
-// batched call saves.  uvar [items, C] (workspace): each item's unbiased variance.
-__global__ void __launch_bounds__(BN_THREADS)
-bn_stats_items_kernel(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_real, const float *__restrict__ gamma,
-                      const float *__restrict__ beta, float eps, float momentum, float *__restrict__ running_mean,
-                      float *__restrict__ running_var, float *__restrict__ mean, float *__restrict__ inv_std,
-                      float *__restrict__ scale, float *__restrict__ shift, float *__restrict__ uvar, double *__restrict__ part,
-                      unsigned int *__restrict__ counter)
-{
-    const long long it = blockIdx.y, o = it * C;
-    if (!bn_stats_body<true>(g + it * P * C, P, C, n_real, gamma, beta, eps, momentum, nullptr, nullptr, mean + o, inv_std + o,
-                             uvar + o, scale + o, shift + o, part + it * gridDim.x * BN_PART * C, counter + 1 + it))
-        return;
     __shared__ bool all_done;
     __threadfence();
     __syncthreads();
@@ -185,8 +164,8 @@ bn_stats_items_kernel(const __nv_bfloat16 *__restrict__ g, long long P, int C, i
     __syncthreads();
     if (!all_done) return;
     __threadfence();
-    // bn_stats_kernel's (1 - momentum) * r + momentum * x compiles to fma(x, momentum, (1 - momentum) * r); written out here so
-    // that the compiler cannot contract the other product
+    // the call-wide (1 - momentum) * r + momentum * x compiles to fma(x, momentum, (1 - momentum) * r); written out here so that
+    // the compiler cannot contract the other product
     for (int c = threadIdx.x; c < n_real; c += BN_THREADS) {      // padded channels have no running statistics
         float rm = running_mean[c], rv = running_var[c];
         for (unsigned i = 0; i < gridDim.y; ++i) {
@@ -197,6 +176,27 @@ bn_stats_items_kernel(const __nv_bfloat16 *__restrict__ g, long long P, int C, i
         running_var[c] = rv;
     }
     if (threadIdx.x == 0) *counter = 0u;
+}
+
+// PER_ITEM: item i = blockIdx.y of a call of gridDim.y items, its P pixels the rows [i * P, (i + 1) * P): the same CTA partition
+// (gridDim.x CTAs) and the same combine as the call-wide pass on those rows alone, so its mean / inv_std / scale / shift
+// ([items, C]) are bit-identical to a single-item call.  var is uvar (workspace): each item's unbiased variance.  counter[1 + i] is
+// item i's CTA counter and counter[0] counts the items that finished; the last CTA of the last one applies every item's running
+// update in item order with the call-wide expression, so the running statistics end bit-identical to B single-item calls in a
+// row.  A second counter rather than a follow-up launch: one launch per norm is what a batched call saves.
+template <bool PER_ITEM>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_stats_kernel(const __nv_bfloat16 *__restrict__ g, long long P, int C, int n_real, const float *__restrict__ gamma,
+                const float *__restrict__ beta, float eps, float momentum, float *__restrict__ running_mean,
+                float *__restrict__ running_var, float *__restrict__ mean, float *__restrict__ inv_std, float *__restrict__ var,
+                float *__restrict__ scale, float *__restrict__ shift, double *__restrict__ part, unsigned int *__restrict__ counter)
+{
+    const long long it = PER_ITEM ? blockIdx.y : 0, o = it * C;
+    const bool last = bn_stats_body<PER_ITEM>(g + it * P * C, P, C, n_real, gamma, beta, eps, momentum, running_mean, running_var,
+                                              mean + o, inv_std + o, var + o, scale + o, shift + o,
+                                              part + it * gridDim.x * BN_PART * C, counter + (PER_ITEM ? 1 + it : 0));
+    if constexpr (PER_ITEM)
+        if (last) bn_items_running_update(C, n_real, momentum, running_mean, running_var, mean, var, counter);
 }
 
 // ------------------------------------------------------------------ apply
@@ -230,20 +230,96 @@ bn_apply_body(const __nv_bfloat16 *g, long long P, int C, const float *__restric
     }
 }
 
+// PER_ITEM: item blockIdx.y's P rows with its own scale / shift (row blockIdx.y of [items, C])
+template <bool PER_ITEM>
 __global__ void __launch_bounds__(BA_THREADS)
 bn_apply_kernel(const __nv_bfloat16 *g, long long P, int C, const float *__restrict__ scale, const float *__restrict__ shift,
                 const __nv_bfloat16 *__restrict__ residual, __nv_bfloat16 *y)
 {
-    bn_apply_body(g, P, C, scale, shift, residual, y);
+    const long long it = PER_ITEM ? blockIdx.y : 0, o = it * P * C;
+    bn_apply_body(g + o, P, C, scale + it * C, shift + it * C, residual ? residual + o : nullptr, y + o);
 }
 
-// per item: item blockIdx.y's P rows with its own scale / shift (row blockIdx.y of [items, C])
-__global__ void __launch_bounds__(BA_THREADS)
-bn_apply_items_kernel(const __nv_bfloat16 *g, long long P, int C, const float *__restrict__ scale, const float *__restrict__ shift,
-                      const __nv_bfloat16 *__restrict__ residual, __nv_bfloat16 *y)
+// ------------------------------------------------------------------ launchers: the call-wide forms pass items = 1
+// The statistics workspace, from its start: the counters (call-wide 1, per item 1 + items), then per item uvar [items, C], then
+// the CTA partials (count, mean, M2 per CTA and channel) of every item; each block before the partials is rounded up to 256 bytes.
+struct BnWorkspace { int64_t counters, uvar, part, bytes; };     // the number of counters, byte offsets, total bytes
+static BnWorkspace bn_ws_layout(bool per_item, int items, int C)
 {
-    const long long it = blockIdx.y, o = it * P * C;
-    bn_apply_body(g + o, P, C, scale + it * C, shift + it * C, residual ? residual + o : nullptr, y + o);
+    const auto round = [](int64_t b) { return (b + 255) / 256 * 256; };
+    const int64_t counters = per_item ? 1 + items : 1, uvar = round(counters * 4);
+    const int64_t part = uvar + (per_item ? round((int64_t)items * C * 4) : 0);
+    return {counters, uvar, part, part + (int64_t)items * BN_MAX_CTAS * BN_PART * C * (int64_t)sizeof(double)};
+}
+
+// CTAs per item of the statistics pass: at most 2 per SM and BN_MAX_CTAS, so an item's partition is a single-item call's
+static long long bn_stats_grid(int64_t pixels, int C)
+{
+    const int ppb = BN_THREADS / (C / 8);
+    const long long blocks = (pixels + ppb - 1) / ppb, cap = 2ll * num_sms() < BN_MAX_CTAS ? 2ll * num_sms() : BN_MAX_CTAS;
+    return blocks > cap ? cap : blocks;
+}
+
+// CTAs per item of the apply pass: the call's CTAs capped at 16 per SM, as for one call
+static long long bn_apply_grid(int items, int64_t pixels, int C)
+{
+    long long blocks = (pixels * (C / 8) + BA_THREADS - 1) / BA_THREADS, cap = 16ll * num_sms() / items;
+    if (cap < 1) cap = 1;
+    return blocks > cap ? cap : blocks;
+}
+
+// The checks after the first null-pointer check, in each entry point's order: [items], C, for the statistics n_real and its
+// parameter pointers (params: none is null), pixels, for the statistics eps / momentum, then the alignment of the or-ed addr.
+static int bn_pass_checks(const char *name, bool stats, bool per_item, int items, int64_t pixels, int C, int n_real, bool params,
+                          float eps, float momentum, uintptr_t addr)
+{
+    if (per_item) RB_CHECK_ARG(items >= 1 && items <= 65535, "%s: items must lie in 1..65535 (got %d)", name, items);
+    RB_CHECK_ARG(bn_channels_ok(C), "%s: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", name, BN_MAX_C, C);
+    if (stats) {
+        RB_CHECK_ARG(n_real >= 1 && n_real <= C, "%s: n_real must lie in 1..C (got %d, C = %d)", name, n_real, C);
+        RB_CHECK_ARG(params, "%s: null pointer", name);
+    }
+    RB_CHECK_ARG(pixels >= 2, "%s: batch statistics need at least 2 pixels%s (got %lld)", name, per_item ? " per item" : "",
+                 (long long)pixels);
+    if (stats)
+        RB_CHECK_ARG(eps > 0.f && momentum >= 0.f && momentum <= 1.f, "%s: bad eps / momentum (%g, %g)", name, eps, momentum);
+    RB_CHECK_ARG((addr & 15) == 0, "%s: tensors must be 16B aligned", name);
+    return READ_OK;
+}
+
+// var: the call-wide pass's optional output; per item the kernel's var is uvar in the workspace
+template <bool PER_ITEM>
+static int bn_stats_launch(const char *name, const void *g, int items, int64_t pixels, int C, int n_real, const float *gamma,
+                           const float *beta, float eps, float momentum, float *running_mean, float *running_var, float *mean,
+                           float *inv_std, float *var, float *scale, float *shift, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(g && mean && inv_std && scale && shift && workspace, "%s: null pointer", name);
+    if (const int rc = bn_pass_checks(name, true, PER_ITEM, items, pixels, C, n_real, gamma && beta && running_mean && running_var,
+                                      eps, momentum, reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(workspace)))
+        return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const BnWorkspace ws = bn_ws_layout(PER_ITEM, items, C);
+    char *w = (char *)workspace;
+    RB_CUDA(cudaMemsetAsync(w, 0, (size_t)ws.counters * sizeof(unsigned int), st));
+    bn_stats_kernel<PER_ITEM><<<dim3((unsigned)bn_stats_grid(pixels, C), (unsigned)items), BN_THREADS, 0, st>>>(
+        (const __nv_bfloat16 *)g, (long long)pixels, C, n_real, gamma, beta, eps, momentum, running_mean, running_var, mean, inv_std,
+        PER_ITEM ? (float *)(w + ws.uvar) : var, scale, shift, (double *)(w + ws.part), (unsigned int *)w);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+template <bool PER_ITEM>
+static int bn_apply_launch(const char *name, const void *g, int items, int64_t pixels, int C, const float *scale, const float *shift,
+                           const void *residual, void *y, void *stream)
+{
+    RB_CHECK_ARG(g && scale && shift && y, "%s: null pointer", name);
+    const uintptr_t addr = reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(residual) | reinterpret_cast<uintptr_t>(y) |
+                           reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift);
+    if (const int rc = bn_pass_checks(name, false, PER_ITEM, items, pixels, C, 0, true, 0.f, 0.f, addr)) return rc;
+    bn_apply_kernel<PER_ITEM><<<dim3((unsigned)bn_apply_grid(items, pixels, C), (unsigned)items), BA_THREADS, 0, (cudaStream_t)stream>>>(
+        (const __nv_bfloat16 *)g, (long long)pixels, C, scale, shift, (const __nv_bfloat16 *)residual, (__nv_bfloat16 *)y);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
 }
 
 }  // namespace rb
@@ -252,116 +328,39 @@ using namespace rb;
 
 extern "C" {
 
-int64_t read_bn_workspace_bytes(int C)
+int64_t read_bn_workspace_bytes(int C) { return bn_channels_ok(C) ? bn_ws_layout(false, 1, C).bytes : -1; }
+
+int64_t read_bn_workspace_bytes_items(int items, int C)
 {
-    if (!bn_channels_ok(C)) return -1;
-    return 256 + (int64_t)BN_MAX_CTAS * BN_PART * C * (int64_t)sizeof(double);
+    return bn_channels_ok(C) && items >= 1 && items <= 65535 ? bn_ws_layout(true, items, C).bytes : -1;
 }
 
 int read_bn_batch_stats(const void *g, int64_t pixels, int C, int n_real, const float *gamma, const float *beta, float eps,
                         float momentum, float *running_mean, float *running_var, float *mean, float *inv_std, float *var,
                         float *scale, float *shift, void *workspace, void *stream)
 {
-    RB_CHECK_ARG(g && mean && inv_std && scale && shift && workspace, "bn_batch_stats: null pointer");
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_batch_stats: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", BN_MAX_C, C);
-    RB_CHECK_ARG(n_real >= 1 && n_real <= C, "bn_batch_stats: n_real must lie in 1..C (got %d, C = %d)", n_real, C);
-    RB_CHECK_ARG(gamma && beta && running_mean && running_var, "bn_batch_stats: null pointer");
-    RB_CHECK_ARG(pixels >= 2, "bn_batch_stats: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(eps > 0.f && momentum >= 0.f && momentum <= 1.f, "bn_batch_stats: bad eps / momentum (%g, %g)", eps, momentum);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
-                 "bn_batch_stats: tensors must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    const int ppb = BN_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb;
-    const long long cap = 2ll * num_sms() < BN_MAX_CTAS ? 2ll * num_sms() : BN_MAX_CTAS;
-    if (blocks > cap) blocks = cap;
-    unsigned int *counter = (unsigned int *)workspace;
-    RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), st));
-    bn_stats_kernel<<<(unsigned)blocks, BN_THREADS, 0, st>>>((const __nv_bfloat16 *)g, (long long)pixels, C, n_real, gamma, beta,
-                                                            eps, momentum, running_mean, running_var, mean, inv_std, var, scale,
-                                                            shift, (double *)((char *)workspace + 256), counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_stats_launch<false>("bn_batch_stats", g, 1, pixels, C, n_real, gamma, beta, eps, momentum, running_mean, running_var,
+                                  mean, inv_std, var, scale, shift, workspace, stream);
 }
 
 int read_bn_apply(const void *g, int64_t pixels, int C, const float *scale, const float *shift, const void *residual, void *y,
                   void *stream)
 {
-    RB_CHECK_ARG(g && scale && shift && y, "bn_apply: null pointer");
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_apply: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", BN_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "bn_apply: batch statistics need at least 2 pixels (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(residual) | reinterpret_cast<uintptr_t>(y) |
-                   reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift)) & 15) == 0,
-                 "bn_apply: tensors must be 16B aligned");
-    const long long n = pixels * (C / 8);
-    long long blocks = (n + BA_THREADS - 1) / BA_THREADS;
-    if (blocks > 16ll * num_sms()) blocks = 16ll * num_sms();
-    bn_apply_kernel<<<(unsigned)blocks, BA_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)g, (long long)pixels, C, scale, shift, (const __nv_bfloat16 *)residual, (__nv_bfloat16 *)y);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-// ------------------------------------------------------------------ per item
-// workspace of the per-item statistics: the counters (1 + items), uvar [items, C] and the CTA partials of every item
-static int64_t bn_items_counter_bytes(int items) { return ((int64_t)(1 + items) * 4 + 255) / 256 * 256; }
-static int64_t bn_items_uvar_bytes(int items, int C) { return ((int64_t)items * C * 4 + 255) / 256 * 256; }
-
-int64_t read_bn_workspace_bytes_items(int items, int C)
-{
-    if (!bn_channels_ok(C) || items < 1 || items > 65535) return -1;
-    return bn_items_counter_bytes(items) + bn_items_uvar_bytes(items, C) +
-           (int64_t)items * BN_MAX_CTAS * BN_PART * C * (int64_t)sizeof(double);
+    return bn_apply_launch<false>("bn_apply", g, 1, pixels, C, scale, shift, residual, y, stream);
 }
 
 int read_bn_batch_stats_items(const void *g, int items, int64_t pixels, int C, int n_real, const float *gamma, const float *beta,
                               float eps, float momentum, float *running_mean, float *running_var, float *mean, float *inv_std,
                               float *scale, float *shift, void *workspace, void *stream)
 {
-    RB_CHECK_ARG(g && mean && inv_std && scale && shift && workspace, "bn_batch_stats_items: null pointer");
-    RB_CHECK_ARG(items >= 1 && items <= 65535, "bn_batch_stats_items: items must lie in 1..65535 (got %d)", items);
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_batch_stats_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", BN_MAX_C, C);
-    RB_CHECK_ARG(n_real >= 1 && n_real <= C, "bn_batch_stats_items: n_real must lie in 1..C (got %d, C = %d)", n_real, C);
-    RB_CHECK_ARG(gamma && beta && running_mean && running_var, "bn_batch_stats_items: null pointer");
-    RB_CHECK_ARG(pixels >= 2, "bn_batch_stats_items: batch statistics need at least 2 pixels per item (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(eps > 0.f && momentum >= 0.f && momentum <= 1.f, "bn_batch_stats_items: bad eps / momentum (%g, %g)", eps, momentum);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
-                 "bn_batch_stats_items: tensors must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    const int ppb = BN_THREADS / (C / 8);
-    long long blocks = (pixels + ppb - 1) / ppb;                  // per item, as read_bn_batch_stats for `pixels`
-    const long long cap = 2ll * num_sms() < BN_MAX_CTAS ? 2ll * num_sms() : BN_MAX_CTAS;
-    if (blocks > cap) blocks = cap;
-    char *ws = (char *)workspace;
-    unsigned int *counter = (unsigned int *)ws;
-    float *uvar = (float *)(ws + bn_items_counter_bytes(items));
-    double *part = (double *)(ws + bn_items_counter_bytes(items) + bn_items_uvar_bytes(items, C));
-    RB_CUDA(cudaMemsetAsync(counter, 0, (size_t)(1 + items) * sizeof(unsigned int), st));
-    bn_stats_items_kernel<<<dim3((unsigned)blocks, (unsigned)items), BN_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)g, (long long)pixels, C, n_real, gamma, beta, eps, momentum, running_mean, running_var, mean, inv_std,
-        scale, shift, uvar, part, counter);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_stats_launch<true>("bn_batch_stats_items", g, items, pixels, C, n_real, gamma, beta, eps, momentum, running_mean,
+                                 running_var, mean, inv_std, nullptr, scale, shift, workspace, stream);
 }
 
 int read_bn_apply_items(const void *g, int items, int64_t pixels, int C, const float *scale, const float *shift, const void *residual,
                         void *y, void *stream)
 {
-    RB_CHECK_ARG(g && scale && shift && y, "bn_apply_items: null pointer");
-    RB_CHECK_ARG(items >= 1 && items <= 65535, "bn_apply_items: items must lie in 1..65535 (got %d)", items);
-    RB_CHECK_ARG(bn_channels_ok(C), "bn_apply_items: C must be 16, 32, 64 or a multiple of 64 up to %d (got %d)", BN_MAX_C, C);
-    RB_CHECK_ARG(pixels >= 2, "bn_apply_items: batch statistics need at least 2 pixels per item (got %lld)", (long long)pixels);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(residual) | reinterpret_cast<uintptr_t>(y) |
-                   reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(shift)) & 15) == 0,
-                 "bn_apply_items: tensors must be 16B aligned");
-    const long long n = pixels * (C / 8);
-    long long blocks = (n + BA_THREADS - 1) / BA_THREADS, cap = 16ll * num_sms() / items;   // the call's CTAs as for one call
-    if (cap < 1) cap = 1;
-    if (blocks > cap) blocks = cap;
-    bn_apply_items_kernel<<<dim3((unsigned)blocks, (unsigned)items), BA_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)g, (long long)pixels, C, scale, shift, (const __nv_bfloat16 *)residual, (__nv_bfloat16 *)y);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return bn_apply_launch<true>("bn_apply_items", g, items, pixels, C, scale, shift, residual, y, stream);
 }
 
 }  // extern "C"
