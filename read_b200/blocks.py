@@ -268,15 +268,12 @@ def conv_wgrad(lib, dfm, x, B, Hout, Wout, C, k, stride, dwf, dwm, st):
     [B,stride*Hout,stride*Wout,Cin] (NHWC bf16); under torch.use_deterministic_algorithms(True) with the split-K partials added in
     a fixed order."""
     Hin, Win, Cin = x.shape[1], x.shape[2], x.shape[3]
+    args = [dfm.data_ptr(), x.data_ptr(), B, Hin, Win, Hout, Wout, C, Cin, k, stride, dwf.data_ptr(), dwm.data_ptr()]
     if torch.are_deterministic_algorithms_enabled():
         ws = ops.det_workspace(lib.read_conv_wgrad_det_workspace_bytes(B, Hout, Wout, C, Cin, k, stride), dfm.device, "conv wgrad")
-        L.check(lib.read_conv_wgrad_det(dfm.data_ptr(), x.data_ptr(), B, Hin, Win, Hout, Wout, C, Cin, k, stride, dwf.data_ptr(),
-                                        dwm.data_ptr(), ws.data_ptr(), st))
-    elif k == 3 and stride == 1:
-        L.check(lib.read_conv3x3_wgrad(dfm.data_ptr(), x.data_ptr(), B, Hout, Wout, C, Cin, dwf.data_ptr(), dwm.data_ptr(), st))
+        L.check(lib.read_conv_wgrad_det(*args, ws.data_ptr(), st))
     else:
-        L.check(lib.read_conv_wgrad(dfm.data_ptr(), x.data_ptr(), B, Hin, Win, Hout, Wout, C, Cin, k, stride, dwf.data_ptr(),
-                                    dwm.data_ptr(), st))
+        L.check(lib.read_conv_wgrad(*args, st))
 
 
 def _out_grad(gout, C):

@@ -6,11 +6,12 @@
 //                    (conv_tc.cu: read_pack_weights_tc_dgrad); the ResBlock skip enters through its residual operand.  An
 //                    8-channel input (the descriptor pyramid) has its own kernel in this file (dgrad_cin8_kernel)
 //   weight gradient  dW[2C][9][Cin] = sum over pixels of [df | dm]^T x im2col(x): the tensor-core kernel of this file
+//                    (wgrad_kernel; its three entry points launch it through wgrad_launch)
 // The 1x1 and stride-2 3x3 / 4x4 convs of train_precision 'bf16_all' (blocks.py: MultiSourceConvFn) use the same gate backward,
 // the weight-gradient kernel's other instances (read_conv_wgrad) and, for a stride-2 conv, the input-gradient kernel
 // dgrad_s2_kernel of this file; a 1x1 conv's input gradient is a RAW 1x1 plan of the TMA kernel.
 // Both kernels read [f | m] / [df | dm] rows in the column order of the forward RAW output: blocks of 2*half columns
-// (half = min(C, 64), the forward plan's n_tile / 2), the conv_f half of a block first.
+// (half = min(C, 64) = fm_half(C), the forward plan's n_tile / 2), the conv_f half of a block first.
 #include "common.cuh"
 #include "conv_common.cuh"
 #include "ptx.cuh"
@@ -18,6 +19,10 @@
 namespace rb {
 
 __device__ __forceinline__ int fm_col(int co, int half) { return (co / half) * 2 * half + co % half; }
+static int fm_half(int C) { return C < 64 ? C : 64; }
+// the Cout whose [df | dm] in that order the weight-gradient and stride-2 input-gradient passes take: 16, 32, 64 or a multiple
+// of 64 (the gate passes also take 48: gate_channels_ok)
+static bool fm_cout_ok(int Cout) { return Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0)); }
 
 // ------------------------------------------------------------------ gate backward
 // y = scale * A(f + b_f) * sigmoid(m + b_m) + shift, scale = gamma * inv_std, shift = beta - mean * scale:
@@ -306,8 +311,7 @@ bn_bwd_reduce_kernel(const __nv_bfloat16 *__restrict__ dy, const __nv_bfloat16 *
 // partial block: its loads are zero-filled beyond Cin and beyond 2C, and only real (column, channel) pairs are stored.
 // The kernel is a template over the filter size KS and the stride (pad (KS - 1) / 2 rounded up: 0 for 1x1, 1 otherwise):
 // 32 output pixels read the x halo of KR filter rows x (STRIDE * 31 + KS) input pixels, tap (ky, kx) of output pixel p sits at
-// halo pixel STRIDE * p + kx.  A CTA holds the taps of KR filter rows; a 4x4 filter is split into two groups of two rows over
-// blockIdx.z (16 taps would take 128 accumulators per thread), the other sizes keep all rows (KR = KS).
+// halo pixel STRIDE * p + kx.  A CTA holds the taps of KR = wg_rows(KS) filter rows (blockIdx.z: input-channel block x row group).
 constexpr int WG_THREADS = 256, WG_PX = 32, WG_M = 64, WG_N = 32;
 constexpr uint32_t WG_A_BYTES = WG_PX * WG_M * 2;                  // 128-byte rows
 __host__ __device__ constexpr int wg_halo(int KS, int STRIDE) { return STRIDE * (WG_PX - 1) + KS; }
@@ -333,7 +337,7 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4],
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// H, W: the output (= [df | dm]) size; the input x is [B][STRIDE * H][STRIDE * W][Cin] (the callers check Hin == STRIDE * Hout).
+// H, W: the output (= [df | dm]) size; the input x is [B][STRIDE * H][STRIDE * W][Cin] (wgrad_launch checks Hin == STRIDE * Hout).
 // DET (torch.use_deterministic_algorithms): instead of the atomics, split blockIdx.x stores its partial sums to its own copy of
 // the gradients, part[split][2][C][Cin][KS][KS] (conv_f, then conv_m); wgrad_split_sum_kernel adds the copies in split order.
 template <int KS, int STRIDE, int KR, bool DET>
@@ -442,20 +446,13 @@ wgrad_body(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restric
         }
 }
 
-template <int KS, int STRIDE, int KR>
+// the atomic form (DET = false) accumulates into dwf / dwm and ignores part, the DET form writes part and ignores dwf / dwm
+template <int KS, int STRIDE, int KR, bool DET>
 __global__ void __launch_bounds__(WG_THREADS)
 wgrad_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
-             int half, float *__restrict__ dwf, float *__restrict__ dwm)
+             int half, float *__restrict__ dwf, float *__restrict__ dwm, float *__restrict__ part)
 {
-    wgrad_body<KS, STRIDE, KR, false>(dfm, x, B, H, W, C, Cin, half, dwf, dwm, nullptr);
-}
-
-template <int KS, int STRIDE, int KR>
-__global__ void __launch_bounds__(WG_THREADS)
-wgrad_det_kernel(const __nv_bfloat16 *__restrict__ dfm, const __nv_bfloat16 *__restrict__ x, int B, int H, int W, int C, int Cin,
-                 int half, float *__restrict__ part)
-{
-    wgrad_body<KS, STRIDE, KR, true>(dfm, x, B, H, W, C, Cin, half, nullptr, nullptr, part);
+    wgrad_body<KS, STRIDE, KR, DET>(dfm, x, B, H, W, C, Cin, half, dwf, dwm, part);
 }
 
 // dwf[e] / dwm[e] += the splits' copies of element e added in split order, from 0
@@ -467,52 +464,6 @@ __global__ void wgrad_split_sum_kernel(const float *__restrict__ part, int split
         for (int k = 0; k < splits; ++k) s += __ldcg(part + k * 2 * nw + e);
         (e < nw ? dwf : dwm)[e < nw ? e : e - nw] += s;
     }
-}
-
-// the launch geometry of wgrad_kernel<KS, STRIDE, KR>: splits (blockIdx.x), column blocks, input-channel blocks x filter-row groups
-template <int KS, int KR>
-static void wgrad_grid(int B, int H, int W, int Cout, int Cin, long long &s, int &mb, int &nz)
-{
-    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
-    mb = (2 * Cout + WG_M - 1) / WG_M;
-    nz = ((Cin + WG_N - 1) / WG_N) * (KS / KR);
-    s = (2ll * num_sms() + mb * nz - 1) / (mb * nz);
-    if (s > chunks) s = chunks;
-}
-
-template <int KS, int STRIDE, int KR>
-static int launch_wgrad_det(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm,
-                            void *workspace, cudaStream_t st)
-{
-    long long s;
-    int mb, nz;
-    wgrad_grid<KS, KR>(B, H, W, Cout, Cin, s, mb, nz);
-    RB_CHECK_ARG(s <= 0x7FFFFFFF && nz <= 65535 && mb <= 65535, "conv_wgrad_det: too large");
-    float *part = (float *)workspace;
-    wgrad_det_kernel<KS, STRIDE, KR><<<dim3((unsigned)s, mb, nz), WG_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, part);
-    RB_LAUNCH_CHECK();
-    const long long nw = (long long)Cout * Cin * KS * KS;
-    long long blocks = (2 * nw + 255) / 256;
-    if (blocks > 16ll * num_sms()) blocks = 16ll * num_sms();
-    wgrad_split_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(part, (int)s, nw, dwf, dwm);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
-}
-
-template <int KS, int STRIDE, int KR>
-static int launch_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm,
-                        cudaStream_t st)
-{
-    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
-    const int mb = (2 * Cout + WG_M - 1) / WG_M, nz = ((Cin + WG_N - 1) / WG_N) * (KS / KR);
-    long long s = (2ll * num_sms() + mb * nz - 1) / (mb * nz);
-    if (s > chunks) s = chunks;
-    RB_CHECK_ARG(s <= 0x7FFFFFFF && nz <= 65535 && mb <= 65535, "conv_wgrad: too large");
-    wgrad_kernel<KS, STRIDE, KR><<<dim3((unsigned)s, mb, nz), WG_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
 }
 
 // ------------------------------------------------------------------ input gradient of an 8-channel input
@@ -814,7 +765,7 @@ static int gate_backward_launch(const char *name, int items, const void *dy, con
     if (DET) RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
     auto k = elu ? gate_bwd_kernel<true, BATCH, DET, PER_ITEM> : gate_bwd_kernel<false, BATCH, DET, PER_ITEM>;
     k<<<dim3((unsigned)gate_grid(items, DET, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_scale, bn_mean,
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, fm_half(C), bias_f, bias_m, bn_scale, bn_mean,
         bn_inv_std, (__nv_bfloat16 *)dfm, dbias_f, dbias_m, dgamma, dbeta, sum_dy, sum_dy_xhat,
         DET ? (float *)((char *)workspace + 256) : nullptr, counter);
     RB_LAUNCH_CHECK();
@@ -834,8 +785,75 @@ static int bn_reduce_launch(const char *name, int items, const void *dy, const v
     if (DET) RB_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned), st));
     auto k = elu ? bn_bwd_reduce_kernel<true, DET, PER_ITEM> : bn_bwd_reduce_kernel<false, DET, PER_ITEM>;
     k<<<dim3((unsigned)gate_grid(items, DET, pixels, C), (unsigned)items), GB_THREADS, 0, st>>>(
-        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, C < 64 ? C : 64, bias_f, bias_m, bn_mean,
+        (const __nv_bfloat16 *)dy, (const __nv_bfloat16 *)fm, (long long)pixels, C, fm_half(C), bias_f, bias_m, bn_mean,
         bn_inv_std, sum_dy, sum_dy_xhat, DET ? (float *)((char *)workspace + 256) : nullptr, counter);
+    RB_LAUNCH_CHECK();
+    return READ_OK;
+}
+
+// ------------------------------------------------------------------ launcher of the weight gradient
+// The three entry points are forms of one pass: read_conv3x3_wgrad is k = 3, stride 1; DET (read_conv_wgrad_det) stores each
+// split's partial dW in the workspace and adds them in split order with wgrad_split_sum_kernel.
+static bool wgrad_channels_ok(int Cout, int Cin) { return (Cin == 8 || Cin == 16 || (Cin % 32 == 0 && Cin > 0)) && fm_cout_ok(Cout); }
+static bool wgrad_geom_ok(int k, int stride) { return (stride == 1 && (k == 1 || k == 3)) || (stride == 2 && (k == 3 || k == 4)); }
+
+// Filter rows per CTA: a 4x4 filter runs as two groups of two rows over blockIdx.z (16 taps would take 128 accumulators per
+// thread), every other size as one group of all its rows.
+constexpr int wg_rows(int k) { return k == 4 ? 2 : k; }
+
+struct WgradGrid {
+    long long s;   // splits of the 32-pixel row segments (blockIdx.x)
+    int mb, nz;    // column blocks (blockIdx.y), input-channel blocks x filter-row groups (blockIdx.z)
+};
+
+// The one split rule: about 2 CTAs per SM, at most one per segment.  The DET kernel writes s copies of dW into a workspace that
+// read_conv_wgrad_det_workspace_bytes sizes with this same s.
+static WgradGrid wgrad_grid(int k, int B, int H, int W, int Cout, int Cin)
+{
+    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
+    const int mb = (2 * Cout + WG_M - 1) / WG_M, nz = ((Cin + WG_N - 1) / WG_N) * (k / wg_rows(k));
+    const long long s = (2ll * num_sms() + mb * nz - 1) / (mb * nz);
+    return {s < chunks ? s : chunks, mb, nz};
+}
+
+using WgradKernel = void (*)(const __nv_bfloat16 *, const __nv_bfloat16 *, int, int, int, int, int, int, float *, float *, float *);
+template <int KS, int STRIDE>
+static WgradKernel wgrad_instance(bool det)
+{
+    return det ? wgrad_kernel<KS, STRIDE, wg_rows(KS), true> : wgrad_kernel<KS, STRIDE, wg_rows(KS), false>;
+}
+
+// The checks keep each entry point's order and text: read_conv3x3_wgrad passes a geometry that cannot fail them, DET checks the
+// geometry in one message and the workspace with the alignment.
+static int wgrad_launch(const char *name, bool det, const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout,
+                        int Cout, int Cin, int k, int stride, float *dwf, float *dwm, void *workspace, void *stream)
+{
+    RB_CHECK_ARG(dfm && x && dwf && dwm && (!det || workspace), "%s: null pointer", name);
+    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "%s: bad shape", name);
+    const bool geom = wgrad_geom_ok(k, stride), match = geom && Hin == stride * Hout && Win == stride * Wout;
+    if (det) {
+        RB_CHECK_ARG(match, "%s: k=%d stride=%d input %dx%d output %dx%d is not 1x1 / 3x3 stride 1 or 3x3 / 4x4 stride 2 "
+                            "(input = stride x output)", name, k, stride, Hin, Win, Hout, Wout);
+    } else {
+        RB_CHECK_ARG(geom, "%s: k=%d stride=%d is not one of 1x1 / 3x3 stride 1, 3x3 / 4x4 stride 2", name, k, stride);
+        RB_CHECK_ARG(match, "%s: input %dx%d does not match output %dx%d at stride %d (stride 2 needs an even input)", name, Hin, Win,
+                     Hout, Wout, stride);
+    }
+    RB_CHECK_ARG(wgrad_channels_ok(Cout, Cin),
+                 "%s: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", name, Cin, Cout);
+    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
+                 "%s: tensors%s must be 16B aligned", name, det ? " and workspace" : "");
+    const WgradGrid g = wgrad_grid(k, B, Hout, Wout, Cout, Cin);
+    RB_CHECK_ARG(g.s <= 0x7FFFFFFF && g.nz <= 65535 && g.mb <= 65535, "%s: too large", name);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const WgradKernel kernel = k == 1 ? wgrad_instance<1, 1>(det) : stride == 1 ? wgrad_instance<3, 1>(det)
+                             : k == 3 ? wgrad_instance<3, 2>(det) : wgrad_instance<4, 2>(det);
+    kernel<<<dim3((unsigned)g.s, g.mb, g.nz), WG_THREADS, 0, st>>>((const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, Hout,
+                                                                   Wout, Cout, Cin, fm_half(Cout), dwf, dwm, (float *)workspace);
+    RB_LAUNCH_CHECK();
+    if (!det) return READ_OK;
+    const long long nw = (long long)Cout * Cin * k * k;
+    wgrad_split_sum_kernel<<<grid_for(2 * nw), 256, 0, st>>>((const float *)workspace, (int)g.s, nw, dwf, dwm);
     RB_LAUNCH_CHECK();
     return READ_OK;
 }
@@ -892,23 +910,7 @@ int read_gate_backward_batch_stats_items(const void *dy, const void *fm, int ite
 
 int read_conv3x3_wgrad(const void *dfm, const void *x, int B, int H, int W, int Cout, int Cin, float *dwf, float *dwm, void *stream)
 {
-    RB_CHECK_ARG(dfm && x && dwf && dwm, "conv3x3_wgrad: null pointer");
-    RB_CHECK_ARG(B >= 1 && H >= 1 && W >= 1, "conv3x3_wgrad: bad shape");
-    RB_CHECK_ARG((Cin == 8 || Cin == 16 || (Cin % 32 == 0 && Cin > 0)) &&
-                     (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
-                 "conv3x3_wgrad: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin,
-                 Cout);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x)) & 15) == 0,
-                 "conv3x3_wgrad: tensors must be 16B aligned");
-    const long long chunks = (long long)B * H * ((W + WG_PX - 1) / WG_PX);
-    const int mb = (2 * Cout + WG_M - 1) / WG_M, nb = (Cin + WG_N - 1) / WG_N;
-    long long s = (2ll * num_sms() + mb * nb - 1) / (mb * nb);
-    if (s > chunks) s = chunks;
-    RB_CHECK_ARG(s <= 0x7FFFFFFF && nb <= 65535 && mb <= 65535, "conv3x3_wgrad: too large");
-    wgrad_kernel<3, 1, 3><<<dim3((unsigned)s, mb, nb), WG_THREADS, 0, (cudaStream_t)stream>>>(
-        (const __nv_bfloat16 *)dfm, (const __nv_bfloat16 *)x, B, H, W, Cout, Cin, Cout < 64 ? Cout : 64, dwf, dwm);
-    RB_LAUNCH_CHECK();
-    return READ_OK;
+    return wgrad_launch("conv3x3_wgrad", false, dfm, x, B, H, W, H, W, Cout, Cin, 3, 1, dwf, dwm, nullptr, stream);
 }
 
 int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, int B, int H, int W, int Cout, void *dx, void *stream)
@@ -924,42 +926,22 @@ int read_conv3x3_dgrad_cin8(const void *dfm, const float *wf, const float *wm, i
     return launch_dgrad_cin8<128>(dfm, wf, wm, B, H, W, dx, st);
 }
 
-static bool wgrad_channels_ok(int Cout, int Cin)
-{
-    return (Cin == 8 || Cin == 16 || (Cin % 32 == 0 && Cin > 0)) && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0)));
-}
-
 int read_conv_wgrad(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
                     int stride, float *dwf, float *dwm, void *stream)
 {
-    RB_CHECK_ARG(dfm && x && dwf && dwm, "conv_wgrad: null pointer");
-    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_wgrad: bad shape");
-    RB_CHECK_ARG((stride == 1 && (k == 1 || k == 3)) || (stride == 2 && (k == 3 || k == 4)),
-                 "conv_wgrad: k=%d stride=%d is not one of 1x1 / 3x3 stride 1, 3x3 / 4x4 stride 2", k, stride);
-    RB_CHECK_ARG(Hin == stride * Hout && Win == stride * Wout,
-                 "conv_wgrad: input %dx%d does not match output %dx%d at stride %d (stride 2 needs an even input)", Hin, Win, Hout,
-                 Wout, stride);
-    RB_CHECK_ARG(wgrad_channels_ok(Cout, Cin),
-                 "conv_wgrad: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x)) & 15) == 0,
-                 "conv_wgrad: tensors must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (k == 1) return launch_wgrad<1, 1, 1>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
-    if (stride == 1) return launch_wgrad<3, 1, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
-    if (k == 3) return launch_wgrad<3, 2, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
-    return launch_wgrad<4, 2, 2>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, st);
+    return wgrad_launch("conv_wgrad", false, dfm, x, B, Hin, Win, Hout, Wout, Cout, Cin, k, stride, dwf, dwm, nullptr, stream);
 }
 
 int read_pack_weights_dgrad_s2(const float *wf, const float *wm, int Cout, int Cin, int k, void *out_bf16, void *stream)
 {
     RB_CHECK_ARG(wf && wm && out_bf16, "pack_dgrad_s2: null pointer");
     RB_CHECK_ARG(k == 3 || k == 4, "pack_dgrad_s2: k must be 3 or 4 (got %d)", k);
-    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
+    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && fm_cout_ok(Cout),
                  "pack_dgrad_s2: Cin must be a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
     const long long total = (long long)k * k * Cin * 2 * Cout;
     long long blocks = (total + 255) / 256;
     if (blocks > 65535) blocks = 65535;
-    pack_dgrad_s2_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, k, Cout < 64 ? Cout : 64,
+    pack_dgrad_s2_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(wf, wm, Cout, Cin, k, fm_half(Cout),
                                                                              (__nv_bfloat16 *)out_bf16);
     RB_LAUNCH_CHECK();
     return READ_OK;
@@ -970,7 +952,7 @@ int read_conv_dgrad_s2(const void *dfm, const void *wt, int B, int Hout, int Wou
     RB_CHECK_ARG(dfm && wt && dx, "conv_dgrad_s2: null pointer");
     RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_dgrad_s2: bad shape");
     RB_CHECK_ARG(k == 3 || k == 4, "conv_dgrad_s2: k must be 3 or 4 (got %d)", k);
-    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && (Cout == 16 || (Cout % 32 == 0 && Cout > 0 && (Cout <= 64 || Cout % 64 == 0))),
+    RB_CHECK_ARG(Cin % 32 == 0 && Cin > 0 && fm_cout_ok(Cout),
                  "conv_dgrad_s2: Cin must be a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
     RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(wt) | reinterpret_cast<uintptr_t>(dx)) & 15) == 0,
                  "conv_dgrad_s2: tensors must be 16B aligned");
@@ -1032,41 +1014,16 @@ int read_gate_backward_batch_stats_items_det(const void *dy, const void *fm, int
                                                   nullptr, nullptr, workspace, stream);
 }
 
-static bool wgrad_geom_ok(int Hin, int Win, int Hout, int Wout, int k, int stride)
-{
-    return ((stride == 1 && (k == 1 || k == 3)) || (stride == 2 && (k == 3 || k == 4))) && Hin == stride * Hout &&
-           Win == stride * Wout;
-}
-
 int64_t read_conv_wgrad_det_workspace_bytes(int B, int Hout, int Wout, int Cout, int Cin, int k, int stride)
 {
-    if (B < 1 || Hout < 1 || Wout < 1 || !wgrad_channels_ok(Cout, Cin) || !wgrad_geom_ok(stride * Hout, stride * Wout, Hout, Wout, k, stride))
-        return -1;
-    long long s;
-    int mb, nz;
-    if (k == 4) wgrad_grid<4, 2>(B, Hout, Wout, Cout, Cin, s, mb, nz);
-    else if (k == 3) wgrad_grid<3, 3>(B, Hout, Wout, Cout, Cin, s, mb, nz);
-    else wgrad_grid<1, 1>(B, Hout, Wout, Cout, Cin, s, mb, nz);
-    return s * 2 * (int64_t)Cout * Cin * k * k * (int64_t)sizeof(float);
+    if (B < 1 || Hout < 1 || Wout < 1 || !wgrad_channels_ok(Cout, Cin) || !wgrad_geom_ok(k, stride)) return -1;
+    return wgrad_grid(k, B, Hout, Wout, Cout, Cin).s * 2 * (int64_t)Cout * Cin * k * k * (int64_t)sizeof(float);
 }
 
 int read_conv_wgrad_det(const void *dfm, const void *x, int B, int Hin, int Win, int Hout, int Wout, int Cout, int Cin, int k,
                         int stride, float *dwf, float *dwm, void *workspace, void *stream)
 {
-    RB_CHECK_ARG(dfm && x && dwf && dwm && workspace, "conv_wgrad_det: null pointer");
-    RB_CHECK_ARG(B >= 1 && Hout >= 1 && Wout >= 1, "conv_wgrad_det: bad shape");
-    RB_CHECK_ARG(wgrad_geom_ok(Hin, Win, Hout, Wout, k, stride),
-                 "conv_wgrad_det: k=%d stride=%d input %dx%d output %dx%d is not 1x1 / 3x3 stride 1 or 3x3 / 4x4 stride 2 "
-                 "(input = stride x output)", k, stride, Hin, Win, Hout, Wout);
-    RB_CHECK_ARG(wgrad_channels_ok(Cout, Cin),
-                 "conv_wgrad_det: Cin must be 8, 16 or a multiple of 32 and Cout 16, 32, 64 or a multiple of 64 (got %d, %d)", Cin, Cout);
-    RB_CHECK_ARG(((reinterpret_cast<uintptr_t>(dfm) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(workspace)) & 15) == 0,
-                 "conv_wgrad_det: tensors and workspace must be 16B aligned");
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (k == 1) return launch_wgrad_det<1, 1, 1>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
-    if (stride == 1) return launch_wgrad_det<3, 1, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
-    if (k == 3) return launch_wgrad_det<3, 2, 3>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
-    return launch_wgrad_det<4, 2, 2>(dfm, x, B, Hout, Wout, Cout, Cin, dwf, dwm, workspace, st);
+    return wgrad_launch("conv_wgrad_det", true, dfm, x, B, Hin, Win, Hout, Wout, Cout, Cin, k, stride, dwf, dwm, workspace, stream);
 }
 
 }  // extern "C"
