@@ -359,6 +359,39 @@ int read_upsample_bilinear4(const void *in, int act_dtype, int B, int h, int w, 
  * RGB planes [3,H,W] f32 -> [H,W,4] f32 (alpha constant), optionally flipped vertically. */
 int read_frame_to_rgba(const float *rgb_planes, int H, int W, int flip_vertical, float alpha, float *out_hwc4, void *stream);
 
+/* Point-cloud views (the reference viewer's non-neural path: NNScene's GLSL program, READ/gl/programs.py:60-300; DESIGN.md §4.3).
+ * Shades level 0 of a 1-view z-buffer [H,W] (rasterised by any of the entry points above) into [H,W,4] f32, one 16-byte store
+ * per pixel; with flip_vertical, output row y is z-buffer row H-1-y (as read_frame_to_rgba).  An empty pixel gets clear[];
+ * a drawn pixel gets (r, g, b, 1) from its point, id = the key's low 32 bits, clamped to n - 1 for the table reads.
+ * Colour per mode (mode0 of the shader; sub = submode, the shader's mode1), every operation an IEEE round-to-nearest one in
+ * the order written, no contraction; half(v) = v*0.5 + 0.5, normalize(v) = v_i / sqrt((v0*v0 + v1*v1) + v2*v2):
+ *   COLOR   colors[id].rgb (the point colours, or the PCA colours the host computed)
+ *   NORMALS sub 0: half(n);  1: half(normalize(d - (2*dot(n, d))*n)) with d = normalize(cam - p), dot(a, b) = (a0*b0 + a1*b1) + a2*b2;
+ *           2: half(normalize(m_view rows 0..2 . (cam + n, 1))), row i . v = ((m[i0]*v0 + m[i1]*v1) + m[i2]*v2) + m[i3];
+ *           3: half(normalize(cam - p));  4: n
+ *   DEPTH   (c2, c2, c2), c2 = fadd(fma(z, m[10], fma(y, m[9], x*m[8])), m[11]) of total_m: the rasterizer's own clip z
+ *   UV      sub 0: (float(id), 0, 0) of the unclamped id;  1..4: (0, 0, 0)
+ *   XYZ     (p - lo) / ((hi - lo) + 1e-9f) per axis
+ *   LABEL   (n.x / 255, 0, 0)
+ * with p = xyz[id] ([n,3] f32), n = normals[id].xyz.  colors and normals are [n,4] f32 rows (16-byte aligned); a table the mode
+ * does not read may be NULL.  A zero vector normalises to NaN. */
+enum { READ_VIEW_COLOR = 0, READ_VIEW_NORMALS = 1, READ_VIEW_DEPTH = 2, READ_VIEW_UV = 3, READ_VIEW_XYZ = 4, READ_VIEW_LABEL = 5 };
+typedef struct {
+    int32_t mode;            /* READ_VIEW_* */
+    int32_t submode;         /* 0..4 */
+    const float *colors;     /* [n,4] f32 */
+    const float *normals;    /* [n,4] f32 */
+    const float *xyz;        /* [n,3] f32 */
+    int64_t n;               /* rows of the tables (>= 1 when the mode reads one) */
+    float total_m[16];       /* row-major proj @ inv(view), as the rasterizer took it */
+    float m_view[16];        /* row-major inv(view) */
+    float cam[3];            /* view[:3, 3] */
+    float lo[3], hi[3];      /* the cloud's per-axis min and max */
+    float clear[4];
+    int32_t flip_vertical;
+} read_point_view_desc;
+int read_point_view(const uint64_t *zbuf_level0, int H, int W, const read_point_view_desc *desc, float *out_hwc4, void *stream);
+
 /* Net-input staging for NetAndTexture's viewer options on the fused path (READ/models/compose.py:162-171): src = f32 NHWC
  * features [B,hs,ws,C] at render resolution; factor = supersampling (bilinear reduce exactly as F.interpolate(scale_factor=1/ss,
  * mode='bilinear')); last (nullable) = f32 [B,hs/factor,ws/factor,C] temporal-average state: out = (cur + last) / 2 when

@@ -63,6 +63,16 @@ class ReadSpriteDesc(ctypes.Structure):
     _fields_ = [("size", ctypes.c_float * MAX_LEVELS), ("relative", ctypes.c_int32 * MAX_LEVELS), ("point_sizes", c_vp)]
 
 
+VIEW_MODES = {"color": 0, "normals": 1, "depth": 2, "uv": 3, "xyz": 4, "label": 5}   # READ_VIEW_*
+
+
+class ReadPointViewDesc(ctypes.Structure):
+    _fields_ = [("mode", ctypes.c_int32), ("submode", ctypes.c_int32), ("colors", c_vp), ("normals", c_vp), ("xyz", c_vp),
+                ("n", c_i64), ("total_m", ctypes.c_float * 16), ("m_view", ctypes.c_float * 16), ("cam", ctypes.c_float * 3),
+                ("lo", ctypes.c_float * 3), ("hi", ctypes.c_float * 3), ("clear", ctypes.c_float * 4),
+                ("flip_vertical", ctypes.c_int32)]
+
+
 class ReadHaloDesc(ctypes.Structure):
     _fields_ = [("src_up", c_vp), ("src_dn", c_vp), ("peer_up_slot", c_vp), ("peer_dn_slot", c_vp),
                 ("peer_up_flag", c_vp), ("peer_dn_flag", c_vp), ("slot_from_up", c_vp), ("slot_from_dn", c_vp),
@@ -193,6 +203,7 @@ _SIGS = {
     "read_conv_plan_destroy": (None, [c_vp]),
     "read_upsample_bilinear4": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_frame_to_rgba": (c_int, [c_vp, c_int, c_int, c_int, ctypes.c_float, c_vp, c_vp]),
+    "read_point_view": (c_int, [c_vp, c_int, c_int, ctypes.POINTER(ReadPointViewDesc), c_vp, c_vp]),
     "read_nchw_f32_to_nhwc": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_nhwc_to_nchw_f32": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "read_launch_count": (c_i64, []),

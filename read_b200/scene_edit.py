@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import ops
+from . import point_views
 from . import sprites
 from .texture import PointTexture
 
@@ -61,6 +62,7 @@ class SceneComposer:
         self._seg_is_scene = np.empty((0,), dtype=bool)
         self._seg_own_vis = np.empty((0,), dtype=bool)
         self._seg_of = {}        # (kind, index) of an object or instance -> its segment
+        self._tables = {}        # composed [total, 4] attribute tables, built on first use after a scene is added
         self.total = 0
 
     # ------------------------------------------------------------------ layout
@@ -69,12 +71,15 @@ class SceneComposer:
         if n > ops.MAX_SEGMENTS:
             raise ValueError(f"read_b200: a composed scene holds at most {ops.MAX_SEGMENTS} segments (scenes + objects + instances)")
 
-    def add_scene(self, xyz, texture, placement=None, point_sizes=None):
+    def add_scene(self, xyz, texture, placement=None, point_sizes=None, colors=None, normals=None):
         """Add a cloud ``xyz`` [N,3] with its descriptors (``[1,8,N]`` tensor or ``PointTexture``) and an optional 4x4
         ``placement`` into the composed world.  Returns the scene's handle; its points' global ids are ``handle.base + id``.
-        ``point_sizes``: optional [N] per-point sprite sizes (read_b200.sprites), shared by the scene's objects and instances."""
+        ``point_sizes``: optional [N] per-point sprite sizes (read_b200.sprites), shared by the scene's objects and instances.
+        ``colors`` / ``normals``: optional [N,3] per-point attributes for ``SceneRenderer.render_points``, shared likewise."""
         n = int(xyz.shape[0])
         sizes = None if point_sizes is None else sprites.check_point_sizes(point_sizes, n)
+        attrs = {k: None if v is None else point_views.attribute_table(v, n, k, self.device)
+                 for k, v in (("colors", colors), ("normals", normals))}
         if self.total + n >= 1 << 31:
             raise ValueError(f"read_b200: a composed scene of {self.total + n} points is too large; point ids must stay below 2^31")
         activation = texture.activation if isinstance(texture, PointTexture) else 'none'
@@ -96,7 +101,8 @@ class SceneComposer:
         h = _Handle("scene", len(self._scenes))
         h.base = self.total
         self._scenes.append(dict(xyz=xyz.to(self.device).contiguous(), base=self.total, n=n, P=P, visible=True, objects=[],
-                                 sizes=None if sizes is None else sizes.to(self.device)))
+                                 sizes=None if sizes is None else sizes.to(self.device), **attrs))
+        self._tables = {}
         self._scene_P = np.concatenate([self._scene_P, P[None]])
         self._scene_vis = np.append(self._scene_vis, True)
         self.total += n
@@ -196,6 +202,25 @@ class SceneComposer:
         if self._tex is None:
             raise ValueError("read_b200: the composition holds no scene")
         return self._tex
+
+    @property
+    def colors(self):
+        """The scenes' colours as one [total, 4] f32 table in global-id order (zeros for a scene without), or None if no scene
+        has colours."""
+        return self._table("colors")
+
+    @property
+    def normals(self):
+        """The scenes' normals, as ``colors``."""
+        return self._table("normals")
+
+    def _table(self, name):
+        if name not in self._tables:
+            parts = [sc[name] for sc in self._scenes]
+            self._tables[name] = None if all(p is None for p in parts) else torch.cat(
+                [torch.zeros((sc["n"], 4), dtype=torch.float32, device=self.device) if p is None else p
+                 for sc, p in zip(self._scenes, parts)])
+        return self._tables[name]
 
     @property
     def store(self):

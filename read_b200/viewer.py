@@ -11,6 +11,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from . import point_views
 from . import sprites
 from .compose import NetAndTexture
 from .texture import PointTexture
@@ -19,7 +20,8 @@ from .unet import UNet
 
 class FrameRenderer:
     def __init__(self, xyz, net_state_dict, texture, viewport_size, supersampling=1, temporal_average=False,
-                 device=None, flip_vertical=False, n_levels=4, return_net_input=True, input_format=None, point_sizes=None):
+                 device=None, flip_vertical=False, n_levels=4, return_net_input=True, input_format=None, point_sizes=None,
+                 colors=None, normals=None):
         """xyz: [N,3] float32 (numpy / tensor); net_state_dict: UNet checkpoint ``state_dict``; texture: the
         ``[1,8,N]`` descriptor tensor (``PointTexture.texture_``) or a ``PointTexture``; viewport_size: (W, H) of the output
         frame.  ``supersampling`` / ``temporal_average``: the options of READ/gl/nn.py:76,100-103 (the pyramid is rendered at
@@ -27,7 +29,9 @@ class FrameRenderer:
         path.  ``return_net_input=False`` skips materialising the reference's ``net_input`` list (4 small transposes).
         ``input_format``: the checkpoint's format string (``args.input_format``); its first ``n_levels`` keys' ``_pN`` / ``_psN``
         point sizes are drawn as point sprites (read_b200.sprites).  ``point_sizes``: optional [N] per-point sizes (the scene's
-        ``point_sizes``), which replace the keys' sizes where > 0; without ``input_format`` every level is a ``_p1`` key."""
+        ``point_sizes``), which replace the keys' sizes where > 0; without ``input_format`` every level is a ``_p1`` key.
+        ``colors`` / ``normals``: optional [N,3] per-point colours (``scene_data['pointcloud']['rgb']``) and normals, the
+        attributes ``render_points`` draws; uploaded once."""
         W, H = int(viewport_size[0]), int(viewport_size[1])
         factor = 16
         assert W % 16 == 0, f'set width {factor * (W // factor)}'          # READ/gl/nn.py:107-109
@@ -68,6 +72,12 @@ class FrameRenderer:
         self._cam_host = [torch.empty((1, 4, 4), dtype=torch.float32).pin_memory() for _ in range(4)]
         self._cam_used = [None] * 4
         self._cam_i = 0
+        n = self.xyz.shape[0]
+        self.colors = None if colors is None else point_views.attribute_table(colors, n, "colors", self.device)
+        self.normals = None if normals is None else point_views.attribute_table(normals, n, "normals", self.device)
+        self._views = point_views.ViewState(W, H, self.device)
+        self._points_store = None          # sorted store for point-sprite views when the frame path keeps none
+        self._bounds = None
 
     def _upload_camera(self, total_m):
         i = self._cam_i
@@ -110,6 +120,42 @@ class FrameRenderer:
                                              rgba.data_ptr(), L.stream_ptr()))
         return {'output': rgba, 'net_input': net_input}
 
+    def render_points(self, proj_matrix, view_matrix, mode='color', submode=0, point_size=1, relative=False,
+                      clear_color=(0., 0., 0., 1.)):
+        """The reference viewer's point-cloud view (viewer.py:263-285): -> {'output': [H,W,4] f32 cuda tensor}, a fresh tensor whose
+        rows are in ``infer``'s order (flipped the same way with ``flip_vertical``).  Each pixel shows its winning point (the
+        z-buffer's minimum depth, ties to the lowest id) coloured by ``mode``: 'color' (the ``colors`` table), 'pca' (a 3-component
+        PCA of the descriptors, ``--pca``), 'normals' (``submode`` 0..4: model, reflection, camera frame, view direction, raw),
+        'depth' (clip-space z), 'uv' (submode 0: the point id), 'xyz' (position in the cloud's bounding box) or 'label' (normal x
+        / 255); an empty pixel gets ``clear_color``.  ``point_size`` (1..64) and ``relative`` (size / clip z) draw point sprites
+        with the scene's per-point sizes, as the frame path's ``_pN`` / ``_psN`` keys do; a per-point size of 0 keeps
+        ``point_size`` (GL would draw such a point at size 0).  Arithmetic: include/read_b200.h, read_point_view."""
+        clear = point_views.check_view_args(mode, submode, point_size, clear_color)
+        table = point_views.table_for(mode, self.colors, self.normals,
+                                      lambda: self._views.pca(self.model._texture(0).texture_))
+        total = self.total_matrix(proj_matrix, view_matrix)
+        m = self._upload_camera(total)
+        pyr = self._views.pyramid()
+        store = self.store
+        with torch.no_grad():
+            if point_size != 1 or relative or (store is not None and store.psize is not None):
+                if store is None:
+                    if self._points_store is None:
+                        self._points_store = ops.SortedPoints(self.xyz)
+                    store = self._points_store
+                ops.raster_project_sprites(pyr, store, m, [(float(point_size), bool(relative))])
+            elif store is not None:
+                ops.raster_project_sorted(pyr, store, m)
+            else:
+                ops.raster_project(pyr, self.xyz, m)
+            if mode == 'xyz' and self._bounds is None:
+                self._bounds = (self.xyz.min(0).values.cpu().numpy(), self.xyz.max(0).values.cpu().numpy())
+            lo, hi = self._bounds if mode == 'xyz' else ((0., 0., 0.), (0., 0., 0.))
+            geometry = mode in ('normals', 'depth', 'xyz')
+            out = point_views.shade(pyr, mode, submode, table, self.xyz if geometry else None, total, view_matrix, lo, hi,
+                                    clear, self.flip_vertical)
+        return {'output': out}
+
 
 class SceneRenderer:
     """``FrameRenderer`` for a composed scene (read_b200.scene_edit.SceneComposer): several scenes, moved / hidden / instanced
@@ -147,6 +193,7 @@ class SceneRenderer:
         self._m_host = [torch.empty(ops.MAX_SEGMENTS * 65, dtype=torch.uint8).pin_memory() for _ in range(4)]
         self._m_used = [None] * 4
         self._m_i = 0
+        self._views = point_views.ViewState(W, H, self.device)
 
     def _upload(self, seg_m, visible):
         """-> (seg_m, visible) on the device: [nseg, 1, 4, 4] f32 and [nseg] uint8."""
@@ -183,3 +230,27 @@ class SceneRenderer:
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
                                              rgba.data_ptr(), L.stream_ptr()))
         return {'output': rgba, 'net_input': net_input}
+
+    def render_points(self, proj_matrix, view_matrix, mode='color', submode=0, point_size=1, relative=False,
+                      clear_color=(0., 0., 0., 1.)):
+        """``FrameRenderer.render_points`` for the composed scene, in the modes a pixel's id alone determines: 'color', 'pca' (over
+        the composed descriptor table), 'uv' (the global id) and 'label', with the tables of ``SceneComposer.add_scene``
+        concatenated in global-id order.  'normals', 'depth' and 'xyz' need the point's world position, which an instance's
+        id does not give (every instance of an object carries the object's ids): they raise ValueError."""
+        clear = point_views.check_view_args(mode, submode, point_size, clear_color)
+        if mode not in point_views.ID_MODES:
+            raise ValueError(f"read_b200: mode {mode!r} needs the point's world position, which a composed scene's ids do not "
+                             f"identify; a composed scene draws the modes {point_views.ID_MODES}")
+        comp = self.composer
+        table = point_views.table_for(mode, comp.colors, comp.normals, lambda: self._views.pca(comp.texture.texture_))
+        store = comp.store
+        seg_m, visible = self._upload(comp.segment_matrices(FrameRenderer.total_matrix(proj_matrix, view_matrix)),
+                                      store.visible_flags())
+        pyr = self._views.pyramid()
+        with torch.no_grad():
+            if point_size != 1 or relative or store.psize is not None:
+                ops.raster_project_sprites(pyr, store, seg_m, [(float(point_size), bool(relative))], visible=visible)
+            else:
+                ops.raster_project_segments_culled(pyr, store, seg_m, visible)
+            out = point_views.shade(pyr, mode, submode, table, None, None, None, None, None, clear, self.flip_vertical)
+        return {'output': out}
