@@ -8,7 +8,8 @@ per pyramid level, READ/models/texture.py:55-63) and a dense ``torch.optim.RMSpr
   accumulator and flags the touched points (``texture_.grad`` stays ``None``: nothing dense is ever materialised);
 * ``SparseRMSprop`` is a drop-in for the reference's descriptor optimizer (same hyper-parameters, ``param_groups`` whose ``lr`` the
   pipeline rescales, ``step() / zero_grad() / state_dict()``): it updates only touched points, with the skipped ``square_avg``
-  decays applied lazily - the result equals the dense optimizer's.  ``PointTexture.reg_loss`` (``--reg_weight``) in sparse mode
+  decays applied lazily - the result equals the dense optimizer's.  With weight decay every point has a gradient, so every
+  point is updated on every step.  ``PointTexture.reg_loss`` (``--reg_weight``) in sparse mode
   back-propagates one scalar per texture (``_RegLoss``), and the step after it updates every point with that term added;
 * ``exchange_sparse_grads`` is the data-parallel join: ranks all-gather their touched ``(id, grad[D])`` rows (a few MB) instead
   of all-reducing ``[N, D]`` gradients or re-broadcasting the texture as ``nn.DataParallel`` does (train.py:138-139).
@@ -111,7 +112,10 @@ class SparseRMSprop:
     """RMSprop (torch defaults: alpha 0.99, eps 1e-8, no momentum, not centered) over PointTexture descriptors, touching only the
     points that received a gradient since the last step.  ``textures``: one PointTexture or a list (one param group each, like the
     reference's multi-scene ``extra_optimizer``, ogl.py:136-144).  A texture whose regulariser was back-propagated since its last
-    step (a pending ``reg_coef``) gets the dense-term step instead: every point, with g = accumulated row + reg_coef * param."""
+    step (a pending ``reg_coef``) gets the dense-term step instead: every point, with g = accumulated row + reg_coef * param.
+    A param group with ``weight_decay != 0`` takes that every-point step on every step (with a zero coefficient when no
+    regulariser is pending): torch.optim.RMSprop adds weight_decay * param to the zero gradient of a point outside the batch, so
+    with weight decay every point moves every step, and skipping the untouched ones would not give the dense optimizer's result."""
 
     def __init__(self, textures, lr=1e-2, alpha=0.99, eps=1e-8, weight_decay=0.0):
         if not isinstance(textures, (list, tuple)):
@@ -132,6 +136,12 @@ class SparseRMSprop:
                                       "last_step": torch.zeros((sp.N,), dtype=torch.int32, device=t.texture_.device)}
         return st
 
+    def _zero_coef(self, t):
+        z = getattr(self, "_zero", None)
+        if z is None or z.device != t.texture_.device:
+            z = self._zero = torch.zeros((), dtype=torch.float32, device=t.texture_.device)
+        return z
+
     def zero_grad(self, set_to_none=True):
         """Gradient rows are cleared by ``step`` itself; calling this before the first backward is harmless."""
         for t in self.textures:
@@ -148,11 +158,13 @@ class SparseRMSprop:
             args = (t.texture_.data_ptr(), shadow.data_ptr(), sp.grad.data_ptr(), sp.touched.data_ptr(), st["square_avg"].data_ptr(),
                     st["last_step"].data_ptr(), sp.N, sp.D, self._steps, float(g["lr"]), float(g["alpha"]), float(g["eps"]),
                     float(g["weight_decay"]))
-            if sp.reg_coef is None:
-                L.check(lib.read_sparse_rmsprop_step(*args, sp_))
-            else:                                    # the regulariser's gradient reaches every point: the dense-term step
+            if sp.reg_coef is not None:              # the regulariser's gradient reaches every point: the dense-term step
                 coef, sp.reg_coef = sp.reg_coef, None
                 L.check(lib.read_sparse_rmsprop_step_reg(*args, coef.data_ptr(), sp_))
+            elif float(g["weight_decay"]) != 0.0:    # so does weight decay's: the same step with a zero coefficient
+                L.check(lib.read_sparse_rmsprop_step_reg(*args, self._zero_coef(t).data_ptr(), sp_))
+            else:
+                L.check(lib.read_sparse_rmsprop_step(*args, sp_))
         return loss
 
     def dense_square_avg(self, t):
