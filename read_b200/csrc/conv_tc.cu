@@ -431,8 +431,11 @@ gated_conv_tc_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ 
 // Warp roles: the producer warp as above; each consumer warpgroup takes whole tiles (the CTA's even / odd ones), so one
 // warpgroup's epilogue runs under the other's MMAs.  One CTA per SM (72 + 64 registers per thread are live across the MMAs).
 constexpr int WS_E_STAGES = 4;                 // two per consumer warpgroup: tile k uses stage k % 4
-constexpr uint32_t WS_ROW_BYTES = (TC_TW + 2) * 16u;                  // one halo row of one 8-channel chunk
-constexpr uint32_t WS_CHUNK_BYTES = ((TC_TH + 2) * WS_ROW_BYTES + 127u) & ~127u;   // TMA destinations are 128 B aligned
+// one halo row of one 8-channel chunk, and the chunk, of a TW x TH-pixel tile (TMA destinations are 128 B aligned)
+__host__ __device__ constexpr uint32_t ws_row_bytes(int tw) { return (uint32_t)(tw + 2) * 16u; }
+__host__ __device__ constexpr uint32_t ws_chunk_bytes(int tw, int th) { return ((uint32_t)(th + 2) * ws_row_bytes(tw) + 127u) & ~127u; }
+constexpr uint32_t WS_ROW_BYTES = ws_row_bytes(TC_TW);
+constexpr uint32_t WS_CHUNK_BYTES = ws_chunk_bytes(TC_TW, TC_TH);
 constexpr uint32_t WS_BLOCK_BYTES = 128u * 32u * 2u;   // one 32-channel block of an epilogue stage
 
 // The shared memory of a weight-stationary body with E epilogue stages, from its 1 KB aligned base (offsets and sizes:
@@ -440,7 +443,7 @@ constexpr uint32_t WS_BLOCK_BYTES = 128u * 32u * 2u;   // one 32-channel block o
 template <int E>
 struct WsSmem {
     uint32_t base, b_region, e_region;
-    uint32_t afull0, aempty0, bres, efull0, eempty0;
+    uint32_t afull0, aempty0, bfull0, bempty0, bres, efull0, eempty0;
     float4 *par;
     __device__ __forceinline__ explicit WsSmem(const TcArgs &a)
     {
@@ -451,15 +454,16 @@ struct WsSmem {
         uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (base - s_u32(smem_raw)) + a.e_region_off + E * a.e_bytes);
         const uint32_t bar0 = s_u32(bars);
         afull0 = bar0 + 8 * BAR_AFULL, aempty0 = bar0 + 8 * BAR_AEMPTY, bres = bar0 + 8 * BAR_BRES;
+        bfull0 = bar0 + 8 * BAR_BFULL, bempty0 = bar0 + 8 * BAR_BEMPTY;
         efull0 = bar0 + 8 * tc_bar_slots(E).efull, eempty0 = bar0 + 8 * tc_bar_slots(E).eempty;
         par = reinterpret_cast<float4 *>(bars + tc_bar_slots(E).params);
     }
 };
 
-// Prologue of the weight-stationary bodies (C = 32 and 64 channels): per-channel parameters, descriptor prefetch, and
-// the barriers, with a_arrivals per halo stage (the warps that read it) and e_arrivals per epilogue stage (the warpgroups that
-// store from it).
-template <int E>
+// Prologue of the role-swapped bodies: per-channel parameters, descriptor prefetch, and the barriers, with a_arrivals per
+// halo stage (the warps that read it; with STREAMED weights also per weight stage) and e_arrivals per epilogue stage (the
+// warpgroups that store from it).
+template <int E, bool STREAMED = false>
 __device__ __forceinline__ void ws_prologue(const WsSmem<E> &sm, const TcMaps &tm, const CUtensorMap &tmB, const TcArgs &a,
                                             uint32_t a_arrivals, uint32_t e_arrivals)
 {
@@ -473,6 +477,11 @@ __device__ __forceinline__ void ws_prologue(const WsSmem<E> &sm, const TcMaps &t
             mbar_init(sm.afull0 + 8 * s, 1);
             mbar_init(sm.aempty0 + 8 * s, a_arrivals);
         }
+        if (STREAMED)
+            for (int s = 0; s < a.b_stages; ++s) {
+                mbar_init(sm.bfull0 + 8 * s, 1);
+                mbar_init(sm.bempty0 + 8 * s, a_arrivals);
+            }
         for (int s = 0; s < E; ++s) {
             mbar_init(sm.efull0 + 8 * s, 1);
             mbar_init(sm.eempty0 + 8 * s, e_arrivals);
@@ -483,11 +492,11 @@ __device__ __forceinline__ void ws_prologue(const WsSmem<E> &sm, const TcMaps &t
     __syncthreads();
 }
 
-// Producer: tile tc's halo into the next stage (as, aph) of the halo ring, as C / 8 unswizzled 8-channel chunks from pixel
-// (x0 - 1, y0 - 1)
-template <int C, int E>
+// Producer: the halo of tile tc (TW x TH pixels from (x0, y0)) into the next stage (as, aph) of the halo ring, as C / 8
+// unswizzled 8-channel chunks of input channels c0 .. c0 + C - 1 from pixel (x0 - 1, y0 - 1)
+template <int C, int E, int TW = TC_TW, int TH = TC_TH>
 __device__ __forceinline__ void ws_load_halo(const WsSmem<E> &sm, const TcMaps &tm, const TcArgs &a, const TileCoord &tc,
-                                             uint32_t &as, uint32_t &aph)
+                                             uint32_t &as, uint32_t &aph, int c0 = 0)
 {
     mbar_wait(sm.aempty0 + 8 * as, aph ^ 1u);
     if (elect_one()) {
@@ -495,17 +504,17 @@ __device__ __forceinline__ void ws_load_halo(const WsSmem<E> &sm, const TcMaps &
         mbar_arrive_expect_tx(full, a.a_tx_bytes);
 #pragma unroll
         for (int c = 0; c < C / 8; ++c)
-            tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * WS_CHUNK_BYTES, 8 * c, tc.tx * TC_TW - 1, tc.ty * TC_TH - 1, tc.b);
+            tma_load_4d(&tm.a[0], full, dst + (uint32_t)c * ws_chunk_bytes(TW, TH), c0 + 8 * c, tc.tx * TW - 1, tc.ty * TH - 1, tc.b);
     }
     __syncwarp();
     if (++as == (uint32_t)a.a_stages) { as = 0; aph ^= 1u; }
 }
 
-// Producer: tile tc's residual into the next epilogue stage (es, eph), as C / 32 boxes of 32 channels, block h at h * 8 KB; a
-// plain arrival without a residual
-template <int C, int E>
+// Producer: the residual of tile tc (TW x TH pixels), output channels c0 .. c0 + C - 1, into the next epilogue stage (es, eph),
+// as C / 32 boxes of 32 channels, block h at h * TW * TH * 64 bytes; a plain arrival without a residual
+template <int C, int E, int TW = TC_TW, int TH = TC_TH>
 __device__ __forceinline__ void ws_load_residual(const WsSmem<E> &sm, const TcMaps &tm, const TcArgs &a, const TileCoord &tc,
-                                                 uint32_t &es, uint32_t &eph)
+                                                 uint32_t &es, uint32_t &eph, int c0 = 0)
 {
     mbar_wait(sm.eempty0 + 8 * es, eph ^ 1u);
     if (elect_one()) {
@@ -514,27 +523,32 @@ __device__ __forceinline__ void ws_load_residual(const WsSmem<E> &sm, const TcMa
         if (a.epi.residual)
 #pragma unroll
             for (int h = 0; h < C / 32; ++h)
-                tma_load_4d(&tm.res, full, dst + (uint32_t)h * WS_BLOCK_BYTES, 32 * h, tc.tx * TC_TW, tc.ty * TC_TH, tc.b);
+                tma_load_4d(&tm.res, full, dst + (uint32_t)h * (TW * TH * 64u), c0 + 32 * h, tc.tx * TW, tc.ty * TH, tc.b);
     }
     __syncwarp();
     if (++es == (uint32_t)E) { es = 0; eph ^= 1u; }
 }
 
-// Consumer: tile rows j0 .. j0 + 3 of the epilogue, in place in the warpgroup's 64-byte-swizzled [128 px][32 ch] block st of an
-// epilogue stage.  acc holds both gates of this thread's channel (parameters par) for two pixels of every tile row.  The
-// residual comes in with ldmatrix.trans, the arithmetic is epilogue_smem's per element, and the bf16 output goes back with
-// stmatrix.trans.
-__device__ __forceinline__ void ws_epilogue_rows(const float (&acc)[64], int j0, uint32_t st, float4 par, const EpiArgs &e)
+// Consumer: NR (4 or 1) tile rows j0 .. of the epilogue, pixels x0 .. x0 + 7 of each, in place in the warpgroup's
+// 64-byte-swizzled [TH rows][TW px][32 ch] block st of an epilogue stage.  acc holds both gates of this thread's channel
+// (parameters par) for two pixels of every 8-pixel row of the block: row j at acc[4 j ..].  The residual comes in with
+// ldmatrix.trans, the arithmetic is epilogue_smem's per element, and the bf16 output goes back with stmatrix.trans.
+template <int NA = 64, int TW = TC_TW, int NR = 4>
+__device__ __forceinline__ void ws_epilogue_rows(const float (&acc)[NA], int j0, uint32_t st, float4 par, const EpiArgs &e, int x0 = 0)
 {
+    static_assert(NR == 4 || NR == 1, "ldmatrix / stmatrix of four or one 8x8 blocks");
     const int lane = threadIdx.x & 31, wiw = (threadIdx.x >> 5) & 3;
-    // this lane's ldmatrix / stmatrix row: pixel lane & 7 of tile row j0 + (lane >> 3), channels 8 wiw ..
-    const uint32_t e_row = ((uint32_t)(lane >> 3) * TC_TW + (lane & 7)) * 64u + 16u * wiw;
-    const uint32_t addr = st + swz(e_row + (uint32_t)j0 * TC_TW * 64u, 64u);
-    uint32_t rv[4] = {0u, 0u, 0u, 0u};
-    if (e.residual) ldmatrix_x4_trans(addr, rv);
-    uint32_t ov[4];
+    // this lane's ldmatrix / stmatrix row: pixel x0 + (lane & 7) of tile row j0 + (lane >> 3), channels 8 wiw ..
+    const uint32_t e_row = ((uint32_t)(lane >> 3) * TW + (lane & 7)) * 64u + 16u * wiw;
+    const uint32_t addr = st + swz(e_row + ((uint32_t)j0 * TW + (uint32_t)x0) * 64u, 64u);
+    uint32_t rv[NR] = {};
+    if (e.residual) {
+        if constexpr (NR == 4) ldmatrix_x4_trans(addr, rv);
+        else ldmatrix_x1_trans(addr, rv);
+    }
+    uint32_t ov[NR];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
+    for (int i = 0; i < NR; ++i) {
         const int j = j0 + i;
         const float f0 = acc[4 * j] + par.x, f1 = acc[4 * j + 1] + par.x;
         const float m0 = acc[4 * j + 2] + par.y, m1 = acc[4 * j + 3] + par.y;
@@ -549,18 +563,20 @@ __device__ __forceinline__ void ws_epilogue_rows(const float (&acc)[64], int j0,
         const float2 rs = bf16x2_val(rv[i]);             // zero without a residual
         ov[i] = bf16x2_bits(y0 + rs.x, y1 + rs.y);
     }
-    stmatrix_x4_trans(addr, ov);
+    if constexpr (NR == 4) stmatrix_x4_trans(addr, ov);
+    else stmatrix_x1_trans(addr, ov);
 }
 
-// Consumer: the warpgroup's finished block st, output channels c0 .. c0 + 31 of tile t, made visible to the TMA unit and stored
-// by the issuer (the TMA unit clips the box at the image edge)
+// Consumer: the warpgroup's finished block st, output channels c0 .. c0 + 31 of the TW x TH-pixel tile t, made visible to the
+// TMA unit and stored by the issuer (the TMA unit clips the box at the image edge)
+template <int TW = TC_TW, int TH = TC_TH>
 __device__ __forceinline__ void ws_store_block(const TcMaps &tm, const TcArgs &a, uint32_t st, int c0, int t, int wg, bool issuer)
 {
     fence_proxy_async_smem();
     named_bar_sync(1 + wg, 128);
     if (issuer) {
         const TileCoord tc = decode_tile(t, a);
-        tma_store_4d(&tm.out, st, c0, tc.tx * TC_TW, tc.ty * TC_TH, tc.b);
+        tma_store_4d(&tm.out, st, c0, tc.tx * TW, tc.ty * TH, tc.b);
         bulk_commit_group();
     }
 }
@@ -770,6 +786,136 @@ gated_conv_tc_ws64_kernel(const __grid_constant__ TcMaps tm, const __grid_consta
     if (issuer) bulk_wait_group<0>();
 }
 
+// ------------------------------------------------------------------ role-swapped body with streamed weights: 3x3 stride-1, C -> C, C = 128 / 256
+// The 64-channel body's role swap for the layers whose weights (576 KB / 2.25 MB) do not fit shared memory.  The general body
+// streams an n-tile's whole weight set out of L2 for every 128-pixel tile, so each weight byte feeds 128 pixels; here a work
+// unit is (16 x R-pixel tile, n-tile of 64 output channels), and each weight byte feeds 16 R = 256 or 272 pixels:
+//   D[128 weight rows = 64 conv_f + 64 conv_m][16 R pixels] += W[128, K = 9 taps x C] X[16 R, K]
+//   A (weights)  streamed through the weight ring, one stage per (K chunk of 64 channels, tap): the n-tile's packed 128 x 64 tile
+//                loaded as sixteen 8-row boxes in the 64-channel body's order (f-group g, m-group g, f-group g + 1, ...), so
+//                warpgroup h reads its 64 rows (conv_f and conv_m of channels 32h .. 32h + 31) at h * 8 KB.  The packing is
+//                the general body's.
+//   B (pixels)   one halo stage per K chunk: [8-channel chunk][R + 2 rows][18 px][16 B], unswizzled.  Each K step is two
+//                m64n(8R)k16 with the same A descriptor, for pixel columns 0..7 and 8..15 of the tile (128 B apart): SBO = the
+//                halo row (288 B), LBO = the chunk stride, tap (ky, kx) at + ky * 288 + kx * 16 B.
+//   K order      K chunk, tap, 16-wide step: the general body's, so each output sums its products in the same order.
+//   accumulators one set of 2 x 4R per thread (both gates of one channel, two pixels of every 8-pixel row of the tile).
+//   epilogue     ws_epilogue_rows / ws_store_block over [R rows][16 px][32 ch] blocks; it does not overlap the MMAs (the
+//                producer keeps loading the next unit's halo and weights meanwhile).
+// R = 16 or 17 is chosen per layer by tc_wss_rows.  One CTA per SM, at most 168 registers per thread: nine warps spread over
+// the SM's four register-file quarters put three warps in one of them.  The ring sizes are compile-time so that every stage
+// index and phase is a bit field of one running count.
+constexpr int WSS_TW = 16;                                 // tile width in pixels
+constexpr int WSS_A_STAGES = 2, WSS_B_STAGES = 4;          // halo stages, weight stages
+constexpr uint32_t WSS_STAGE_BYTES = 128u * 64u * 2u;     // one weight stage: 128 packed rows of one tap and K chunk
+
+template <int R>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gated_conv_tc_wss_kernel(const __grid_constant__ TcMaps tm, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcArgs a)
+{
+    constexpr uint32_t ROW = ws_row_bytes(WSS_TW), CHUNK = ws_chunk_bytes(WSS_TW, R);
+    constexpr uint32_t BLOCK = WSS_TW * R * 64u;        // one warpgroup's [R][16 px][32 ch] block of an epilogue stage
+    const WsSmem<TC_E_STAGES> sm(a);
+    ws_prologue<TC_E_STAGES, true>(sm, tm, tmB, a, TC_CONSUMER_WARPS, 2);   // both warpgroups read every stage
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const int total = a.tiles_x * a.tiles_y * a.B * a.n_tiles;
+    const int n_total = a.n_tile * a.n_tiles;
+
+    if (warp == TC_PRODUCER_WARP) {
+        if (a.pdl) pdl_wait();
+        uint32_t as = 0, aph = 0, es = 0, eph = 0, nb = 0;
+        for (int t = blockIdx.x; t < total; t += gridDim.x) {
+            const TileCoord tc_ = decode_tile(t, a);
+            for (int kc = 0; kc < a.kchunks; ++kc) {
+                ws_load_halo<64, TC_E_STAGES, WSS_TW, R>(sm, tm, a, tc_, as, aph, 64 * kc);
+                for (int tap = 0; tap < 9; ++tap, ++nb) {
+                    const uint32_t bs = nb % WSS_B_STAGES;
+                    mbar_wait(sm.bempty0 + 8 * bs, ((nb / WSS_B_STAGES) & 1u) ^ 1u);
+                    if (elect_one()) {
+                        const uint32_t full = sm.bfull0 + 8 * bs, dst = sm.b_region + bs * WSS_STAGE_BYTES;
+                        const int row0 = (tap * a.kchunks + kc) * n_total + tc_.nt * a.n_tile;
+                        mbar_arrive_expect_tx(full, WSS_STAGE_BYTES);
+                        for (int g = 0; g < 8; ++g) {
+                            tma_load_2d(&tmB, full, dst + (uint32_t)g * 2048u, 0, row0 + 8 * g);                // conv_f channels 8g ..
+                            tma_load_2d(&tmB, full, dst + (uint32_t)g * 2048u + 1024u, 0, row0 + 64 + 8 * g);   // conv_m, the same
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+            ws_load_residual<64, TC_E_STAGES, WSS_TW, R>(sm, tm, a, tc_, es, eph, tc_.nt * 64);
+        }
+        return;
+    }
+
+    const int wg = warp >> 2, wiw = warp & 3;
+    if (a.pdl) pdl_wait();        // the outputs may still be read by earlier kernels
+    const bool issuer = wiw == 0 && lane == 0;      // issues the warpgroup's TMA stores and releases its epilogue stages
+    // halo and weight stages consumed so far: stage = count % stages, phase = (count / stages) & 1
+    uint32_t na = 0, nb = 0;
+    auto release = [&](uint32_t bar) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar);
+    };
+    for (int k = 0, t = blockIdx.x; t < total; ++k, t += gridDim.x) {
+        const TileCoord tc_ = decode_tile(t, a);
+        float acc[2][4 * R];
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+#pragma unroll
+            for (int i = 0; i < 4 * R; ++i) acc[c][i] = 0.f;
+        // a weight stage is released once the MMA group after the one that read it has been issued and the one that read it
+        // has retired (wgmma_wait<1>); a halo stage likewise after its last tap's group
+        for (int kc = 0; kc < a.kchunks; ++kc, ++na) {
+            mbar_wait(sm.afull0 + 8 * (na % WSS_A_STAGES), (na / WSS_A_STAGES) & 1u);
+            const uint32_t halo = sm.base + (na % WSS_A_STAGES) * a.a_bytes;
+#pragma unroll
+            for (int tap = 0; tap < 9; ++tap, ++nb) {
+                const uint32_t bs = nb % WSS_B_STAGES;
+                mbar_wait(sm.bfull0 + 8 * bs, (nb / WSS_B_STAGES) & 1u);
+                // warpgroup-uniform weight base through a shuffle, recomputed per group (see gated_conv_tc_ws64_kernel)
+                const uint32_t w_base = sm.b_region + bs * WSS_STAGE_BYTES + (uint32_t)__shfl_sync(0xffffffffu, wg, 0) * 8192u;
+                const uint32_t x_base = halo + (uint32_t)(tap / 3) * ROW + (uint32_t)(tap % 3) * 16u;
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const uint64_t wd = wgmma_desc(w_base + 32u * kk, 128u);
+                        const uint64_t xd = wgmma_desc_noswz(x_base + 2u * kk * CHUNK + 128u * c, CHUNK, ROW);
+                        if constexpr (R == 16) wgmma_ss_m64n128k16(acc[c], wd, xd, 1u);
+                        else wgmma_ss_m64n136k16(acc[c], wd, xd, 1u);
+                    }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (tap > 0 || kc > 0) release(sm.bempty0 + 8 * ((nb - 1u) % WSS_B_STAGES));
+                if (tap == 0 && kc > 0) release(sm.aempty0 + 8 * ((na - 1u) % WSS_A_STAGES));
+            }
+        }
+        const uint32_t es = (uint32_t)k % TC_E_STAGES;
+        release_epilogue_stage(issuer, k > 0 ? (int)((uint32_t)(k - 1) % TC_E_STAGES) : -1, sm.eempty0);
+        wgmma_wait<0>();
+#pragma unroll
+        for (int c = 0; c < 2; ++c) wgmma_fence_acc(acc[c]);
+        release(sm.bempty0 + 8 * ((nb - 1u) % WSS_B_STAGES));
+        release(sm.aempty0 + 8 * ((na - 1u) % WSS_A_STAGES));
+
+        const float4 par = sm.par[tc_.nt * 64 + 32 * wg + 8 * wiw + (lane >> 2)];
+        mbar_wait(sm.efull0 + 8 * es, ((uint32_t)k / TC_E_STAGES) & 1u);
+        const uint32_t st = sm.e_region + es * a.e_bytes + (uint32_t)wg * BLOCK;
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+#pragma unroll
+            for (int j0 = 0; j0 + 4 <= R; j0 += 4) ws_epilogue_rows<4 * R, WSS_TW, 4>(acc[c], j0, st, par, a.epi, 8 * c);
+#pragma unroll
+            for (int j = R / 4 * 4; j < R; ++j) ws_epilogue_rows<4 * R, WSS_TW, 1>(acc[c], j, st, par, a.epi, 8 * c);
+        }
+        ws_store_block<WSS_TW, R>(tm, a, st, tc_.nt * 64 + 32 * wg, t, wg, issuer);
+    }
+    if (issuer) bulk_wait_group<0>();
+}
+
 // ------------------------------------------------------------------ weight packing
 // out[((tap*kchunks + kc) * n_total + n) * cin_blk + kk],  n -> (tile nt, f|m half, channel)
 __global__ void pack_tc_kernel(const float *__restrict__ wf, const float *__restrict__ wm, int Cout, int cout_pad, int Cin,
@@ -943,46 +1089,71 @@ struct TcPlan {
     TcArgs args;
     size_t smem_bytes;
     int reverse;
-    int ws;                                // 0, or the channel count of a weight-stationary layer (tc_ws_layer): 32 runs
-                                           // gated_conv_tc_ws_kernel, 64 gated_conv_tc_ws64_kernel
+    int ws;                                // 0, or the channel count of a role-swapped layer (tc_ws_layer): 32 runs
+                                           // gated_conv_tc_ws_kernel, 64 gated_conv_tc_ws64_kernel, 128 and 256
+                                           // gated_conv_tc_wss_kernel<tile_h>
+    int tile_h;                            // output tile rows: TC_TH, or R of gated_conv_tc_wss_kernel<R>
 };
 
-// The layers of the weight-stationary bodies: 3x3 stride-1 C -> C gated convs, C = 32 or 64, with an NHWC output and at most
-// a residual
+// The layers of the role-swapped bodies: 3x3 stride-1 C -> C gated convs, C = 32 or 64 (weight-stationary) or 128 or 256
+// (streamed weights), with an NHWC output and at most a residual
 static bool tc_ws_layer(const read_conv_desc &d)
 {
-    return d.k == 3 && d.stride == 1 && (d.Cin == 32 || d.Cin == 64) && d.Cout == d.Cin && d.n_src == 1 &&
-           d.out_mode == READ_OUT_NHWC && d.out2 == nullptr && d.addin == nullptr;
+    return d.k == 3 && d.stride == 1 && (d.Cin == 32 || d.Cin == 64 || d.Cin == 128 || d.Cin == 256) && d.Cout == d.Cin &&
+           d.n_src == 1 && d.out_mode == READ_OUT_NHWC && d.out2 == nullptr && d.addin == nullptr;
 }
 
-// The plan values that depend on the kernel body, for a layer whose halo tile is a_tx_bytes and whose weights, like its
-// activations, have the swizzle sw of their K chunk.  The weight-stationary bodies read the halo as unswizzled 8-channel chunks
-// and load the residual and store the output as 32-channel blocks of whole tiles; the 64-channel body loads its weights as
-// 8-row boxes, one swizzle atom each, to interleave conv_f and conv_m.
+// Tile rows R of a streamed-weight role-swapped layer (gated_conv_tc_wss_kernel<R>, R = 16 or 17): the fewest pixel slots on
+// the busiest CTA, ceil(units / SMs) x 16 R, and on a tie the fewer halo rows loaded
+static int tc_wss_rows(const read_conv_desc &d, int n_tiles)
+{
+    const long long ctas = num_sms(), tiles_x = (d.Wout + WSS_TW - 1) / WSS_TW;
+    int best = 0;
+    long long best_slots = 0, best_halo = 0;
+    for (int r = 16; r <= 17; ++r) {
+        const long long tiles_y = (d.Hout + r - 1) / r, units = tiles_x * tiles_y * d.B * n_tiles;
+        const long long slots = (units + ctas - 1) / ctas * WSS_TW * r, halo = tiles_y * (r + 2);
+        if (!best || slots < best_slots || (slots == best_slots && halo < best_halo)) {
+            best = r;
+            best_slots = slots;
+            best_halo = halo;
+        }
+    }
+    return best;
+}
+
+// The plan values that depend on the kernel body, for a layer whose weights, like its activations, have the swizzle sw of
+// their K chunk.  The role-swapped bodies read the halo as unswizzled 8-channel chunks and load the residual and store the
+// output as 32-channel blocks of whole tiles; from 64 channels they load their weights as 8-row boxes, one swizzle atom each,
+// to interleave conv_f and conv_m, and from 128 channels their tiles are 16 pixels wide and tc_wss_rows high.
 struct TcBodyLayout {
     int ws;                                // TcPlan::ws
+    int tile_w, tile_h;                    // pixels of the output tile
     int halo_c;                            // channels of one halo box
     CUtensorMapSwizzle halo_sw;
     int w_rows;                            // rows of one weight box
     int epi_c, out_rows;                   // channels of the output and residual boxes, rows of the output box
-    uint32_t tile_bytes;                   // TcArgs::tile_bytes
+    uint32_t tile_bytes;                   // TcArgs::tile_bytes, 0: the halo tile's bytes
     int e_stages;                          // epilogue stages
 };
-static TcBodyLayout tc_body_layout(const read_conv_desc &d, const TcGeom &g, uint32_t a_tx_bytes, CUtensorMapSwizzle sw)
+static TcBodyLayout tc_body_layout(const read_conv_desc &d, const TcGeom &g, CUtensorMapSwizzle sw)
 {
     const int oc = d.out_mode == READ_OUT_RAW_NHWC ? g.n_tile : g.n_tile / 2;     // channels of one output pixel in the tile
-    TcBodyLayout L{0, g.cin_blk, sw, g.n_tile, oc < 64 ? oc : 64, TC_TH / 2, a_tx_bytes, TC_E_STAGES};
+    TcBodyLayout L{0, TC_TW, TC_TH, g.cin_blk, sw, g.n_tile, oc < 64 ? oc : 64, TC_TH / 2, 0, TC_E_STAGES};
     if (tc_ws_layer(d)) {
         L.ws = d.Cin;
+        if (d.Cin >= 128) {
+            L.tile_w = WSS_TW;
+            L.tile_h = tc_wss_rows(d, g.n_tiles);
+        }
         L.halo_c = 8;
         L.halo_sw = CU_TENSOR_MAP_SWIZZLE_NONE;
-        if (d.Cin == 64) L.w_rows = 8;
+        if (d.Cin >= 64) L.w_rows = 8;
         L.epi_c = 32;
-        L.out_rows = TC_TH;
-        L.tile_bytes = (uint32_t)(d.Cin / 8) * WS_CHUNK_BYTES;
+        L.out_rows = L.tile_h;
+        L.tile_bytes = (uint32_t)(g.cin_blk / 8) * ws_chunk_bytes(L.tile_w, L.tile_h);
         if (d.Cin == 32) L.e_stages = WS_E_STAGES;
     }
-    L.tile_bytes = (L.tile_bytes + 1023u) & ~1023u;   // tiles stay 1 KB aligned (swizzle patterns are address based)
     return L;
 }
 
@@ -1004,18 +1175,18 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     RB_CHECK_ARG(d.addin == nullptr || (reinterpret_cast<uintptr_t>(d.addin) & 15) == 0, "wgmma conv: addin must be 16B aligned");
     RB_CHECK_ARG(d.out2 == nullptr || ((reinterpret_cast<uintptr_t>(d.out2) | reinterpret_cast<uintptr_t>(d.out2_mul)) & 15) == 0,
                  "wgmma conv: out2 and out2_mul must be 16B aligned");
-    const long long tiles = (long long)((d.Wout + TC_TW - 1) / TC_TW) * ((d.Hout + TC_TH - 1) / TC_TH) * d.B * g.n_tiles;
+    const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                  : (g.cin_blk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+    const TcBodyLayout L = tc_body_layout(d, g, sw);
+    const long long tiles = (long long)((d.Wout + L.tile_w - 1) / L.tile_w) * ((d.Hout + L.tile_h - 1) / L.tile_h) * d.B * g.n_tiles;
     RB_CHECK_ARG(tiles < (1ll << 31), "wgmma conv: too many tiles");
     TcPlan *p = new (std::nothrow) TcPlan{};
     RB_CHECK_ARG(p != nullptr, "wgmma conv: out of host memory");
 
     const bool s2 = d.stride == 2;
-    const int halo_rows = s2 ? TC_TH + 1 : TC_TH + d.k - 1;
-    const int halo_w = s2 ? TC_TW + 1 : TC_TW + d.k - 1;
+    const int halo_rows = s2 ? L.tile_h + 1 : L.tile_h + d.k - 1;
+    const int halo_w = s2 ? L.tile_w + 1 : L.tile_w + d.k - 1;
     const uint32_t a_tx_bytes = (uint32_t)halo_rows * halo_w * g.cin_blk * 2u;
-    const CUtensorMapSwizzle sw = g.cin_blk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                  : (g.cin_blk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-    const TcBodyLayout L = tc_body_layout(d, g, a_tx_bytes, sw);
     p->ws = L.ws;
     for (int si = 0; si < d.n_src; ++si) {   // activations: dims {C, W, H, B}; box = one halo tile (all filter taps)
         const read_src &sv = d.src[si];
@@ -1067,10 +1238,10 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     const int half = g.n_tile / 2;
     if (!nchw) {
         const int out_c = raw ? 2 * d.Cout : d.Cout, acb = g.n_tile < 64 ? g.n_tile : 64;     // out_c: also the residual's
-        bool ok = enc_epi(&p->tmA.out, d.out, out_c, d.Wout, d.Hout, L.epi_c, TC_TW, L.out_rows, "out");
+        bool ok = enc_epi(&p->tmA.out, d.out, out_c, d.Wout, d.Hout, L.epi_c, L.tile_w, L.out_rows, "out");
         if (ok && d.out2) ok = enc_epi(&p->tmA.out2, d.out2, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH / 2, "out2");
         if (ok && d.out2) ok = enc_epi(&p->tmA.mul, d.out2_mul, d.Cout, d.Wout, d.Hout, half, TC_TW, TC_TH, "out2_mul");
-        if (ok && d.residual) ok = enc_epi(&p->tmA.res, d.residual, out_c, d.Wout, d.Hout, L.epi_c, TC_TW, TC_TH, "residual");
+        if (ok && d.residual) ok = enc_epi(&p->tmA.res, d.residual, out_c, d.Wout, d.Hout, L.epi_c, L.tile_w, L.tile_h, "residual");
         if (ok && d.addin) ok = enc_epi(&p->tmA.add, d.addin, g.n_tile, d.addin_W, d.addin_H, acb, TC_TW / 2, TC_TH / 2, "addin");
         if (!ok) {
             delete p;
@@ -1081,8 +1252,9 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     a.B = d.B; a.H = d.Hout; a.W = d.Wout; a.Cin = d.Cin; a.Cout = d.Cout; a.cout_pad = g.cout_pad;
     a.ksize = d.k; a.pad = d.pad;
     a.cin_blk = g.cin_blk; a.kchunks = g.kchunks; a.n_tile = g.n_tile; a.n_tiles = g.n_tiles;
-    a.tiles_x = (d.Wout + TC_TW - 1) / TC_TW;
-    a.tiles_y = (d.Hout + TC_TH - 1) / TC_TH;
+    a.tiles_x = (d.Wout + L.tile_w - 1) / L.tile_w;
+    a.tiles_y = (d.Hout + L.tile_h - 1) / L.tile_h;
+    p->tile_h = L.tile_h;
     a.halo_w = halo_w;
     a.stride = d.stride;
     a.n_src = d.n_src;
@@ -1102,14 +1274,14 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
         }
     }
     a.a_tx_bytes = a_tx_bytes;
-    a.tile_bytes = L.tile_bytes;
+    a.tile_bytes = ((L.tile_bytes ? L.tile_bytes : a_tx_bytes) + 1023u) & ~1023u;   // 1 KB aligned (swizzle patterns are address based)
     a.a_bytes = s2 ? 4u * a.tile_bytes : a.tile_bytes;
     a.b_bytes = (uint32_t)g.n_tile * g.cin_blk * 2u;
     const uint32_t total_b = (uint32_t)(d.k * d.k * g.kchunks) * a.b_bytes;
-    // epilogue stage: out region (128 pixels of the tile's output channels), out2 region, add-in region (32 pixels x N);
+    // epilogue stage: out region (the tile's pixels x its output channels), out2 region, add-in region (32 pixels x N);
     // every region is a multiple of 1 KB, so each keeps the 1 KB alignment of the swizzle patterns
     if (!nchw) {
-        const uint32_t out_b = 128u * (raw ? 2u : 1u) * (uint32_t)g.n_tile;
+        const uint32_t out_b = (uint32_t)(L.tile_w * L.tile_h) * (raw ? 2u : 1u) * (uint32_t)g.n_tile;
         const uint32_t out2_b = d.out2 ? 128u * (uint32_t)g.n_tile : 0u, add_b = d.addin ? 64u * (uint32_t)g.n_tile : 0u;
         a.e_out2_off = out_b;
         a.e_add_off = out_b + out2_b;
@@ -1127,7 +1299,20 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     const uint32_t budget = a.ctas_per_sm > 1 ? budget_2 : budget_1;
     a.b_resident = (g.n_tiles == 1 && total_b <= TC_RESIDENT_MAX && total_b + e_ring + 2 * a.a_bytes <= budget) ? 1 : 0;
     uint32_t b_region_bytes;
-    if (a.b_resident) {
+    if (p->ws >= 128) {
+        // streamed-weight role swap: two halo stages, four 16 KB weight stages and the epilogue ring; at 256 channels and
+        // R = 17 two 44 KB halo stages, two 34 KB epilogue stages and 5.6 KB of alignment pad, barriers and parameters,
+        // 225.6 KB of the 227 KB a CTA may have
+        a.a_stages = WSS_A_STAGES;
+        a.b_stages = WSS_B_STAGES;
+        b_region_bytes = (uint32_t)a.b_stages * a.b_bytes;
+        if (a.a_stages * a.a_bytes + b_region_bytes + e_ring > budget) {
+            set_error("wgmma conv: streamed-weight role-swapped layer does not fit shared memory (%u B needed)",
+                      a.a_stages * a.a_bytes + b_region_bytes + e_ring + fixed);
+            delete p;
+            return READ_ERR_UNSUPPORTED;
+        }
+    } else if (a.b_resident) {
         int st = (int)((budget - total_b - e_ring) / a.a_bytes);
         a.a_stages = st > TC_MAX_STAGES ? TC_MAX_STAGES : st;
         a.b_stages = 0;
@@ -1146,7 +1331,7 @@ int tc_plan_create(const read_conv_desc &d, TcPlan **out)
     }
     // the weight-stationary bodies rely on both.  At 64 channels: 144 KB of weights, two 23 KB halo stages, two 16 KB epilogue
     // stages and about 2.7 KB of alignment pad, barriers and parameters, 224.7 KB of the 227 KB a CTA may have
-    if (p->ws && (!a.b_resident || a.a_stages < 2)) {
+    if (p->ws && p->ws < 128 && (!a.b_resident || a.a_stages < 2)) {
         set_error("wgmma conv: weight-stationary layer without resident weights or two A stages (%u B of shared memory needed)",
                   total_b + e_ring + 2 * a.a_bytes + fixed);
         delete p;
@@ -1228,6 +1413,8 @@ int tc_plan_launch(const TcPlan *p, cudaStream_t st, int max_ctas)
     int rc;
     if (p->ws == 32) rc = launch_tc(gated_conv_tc_ws_kernel, p, a, lcfg);
     else if (p->ws == 64) rc = launch_tc(gated_conv_tc_ws64_kernel, p, a, lcfg);
+    else if (p->ws >= 128 && p->tile_h == 16) rc = launch_tc(gated_conv_tc_wss_kernel<16>, p, a, lcfg);
+    else if (p->ws >= 128 && p->tile_h == 17) rc = launch_tc(gated_conv_tc_wss_kernel<17>, p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 1) rc = launch_tc_kn<1, 1>(p, a, lcfg);
     else if (a.stride == 1 && a.ksize == 3) rc = launch_tc_kn<3, 1>(p, a, lcfg);
     else if (a.stride == 2 && a.ksize == 3) rc = launch_tc_kn<3, 2>(p, a, lcfg);
