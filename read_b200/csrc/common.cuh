@@ -78,6 +78,8 @@ inline int check_tex_table(const read_tex_table *t, int h, int w, bool forward, 
 // max positive int64: larger than any real key (depth bits <= 0x3F800000) under BOTH signed and unsigned
 // comparison, so a min-reduction may be typed int64 (torch.distributed / ncclInt64) or uint64.
 static constexpr unsigned long long ZBUF_EMPTY = 0x7FFFFFFFFFFFFFFFull;
+// the point a key names: its low 32 bits, and point 0 for an empty pixel (the reference's index maps hold 0 there)
+__device__ __forceinline__ unsigned zbuf_point_id(unsigned long long key) { return key == ZBUF_EMPTY ? 0u : (unsigned)key; }
 
 struct LevelGeom {
     int w[READ_MAX_LEVELS], h[READ_MAX_LEVELS];

@@ -419,10 +419,8 @@ int read_frame_to_rgba(const float *rgb_planes, int H, int W, int flip_vertical,
     RB_CHECK_ARG((reinterpret_cast<uintptr_t>(out_hwc4) & 15) == 0, "frame_to_rgba: output must be 16-byte aligned");
     const long long n = (long long)H * W;
     if (n == 0) return READ_OK;
-    long long blocks = (n + 255) / 256;
-    if (blocks > (long long)num_sms() * 16) blocks = (long long)num_sms() * 16;
-    frame_to_rgba_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(rgb_planes, H, W, flip_vertical, alpha,
-                                                                             reinterpret_cast<float4 *>(out_hwc4));
+    frame_to_rgba_kernel<<<grid_for(n), 256, 0, (cudaStream_t)stream>>>(rgb_planes, H, W, flip_vertical, alpha,
+                                                                        reinterpret_cast<float4 *>(out_hwc4));
     RB_LAUNCH_CHECK();
     return READ_OK;
 }

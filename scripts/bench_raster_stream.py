@@ -60,15 +60,11 @@ tex = torch.rand((N, 8), device=dev)
 pyr4 = ops.Pyramid(1, W, H, 4, dev)
 outs = [torch.empty((1, H >> l, W >> l, 8), dtype=torch.bfloat16, device=dev) for l in range(4)]
 pyr4.clear()
-gts = {0: [], 1: [], 2: [], 3: []}
+gts = []
 for rep in range(10):
-    for v in (0, 1, 2, 3):
-        setopt(gather_variant=v)
-        ops.raster_project_sorted(pyr4, store, mats[0]); torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(); ops.pyramid_resolve_gather(tex, pyr4, outs, L.FEAT_NHWC_BF16, reset_level0=True); b.record(); torch.cuda.synchronize()
-        gts[v].append(a.elapsed_time(b) * 1e3)
-setopt(gather_variant=0)
-for v in (0, 1, 2, 3):
-    ts = sorted(gts[v][2:])
-    print(f"pyramid_resolve_gather variant {v}: median {ts[len(ts)//2]:6.1f} us  best {ts[0]:6.1f} us")
+    ops.raster_project_sorted(pyr4, store, mats[0]); torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record(); ops.pyramid_resolve_gather(tex, pyr4, outs, L.FEAT_NHWC_BF16, reset_level0=True); b.record(); torch.cuda.synchronize()
+    gts.append(a.elapsed_time(b) * 1e3)
+ts = sorted(gts[2:])
+print(f"pyramid_resolve_gather: median {ts[len(ts)//2]:6.1f} us  best {ts[0]:6.1f} us")
