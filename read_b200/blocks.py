@@ -2,9 +2,9 @@
 
 ``UNet.train_precision = 'bf16'`` sends 78 of the net's 99 convs here; the other 21 (the 1x1 and stride-2 convs), the
 interpolations, concats and FAM products / sums stay on torch operators in the same autograd graph.  ``'bf16_all'`` also sends
-those 21 convs here (``MultiSourceConvFn``, at the end of this file).
-* ``ResStackFn``: each of the 8 residual block stacks (Encoder.0-3, Decoder.0-3: 4 ResBlocks = 8 convs at constant C, 64 convs).
-* ``GatedConvFn``: one conv with an optional residual, for the 14 single convs feat_extract.0 (8 -> 32), feat_extract.5 (32 -> 3,
+those 21 convs here (``gated_conv_srcs``).  One autograd Function, ``ConvChainFn``, runs every call:
+* ``stack_forward``: each of the 8 residual block stacks (Encoder.0-3, Decoder.0-3: 4 ResBlocks = 8 convs at constant C, 64 convs).
+* ``gated_conv``: one conv with an optional residual, for the 14 single convs feat_extract.0 (8 -> 32), feat_extract.5 (32 -> 3,
   the RGB output, run padded to C = 16), SCM*.main.0 (8 -> 16 / 32 / 64), SCM*.main.2, AFFs.*.conv.1 and FAM*.merge.
 
 Forward: NCHW f32 -> NHWC bf16 once, launches of the TMA wgmma kernel (in a stack the second conv of each ResBlock adds the skip in
@@ -14,10 +14,11 @@ with a RAW launch of the same kernel.  That costs one extra forward conv per con
 what saving [f | m] as well would take (C5, 8 crops of 256^2: about 1 GB instead of 3 GB across the 8 stacks, and 147 MB for the
 14 single convs).
 
-Backward, per conv, last to first (csrc/conv_bwd.cu): recompute [f | m]; gate backward -> [df | dm] and the bias / BatchNorm-affine
-gradients; weight gradient (tensor-core kernel, fp32 atomics into the torch-layout gradients; skipped when no weight needs one);
-input gradient = RAW launch of the TMA kernel over [df | dm] with flipped, transposed filters, the ResBlock skip added through its
-residual operand, or for an 8-channel input (the descriptor pyramid) the dedicated dgrad_cin8 kernel.
+Backward, per conv, last to first (csrc/conv_bwd.cu, conv_backward): recompute [f | m]; gate backward -> [df | dm] and the bias /
+BatchNorm-affine gradients; weight gradient (tensor-core kernel, fp32 atomics into the torch-layout gradients; skipped when no
+weight needs one); input gradient (input_grad) = RAW launch of the TMA kernel over [df | dm] with flipped, transposed filters, the
+ResBlock skip added through its residual operand, or for an 8-channel input (the descriptor pyramid) the dedicated dgrad_cin8
+kernel; a stride-2 conv's has its own kernel, and a 1x1 conv's runs as RAW 1x1 plans per source.
 
 BatchNorm is per conv, from the mode of that conv's norm at forward time:
 * eval mode (running statistics, as the reference trains with eval_in_train): folded into scale / shift like the inference engine,
@@ -114,10 +115,12 @@ def filter_key(mod, wf, wm, C, srcs=None):
 
 
 def _packed(mod, wf, wm, C, srcs):
-    """The fp32 filters padded to C channels and the bf16 forward (and 3x3 input-gradient) filters of ``mod``, from the cache when
-    the weights are unchanged.  The dict also holds the filters backward packs lazily (dgrad_s2_filters, recompute_fm,
-    dgrad_1x1); entries are only ever added, and a new weight version starts a new dict, so a FoldedConv of an earlier forward
-    keeps the filters it was built with.  Writes that bypass the version counter (through ``.data``) are not seen."""
+    """The fp32 filters padded to C channels and the bf16 forward and backward filters of ``mod``, from the cache when the weights
+    are unchanged: for a 3x3 stride-1 conv the forward and input-gradient filters, for a 1x1 or stride-2 conv over ``srcs`` the
+    forward filters and those its backward launches take (the stride-2 input-gradient filters, _fm64_filters,
+    _dgrad1x1_filters), so that a backward packs nothing.  Entries are only ever added, and a new weight version starts a new
+    dict, so a FoldedConv of an earlier forward keeps the filters it was built with.  Writes that bypass the version counter
+    (through ``.data``) are not seen."""
     key = filter_key(mod, wf, wm, C, srcs)
     ent = _FILTERS.get(mod) if cache_filters else None
     if ent is not None and ent[0] == key:
@@ -127,46 +130,75 @@ def _packed(mod, wf, wm, C, srcs):
     pad = lambda t: _pad_rows(t.detach().float(), C).contiguous()
     pk = {'wf': pad(wf), 'wm': pad(wm), 'w_dgrad': None}       # an 8-channel input's gradient kernel reads wf / wm itself
     pk['w_tc'] = torch.empty(lib.read_tc_weight_elems(C, cin, mod.k), dtype=torch.bfloat16, device=wf.device)
-    if (mod.k, mod.stride) != (3, 1):
-        L.check(lib.read_pack_weights_tc_for(ctypes.byref(_desc(srcs, C, mod.k, mod.stride)), pk['wf'].data_ptr(),
-                                             pk['wm'].data_ptr(), pk['w_tc'].data_ptr(), st))
-    else:
+    if (mod.k, mod.stride) == (3, 1):
         L.check(lib.read_pack_weights_tc(pk['wf'].data_ptr(), pk['wm'].data_ptr(), C, cin, 3, pk['w_tc'].data_ptr(), st))
         if cin != 8:
             pk['w_dgrad'] = torch.empty(lib.read_tc_weight_elems(cin // 2, 2 * C, 3), dtype=torch.bfloat16, device=wf.device)
             L.check(lib.read_pack_weights_tc_dgrad(pk['wf'].data_ptr(), pk['wm'].data_ptr(), C, cin, pk['w_dgrad'].data_ptr(), st))
-    if (mod.k, mod.stride) != (3, 1):
-        # the backward's filters too, so that a backward packs nothing (its launches are the same on every call)
-        c = _Filters(pk, C, mod.k, mod.stride)
-        if mod.stride == 2:
-            dgrad_s2_filters(c)
+    else:
+        L.check(lib.read_pack_weights_tc_for(ctypes.byref(_desc(srcs, C, mod.k, mod.stride)), pk['wf'].data_ptr(),
+                                             pk['wm'].data_ptr(), pk['w_tc'].data_ptr(), st))
+        if mod.stride == 2:             # the flipped-by-phase filters [k*k][Cin][2C] of the stride-2 input-gradient kernel
+            pk['s2'] = torch.empty((mod.k * mod.k, cin, 2 * C), dtype=torch.bfloat16, device=wf.device)
+            L.check(lib.read_pack_weights_dgrad_s2(pk['wf'].data_ptr(), pk['wm'].data_ptr(), C, cin, mod.k, pk['s2'].data_ptr(),
+                                                   st))
         else:
             if C > 64:
-                _fm64_filters(lib, srcs, c)
+                _fm64_filters(lib, pk, C, srcs)
             c0 = 0
             for s in srcs:
-                for a in range(c0, c0 + s.shape[3], 128):
-                    _dgrad1x1_filters(lib, c, a, min(128, c0 + s.shape[3] - a), wf.device)
+                _dgrad1x1_filters(lib, pk, C, c0, s.shape[3])
                 c0 += s.shape[3]
     if cache_filters:
         _FILTERS[mod] = (key, pk)
     return pk
 
 
-class _Filters:
-    """The attributes of a FoldedConv the filter packers read."""
+def _fm64_filters(lib, pk, C, srcs):
+    """The forward filters of each 64-channel block of a 1x1 conv wider than 64 (recompute_fm) from its filters ``pk``
+    (_packed) at C channels, packed once per entry."""
+    ws = pk.get('fm64')
+    if ws is None:
+        wf, wm = pk['wf'], pk['wm']
+        d64 = _desc(srcs, 64, 1, 1)
+        ws = [torch.empty(lib.read_tc_weight_elems(64, d64.Cin, 1), dtype=torch.bfloat16, device=wf.device) for _ in range(C // 64)]
+        for b, w in enumerate(ws):
+            L.check(lib.read_pack_weights_tc_for(ctypes.byref(d64), wf[64 * b: 64 * b + 64].data_ptr(),
+                                                 wm[64 * b: 64 * b + 64].data_ptr(), w.data_ptr(), L.stream_ptr()))
+        pk['fm64'] = ws
+    return ws
 
-    def __init__(self, pk, C, k, stride):
-        self.pk, self.wf, self.wm, self.C, self.k, self.stride = pk, pk['wf'], pk['wm'], C, k, stride
+
+def _dgrad1x1_filters(lib, pk, C, c0, cs):
+    """The transposed filters of the RAW 1x1 input-gradient plans (dgrad_1x1) of input channels c0 .. c0 + cs - 1 of a 1x1 conv
+    with filters ``pk`` (_packed) at C channels, one plan per 128 channels: a list of (a, cn, filters of channels a .. a + cn - 1),
+    each packed once per entry."""
+    wf, wm = pk['wf'], pk['wm']
+    plans = []
+    for a in range(c0, c0 + cs, 128):
+        cn = min(128, c0 + cs - a)
+        w = pk.get(('d1x1', a, cn))
+        if w is None:
+            w = torch.empty(lib.read_tc_weight_elems(max(cn, 32) // 2, 2 * C, 1), dtype=torch.bfloat16, device=wf.device)
+            L.check(lib.read_pack_weights_tc_dgrad1x1(wf.data_ptr(), wm.data_ptr(), C, wf.shape[1], a, cn, w.data_ptr(),
+                                                      L.stream_ptr()))
+            pk[('d1x1', a, cn)] = w
+        plans.append((a, cn, w))
+    return plans
+
+
+def dgrad_s2_filters(c):
+    """The flipped-by-phase filters [k*k][Cin][2C] (bf16) of the stride-2 input-gradient kernel for the stride-2 FoldedConv
+    ``c``, packed with its forward filters (_packed)."""
+    return c.pk['s2']
 
 
 class FoldedConv:
     """One GatedConv's live parameters for this step: its BatchNorm and the bf16 filters of the forward conv (also used for the RAW
     recompute) and of the input gradient.  ``cout`` > the conv's C pads it with zero filters, biases and BatchNorm scale / shift
     (the RGB output conv, C = 3, runs as C = 16; SCM*.main.3, C = 56 / 120 / 248, as 64 / 128 / 256): the padded channels compute
-    0 and get 0 gradients.  A 1x1 or stride-2 conv (k in {1, 3, 4}, stride in {1, 2}) packs its forward filters for the launch
-    over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks); its input-gradient filters are packed in
-    backward (dgrad_s2_filters, dgrad_1x1).
+    0 and get 0 gradients.  A 1x1 or stride-2 conv (k in {1, 3, 4}, stride in {1, 2}) packs its forward and backward filters
+    for the launches over ``srcs`` (the NHWC sources, whose channel counts set a concat's K chunks).
     An eval-mode norm is folded into scale / shift from its running statistics.  A train-mode norm (``batch``) runs the forward
     launch with the identity epilogue ``fwd_par``; mean / inv / scale / shift are then filled by bn_forward from the batch, per
     batch item ([items, C]) when ``items`` is given (per-item statistics), else per channel ([C])."""
@@ -318,70 +350,133 @@ def dgrad(dfm, conv, residual=None):
     return out
 
 
+def padded_channels(c):
+    """The channel count a conv with C = c runs at: 16, 32, 64 or a multiple of 64 (the counts the gate backward, the weight
+    gradient and the RAW 1x1 plans take)."""
+    return 16 if c <= 16 else 32 if c <= 32 else 64 * ((c + 63) // 64)
+
+
+def recompute_fm(lib, srcs, c):
+    """[f | m] (RAW column order) of the FoldedConv ``c`` over the NHWC sources, launched with the conv's own epilogue
+    parameters (RAW output reads none of them).  A RAW 1x1 plan takes at most 64 output channels (one N tile), so a wider 1x1
+    conv is recomputed per 64-channel block with that block's filters: block b of the RAW order is [f | m] of channels
+    64b .. 64b + 63."""
+    d = _desc(srcs, c.C, c.k, c.stride)
+    B, H, W = d.B, d.Hout, d.Wout
+    if c.k != 1 or c.C <= 64:
+        fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=srcs[0].device)
+        _launch(lib, srcs, c.C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm, k=c.k, stride=c.stride)
+        return fm
+    blocks_ = []
+    for w in _fm64_filters(lib, c.pk, c.C, srcs):
+        out = torch.empty((B, H, W, 128), dtype=torch.bfloat16, device=srcs[0].device)
+        _launch(lib, srcs, 64, w, c.par, c.elu, L.OUT_RAW_NHWC, out, k=1)
+        blocks_.append(out)
+    return torch.cat(blocks_, -1)
+
+
+def dgrad_1x1(dfm, c, c0, cs):
+    """Input gradient [B,H,W,cs] (bf16) of input channels c0 .. c0 + cs - 1 of the 1x1 FoldedConv ``c``: RAW 1x1 plans over
+    [df | dm] with transposed filters, one per 128 channels (the plans' widest N tile); 16 channels run padded to 32."""
+    lib = L.load()
+    B, H, W, _ = dfm.shape
+    parts = []
+    for _, cn, w in _dgrad1x1_filters(lib, c.pk, c.C, c0, cs):
+        n_out = max(cn, 32)
+        out = torch.empty((B, H, W, n_out), dtype=torch.bfloat16, device=dfm.device)
+        _launch_raw(lib, dfm, n_out // 2, w, out, k=1)
+        parts.append(out if cn == n_out else out[..., :cn])
+    return parts[0] if len(parts) == 1 else torch.cat(parts, -1)
+
+
+def input_grad(dfm, c, src, c0, residual=None):
+    """Input gradient (NHWC bf16, the shape of ``src``) of the NHWC source ``src`` of the FoldedConv ``c``, input channels
+    c0 .. c0 + Cs - 1 of its concat, from [df | dm] in RAW column order: the stride-2 kernel, a 1x1 conv's RAW plans (dgrad_1x1),
+    or a 3x3 stride-1 conv's dgrad, plus ``residual``."""
+    if c.stride == 2:
+        B, Hout, Wout, _ = dfm.shape
+        dx = torch.empty_like(src)
+        L.check(L.load().read_conv_dgrad_s2(dfm.data_ptr(), dgrad_s2_filters(c).data_ptr(), B, Hout, Wout, c.C,
+                                            src.shape[3], c.k, dx.data_ptr(), L.stream_ptr()))
+        return dx
+    if c.k == 1:
+        return dgrad_1x1(dfm, c, c0, src.shape[3])
+    return dgrad(dfm, c, residual)
+
+
+def conv_backward(lib, c, srcs, g, need, cout, need_src, residual=None, nchw=False):
+    """Backward of the FoldedConv ``c`` over the NHWC sources ``srcs`` from its output gradient ``g`` (NHWC bf16): [f | m]
+    recomputed, the 6 parameters' gradients (_param_grads with their flags ``need`` and real channel count ``cout``), then the
+    input gradient of each source whose ``need_src`` flag is set (input_grad, ``residual`` added in a 3x3 conv's rounding), NCHW
+    f32 with ``nchw``, else NHWC bf16; None for the others.  Returns (parameter gradients, input gradients)."""
+    fm = recompute_fm(lib, srcs, c)
+    dfm = torch.empty_like(fm)
+    grads = _param_grads(lib, g, fm, c, dfm, srcs, need, cout)
+    del fm                                                                 # the input gradient reads [df | dm] only
+    dxs, c0 = [], 0
+    for s, n in zip(srcs, need_src):
+        dx = input_grad(dfm, c, s, c0, residual) if n else None
+        dxs.append(ops.nhwc_to_nchw(dx.contiguous()) if nchw and n else dx)
+        c0 += s.shape[3]
+    return grads, dxs
+
+
 def _check_cuda(x):
     if not x.is_cuda:
         raise RuntimeError("read_b200: train_precision='bf16' runs the gated 3x3 convs on the H100 kernels and needs CUDA tensors")
     L.require_device(x.device.index)
 
 
-class ResStackFn(torch.autograd.Function):
-    """x (NCHW f32) -> the 4-ResBlock stack; ``mods`` = the stack's 8 GatedConvs in order, ``params`` = per conv (conv_f.weight,
-    conv_f.bias, conv_m.weight, conv_m.bias, norm.weight, norm.bias)."""
+class ConvChainFn(torch.autograd.Function):
+    """The gated convs ``mods`` in turn over NCHW f32 tensors.  ``tensors`` = the ``n_src`` sources, a residual slot (None, or a
+    tensor the output's shape that a one-conv call adds) and per conv its 6 parameters (stack_params).  Conv 0 reads the sources
+    (a 1x1 conv several as a virtual concat), conv i > 0 the output of conv i - 1.  More than one conv is a chain of ResBlocks:
+    the second conv of each pair adds the pair's input.  Each conv runs at padded_channels of its C.  ``per_item``: a train-mode
+    norm normalises each batch item with its own statistics."""
 
     @staticmethod
-    def forward(ctx, x, mods, *params):
-        return ResStackFn._forward(ctx, x, mods, params, None)
-
-    @staticmethod
-    def _forward(ctx, x, mods, params, items):
-        _check_cuda(x)
+    def forward(ctx, mods, n_src, per_item, *tensors):
+        xs, residual, params = tensors[:n_src], tensors[n_src], tensors[n_src + 1:]
+        _check_cuda(xs[0])
         lib = L.load()
-        convs = [FoldedConv(m, *params[6 * i: 6 * i + 6], items=items) for i, m in enumerate(mods)]   # packed before the first launch
-        t = ops.nchw_to_nhwc(x.detach().float().contiguous(), True)
-        C = t.shape[3]
-        saved = []
-        for r in range(0, len(convs), 2):
-            h = torch.empty_like(t)
-            conv_forward(lib, t, convs[r], h)
-            y = torch.empty_like(t)
-            conv_forward(lib, h, convs[r + 1], y, residual=t)
-            saved += [t, h]
-            t = y
-        ctx.convs, ctx.n_inputs = convs, len(saved)
+        nhwc = lambda t: ops.nchw_to_nhwc(t.detach().float().contiguous(), True)
+        srcs = [nhwc(x) for x in xs]
+        res = None if residual is None else nhwc(residual)
+        items = xs[0].shape[0] if per_item else None
+        # every conv's filters packed before the first launch
+        convs = [FoldedConv(m, *params[6 * i: 6 * i + 6], cout=padded_channels(params[6 * i].shape[0]),
+                            srcs=srcs if i == 0 else None, items=items) for i, m in enumerate(mods)]
+        ins = [srcs]                                                       # the input of each conv, then the output
+        for i, c in enumerate(convs):
+            d = _desc(ins[i], c.C, c.k, c.stride)
+            y = torch.empty((d.B, d.Hout, d.Wout, c.C), dtype=torch.bfloat16, device=srcs[0].device)
+            conv_forward(lib, ins[i], c, y, residual=ins[i - 1][0] if len(convs) > 1 and i % 2 else res)
+            ins.append([y])
+        ctx.convs, ctx.conv, ctx.n_src = convs, convs[-1], n_src     # ctx.conv: the conv whose output the call returns
         # the parameters are saved too: the folded / packed copies in ctx.convs alias or derive from them, and saving them makes
         # autograd raise if one is modified in place between forward and backward
-        ctx.save_for_backward(*saved, *params)
-        return ops.nhwc_to_nchw(t)
+        ctx.save_for_backward(*(t for ts in ins[:-1] for t in ts), *params)
+        y, cout = ops.nhwc_to_nchw(ins[-1][0]), params[-6].shape[0]
+        return y if cout == convs[-1].C else y[:, :cout].contiguous()
 
     @staticmethod
     def backward(ctx, gout):
-        lib = L.load()
-        inputs, convs = ctx.saved_tensors[:ctx.n_inputs], ctx.convs
-        B, H, W, C = inputs[0].shape
-        g = _out_grad(gout, C)                                            # gradient of the stack's output, NHWC bf16
-        fm = torch.empty((B, H, W, 2 * C), dtype=torch.bfloat16, device=inputs[0].device)
-        dfm = torch.empty_like(fm)
-        grads = [None] * (6 * len(convs))
-        g_block = g
+        lib, convs, n_src, need = L.load(), ctx.convs, ctx.n_src, ctx.needs_input_grad
+        n_in = n_src + len(convs) - 1
+        saved = ctx.saved_tensors
+        ins, params = [saved[:n_src]] + [saved[i:i + 1] for i in range(n_src, n_in)], saved[n_in:]
+        g = g_block = _out_grad(gout, ctx.conv.C)                           # the gradient of the output, NHWC bf16
+        grads, chain = [None] * len(params), len(convs) > 1
         for i in reversed(range(len(convs))):
-            c, x_in = convs[i], inputs[i]
-            if i % 2 == 1:
-                g_block = g                                               # gradient of this ResBlock's output
-            _launch(lib, x_in, C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-            grads[6 * i: 6 * i + 6] = _param_grads(lib, g, fm, c, dfm, [x_in], ctx.needs_input_grad[2 + 6 * i: 8 + 6 * i], C)
-            if i > 0 or ctx.needs_input_grad[0]:
-                # the first conv of a ResBlock adds the gradient that reaches its input through the skip
-                g = dgrad(dfm, c, residual=g_block if i % 2 == 0 else None)
-        dx = ops.nhwc_to_nchw(g) if ctx.needs_input_grad[0] else None
-        return (dx, None, *grads)
-
-
-class ResStackItemsFn(ResStackFn):
-    """ResStackFn with per-item statistics for its train-mode norms (each batch item normalised with its own)."""
-
-    @staticmethod
-    def forward(ctx, x, mods, *params):
-        return ResStackFn._forward(ctx, x, mods, params, x.shape[0])
+            if chain and i % 2 == 1:
+                g_block = g                                                # the gradient of this ResBlock's output
+            p = 4 + n_src + 6 * i                                          # needs_input_grad of the conv's 6 parameters
+            # the first conv of a ResBlock adds the gradient that reaches its input through the skip
+            grads[6 * i: 6 * i + 6], dxs = conv_backward(lib, convs[i], ins[i], g, need[p: p + 6], params[6 * i].shape[0],
+                                                         need[3: 3 + n_src] if i == 0 else [True],
+                                                         g_block if chain and i % 2 == 0 else None, nchw=i == 0)
+            g = dxs[0]
+        return (None, None, None, *dxs, gout if need[3 + n_src] else None, *grads)
 
 
 def _stack_names(net, prefix):
@@ -394,24 +489,19 @@ def stack_convs(net, prefix):
 
 
 def res_stack(net, prefix, x, batch_stats=False, per_item=False):
-    """bf16 forward of one EBlock / DBlock of ``net`` on the wgmma kernels, differentiable through ResStackFn."""
+    """bf16 forward of one EBlock / DBlock of ``net`` on the wgmma kernels, differentiable (stack_forward)."""
     return stack_forward(stack_convs(net, prefix), x, batch_stats=batch_stats, names=_stack_names(net, prefix),
                          per_item=per_item)
 
 
 def stack_params(mods):
-    """ResStackFn's parameter list for the GatedConvs ``mods``."""
+    """ConvChainFn's parameter list for the GatedConvs ``mods``: per conv (conv_f.weight, conv_f.bias, conv_m.weight,
+    conv_m.bias, norm.weight, norm.bias)."""
     params = []
     for m in mods:
         b = m.block
         params += [b['conv_f'].weight, b['conv_f'].bias, b['conv_m'].weight, b['conv_m'].bias, b['norm'].weight, b['norm'].bias]
     return params
-
-
-def _check_eval(mods):
-    if any(m.block['norm'].training for m in mods):
-        raise RuntimeError("read_b200: train_precision='bf16' folds BatchNorm with its running statistics; put the net in eval() "
-                           "mode (the reference trains with eval-mode BatchNorm)")
 
 
 def _label(mod, name):
@@ -423,13 +513,13 @@ def check_norms(mods, batch_stats, pixels, names=None, per_item=False):
     statistics kernels implement (momentum set, running statistics tracked, affine) and the conv must have at least 2 output
     pixels (``pixels`` = B * H_out * W_out, or H_out * W_out per item with ``per_item``; torch raises for 1 too); otherwise a
     ValueError names the layer."""
-    if not batch_stats:
-        _check_eval(mods)
-        return
     for i, m in enumerate(mods):
         n = m.block['norm']
         if not n.training:
             continue
+        if not batch_stats:
+            raise RuntimeError("read_b200: train_precision='bf16' folds BatchNorm with its running statistics; put the net in "
+                               "eval() mode (the reference trains with eval-mode BatchNorm)")
         label = _label(m, names[i] if names else None)
         if n.momentum is None:
             raise ValueError(f"read_b200: {label}: train-mode BatchNorm with momentum=None (cumulative moving average) is not "
@@ -447,215 +537,32 @@ def stack_forward(mods, x, batch_stats=False, names=None, per_item=False):
     whose norm is in train mode normalises with batch statistics (else such a conv raises), each batch item with its own with
     ``per_item``; ``names`` label the convs in errors."""
     check_norms(mods, batch_stats, (1 if per_item else x.shape[0]) * x.shape[2] * x.shape[3], names, per_item)
-    return (ResStackItemsFn if per_item else ResStackFn).apply(x, list(mods), *stack_params(mods))
-
-
-class GatedConvFn(torch.autograd.Function):
-    """x (NCHW f32) -> mod(x) [+ residual] for one gated 3x3 stride-1 conv ``mod``; ``params`` = (conv_f.weight, conv_f.bias,
-    conv_m.weight, conv_m.bias, norm.weight, norm.bias).  A conv with C < 16 (the RGB output conv) runs padded to C = 16."""
-
-    @staticmethod
-    def forward(ctx, x, residual, mod, *params):
-        return GatedConvFn._forward(ctx, x, residual, mod, params, None)
-
-    @staticmethod
-    def _forward(ctx, x, residual, mod, params, items):
-        _check_cuda(x)
-        lib = L.load()
-        cout = params[0].shape[0]
-        conv = FoldedConv(mod, *params, cout=max(cout, 16), items=items)
-        if residual is not None and conv.C != cout:
-            raise ValueError("read_b200: a residual needs C >= 16")
-        t = ops.nchw_to_nhwc(x.detach().float().contiguous(), True)
-        B, H, W, _ = t.shape
-        r = None if residual is None else ops.nchw_to_nhwc(residual.detach().float().contiguous(), True)
-        y = torch.empty((B, H, W, conv.C), dtype=torch.bfloat16, device=t.device)
-        conv_forward(lib, t, conv, y, residual=r)
-        ctx.conv, ctx.cout = conv, cout
-        ctx.save_for_backward(t, *params)              # the parameters: an in-place update before backward raises
-        y = ops.nhwc_to_nchw(y)
-        return y if cout == conv.C else y[:, :cout].contiguous()
-
-    @staticmethod
-    def backward(ctx, gout):
-        lib = L.load()
-        x_in, c, cout = ctx.saved_tensors[0], ctx.conv, ctx.cout
-        need = ctx.needs_input_grad
-        B, H, W, _ = x_in.shape
-        g = _out_grad(gout, c.C)
-        fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=x_in.device)
-        dfm = torch.empty_like(fm)
-        _launch(lib, x_in, c.C, c.w_tc, c.par, c.elu, L.OUT_RAW_NHWC, fm)
-        grads = _param_grads(lib, g, fm, c, dfm, [x_in], need[3:], cout)
-        dx = ops.nhwc_to_nchw(dgrad(dfm, c)) if need[0] else None
-        return (dx, gout if need[1] else None, None, *grads)
-
-
-class GatedConvItemsFn(GatedConvFn):
-    """GatedConvFn with per-item statistics for a train-mode norm (each batch item normalised with its own)."""
-
-    @staticmethod
-    def forward(ctx, x, residual, mod, *params):
-        return GatedConvFn._forward(ctx, x, residual, mod, params, x.shape[0])
+    return ConvChainFn.apply(list(mods), 1, per_item, x, None, *stack_params(mods))
 
 
 def gated_conv(mod, x, residual=None, batch_stats=False, name=None, per_item=False):
     """bf16 forward of the gated 3x3 stride-1 conv ``mod`` (a GatedConv) on the wgmma kernels, plus ``residual`` (NCHW, the
-    output's shape) when given, differentiable through GatedConvFn.  ``batch_stats``: a train-mode norm normalises with batch
-    statistics (else it raises), each batch item with its own with ``per_item``; ``name`` labels the layer in errors."""
+    output's shape) when given, differentiable.  A conv with C < 16 (the RGB output conv) runs padded to C = 16 and takes no
+    residual.  ``batch_stats``: a train-mode norm normalises with batch statistics (else it raises), each batch item with its own
+    with ``per_item``; ``name`` labels the layer in errors."""
     if mod.k != 3 or mod.stride != 1:
         raise ValueError(f"read_b200: gated_conv runs 3x3 stride-1 convs only (got k={mod.k}, stride={mod.stride})")
     check_norms([mod], batch_stats, (1 if per_item else x.shape[0]) * x.shape[2] * x.shape[3], [name], per_item)
-    return (GatedConvItemsFn if per_item else GatedConvFn).apply(x, residual, mod, *stack_params([mod]))
+    cout = mod.block['conv_f'].weight.shape[0]
+    if residual is not None and padded_channels(cout) != cout:
+        raise ValueError("read_b200: a residual needs C >= 16")
+    return ConvChainFn.apply([mod], 1, per_item, x, residual, *stack_params([mod]))
 
 
-# ------------------------------------------------------------------ the 1x1 and stride-2 convs ('bf16_all')
-GEOMETRIES = ((1, 1), (3, 2), (4, 2))        # (k, stride) of the convs MultiSourceConvFn runs
-
-
-def padded_channels(c):
-    """The channel count a conv with C = c runs at: 16, 32, 64 or a multiple of 64 (the counts the gate backward, the weight
-    gradient and the RAW 1x1 plans take)."""
-    return 16 if c <= 16 else 32 if c <= 32 else 64 * ((c + 63) // 64)
-
-
-def recompute_fm(lib, srcs, c):
-    """[f | m] (RAW column order) of the FoldedConv ``c`` over the NHWC sources.  A RAW 1x1 plan takes at most 64 output channels
-    (one N tile), so a wider 1x1 conv is recomputed per 64-channel block with that block's filters: block b of the RAW order is
-    [f | m] of channels 64b .. 64b + 63."""
-    d = _desc(srcs, c.C, c.k, c.stride)
-    B, H, W = d.B, d.Hout, d.Wout
-    if c.k != 1 or c.C <= 64:
-        fm = torch.empty((B, H, W, 2 * c.C), dtype=torch.bfloat16, device=srcs[0].device)
-        _launch_raw(lib, srcs, c.C, c.w_tc, fm, k=c.k, stride=c.stride)
-        return fm
-    blocks_ = []
-    for w in _fm64_filters(lib, srcs, c):
-        out = torch.empty((B, H, W, 128), dtype=torch.bfloat16, device=srcs[0].device)
-        _launch_raw(lib, srcs, 64, w, out, k=1)
-        blocks_.append(out)
-    return torch.cat(blocks_, -1)
-
-
-def _fm64_filters(lib, srcs, c):
-    """The forward filters of each 64-channel block of a 1x1 FoldedConv wider than 64 (recompute_fm), packed once per entry."""
-    ws = c.pk.get('fm64')
-    if ws is None:
-        d64 = _desc(srcs, 64, 1, 1)
-        ws = [torch.empty(lib.read_tc_weight_elems(64, d64.Cin, 1), dtype=torch.bfloat16, device=c.wf.device)
-              for _ in range(c.C // 64)]
-        for b, w in enumerate(ws):
-            L.check(lib.read_pack_weights_tc_for(ctypes.byref(d64), c.wf[64 * b: 64 * b + 64].data_ptr(),
-                                                 c.wm[64 * b: 64 * b + 64].data_ptr(), w.data_ptr(), L.stream_ptr()))
-        c.pk['fm64'] = ws
-    return ws
-
-
-def _dgrad1x1_filters(lib, c, a, cn, device):
-    """The transposed filters of the RAW 1x1 input-gradient plan for input channels a .. a + cn - 1 (dgrad_1x1)."""
-    w = c.pk.get(('d1x1', a, cn))
-    if w is None:
-        n_out = max(cn, 32)
-        w = torch.empty(lib.read_tc_weight_elems(n_out // 2, 2 * c.C, 1), dtype=torch.bfloat16, device=device)
-        L.check(lib.read_pack_weights_tc_dgrad1x1(c.wf.data_ptr(), c.wm.data_ptr(), c.C, c.wf.shape[1], a, cn, w.data_ptr(),
-                                                  L.stream_ptr()))
-        c.pk[('d1x1', a, cn)] = w
-    return w
-
-
-def dgrad_s2_filters(c):
-    """The flipped-by-phase filters [k*k][Cin][2C] (bf16) of the stride-2 input-gradient kernel for the FoldedConv ``c``."""
-    w = c.pk.get('s2')
-    if w is None:
-        cin = c.wf.shape[1]
-        w = torch.empty((c.k * c.k, cin, 2 * c.C), dtype=torch.bfloat16, device=c.wf.device)
-        L.check(L.load().read_pack_weights_dgrad_s2(c.wf.data_ptr(), c.wm.data_ptr(), c.C, cin, c.k, w.data_ptr(), L.stream_ptr()))
-        c.pk['s2'] = w
-    return w
-
-
-def dgrad_1x1(dfm, c, c0, cs):
-    """Input gradient [B,H,W,cs] (bf16) of input channels c0 .. c0 + cs - 1 of the 1x1 FoldedConv ``c``: RAW 1x1 plans over
-    [df | dm] with transposed filters, one per 128 channels (the plans' widest N tile); 16 channels run padded to 32."""
-    lib = L.load()
-    B, H, W, _ = dfm.shape
-    parts = []
-    for a in range(c0, c0 + cs, 128):
-        cn = min(128, c0 + cs - a)
-        n_out = max(cn, 32)
-        w = _dgrad1x1_filters(lib, c, a, cn, dfm.device)
-        out = torch.empty((B, H, W, n_out), dtype=torch.bfloat16, device=dfm.device)
-        _launch_raw(lib, dfm, n_out // 2, w, out, k=1)
-        parts.append(out if cn == n_out else out[..., :cn])
-    return parts[0] if len(parts) == 1 else torch.cat(parts, -1)
-
-
-class MultiSourceConvFn(torch.autograd.Function):
-    """The gated 1x1 or stride-2 3x3 / 4x4 conv ``mod`` over the NCHW f32 tensors ``xs`` (a 1x1 conv reads several as a virtual
-    concat along channels); ``params`` = (conv_f.weight, conv_f.bias, conv_m.weight, conv_m.bias, norm.weight, norm.bias).  A conv
-    whose C is not 16, 32, 64 or a multiple of 64 runs padded (padded_channels)."""
-
-    @staticmethod
-    def forward(ctx, mod, n_src, *args):
-        return MultiSourceConvFn._forward(ctx, mod, n_src, args, False)
-
-    @staticmethod
-    def _forward(ctx, mod, n_src, args, per_item):
-        xs, params = args[:n_src], args[n_src:]
-        _check_cuda(xs[0])
-        lib = L.load()
-        cout = params[0].shape[0]
-        ts = [ops.nchw_to_nhwc(x.detach().float().contiguous(), True) for x in xs]
-        conv = FoldedConv(mod, *params, cout=padded_channels(cout), srcs=ts, items=xs[0].shape[0] if per_item else None)
-        d = _desc(ts, conv.C, mod.k, mod.stride)
-        y = torch.empty((d.B, d.Hout, d.Wout, conv.C), dtype=torch.bfloat16, device=ts[0].device)
-        conv_forward(lib, ts, conv, y)
-        ctx.conv, ctx.cout, ctx.n_src = conv, cout, n_src
-        ctx.save_for_backward(*ts, *params)            # the parameters: an in-place update before backward raises
-        y = ops.nhwc_to_nchw(y)
-        return y if cout == conv.C else y[:, :cout].contiguous()
-
-    @staticmethod
-    def backward(ctx, gout):
-        lib, st = L.load(), L.stream_ptr()
-        n_src, c, cout = ctx.n_src, ctx.conv, ctx.cout
-        ts = ctx.saved_tensors[:n_src]
-        need = ctx.needs_input_grad[2:]                                    # the sources, then the 6 parameters
-        g = _out_grad(gout, c.C)
-        B, Hout, Wout, C = g.shape
-        fm = recompute_fm(lib, ts, c)
-        dfm = torch.empty_like(fm)
-        grads = _param_grads(lib, g, fm, c, dfm, ts, need[n_src:], cout)
-        del fm                                                             # the input gradient reads [df | dm] only
-        dxs = [None] * n_src
-        c0 = 0
-        for i, t in enumerate(ts):
-            cs = t.shape[3]
-            if need[i]:
-                if c.stride == 2:
-                    dx = torch.empty_like(t)
-                    L.check(lib.read_conv_dgrad_s2(dfm.data_ptr(), dgrad_s2_filters(c).data_ptr(), B, Hout, Wout, C, cs, c.k,
-                                                   dx.data_ptr(), st))
-                else:
-                    dx = dgrad_1x1(dfm, c, c0, cs)
-                dxs[i] = ops.nhwc_to_nchw(dx.contiguous())
-            c0 += cs
-        return (None, None, *dxs, *grads)
-
-
-class MultiSourceConvItemsFn(MultiSourceConvFn):
-    """MultiSourceConvFn with per-item statistics for a train-mode norm (each batch item normalised with its own)."""
-
-    @staticmethod
-    def forward(ctx, mod, n_src, *args):
-        return MultiSourceConvFn._forward(ctx, mod, n_src, args, True)
+GEOMETRIES = ((1, 1), (3, 2), (4, 2))        # (k, stride) of the convs gated_conv_srcs runs
 
 
 def gated_conv_srcs(mod, xs, name=None, batch_stats=False, per_item=False):
     """bf16 forward of the gated 1x1 or stride-2 conv ``mod`` (a GatedConv) over the NCHW tensors ``xs`` on the wgmma kernels,
-    differentiable through MultiSourceConvFn.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels);
-    a stride-2 conv takes one source of even height and width.  ``name`` labels the layer in errors.  ``batch_stats``: a
-    train-mode norm normalises with batch statistics (else it raises), each batch item with its own with ``per_item``."""
+    differentiable.  A 1x1 conv reads several sources as one concat (each a multiple of 32 channels); a stride-2 conv takes one
+    source of even height and width.  A conv whose C is not 16, 32, 64 or a multiple of 64 runs padded (padded_channels).
+    ``name`` labels the layer in errors.  ``batch_stats``: a train-mode norm normalises with batch statistics (else it raises),
+    each batch item with its own with ``per_item``."""
     label = _label(mod, name)
     xs = list(xs)
     if (mod.k, mod.stride) not in GEOMETRIES:
@@ -671,4 +578,4 @@ def gated_conv_srcs(mod, xs, name=None, batch_stats=False, per_item=False):
                          f"{xs[0].shape[2]}x{xs[0].shape[3]})")
     pixels = (1 if per_item else xs[0].shape[0]) * (xs[0].shape[2] // mod.stride) * (xs[0].shape[3] // mod.stride)
     check_norms([mod], batch_stats, pixels, [label], per_item)
-    return (MultiSourceConvItemsFn if per_item else MultiSourceConvFn).apply(mod, len(xs), *xs, *stack_params([mod]))
+    return ConvChainFn.apply([mod], len(xs), per_item, *xs, None, *stack_params([mod]))

@@ -1,5 +1,5 @@
 // Backward of the gated 3x3 stride-1 convs (the residual blocks EBlock / DBlock, READ/models/unet.py:56-76, and the single convs
-// around them) for bf16 training (read_b200/blocks.py: ResStackFn, GatedConvFn).  Per conv, last to first:
+// around them) for bf16 training (read_b200/blocks.py: ConvChainFn, conv_backward).  Per conv, last to first:
 //   gate backward    one elementwise pass over dY and the recomputed pre-activation [f | m] -> [df | dm] (bf16) and the fp32
 //                    per-channel sums dbias_f, dbias_m, dgamma, dbeta of the eval-mode BatchNorm
 //   input gradient   the TMA wgmma conv kernel in RAW mode over [df | dm] with flipped, transposed filters
@@ -7,7 +7,7 @@
 //                    8-channel input (the descriptor pyramid) has its own kernel in this file (dgrad_cin8_kernel)
 //   weight gradient  dW[2C][9][Cin] = sum over pixels of [df | dm]^T x im2col(x): the tensor-core kernel of this file
 //                    (wgrad_kernel; its three entry points launch it through wgrad_launch)
-// The 1x1 and stride-2 3x3 / 4x4 convs of train_precision 'bf16_all' (blocks.py: MultiSourceConvFn) use the same gate backward,
+// The 1x1 and stride-2 3x3 / 4x4 convs of train_precision 'bf16_all' (blocks.py: gated_conv_srcs) use the same gate backward,
 // the weight-gradient kernel's other instances (read_conv_wgrad) and, for a stride-2 conv, the input-gradient kernel
 // dgrad_s2_kernel of this file; a 1x1 conv's input gradient is a RAW 1x1 plan of the TMA kernel.
 // Both kernels read [f | m] / [df | dm] rows in the column order of the forward RAW output: blocks of 2*half columns

@@ -241,7 +241,7 @@ def main():
             row[kname + "_us"] = a.elapsed_time(b) / 20 * 1e3
         single.append(row)
 
-    # forward + backward of the 14 single convs at their C5 shapes, fp32 (torch / cuDNN) against bf16 (GatedConvFn)
+    # forward + backward of the 14 single convs at their C5 shapes, fp32 (torch / cuDNN) against bf16 (blocks.gated_conv)
     shapes = [("feat_extract.0", 256), ("feat_extract.5", 256)] + \
              [(f"SCM{i}.main.{j}", 32 << i) for i in range(3) for j in (0, 2)] + \
              [(f"AFFs.{i}.conv.1", 256 >> i) for i in range(3)] + [(f"FAM{i}.merge", 32 << i) for i in range(3)]
@@ -277,7 +277,7 @@ def main():
         runs[tp]["opt_net"].zero_grad(set_to_none=True)
 
     # the 21 1x1 / stride-2 convs at C5: (layer, sources' (channels, resolution)); forward + backward in fp32 (torch, the concat
-    # on torch) against bf16_all (MultiSourceConvFn, a virtual concat), and per conv the backward's pieces
+    # on torch) against bf16_all (blocks.gated_conv_srcs, a virtual concat), and per conv the backward's pieces
     new_convs = [("feat_extract.1", [(32, 256)]), ("feat_extract.2", [(64, 128)]), ("feat_extract.6", [(128, 64)]),
                  ("feat_extract.7", [(256, 32)]), ("feat_extract.3", [(128, 64)]), ("feat_extract.4", [(64, 128)]),
                  ("Convs.0", [(128, 64)] * 2), ("Convs.1", [(64, 128)] * 2), ("Convs.2", [(32, 256)] * 2)] + \
@@ -337,14 +337,9 @@ def main():
                                                 dwf.data_ptr(), dwm.data_ptr(), st))
 
             def dgrad():
-                if fc.stride == 2:
-                    dx = torch.empty_like(ts[0])
-                    L.check(lib.read_conv_dgrad_s2(dfm.data_ptr(), blocks.dgrad_s2_filters(fc).data_ptr(), B_, Ho, Wo, C,
-                                                   ts[0].shape[3], fc.k, dx.data_ptr(), st))
-                    return
                 c0 = 0
                 for t in ts:
-                    blocks.dgrad_1x1(dfm, fc, c0, t.shape[3])
+                    blocks.input_grad(dfm, fc, t, c0)
                     c0 += t.shape[3]
             fns = {
                 "raw_recompute": lambda: blocks.recompute_fm(lib, ts, fc),

@@ -132,22 +132,20 @@ def test_dgrad_raw3x3_is_exact(case):
 
 @gpu
 @pytest.mark.parametrize("case", U.DGRAD1_CASES, ids=lambda c: "src{}-C{}-B{}-{}x{}".format("_".join(map(str, c[0])), *c[1:]))
-def test_dgrad_raw1x1_is_exact_per_source(case):
+def test_dgrad_raw1x1_plans_are_exact_per_source(case):
     srcs, C, B, H, W = case
     lib = L.load()
     cin = sum(srcs)
     dcat, wcat, _ = _dgrad_operands(case, B, H, W, C, cin, 1, U.PADDED.get((1, 1, srcs[0], C)) if len(srcs) == 1 else None)
-    c = blocks._Filters({'wf': wcat[:C].contiguous(), 'wm': wcat[C:].contiguous(), 'w_dgrad': None}, C, 1, 1)
+    c = types.SimpleNamespace(pk={'wf': wcat[:C].contiguous(), 'wm': wcat[C:].contiguous()}, C=C)
     dfm = U.to_raw(dcat).bfloat16().contiguous()
     want = U.dgrad_ref(dcat, wcat, H, W, 1)
     _nonrep_ok(want, f"dgrad 1x1 {case}")
     names = ["b", "y", "x", "c"]
     c0 = 0
     for cs in srcs:
-        for a in range(c0, c0 + cs, 128):
-            cn = min(128, c0 + cs - a)
+        for a, cn, w in blocks._dgrad1x1_filters(lib, c.pk, C, c0, cs):
             n_out = max(cn, 32)
-            w = blocks._dgrad1x1_filters(lib, c, a, cn, dev())
             out = U.Guarded(B * H * W * n_out, torch.bfloat16, dev())
             zeros = torch.zeros(n_out // 2, dtype=torch.float32, device=dev())
             blocks._launch(lib, dfm, n_out // 2, w, (zeros,) * 4, False, L.OUT_RAW_NHWC, out.out, k=1)

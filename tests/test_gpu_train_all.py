@@ -1,5 +1,5 @@
 """-m gpu: bf16 training of the 21 gated 1x1 and stride-2 convs under train_precision='bf16_all' (read_b200/blocks.py:
-MultiSourceConvFn, csrc/conv_bwd.cu) against torch autograd.
+gated_conv_srcs, csrc/conv_bwd.cu) against torch autograd.
 
 Tolerances as for the block stacks (tests/test_gpu_train_blocks.py):
 * one conv of every row (every C) of the 1x1 / stride-2 convs, on ragged B = 2 shapes (stride 2 at even H, W that are not

@@ -1,8 +1,8 @@
-"""-m gpu: bf16 training of the 14 gated 3x3 stride-1 convs outside the residual blocks (read_b200/blocks.py: GatedConvFn,
+"""-m gpu: bf16 training of the 14 gated 3x3 stride-1 convs outside the residual blocks (read_b200/blocks.py: gated_conv,
 csrc/conv_bwd.cu) against torch autograd.
 
 Tolerances as for the block stacks (tests/test_gpu_train_blocks.py):
-* one conv of every row of unet.layer_table that trains through GatedConvFn, at every C it has, on ragged B = 2 shapes, against
+* one conv of every row of unet.layer_table that trains through gated_conv, at every C it has, on ragged B = 2 shapes, against
   float64 autograd of the same module: the output and every gradient (input, conv_f / conv_m weight and bias, BatchNorm weight
   and bias) within relative L2 error 2e-2 and cosine >= 0.999; FAM as a + merge(a * b), the gradients of a and b included;
 * the 8-channel input-gradient kernel alone against torch.nn.grad.conv2d_input on the same bf16 operands: relative L2 <= 1e-3;
@@ -90,7 +90,7 @@ def test_conv_forward_and_grads_match_fp64_autograd(name, cin, cout, elu, B, H, 
 @pytest.mark.parametrize("C,B,H,W", [(64, 2, 45, 67), (128, 2, 29, 35), (256, 2, 13, 19)])
 @pytest.mark.parametrize("fused", [False, True], ids=["torch_sum", "residual"])
 def test_fam_merge_matches_fp64_autograd(C, B, H, W, fused):
-    """a + merge(a * b): with the sum on torch (the net's routing) and through GatedConvFn's residual operand."""
+    """a + merge(a * b): with the sum on torch (the net's routing) and through gated_conv's residual operand."""
     m = _conv(C, C, False, seed=C + H)
     g = torch.Generator().manual_seed(C * H)
     a, b = torch.randn((B, C, H, W), generator=g), torch.rand((B, C, H, W), generator=g)

@@ -1,16 +1,16 @@
-"""-m gpu: per-element checks of the bf16 training autograd Functions of read_b200/blocks.py against the float64 replay of their
+"""-m gpu: per-element checks of the bf16 training autograd Function of read_b200/blocks.py against the float64 replay of its
 launches (tests/train_fn_exact_util.py states the method).
 
-* exact tier, eval-mode BatchNorm: ResStackFn at C = 32 / 64 / 128 / 256 (the role-swapped streamed-weight body with R = 16 and
-  R = 17 tiles), B = 1 / 2 / 3, one pixel wide, a frozen stack and one whose input needs no gradient; GatedConvFn on every
-  3x3 stride-1 row of unet.layer_table outside the stacks (FAM*.merge with its residual); MultiSourceConvFn on every 1x1 and
+* exact tier, eval-mode BatchNorm: block stacks at C = 32 / 64 / 128 / 256 (the role-swapped streamed-weight body with R = 16
+  and R = 17 tiles), B = 1 / 2 / 3, one pixel wide, a frozen stack and one whose input needs no gradient; single convs on every
+  3x3 stride-1 row of unet.layer_table outside the stacks (FAM*.merge with its residual); gated_conv_srcs on every 1x1 and
   stride-2 row.  Every element of the output, the input gradients, dwf, dbias_f, dgamma and dbeta equals the replay; dwm and
   dbias_m are exactly 0; a residual's gradient is the output gradient bit for bit; the folded scale / shift are the intended
   values.  Under torch.use_deterministic_algorithms(True) the same call gives the same bits.
-* train-mode BatchNorm (batch and per-item statistics), GatedConvFn and MultiSourceConvFn on the same operands: the output is a
+* train-mode BatchNorm (batch and per-item statistics), single convs and gated_conv_srcs on the same operands: the output is a
   bit-exact replay of bn_apply with the Function's own statistics, and dbeta (a sum of integer output gradients over every
   item) is exact, with and without the deterministic entry points.
-* bounded tier, GatedConvFn and MultiSourceConvFn in eval, batch and per-item modes, with and without the deterministic entry
+* bounded tier, single convs and gated_conv_srcs in eval, batch and per-item modes, with and without the deterministic entry
   points: unpinned gates (saturated and cancelling sigmoid, nonzero m filters) and ELU's negative branch; every element of the
   output, the input gradients, dwf, dwm, dbias_f, dbias_m and dgamma within its bound, dbeta exact.  The worst err / bound of
   each output is printed.
@@ -43,7 +43,7 @@ def _function_node(out):
         if n is None or id(n) in seen:
             continue
         seen.add(id(n))
-        if hasattr(n, "conv") or hasattr(n, "convs"):
+        if hasattr(n, "convs"):
             return n
         todo += [f for f, _ in n.next_functions]
     raise AssertionError("no blocks Function in the graph")
@@ -76,7 +76,7 @@ def _call(case, mods, xs, res, gout, mode, det):
         torch.cuda.synchronize()
     finally:
         torch.use_deterministic_algorithms(prev)
-    convs = node.convs if case.family == "stack" else [node.conv]
+    convs = node.convs
     grads = []
     for m in ms:
         b = m.block

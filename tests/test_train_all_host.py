@@ -19,10 +19,11 @@ NEW = ({f"feat_extract.{i}" for i in (1, 2, 3, 4, 6, 7)} | {f"Convs.{i}" for i i
 SOURCES = {**{f"AFFs.{i}.conv.0": 4 for i in range(3)}, **{f"Convs.{i}": 2 for i in range(3)}}
 
 
-def test_bf16_all_routing_sends_each_conv_to_one_path(monkeypatch):
-    """Spies stand in for the CUDA Functions: no conv through GatedConv.forward, the 21 1x1 / stride-2 convs through
-    MultiSourceConvFn (AFFs.*.conv.0 with 4 sources, Convs.* with 2, every other one with 1), the 14 single 3x3 stride-1 convs
-    through GatedConvFn, the 64 block convs through res_stack; each conv once, and every used parameter gets a gradient."""
+def test_bf16_all_routing_sends_each_conv_through_one_call(monkeypatch):
+    """A spy stands in for the CUDA Function: no conv through GatedConv.forward, the 21 1x1 / stride-2 convs through
+    gated_conv_srcs (AFFs.*.conv.0 with 4 sources, Convs.* with 2, every other one with 1), the 14 single 3x3 stride-1 convs
+    through gated_conv, the 64 block convs through res_stack (8 convs a call); each conv once, and every used parameter gets a
+    gradient."""
     assert len(SINGLE) == 14 and len(BLOCKS) == 64 and len(NEW) == 21
     net = UNet().eval()
     net.train_precision = 'bf16_all'
@@ -34,35 +35,28 @@ def test_bf16_all_routing_sends_each_conv_to_one_path(monkeypatch):
         torch_calls.append(names[id(self)])
         return orig(self, x)
 
-    class SpySingle:
-        @staticmethod
-        def apply(x, residual, mod, *params):
-            single_calls.append(names[id(mod)])
-            y = orig(mod, x)
-            return y if residual is None else y + residual
-
-    class SpyNew:
-        @staticmethod
-        def apply(mod, n_src, *args):
-            xs, params = args[:n_src], args[n_src:]
-            assert len(params) == 6 and params[0] is mod.block['conv_f'].weight
-            name = names[id(mod)]
+    def spy_apply(mods, n_src, per_item, *tensors):
+        xs, residual, params = tensors[:n_src], tensors[n_src], tensors[n_src + 1:]
+        assert len(params) == 6 * len(mods) and params[0] is mods[0].block['conv_f'].weight and not per_item
+        if len(mods) == 8:
+            for m in mods:
+                stack_calls.append(names[id(m)])
+            x = xs[0]
+            for r in range(0, 8, 2):
+                x = orig(mods[r + 1], orig(mods[r], x)) + x
+            return x
+        mod, = mods
+        name = names[id(mod)]
+        if (mod.k, mod.stride) == (3, 1):
+            single_calls.append(name)
+        else:
             assert name not in new_calls, name
             new_calls[name] = n_src
-            return orig(mod, torch.cat(xs, 1) if n_src > 1 else xs[0])
-
-    def spy_stack(net_, prefix, x):
-        for m in blocks.stack_convs(net_, prefix):
-            stack_calls.append(names[id(m)])
-        for r in range(net_.num_res):
-            p = f"{prefix}.layers.{r}"
-            x = orig(net_.get_submodule(p + ".main.1"), orig(net_.get_submodule(p + ".main.0"), x)) + x
-        return x
+        y = orig(mod, torch.cat(xs, 1) if n_src > 1 else xs[0])
+        return y if residual is None else y + residual
 
     monkeypatch.setattr(GatedConv, 'forward', spy_forward)
-    monkeypatch.setattr(blocks, 'GatedConvFn', SpySingle)
-    monkeypatch.setattr(blocks, 'MultiSourceConvFn', SpyNew)
-    monkeypatch.setattr(blocks, 'res_stack', spy_stack)
+    monkeypatch.setattr(blocks.ConvChainFn, 'apply', spy_apply)
     g = torch.Generator().manual_seed(0)
     xs = [torch.rand((1, 8, 32 >> l, 32 >> l), generator=g) for l in range(4)]
     out = net(*xs)
@@ -107,6 +101,11 @@ def test_gated_conv_srcs_rejects_what_it_does_not_run():
 
 def test_padded_channels():
     assert [blocks.padded_channels(c) for c in (3, 16, 32, 56, 64, 120, 128, 248, 256)] == [16, 16, 32, 64, 64, 128, 128, 256, 256]
+    # every 3x3 conv of the net runs at max(C, 16): the RGB output conv (C = 3) at 16, every other one at its own C
+    rows = [(name, cout) for name, cin, cout, k, s, _ in layer_table() if k == 3]
+    assert {cout for _, cout in rows} == {3, 16, 32, 64, 128, 256}
+    for name, cout in rows:
+        assert blocks.padded_channels(cout) == max(cout, 16), name
 
 
 P, ODD = 0x1000, 0x1008

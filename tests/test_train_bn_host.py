@@ -15,7 +15,7 @@ NEW = ({f"feat_extract.{i}" for i in (1, 2, 3, 4, 6, 7)} | {f"Convs.{i}" for i i
 
 
 def _spy_run(monkeypatch, tp):
-    """The net in train() under ``tp``, with spies standing in for the CUDA Functions; returns the convs each path saw."""
+    """The net in train() under ``tp``, with a spy standing in for the CUDA Function; returns the convs each path saw."""
     net = UNet().train()
     net.train_precision = tp
     names = {id(m): n for n, m in net.named_modules()}
@@ -26,43 +26,30 @@ def _spy_run(monkeypatch, tp):
         seen["torch"].append(names[id(self)])
         return orig(self, x)
 
-    class SpySingle:
-        @staticmethod
-        def apply(x, residual, mod, *params):
-            assert mod.block['norm'].training and len(params) == 6
-            seen["single"].append(names[id(mod)])
-            y = orig(mod, x)
-            return y if residual is None else y + residual
-
-    class SpyMulti:
-        @staticmethod
-        def apply(mod, n_src, *args):
-            assert mod.block['norm'].training
-            seen["multi"].append(names[id(mod)])
-            xs = args[:n_src]
-            return orig(mod, torch.cat(xs, 1) if n_src > 1 else xs[0])
-
-    def spy_stack(net_, prefix, x, batch_stats=False):
-        assert batch_stats
-        for m in blocks.stack_convs(net_, prefix):
-            assert m.block['norm'].training
-            seen["stack"].append(names[id(m)])
-        for r in range(net_.num_res):
-            p = f"{prefix}.layers.{r}"
-            x = orig(net_.get_submodule(p + ".main.1"), orig(net_.get_submodule(p + ".main.0"), x)) + x
-        return x
+    def spy_apply(mods, n_src, per_item, *tensors):
+        xs, residual = tensors[:n_src], tensors[n_src]
+        assert all(m.block['norm'].training for m in mods) and len(tensors) == n_src + 1 + 6 * len(mods) and not per_item
+        if len(mods) == 8:
+            for m in mods:
+                seen["stack"].append(names[id(m)])
+            x = xs[0]
+            for r in range(0, 8, 2):
+                x = orig(mods[r + 1], orig(mods[r], x)) + x
+            return x
+        mod, = mods
+        seen["single" if (mod.k, mod.stride) == (3, 1) else "multi"].append(names[id(mod)])
+        y = orig(mod, torch.cat(xs, 1) if n_src > 1 else xs[0])
+        return y if residual is None else y + residual
 
     monkeypatch.setattr(GatedConv, 'forward', spy_forward)
-    monkeypatch.setattr(blocks, 'GatedConvFn', SpySingle)
-    monkeypatch.setattr(blocks, 'MultiSourceConvFn', SpyMulti)
-    monkeypatch.setattr(blocks, 'res_stack', spy_stack)
+    monkeypatch.setattr(blocks.ConvChainFn, 'apply', spy_apply)
     g = torch.Generator().manual_seed(0)
     out = net(*[torch.rand((1, 8, 32 >> l, 32 >> l), generator=g) for l in range(4)])
     out.mean().backward()
     return seen
 
 
-def test_bf16_all_in_train_mode_sends_every_conv_through_batch_statistics(monkeypatch):
+def test_bf16_all_in_train_mode_runs_every_conv_with_batch_statistics(monkeypatch):
     seen = _spy_run(monkeypatch, 'bf16_all')
     assert seen["torch"] == []
     assert len(seen["stack"]) == len(set(seen["stack"])) == 64 and set(seen["stack"]) == BLOCKS
@@ -70,7 +57,7 @@ def test_bf16_all_in_train_mode_sends_every_conv_through_batch_statistics(monkey
     assert len(seen["multi"]) == len(set(seen["multi"])) == 21 and set(seen["multi"]) == NEW
 
 
-def test_bf16_in_train_mode_keeps_the_21_convs_on_torch(monkeypatch):
+def test_bf16_in_train_mode_leaves_the_21_convs_to_torch(monkeypatch):
     seen = _spy_run(monkeypatch, 'bf16')
     assert len(seen["stack"]) == 64 and len(seen["single"]) == 14 and seen["multi"] == []
     assert len(seen["torch"]) == len(set(seen["torch"])) == 21 and set(seen["torch"]) == NEW

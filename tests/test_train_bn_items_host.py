@@ -72,7 +72,7 @@ def test_per_item_fp32_in_float64_equals_single_item_calls():
 
 
 def _spy_run(monkeypatch, tp, tb, B=3):
-    """The net in train() under ``tp`` / ``tb``, with spies standing in for the CUDA Functions and the per-item torch path; returns
+    """The net in train() under ``tp`` / ``tb``, with spies standing in for the CUDA Function and the per-item torch path; returns
     the convs each path saw and the batch sizes F.batch_norm was called with."""
     net = UNet().train()
     net.train_precision, net.train_batchnorm = tp, tb
@@ -92,41 +92,26 @@ def _spy_run(monkeypatch, tp, tb, B=3):
         seen["bn"].append(x.shape[0])
         return orig_bn(x, *a, **kw)
 
-    def fn(key, per_item):
-        class Spy:
-            @staticmethod
-            def apply(*args):
-                if key == "single":
-                    x, residual, mod = args[:3]
-                    xs = [x]
-                else:
-                    mod, n_src = args[:2]
-                    xs, residual = args[2:2 + n_src], None
-                assert mod.block['norm'].training
-                seen[key + ("_item" if per_item else "")].append(names[id(mod)])
-                x = torch.cat(xs, 1) if len(xs) > 1 else xs[0]
-                y = orig_item(mod, x) if per_item else orig(mod, x)
-                return y if residual is None else y + residual
-        return Spy
-
-    def spy_stack(net_, prefix, x, batch_stats=False, per_item=False):
-        assert batch_stats
-        for m in blocks.stack_convs(net_, prefix):
-            seen["stack_item" if per_item else "stack"].append(names[id(m)])
-        f = orig_item if per_item else orig
-        for r in range(net_.num_res):
-            p = f"{prefix}.layers.{r}"
-            x = f(net_.get_submodule(p + ".main.1"), f(net_.get_submodule(p + ".main.0"), x)) + x
-        return x
+    def spy_apply(mods, n_src, per_item, *tensors):
+        xs, residual = tensors[:n_src], tensors[n_src]
+        assert all(m.block['norm'].training for m in mods) and len(tensors) == n_src + 1 + 6 * len(mods)
+        f, tag = (orig_item, "_item") if per_item else (orig, "")
+        if len(mods) == 8:
+            for m in mods:
+                seen["stack" + tag].append(names[id(m)])
+            x = xs[0]
+            for r in range(0, 8, 2):
+                x = f(mods[r + 1], f(mods[r], x)) + x
+            return x
+        mod, = mods
+        seen[("single" if (mod.k, mod.stride) == (3, 1) else "multi") + tag].append(names[id(mod)])
+        y = f(mod, torch.cat(xs, 1) if n_src > 1 else xs[0])
+        return y if residual is None else y + residual
 
     monkeypatch.setattr(GatedConv, 'forward', spy_forward)
     monkeypatch.setattr(unet_mod, 'gated_conv_per_item', spy_item)
     monkeypatch.setattr(torch.nn.functional, 'batch_norm', spy_bn)
-    monkeypatch.setattr(blocks, 'GatedConvFn', fn("single", False))
-    monkeypatch.setattr(blocks, 'GatedConvItemsFn', fn("single", True))
-    monkeypatch.setattr(blocks, 'MultiSourceConvFn', fn("multi", False))
-    monkeypatch.setattr(blocks, 'MultiSourceConvItemsFn', fn("multi", True))
-    monkeypatch.setattr(blocks, 'res_stack', spy_stack)
+    monkeypatch.setattr(blocks.ConvChainFn, 'apply', spy_apply)
     out = net(*_inputs(B, 32, torch.Generator().manual_seed(0)))
     out.mean().backward()
     return seen
@@ -136,26 +121,26 @@ def _once(names, want):
     return len(names) == len(set(names)) == len(want) and set(names) == want
 
 
-def test_per_item_bf16_all_sends_every_conv_through_the_per_item_path(monkeypatch):
+def test_per_item_bf16_all_runs_every_conv_with_per_item_statistics(monkeypatch):
     seen = _spy_run(monkeypatch, 'bf16_all', 'per_item')
     assert _once(seen["stack_item"], BLOCKS) and _once(seen["single_item"], SINGLE) and _once(seen["multi_item"], NEW)
     assert not (seen["torch"] or seen["torch_item"] or seen["stack"] or seen["single"] or seen["multi"])
 
 
-def test_per_item_bf16_puts_the_21_torch_norms_through_per_item_batch_norm(monkeypatch):
+def test_per_item_bf16_normalises_the_21_torch_convs_per_item(monkeypatch):
     seen = _spy_run(monkeypatch, 'bf16', 'per_item')
     assert _once(seen["stack_item"], BLOCKS) and _once(seen["single_item"], SINGLE)
     assert _once(seen["torch_item"], NEW) and seen["torch"] == [] and seen["multi_item"] == []
     assert seen["bn"] == [1] * (3 * 99)         # the spies of the kernels' paths normalise per item on torch too
 
 
-def test_per_item_fp32_normalises_every_norm_per_item(monkeypatch):
+def test_per_item_fp32_normalises_every_conv_per_item_on_torch(monkeypatch):
     seen = _spy_run(monkeypatch, 'fp32', 'per_item')
     assert _once(seen["torch_item"], BLOCKS | SINGLE | NEW) and seen["torch"] == []     # 99 convs: ConvsOut.* are unused
     assert seen["bn"] == [1] * (3 * 99)
 
 
-def test_batch_mode_is_unchanged(monkeypatch):
+def test_batch_mode_takes_no_per_item_path(monkeypatch):
     seen = _spy_run(monkeypatch, 'bf16_all', 'batch')
     assert _once(seen["stack"], BLOCKS) and _once(seen["single"], SINGLE) and _once(seen["multi"], NEW)
     assert not (seen["torch_item"] or seen["stack_item"] or seen["single_item"] or seen["multi_item"])

@@ -15,9 +15,9 @@ TORCH = ({f"feat_extract.{i}" for i in (1, 2, 3, 4, 6, 7)} | {f"Convs.{i}" for i
          | {f"AFFs.{i}.conv.0" for i in range(3)} | {f"SCM{i}.{n}" for i in range(3) for n in ("main.1", "main.3", "conv")})
 
 
-def test_bf16_routing_sends_each_conv_to_one_path(monkeypatch):
-    """The torch spies stand in for the CUDA Functions: 21 convs through GatedConv.forward, the 14 single 3x3 stride-1 convs
-    through GatedConvFn, the 64 block convs through res_stack, each conv once, in forward and backward."""
+def test_bf16_routing_sends_each_conv_through_one_call(monkeypatch):
+    """The torch spies stand in for the CUDA Function: 21 convs through GatedConv.forward, the 14 single 3x3 stride-1 convs
+    through gated_conv, the 64 block convs through res_stack (8 convs a call), each conv once, in forward and backward."""
     assert len(SINGLE) == 14 and len(BLOCKS) == 64 and len(TORCH) == 21
     net = UNet().eval()
     net.train_precision = 'bf16'
@@ -29,25 +29,24 @@ def test_bf16_routing_sends_each_conv_to_one_path(monkeypatch):
         torch_calls.append(names[id(self)])
         return orig(self, x)
 
-    class SpyFn:
-        @staticmethod
-        def apply(x, residual, mod, *params):
-            assert len(params) == 6 and params[0] is mod.block['conv_f'].weight
-            single_calls.append(names[id(mod)])
-            y = orig(mod, x)
-            return y if residual is None else y + residual
-
-    def spy_stack(net_, prefix, x):
-        for m in blocks.stack_convs(net_, prefix):
-            stack_calls.append(names[id(m)])
-        for r in range(net_.num_res):
-            p = f"{prefix}.layers.{r}"
-            x = orig(net_.get_submodule(p + ".main.1"), orig(net_.get_submodule(p + ".main.0"), x)) + x
-        return x
+    def spy_apply(mods, n_src, per_item, *tensors):
+        xs, residual, params = tensors[:n_src], tensors[n_src], tensors[n_src + 1:]
+        assert len(params) == 6 * len(mods) and params[0] is mods[0].block['conv_f'].weight and not per_item
+        if len(mods) == 8:
+            for m in mods:
+                stack_calls.append(names[id(m)])
+            x = xs[0]
+            for r in range(0, 8, 2):
+                x = orig(mods[r + 1], orig(mods[r], x)) + x
+            return x
+        mod, = mods
+        assert (mod.k, mod.stride) == (3, 1) and n_src == 1, names[id(mod)]
+        single_calls.append(names[id(mod)])
+        y = orig(mod, xs[0])
+        return y if residual is None else y + residual
 
     monkeypatch.setattr(GatedConv, 'forward', spy_forward)
-    monkeypatch.setattr(blocks, 'GatedConvFn', SpyFn)
-    monkeypatch.setattr(blocks, 'res_stack', spy_stack)
+    monkeypatch.setattr(blocks.ConvChainFn, 'apply', spy_apply)
     g = torch.Generator().manual_seed(0)
     xs = [torch.rand((1, 8, 32 >> l, 32 >> l), generator=g) for l in range(4)]
     out = net(*xs)

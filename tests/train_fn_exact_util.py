@@ -1,6 +1,6 @@
-"""Per-element checks of the bf16 training autograd Functions of read_b200/blocks.py (ResStackFn, GatedConvFn, MultiSourceConvFn and
-their per-item forms): a float64 replay of each Function's launch sequence, the exact-tier operands and their precondition, and
-the case lists; shared by test_train_fn_exact_host.py (no GPU) and test_gpu_train_fn_exact.py.
+"""Per-element checks of the bf16 training autograd Function of read_b200/blocks.py (ConvChainFn, as stack_forward, gated_conv and
+gated_conv_srcs call it, in every BatchNorm mode): a float64 replay of each call's launch sequence, the exact-tier operands and
+their precondition, and the case lists; shared by test_train_fn_exact_host.py (no GPU) and test_gpu_train_fn_exact.py.
 
 The replay follows the launches the Functions document and rounds to bf16 (round to nearest even) where they do:
   forward   x -> NHWC bf16 (nchw_to_nhwc); each conv's output bf16(A(f + b_f) * sigmoid(m + b_m) * scale + shift [+ residual]),
@@ -49,8 +49,8 @@ NNZ = 2                     # nonzero f-filter taps per output channel (sparse: 
 # ---------------------------------------------------------------- cases
 @dataclasses.dataclass(frozen=True)
 class Case:
-    """One Function call.  family: 'stack' (ResStackFn, 8 convs at C = cin = cout), 'single' (GatedConvFn, 3x3 stride 1,
-    optional residual) or 'multi' (MultiSourceConvFn over ``srcs``, 1x1 or stride 2).  need: 'all', 'frozen' (no parameter
+    """One Function call.  family: 'stack' (stack_forward, 8 convs at C = cin = cout), 'single' (gated_conv, 3x3 stride 1,
+    optional residual) or 'multi' (gated_conv_srcs over ``srcs``, 1x1 or stride 2).  need: 'all', 'frozen' (no parameter
     needs a gradient) or 'no_x' (the input needs none)."""
     name: str
     family: str
@@ -89,7 +89,7 @@ def _stack(C, B, H, W, **kw):
     return Case(f"C{C}", "stack", (C,), C, 3, 1, B, H, W, **kw)
 
 
-# ResStackFn: C = 32 / 64 (weight-stationary bodies) and 128 / 256 (the role-swapped streamed-weight body, R = 16 on small
+# stacks: C = 32 / 64 (weight-stationary bodies) and 128 / 256 (the role-swapped streamed-weight body, R = 16 on small
 # images); B = 1, 2, 3; H, W multiples of none of 8, 16, 17; one pixel wide.  The large frozen / input-only cases reach R = 17
 # on a 132-SM H100 (test_gpu_train_fn_exact.py asserts which R each case gets).
 STACK_CASES = [
@@ -105,7 +105,7 @@ def _single(name, cin, cout, B, H, W, elu, residual=False, **kw):
     return Case(name, "single", (cin,), cout, 3, 1, B, H, W, elu=elu, residual=residual, **kw)
 
 
-# GatedConvFn: every row of unet.layer_table it runs (feat_extract.0 is the 8-channel dgrad_cin8 path, feat_extract.5 runs
+# single convs: every row of unet.layer_table they run (feat_extract.0 is the 8-channel dgrad_cin8 path, feat_extract.5 runs
 # padded to 16, FAM*.merge with its residual)
 SINGLE_CASES = [
     _single("feat_extract.0", 8, 32, 2, 9, 7, True),
@@ -129,7 +129,7 @@ def _multi(name, srcs, cout, k, stride, B, H, W, elu, **kw):
     return Case(name, "multi", tuple(srcs), cout, k, stride, B, H, W, elu=elu, **kw)
 
 
-# MultiSourceConvFn: every 1x1 and stride-2 row.  AFFs.*.conv.0 read four sources (480 channels, the 256-channel one split into
+# gated_conv_srcs: every 1x1 and stride-2 row.  AFFs.*.conv.0 read four sources (480 channels, the 256-channel one split into
 # two 128-channel input-gradient parts); SCM*.main.3 runs padded (C = 56 / 120 / 248) and, at 120 / 248, recomputes [f | m] per
 # 64-channel block; SCM0.conv has one 256-channel source; Convs.* read two sources of equal width.  Odd H, W for 1x1, even H, W
 # that are not multiples of 16 for stride 2.
@@ -514,7 +514,7 @@ def filter_coverage(mods):
 
 
 # ---------------------------------------------------------------- bounded tier
-# GatedConvFn / MultiSourceConvFn with unpinned gates, ELU's negative branch and every BatchNorm mode, held to per-element bounds.
+# single and multi-source convs with unpinned gates, ELU's negative branch and every BatchNorm mode, held to per-element bounds.
 # Integer inputs and dyadic filters keep the RAW [f | m] recompute exact, so the gate backward sees known bf16 operands and
 # bwd_exact_util.gate_ref bounds [df | dm] per element (REL_BF16 |want| + TAU T).  The statistics are re-anchored at the
 # Function's own (mean, inv_std, scale, shift read from its FoldedConv; bn_fwd_exact pins them per element).  sum dy is exact
