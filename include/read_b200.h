@@ -157,6 +157,33 @@ int read_raster_sprites_segments_culled(const float *pts4, int64_t n, const int3
                                         const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
                                         void *workspace, int64_t workspace_bytes, int B, int W, int H, int L,
                                         const read_sprite_desc *desc, uint64_t *zbuf, void *stream);
+/* Cylindrical panoramas (DESIGN.md §4.4).  view_m / seg_m hold WORLD -> CAMERA matrices (the inverse of a GL camera-to-world
+ * view matrix: x right, y up, looking down -z), [B,16] or [nseg, B, 16].  Per point, in IEEE float32 with no contraction:
+ *   (x, y, z) = rows 0-2 of m (p, 1), in the order of the pinhole path's dot products; f = -z; r = sqrt(x*x + f*f);
+ *   visible only if znear <= r <= zfar;  v = (t_hi - y / r) * k_h, visible only if 0 <= v < H, row = (int)v;
+ *   theta = atan2(x, f) from +, -, *, / (octant reduction and a degree-6 minimax polynomial; |theta| <= float32 pi);
+ *   u = (theta + theta_half) * k_w, col = (int)u; full: col == width wraps to 0, otherwise visible only if 0 <= u < width;
+ *   key = (bits(r) << 32) | id;  pixel (row, col + margin) of the level-0 plane, W = width + 2 margin columns wide;
+ *   full: a point with col < margin also goes to col + margin + width, one with col >= width - margin to col + margin - width.
+ * The constants come from read_b200/panorama.py (Panorama.desc), each computed in float64 and rounded once:
+ *   theta_half = hfov / 2 (float32 pi at 360 degrees), k_w = width / hfov, t_hi = tan(elevation hi), k_h = H / (t_hi - t_lo).
+ * width, margin and H are multiples of 16, 2 margin <= width <= READ_PANORAMA_MAX_WIDTH, margin = 0 unless full.  Level 0 only,
+ * into a cleared pyramid whose levels nest (finish with read_raster_derive_levels or read_pyramid_resolve_gather).  The two
+ * entry points take the stores and arguments of read_raster_project_sorted_views (B <= 8) and
+ * read_raster_project_segments_culled; the culled one drops a unit when, in every view, its box lies entirely beyond zfar. */
+#define READ_PANORAMA_MAX_WIDTH 65536
+typedef struct {
+    float theta_half, k_w, t_hi, k_h, znear, zfar;
+    int32_t width;                               /* W: columns of the panorama, margins excluded */
+    int32_t margin;                              /* M: wrapped columns drawn on each side (full circle only) */
+    int32_t full;                                /* 1: 360 degrees */
+} read_panorama_desc;
+int read_raster_panorama_sorted(const float *pts4, int64_t n, const float *view_m, int B, int W, int H, int L,
+                                const read_panorama_desc *desc, uint64_t *zbuf, void *stream);
+int read_raster_panorama_segments_culled(const float *pts4, int64_t n, const int32_t *seg_table, int nseg, int64_t nunits,
+                                         const float *chunk_boxes, const uint8_t *seg_visible, const float *seg_m,
+                                         void *workspace, int64_t workspace_bytes, int B, int W, int H, int L,
+                                         const read_panorama_desc *desc, uint64_t *zbuf, void *stream);
 /* Bitmask of levels rasterised with direct atomics (bit l set) for this geometry. */
 unsigned read_raster_direct_mask(int W, int H, int L);
 

@@ -63,6 +63,15 @@ class ReadSpriteDesc(ctypes.Structure):
     _fields_ = [("size", ctypes.c_float * MAX_LEVELS), ("relative", ctypes.c_int32 * MAX_LEVELS), ("point_sizes", c_vp)]
 
 
+PANORAMA_MAX_WIDTH = 65536  # READ_PANORAMA_MAX_WIDTH
+
+
+class ReadPanoramaDesc(ctypes.Structure):
+    _fields_ = [("theta_half", ctypes.c_float), ("k_w", ctypes.c_float), ("t_hi", ctypes.c_float), ("k_h", ctypes.c_float),
+                ("znear", ctypes.c_float), ("zfar", ctypes.c_float), ("width", ctypes.c_int32), ("margin", ctypes.c_int32),
+                ("full", ctypes.c_int32)]
+
+
 VIEW_MODES = {"color": 0, "normals": 1, "depth": 2, "uv": 3, "xyz": 4, "label": 5}   # READ_VIEW_*
 
 
@@ -123,6 +132,10 @@ _SIGS = {
                                              ctypes.POINTER(ReadSpriteDesc), c_vp, c_vp]),
     "read_raster_sprites_segments_culled": (c_int, [c_vp, c_i64, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int,
                                                     c_int, c_int, ctypes.POINTER(ReadSpriteDesc), c_vp, c_vp]),
+    "read_raster_panorama_sorted": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, ctypes.POINTER(ReadPanoramaDesc), c_vp,
+                                            c_vp]),
+    "read_raster_panorama_segments_culled": (c_int, [c_vp, c_i64, c_vp, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int,
+                                                     c_int, c_int, ctypes.POINTER(ReadPanoramaDesc), c_vp, c_vp]),
     "read_zbuf_resolve": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
     "read_pcpr_forward": (c_int, [c_vp, c_i64, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "read_texture_to_point_major": (c_int, [c_vp, c_int, c_i64, c_vp, c_vp]),

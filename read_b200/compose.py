@@ -25,6 +25,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from . import panorama as pano_mod
 from . import sprites
 from . import _lib as L
 from .texture import PointTexture, sample_items
@@ -53,6 +54,7 @@ class NetAndTexture(nn.Module):
         self._textures = {tid: tex.cpu() for tid, tex in textures.items()}        # parked until loaded
         self._loaded_textures = []
         self._fused = {}                             # state of the fused path: pyramid, staging buffers, temporal history
+        self._fused_pano = {}                        # the same for panoramas, so frames and panoramas keep their own histories
 
     # ------------------------------------------------------------------ texture residency (compose.py:102-123)
     def load_textures(self, texture_ids):
@@ -182,8 +184,8 @@ class NetAndTexture(nn.Module):
         return (out, net_input) if kwargs.get('return_input') else out
 
     # ------------------------------------------------------------------ fused fast path
-    def _fused_state(self, B, Wr, Hr, n_levels, device, staged, Hn, Wn):
-        st = self._fused
+    def _fused_state(self, B, Wr, Hr, n_levels, device, staged, Hn, Wn, st=None):
+        st = self._fused if st is None else st
         key = (B, Wr, Hr, n_levels, str(device), staged, Hn, Wn)
         if st.get('key') != key:
             st.clear()
@@ -198,7 +200,7 @@ class NetAndTexture(nn.Module):
 
     @torch.no_grad()
     def render(self, xyz, total_m, W, H, texture_id=0, n_levels=4, want_maps=False, return_input=False, clone_output=True,
-               seg_visible=None, input_format=None):
+               seg_visible=None, input_format=None, panorama=None):
         """points [N,3] (cuda f32) or an ``ops.SortedPoints`` store + total_m [B,4,4] (cuda f32) -> RGB [B,3,H,W] f32 (a fresh
         tensor), all on device, one pass over the cloud.  A sorted store serves frames whose levels nest; the result is
         bit-identical to rendering the unsorted cloud (the z-buffer is a min over (depth | original id) keys).
@@ -218,7 +220,13 @@ class NetAndTexture(nn.Module):
         ``input_format``: the checkpoint's format string; its first ``n_levels`` keys give each level's point size (``_pN`` /
         ``_psN``, read_b200.sprites), and a store's per-point sizes (``psize``) apply.  Frames with larger points are drawn as point
         sprites from the store (SortedPoints or SegmentedPoints, whose levels need not nest) and gathered level by level;
-        ``None`` (the default), or only 1-pixel levels and no per-point sizes, renders as without it."""
+        ``None`` (the default), or only 1-pixel levels and no per-point sizes, renders as without it.
+
+        ``panorama``: a ``read_b200.panorama.Panorama`` of ``W`` x ``H`` pixels, drawn from a store (SortedPoints or
+        SegmentedPoints) with ``total_m`` the world -> camera matrices (``Panorama.world_to_camera``; per segment for a segmented
+        store).  The pyramid and the net run at (W + 2 margin) x H, the result is the [B,3,H,W] crop without the margins;
+        ``want_maps`` and ``return_input`` give the full width, margins included.  Panoramas keep a temporal history of their own,
+        apart from the frames'.  Point sprites raise ValueError."""
         segmented = isinstance(xyz, ops.SegmentedPoints)
         store = xyz if segmented or isinstance(xyz, ops.SortedPoints) else None
         pts = store.pts4 if store is not None else xyz
@@ -229,10 +237,18 @@ class NetAndTexture(nn.Module):
         texture = self._texture(texture_id)
         B = total_m.shape[1] if segmented else total_m.shape[0]
         ss = int(self.ss)
+        if panorama is not None:
+            if store is None:
+                raise ValueError("read_b200: panoramas are drawn from an ops.SortedPoints or ops.SegmentedPoints store")
+            if (W, H) != (panorama.width, panorama.height):
+                raise ValueError(f"read_b200: W, H = {W}, {H} for a {panorama!r}")
+            margin = panorama.margin
+            W = panorama.plane_width                            # the pyramid and the net run with the margins
         Wr, Hr = W * ss, H * ss
         eng = self.net.engine(B, H, W, pts.device)
         staged = ss > 1 or bool(self.temporal_average)
-        st = self._fused_state(B, Wr, Hr, n_levels, pts.device, staged, H, W)
+        st = self._fused_state(B, Wr, Hr, n_levels, pts.device, staged, H, W,
+                               None if panorama is None else self._fused_pano)
         pyr = st['pyr']
         if not self.temporal_average:
             st['have_last'] = False
@@ -244,12 +260,23 @@ class NetAndTexture(nn.Module):
         sprite = levels is not None and not sprites.one_pixel(levels, store.psize if store is not None else None)
         if sprite and store is None:
             raise ValueError("read_b200: point sprites are drawn from an ops.SortedPoints or ops.SegmentedPoints store")
+        if sprite and panorama is not None:
+            raise ValueError("read_b200: panoramas draw 1-pixel points; point sprites (_pN / _psN keys, per-point sizes) are "
+                             "drawn on frames only")
         fused_ok = (not sprite and not want_maps and texture.activation == 'none'
                     and ops.fused_resolve_supported(pyr, tex.shape[1]))
 
         if not (fused_ok and st['clean']):
             pyr.clear()
-        if sprite:
+        if panorama is not None:
+            pr = panorama.scaled(ss)
+            if segmented:
+                pano_mod.raster_panorama_segments_culled(pyr, store, total_m, pr, seg_visible)
+            else:
+                pano_mod.raster_panorama_sorted(pyr, store, total_m, pr)
+            if not fused_ok:
+                ops.raster_derive(pyr)
+        elif sprite:
             ops.raster_project_sprites(pyr, store, total_m, levels, visible=seg_visible)
         elif store is not None:
             if pyr.direct_mask != 1:
@@ -277,7 +304,9 @@ class NetAndTexture(nn.Module):
                                                   int(st['have_last']), eng.act_code, eng.inputs[l].data_ptr(), sp))
             st['have_last'] = bool(self.temporal_average)
         out = eng.run()
-        if clone_output:                     # the engine's output buffer is reused by the next frame
+        if panorama is not None and margin:
+            out = out[..., margin:W - margin].contiguous()       # a fresh tensor without the wrapped columns
+        elif clone_output:                   # the engine's output buffer is reused by the next frame
             out = out.clone()
         extras = []
         if want_maps:

@@ -18,6 +18,15 @@ from .texture import PointTexture
 from .unet import UNet
 
 
+def _panorama_result(out, panorama, flip_vertical, net_input):
+    """``infer``'s result for a panorama: the displayable [H,W,4] surface of the net's [1,3,H,W] crop (alpha 1, flipped with
+    ``flip_vertical``) and the net input."""
+    H, W = panorama.height, panorama.width
+    rgba = torch.empty((H, W, 4), dtype=torch.float32, device=out.device)
+    L.check(L.load().read_frame_to_rgba(out.data_ptr(), H, W, int(flip_vertical), 1.0, rgba.data_ptr(), L.stream_ptr()))
+    return {'output': rgba, 'net_input': net_input}
+
+
 class FrameRenderer:
     def __init__(self, xyz, net_state_dict, texture, viewport_size, supersampling=1, temporal_average=False,
                  device=None, flip_vertical=False, n_levels=4, return_net_input=True, input_format=None, point_sizes=None,
@@ -119,6 +128,24 @@ class FrameRenderer:
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
                                              rgba.data_ptr(), L.stream_ptr()))
         return {'output': rgba, 'net_input': net_input}
+
+    def infer_panorama(self, view_matrix, panorama):
+        """A cylindrical panorama (read_b200.panorama.Panorama) from the camera ``view_matrix`` (camera-to-world, GL convention):
+        -> {'output': [H,W,4] f32 cuda tensor, 'net_input': the four [1,8,h,w] net inputs at the rendered width, margins
+        included (None with ``return_net_input=False``)}, as ``infer``.  Drawn from the sorted store (built here once if the
+        frame path keeps none); its temporal history is kept apart from ``infer``'s.  Point sprites raise ValueError."""
+        store = self.store
+        if store is None:
+            if self._points_store is None:
+                self._points_store = ops.SortedPoints(self.xyz)
+            store = self._points_store
+        m = self._upload_camera(panorama.world_to_camera(view_matrix))
+        with torch.no_grad():
+            res = self.model.render(store, m, panorama.width, panorama.height, n_levels=self.n_levels,
+                                    return_input=self.return_net_input, clone_output=False, input_format=self.input_format,
+                                    panorama=panorama)
+        out, net_input = res if self.return_net_input else (res, None)
+        return _panorama_result(out, panorama, self.flip_vertical, net_input)
 
     def render_points(self, proj_matrix, view_matrix, mode='color', submode=0, point_size=1, relative=False,
                       clear_color=(0., 0., 0., 1.)):
@@ -230,6 +257,23 @@ class SceneRenderer:
         L.check(L.load().read_frame_to_rgba(out.data_ptr(), self.H, self.W, int(self.flip_vertical), 1.0,
                                              rgba.data_ptr(), L.stream_ptr()))
         return {'output': rgba, 'net_input': net_input}
+
+    def infer_panorama(self, view_matrix, panorama):
+        """``FrameRenderer.infer_panorama`` for the composed scene: every segment drawn under
+        ``composer.segment_matrices(Panorama.world_to_camera(view_matrix))``, units beyond ``zfar`` in every view culled."""
+        comp = self.composer
+        if comp.texture is not self._tex:                # a scene was added: the composed descriptor table grew
+            self._tex = comp.texture
+            self.model._textures[0] = self._tex
+            self.model.add_module('0', self._tex.to(self.device))
+        store = comp.store
+        seg_m, visible = self._upload(comp.segment_matrices(panorama.world_to_camera(view_matrix)), store.visible_flags())
+        with torch.no_grad():
+            res = self.model.render(store, seg_m, panorama.width, panorama.height, n_levels=self.n_levels,
+                                    return_input=self.return_net_input, clone_output=False, seg_visible=visible,
+                                    input_format=self.input_format, panorama=panorama)
+        out, net_input = res if self.return_net_input else (res, None)
+        return _panorama_result(out, panorama, self.flip_vertical, net_input)
 
     def render_points(self, proj_matrix, view_matrix, mode='color', submode=0, point_size=1, relative=False,
                       clear_color=(0., 0., 0., 1.)):
